@@ -1,4 +1,4 @@
-"""alphafold2_b200 — B200-native (sm_100a) drop-in for the Evoformer trunk hot path of lucidrains/alphafold2.
+"""alphafold2_b200 — H100-native (sm_90a) drop-in for the Evoformer trunk hot path of lucidrains/alphafold2.
 
     from alphafold2_b200 import Alphafold2, Evoformer      # mirrors alphafold2_pytorch/__init__.py:1
 """

@@ -1,11 +1,11 @@
 """ctypes binding of libaf2b200.so (include/af2b200.h).  No torch extension, no pybind: the C ABI is the
 drop-in boundary.  There is deliberately NO fallback: if the library is missing or the device is not
-sm_100, every op raises."""
+sm_90 (H100), every op raises."""
 import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# AF2_LIB_PATH: A/B builds of the same library on one box (tools/gpu_ab.sh); never a different implementation
+# AF2_LIB_PATH: A/B builds of the same library on one machine; never a different implementation
 LIB_PATH = os.environ.get("AF2_LIB_PATH") or os.path.join(_HERE, "csrc", "libaf2b200.so")
 
 _lib = None
@@ -121,7 +121,7 @@ def load():
         if not os.path.isfile(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). alphafold2_b200 has no CPU or PyTorch fallback.")
+                "(nvcc, sm_90a). alphafold2_b200 has no CPU or PyTorch fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(lib, name)

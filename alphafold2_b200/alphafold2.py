@@ -3,7 +3,7 @@
 Same class names, constructor signatures, forward signatures and ``state_dict`` keys as
 ``alphafold2_pytorch/alphafold2.py`` (reference @ 931466e), so reference checkpoints load unchanged and the
 reference's own API smoke tests run against this package.  The forward bodies of every module on the hot
-path (alphafold2.py:69-467) call hand-written sm_100a kernels through the C ABI in include/af2b200.h;
+path (alphafold2.py:69-467) call hand-written sm_90a kernels through the C ABI in include/af2b200.h;
 there is no PyTorch / CPU fallback for them.  Glue outside the trunk (embeddings, pair initialisation,
 distogram head, alphafold2.py:676-726, 811-823) stays plain PyTorch on the device (SURVEY.md §8f n1).
 
@@ -127,7 +127,7 @@ def _forward_only(*tensors):
     """SURVEY.md 8(b) error convention: the kernels are not differentiable.  Silently detaching would return wrong
     (zero) gradients, so a call that autograd would have to record raises instead."""
     if torch.is_grad_enabled() and any(t is not None and torch.is_tensor(t) and t.requires_grad for t in tensors):
-        raise RuntimeError("alphafold2_b200 is forward-only (hand-written sm_100a kernels, no autograd): call it under "
+        raise RuntimeError("alphafold2_b200 is forward-only (hand-written sm_90a kernels, no autograd): call it under "
                            "torch.no_grad() or pass tensors that do not require grad")
 
 
@@ -196,7 +196,7 @@ class Attention(nn.Module):
 
     def forward(self, x, mask=None, attn_bias=None, context=None, context_mask=None, tie_dim=None):
         raise NotImplementedError(
-            "alphafold2_b200.Attention is only executed through AxialAttention (fused sm_100a kernel); "
+            "alphafold2_b200.Attention is only executed through AxialAttention (fused sm_90a kernel); "
             "cross-attention / tied-row attention (templates, extra-MSA stack) are outside the hot path, see DESIGN.md")
 
 
@@ -495,7 +495,7 @@ class Alphafold2(nn.Module):
         _forward_only(seq_embed, msa_embed, embedds)
         for name, val in (("templates_feats", templates_feats), ("templates_angles", templates_angles), ("recyclables", recyclables)):
             if exists(val):
-                raise NotImplementedError(f"{name}: templates / recycling are outside the B200 hot path (SURVEY.md §8f n3 / n4)")
+                raise NotImplementedError(f"{name}: templates / recycling are outside the trunk hot path (SURVEY.md §8f n3 / n4)")
         if self.training and not self._warned_training:
             warnings.warn("alphafold2_b200 is forward-only: running inference semantics (no MLM noising, no autograd)")
             self._warned_training = True
@@ -572,4 +572,4 @@ class Alphafold2(nn.Module):
                 return ret
         raise NotImplementedError(
             "predict_coords=True needs the third-party IPABlock / pytorch3d structure module "
-            "(alphafold2.py:19-20, 841-905), which the reference does not vendor; outside the B200 hot path")
+            "(alphafold2.py:19-20, 841-905), which the reference does not vendor; outside the trunk hot path")

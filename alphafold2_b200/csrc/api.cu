@@ -58,7 +58,7 @@ int sm_count() {
   const int dev = cur_dev();
   if (n[dev] == 0) {
     cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (n[dev] <= 0) n[dev] = 148;
+    if (n[dev] <= 0) n[dev] = 132;
   }
   return n[dev];
 }
@@ -307,52 +307,18 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
   p.cm_inner = c.cm_inner > 0 ? c.cm_inner : 1; p.cm_pitch = c.cm_pitch > 0 ? c.cm_pitch : 1;
   p.tile.mode = c.mode; p.tile.act = c.act; p.tile.layout = c.layout; p.tile.use_rowscale = c.use_rowscale;
   p.tile.out = c.out; p.tile.bias = c.bias; p.tile.ld = c.ld_out;
-  // ---- output path: TMA store through swizzled smem staging whenever the output is a legal TMA tensor ----
-  const bool out_f32 = (c.mode == EPI_RESID_F32 || c.mode == EPI_STORE_F32);
-  const int es = out_f32 ? 4 : 2;
-  const int W = (c.mode == EPI_GATED_BF16) ? BN / 2 : BN;
-  bool direct = false;
-  if (!out_f32 && (W % 64) != 0) direct = true;
-  if ((reinterpret_cast<uintptr_t>(c.out) & 15) != 0) direct = true;
-  if (c.layout == LAYOUT_TOKEN) {
-    if ((c.ld_out * es) % 16 != 0) direct = true;
-    if (c.batch > 1 && (c.out_batch * es) % 16 != 0) direct = true;
-  } else {
-    if (c.cm_pitch != c.cm_inner || (c.ld_out * 2) % 16 != 0 || c.batch != 1 || out_f32) direct = true;
-  }
-  if (c.mode == EPI_RESID_F32 && ((c.ld_resid * 4) % 16 != 0 || (reinterpret_cast<uintptr_t>(c.resid) & 15) != 0)) direct = true;
-  // warp-autonomous residual epilogue: one column tile, one batch, whole accumulator tile valid
-  const bool resid_w = !direct && c.mode == EPI_RESID_F32 && BN == 256 && !c.mn_major && c.batch == 1 && c.N <= 256 &&
-                       p.out_cols == 256;
-  CUtensorMap tc = ta, tr = ta;
-  if (!direct) {
-    const CUtensorMapDataType dt = out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    if (c.layout == LAYOUT_TOKEN) {
-      unsigned long long dc[3] = {(unsigned long long)p.out_cols, (unsigned long long)c.M, (unsigned long long)c.batch};
-      unsigned long long sc[2] = {(unsigned long long)c.ld_out * es, (unsigned long long)(c.batch > 1 ? c.out_batch : c.ld_out * c.M) * es};
-      unsigned bc[3] = {(unsigned)(out_f32 ? 32 : 64), (unsigned)(resid_w ? 32 : 128), 1};
-      AF2_TRY(make_tmap(&tc, c.out, 3, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B, dt));
-      if (c.mode == EPI_RESID_F32) {
-        unsigned long long sr[2] = {(unsigned long long)c.ld_resid * 4, (unsigned long long)c.ld_resid * c.M * 4};
-        AF2_TRY(make_tmap(&tr, c.resid, 3, dc, sr, bc, CU_TENSOR_MAP_SWIZZLE_128B, dt));
-      }
-    } else {
-      unsigned long long dc[3] = {(unsigned long long)c.M, (unsigned long long)p.out_cols, 1ull};
-      unsigned long long sc[2] = {(unsigned long long)c.ld_out * 2, (unsigned long long)c.ld_out * p.out_cols * 2};
-      unsigned bc[3] = {64, 64, 1};
-      AF2_TRY(make_tmap(&tc, c.out, 3, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B, dt));
-    }
-  }
-  p.direct = direct ? 1 : 0;
+  // the epilogue stores straight from the accumulator registers: no output / residual tensor maps
+  const CUtensorMap& tc = ta;
+  const CUtensorMap& tr = ta;
   // compile-time epilogue specialisation for the big-tile instantiation
   int ek = EK_GENERIC;
-  if (!direct && BN == 256) {
+  if (BN == 256) {
     if (c.mode == EPI_STORE_BF16 && c.layout == LAYOUT_TOKEN && c.act == ACT_NONE && !c.use_rowscale) ek = EK_STORE_TOK;
     else if (c.mode == EPI_STORE_BF16 && c.layout == LAYOUT_TOKEN && c.act == ACT_SIGMOID && !c.use_rowscale) ek = EK_STORE_TOK_SIG;
     else if (c.mode == EPI_STORE_BF16 && c.layout == LAYOUT_CHANNEL && c.act == ACT_NONE) ek = EK_STORE_CH;
     else if (c.mode == EPI_GATED_BF16 && c.layout == LAYOUT_TOKEN && c.act == ACT_GELU && !c.use_rowscale) ek = EK_GATED_TOK_GELU;
     else if (c.mode == EPI_GATED_BF16 && c.layout == LAYOUT_CHANNEL && c.act == ACT_SIGMOID) ek = EK_GATED_CH_SIG;
-    else if (c.mode == EPI_RESID_F32) ek = resid_w ? EK_RESID_F32_W : EK_RESID_F32;
+    else if (c.mode == EPI_RESID_F32) ek = EK_RESID_F32;
     else if (c.mode == EPI_STORE_F32) ek = EK_STORE_F32;
   }
   if (c.mn_major) {
@@ -371,7 +337,6 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
       case EK_GATED_TOK_GELU: return launch_gemm_inst<256, 3, false, EK_GATED_TOK_GELU>(ta, tb, tc, tr, p, s);
       case EK_GATED_CH_SIG: return launch_gemm_inst<256, 3, false, EK_GATED_CH_SIG>(ta, tb, tc, tr, p, s);
       case EK_RESID_F32: return launch_gemm_inst<256, 3, false, EK_RESID_F32>(ta, tb, tc, tr, p, s);
-      case EK_RESID_F32_W: return launch_gemm_inst<256, 3, false, EK_RESID_F32_W>(ta, tb, tc, tr, p, s);
       case EK_STORE_F32: return launch_gemm_inst<256, 3, false, EK_STORE_F32>(ta, tb, tc, tr, p, s);
       default: return launch_gemm_inst<256, 3, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
     }
@@ -471,14 +436,7 @@ int launch_chan_to_token_tma(const ChanLnParams& p, long long T, cudaStream_t s)
 }
 
 int g_c2t_tma = 1;   // 0: tile-per-CTA kernel (AF2_C2T_TMA=0)
-int g_attn_bias_t = 0;      // 1: pair bias stored transposed ([h][key][query]) so the bias MMA's B operand is K-major (AF2_ATTN_BIAS_T)
-int g_attn_ident_tmem = 1;  // 1: bias-MMA identity operand in tensor memory (AF2_ATTN_IDENT_TMEM=0: shared-memory strip)
-int g_attn_skip = 0;       // DEBUG timing experiments (AF2_ATTN_SKIP bitmask, results wrong)
-int g_attn_k3 = 0;         // 1: three K stages in the attention kernel's resident-bias mode (AF2_ATTN_K3)
 int g_attn_headmajor = 0;  // EXPERIMENT: attention reads a head-major copy of q|k|v (AF2_ATTN_HEADMAJOR=1)
-long long* g_attn_trace = nullptr;   // device buffer of 1024 stamps when AF2_ATTN_TRACE=1 (debug only)
-int g_attn_l2pf = 0;      // 1: attention K producer prefetches upcoming K / V / Q / gate boxes into L2 (AF2_ATTN_L2PF)
-int g_attn_group = 1;     // 1: attention CTAs grouped per (h, b') unit for 2..8 query blocks (AF2_ATTN_GROUP=0: n > 256 ungrouped)
 int g_gather_fused = 1;   // 1: contractions over all-gathered operand pieces in ONE launch (AF2_GATHER_FUSED=0: one launch per piece)
 
 int launch_chan_to_token(const ChanLnParams& p, cudaStream_t s) {
@@ -525,34 +483,34 @@ int launch_chan_to_token(const ChanLnParams& p, cudaStream_t s) {
 // attention launch (one folded batch group)
 // -------------------------------------------------------------------------------------------------
 template <int DH>
-int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tbias,
-                          const CUtensorMap& tg, const CUtensorMap& to, const AttnParams& p, cudaStream_t s) {
+int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p, cudaStream_t s) {
   using L = AttnSmem<DH>;
-  static bool configured[MAX_DEVICES] = {false};
+  static int configured[MAX_DEVICES] = {0};
   auto kern = attention_tc_kernel<DH>;
-  if (!configured[cur_dev()]) {
-    CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
-    configured[cur_dev()] = true;
+  const int smem = L::bytes(p.n);
+  if (smem > 232448) return fail(AF2_ERR_BAD_ARG, "attention: sequence length %d too long", p.n);
+  if (smem > configured[cur_dev()]) {
+    CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured[cur_dev()] = smem;
   }
   const int nqb = (p.n + 127) / 128;
   const long long items = (long long)nqb * p.heads * p.nbatch;
   if (items <= 0) return AF2_OK;
-  int grid = (int)(items < sm_count() ? items : sm_count());           // persistent CTAs
-  if (nqb >= 2 && nqb <= 8 && g_attn_group) grid = grid / nqb * nqb;    // groups of nqb CTAs share the K/V of their (h, b') units
+  if (items > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "attention: too many work items");
   const double tokens = (double)p.n * p.nbatch;
   ProfScope ps(s, KC_ATTENTION, 4.0 * tokens * p.n * p.heads * DH,
                tokens * p.heads * DH * 2.0 * 5 + (p.has_bias ? (double)p.heads * p.n * p.n * 2 : 0));
-  CUDA_OK(launch_pdl(kern, dim3(grid), dim3(ATTN_THREADS), L::TOTAL, s, tq, tk, tv, tbias, tg, to, p));
+  CUDA_OK(launch_pdl(kern, dim3((unsigned)items), dim3(ATTN_THREADS), smem, s, tq, tk, tv, tq, tq, tq, p));
   return AF2_OK;
 }
 
 // qkv: bf16 [tokens, 3I] (q | k | v), token(b', i) = b' * tok_sb + i * tok_si
 int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nbatch, long long tok_sb, long long tok_si,
                      const __nv_bfloat16* bias, int npad, const uint8_t* mask, const __nv_bfloat16* gate,
-                     __nv_bfloat16* out, cudaStream_t s, const __nv_bfloat16* qkv_hm = nullptr, long long hm_tokens = 0, int bias_t = 0) {
+                     __nv_bfloat16* out, cudaStream_t s, const __nv_bfloat16* qkv_hm = nullptr, long long hm_tokens = 0) {
   const long long I = (long long)heads * dh;
   const long long ld = 3 * I;
-  CUtensorMap tq, tk, tv, tb, tg, to;
+  CUtensorMap tq, tk, tv;
   unsigned long long dims[4] = {(unsigned long long)dh, (unsigned long long)n, (unsigned long long)heads, (unsigned long long)nbatch};
   unsigned long long str[3] = {(unsigned long long)(tok_si * ld * 2), (unsigned long long)(dh * 2), (unsigned long long)(tok_sb * ld * 2)};
   if (qkv_hm) {   // head-major q|k|v [3H][hm_tokens][dh] (experiment AF2_ATTN_HEADMAJOR)
@@ -574,33 +532,18 @@ int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nba
     AF2_TRY(make_tmap(&tk, qkv + I, 4, dims, str, box, swz, bf, promo));
     AF2_TRY(make_tmap(&tv, qkv + 2 * I, 4, dims, str, box, swz, bf, promo));
   }
-  unsigned long long gstr[3] = {(unsigned long long)(tok_si * I * 2), (unsigned long long)(dh * 2), (unsigned long long)(tok_sb * I * 2)};
-  AF2_TRY(make_tmap(&tg, gate, 4, dims, gstr, box, swz, bf, promo));
-  unsigned obox[4] = {(unsigned)dh, 32, 1, 1};            // the output leaves per 32-row quarter of a query block
-  AF2_TRY(make_tmap(&to, out, 4, dims, gstr, obox, swz));
-  if (bias) {
-    unsigned long long bd[3] = {(unsigned long long)npad, (unsigned long long)n, (unsigned long long)heads};
-    unsigned long long bs[2] = {(unsigned long long)npad * 2, (unsigned long long)n * npad * 2};
-    unsigned bb[3] = {64, 128, 1};
-    AF2_TRY(make_tmap(&tb, bias, 3, bd, bs, bb, CU_TENSOR_MAP_SWIZZLE_128B));
-  } else {
-    tb = tq;
-  }
+  if (bias && npad % 2 != 0) return fail(AF2_ERR_BAD_ARG, "attention: bias pitch %d must be even", npad);
+  if (I % 2 != 0) return fail(AF2_ERR_BAD_ARG, "attention: heads * dim_head must be even");
   AttnParams p;
   memset(&p, 0, sizeof(p));
-  p.n = n; p.heads = heads; p.nbatch = nbatch; p.has_bias = bias != nullptr;
+  p.n = n; p.heads = heads; p.nbatch = nbatch; p.has_bias = bias != nullptr; p.bias = bias; p.npad = npad;
   p.mask = mask; p.mask_sb = tok_sb; p.mask_si = tok_si;
   p.gate = gate; p.out = out; p.tok_sb = tok_sb; p.tok_si = tok_si; p.ld_gate = I; p.ld_out = I;
-  p.l2_prefetch = g_attn_l2pf;
-  p.k_stages3 = g_attn_k3;
-  p.dbg_skip = g_attn_skip;
-  p.ident_tmem = g_attn_ident_tmem;
-  p.bias_t = bias_t;
-  p.trace = g_attn_trace;
-  if (dh == 64) return launch_attention_inst<64>(tq, tk, tv, tb, tg, to, p, s);
-  if (dh == 32) return launch_attention_inst<32>(tq, tk, tv, tb, tg, to, p, s);
+  if (dh == 64) return launch_attention_inst<64>(tq, tk, tv, p, s);
+  if (dh == 32) return launch_attention_inst<32>(tq, tk, tv, p, s);
   return fail(AF2_ERR_BAD_ARG, "attention: dim_head %d unsupported (32 or 64)", dh);
 }
+
 
 #include "proj_launch.inl"
 
@@ -675,59 +618,28 @@ long long af2_profile_read(int cls, double* ms, double* flops, double* bytes) {
   return n;
 }
 
-// debug: copies the clock64 stamps of the last fused-projection launch (AF2_PROJ_TRACE=1) to `out` (2048 entries)
-int af2_debug_proj_trace(long long* out) {
-  if (!g_proj_trace) return fail(AF2_ERR_BAD_ARG, "projection trace not enabled (AF2_PROJ_TRACE=1)");
-  CUDA_OK(cudaDeviceSynchronize());
-  CUDA_OK(cudaMemcpy(out, g_proj_trace, 2048 * sizeof(long long), cudaMemcpyDeviceToHost));
-  return AF2_OK;
-}
+// debug entry points kept for ABI compatibility: no kernel of this build records a timeline
+int af2_debug_proj_trace(long long*) { return fail(AF2_ERR_BAD_ARG, "no projection trace in this build"); }
+int af2_debug_attn_trace(long long*) { return fail(AF2_ERR_BAD_ARG, "no attention trace in this build"); }
 
-// debug: copies the clock64 stamps of CTA 0 of the last attention launch (AF2_ATTN_TRACE=1) to `out` (1024 entries) and clears them
-int af2_debug_attn_trace(long long* out) {
-  if (!g_attn_trace) return fail(AF2_ERR_BAD_ARG, "attention trace not enabled (AF2_ATTN_TRACE=1)");
-  CUDA_OK(cudaDeviceSynchronize());
-  CUDA_OK(cudaMemcpy(out, g_attn_trace, 1024 * sizeof(long long), cudaMemcpyDeviceToHost));
-  CUDA_OK(cudaMemset(g_attn_trace, 0, 1024 * sizeof(long long)));
-  return AF2_OK;
-}
-
-void af2_set_proj_mode(int ctas) { g_proj_ctas = ctas < 0 ? 2 : (ctas > 2 ? 2 : ctas); }
+// 0: every LN -> Linear cluster runs as LayerNorm kernel + GEMM; nonzero: on the fused projection kernel
+void af2_set_proj_mode(int ctas) { g_proj_ctas = ctas != 0 ? 2 : 0; }
 
 int af2_check_device(void) {
-  if (const char* e = getenv("AF2_PROJ_CTAS")) af2_set_proj_mode(atoi(e));
   if (const char* e = getenv("AF2_C2T_TMA")) g_c2t_tma = atoi(e) != 0;
-  if (const char* e = getenv("AF2_PROJ_PRODTILES")) g_proj_prod_tiles = atof(e);
-  if (const char* e = getenv("AF2_PROJ_BALANCE")) g_proj_balance = atoi(e) != 0;
-  if (const char* e = getenv("AF2_PROJ_WIDE")) g_proj_wide = atoi(e) != 0;
-  if (const char* e = getenv("AF2_PROJ_L2PF")) g_proj_l2pf = atoi(e) != 0;
   if (const char* e = getenv("AF2_GATHER_FUSED")) g_gather_fused = atoi(e) != 0;
-  if (const char* e = getenv("AF2_ATTN_GROUP")) g_attn_group = atoi(e) != 0;
-  if (const char* e = getenv("AF2_ATTN_L2PF")) g_attn_l2pf = atoi(e) != 0;
+  if (const char* e = getenv("AF2_PROJ_CTAS")) af2_set_proj_mode(atoi(e));
   if (const char* e = getenv("AF2_ATTN_HEADMAJOR")) g_attn_headmajor = atoi(e) != 0;
-  if (const char* e = getenv("AF2_ATTN_K3")) g_attn_k3 = atoi(e) != 0;
-  if (const char* e = getenv("AF2_ATTN_SKIP")) g_attn_skip = atoi(e);
-  if (const char* e = getenv("AF2_ATTN_IDENT_TMEM")) g_attn_ident_tmem = atoi(e) != 0;
-  if (const char* e = getenv("AF2_ATTN_BIAS_T")) g_attn_bias_t = atoi(e) != 0;
-  if (const char* e = getenv("AF2_ATTN_TRACE")) {
-    if (atoi(e) != 0 && !g_attn_trace) {
-      if (cudaMalloc(&g_attn_trace, 1024 * sizeof(long long)) != cudaSuccess) g_attn_trace = nullptr;
-      else cudaMemset(g_attn_trace, 0, 1024 * sizeof(long long));
-    }
-  }
   if (const char* e = getenv("AF2_X_EVICT_LAST")) g_x_evict_last = atoi(e) != 0;
   if (const char* e = getenv("AF2_PDL")) g_pdl = atoi(e) != 0;
-  if (const char* e = getenv("AF2_PROJ_TRACE")) {
-    if (atoi(e) != 0 && !g_proj_trace) {
-      if (cudaMalloc(&g_proj_trace, 2048 * sizeof(long long)) != cudaSuccess) g_proj_trace = nullptr;
-      else cudaMemset(g_proj_trace, 0, 2048 * sizeof(long long));
-    }
-  }
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return fail(AF2_ERR_CUDA, "no CUDA device");
   int major = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return fail(AF2_ERR_UNSUPPORTED_DEVICE, "libaf2b200 is built for sm_100a only; device has compute capability %d.x", major);
+  int minor = 0;
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0)
+    return fail(AF2_ERR_UNSUPPORTED_DEVICE, "libaf2b200 is built for sm_90a only; device has compute capability %d.%d", major, minor);
   return AF2_OK;
 }
 
@@ -750,12 +662,12 @@ int af2_feed_forward(const af2_ff_weights* w, float* x, long long tokens, int d,
   // h = a * gelu(g)
   const int half = w->bn / 2;
   const int n1p = (hidden + half - 1) / half * w->bn;   // packed accumulator columns
-  if (g_proj_ctas > 0 && w->w_cat && w->bn == 256 && proj_dim_ok(d)) {
-    // fused LayerNorm -> Linear -> GEGLU (A-stationary CTA-pair kernel)
+  if (g_proj_ctas > 0 && w->w_cat && w->b_cat && w->bn == 256 && proj_dim_ok(d)) {
+    // fused LayerNorm -> Linear -> GEGLU
     ProjCall pc;
     memset(&pc, 0, sizeof(pc));
     pc.x = x; pc.T = tokens; pc.d = d;
-    pc.w_cat = w->w_cat; pc.w_ext = w->w_ext; pc.nseg = 1;
+    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.nseg = 1;
     pc.seg[0] = ProjOut{n1p / 256, EK_GATED_TOK_GELU, hidden, hbuf, hidden};
     AF2_TRY(launch_proj(pc, s));
   } else {
@@ -808,33 +720,25 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   if (pre_bias) bias = const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(pre_bias));   // [B][H][n][npad], zero padded
 
   // 1. LayerNorm (+ pair bias from the RAW edges; fused when the edges are x itself)
-  const bool fused_proj = g_proj_ctas > 0 && w->w_cat && proj_dim_ok(d) && (I % 8) == 0;
+  const bool fused_proj = g_proj_ctas > 0 && w->w_cat && w->b_cat && proj_dim_ok(d) && (I % 8) == 0;
   LnParams lp;
   memset(&lp, 0, sizeof(lp));
   lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = T; lp.d = d; lp.eps = 1e-5f;
   const bool fuse_bias = has_bias && !pre_bias && edges == x && B == 1;
-  // transposed bias [h][key][query] (K-major operand of the bias MMA) whenever the dedicated pair-bias kernel produces it
-  const bool bias_t = g_attn_bias_t && has_bias && !pre_bias && pair_bias_fast_ok(d, heads) && !(fuse_bias && !fused_proj);
-  // pad key columns are loaded by TMA next to valid ones: keep them finite (zero)
+  // pad key columns of the bias rows are never read, but keep them finite (zero)
   if (has_bias && !pre_bias && npad != n) CUDA_OK(cudaMemsetAsync(bias, 0, (size_t)B * heads * n * npad * 2, s));
-  if (fuse_bias) {
+  if (fuse_bias && pair_bias_fast_ok(d, heads)) {
+    // pair bias from the raw x by the dedicated kernel (the one the sharded schedule uses), LayerNorm without it
+    AF2_TRY(launch_pair_bias(x, T, d, w->w_edge, bias, heads, (long long)n * npad, n, npad, s));
+  } else if (fuse_bias) {
     lp.wb = w->w_edge; lp.bias_out = bias; lp.heads = heads; lp.bias_hs = (long long)n * npad; lp.n_inner = n; lp.pitch = npad;
   }
-  if (!fused_proj) {
-    AF2_TRY(launch_layernorm(lp, s));
-  } else if (fuse_bias) {
-    // pair bias only (raw x . w_edge); the LayerNorm itself is fused into the projection
-    if (pair_bias_fast_ok(d, heads)) {
-      AF2_TRY(launch_pair_bias(x, T, d, w->w_edge, bias, heads, (long long)n * npad, n, npad, s, bias_t ? 1 : 0));
-    } else {
-      lp.y = nullptr;
-      AF2_TRY(launch_layernorm(lp, s));
-    }
-  }
+  if (fused_proj) lp.y = nullptr;          // the fused projection normalises x itself
+  if (lp.y || lp.wb) AF2_TRY(launch_layernorm(lp, s));
   if (has_bias && !fuse_bias && !pre_bias && pair_bias_fast_ok(d, heads)) {
     for (int b = 0; b < B; ++b)
       AF2_TRY(launch_pair_bias(edges + (long long)b * n * n * d, (long long)n * n, d, w->w_edge, bias + (long long)b * heads * n * npad,
-                               heads, (long long)n * npad, n, npad, s, bias_t ? 1 : 0));
+                               heads, (long long)n * npad, n, npad, s));
   } else if (has_bias && !fuse_bias && !pre_bias) {
     for (int b = 0; b < B; ++b) {
       LnParams bp;
@@ -847,11 +751,11 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   }
   // 2. projections
   if (fused_proj) {
-    // one launch: LayerNorm (+ pair bias) -> [q | k | v] and sigmoid(gating)
+    // one launch: LayerNorm -> [q | k | v] and sigmoid(gating)
     ProjCall pc;
     memset(&pc, 0, sizeof(pc));
     pc.x = x; pc.T = T; pc.d = d;
-    pc.w_cat = w->w_cat; pc.w_ext = w->w_ext; pc.nseg = 2;
+    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.nseg = 2;
     pc.seg[0] = ProjOut{(int)((3 * I + 255) / 256), EK_STORE_TOK, (int)(3 * I), qkv, 3 * I};
     pc.seg[1] = ProjOut{(int)((I + 255) / 256), EK_STORE_TOK_SIG, (int)I, gate, I};
     AF2_TRY(launch_proj(pc, s));
@@ -882,7 +786,7 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
     AF2_TRY(launch_attention(qkv + t0 * 3 * I, heads, dim_head, n, nb, tok_sb, tok_si,
                              has_bias ? bias + (long long)b * heads * n * npad : nullptr, npad,
                              mask ? mask + t0 : nullptr, gate + t0 * I, og + t0 * I, s,
-                             (g_attn_headmajor && dim_head % 8 == 0) ? qkv_hm + t0 * 3 * I : nullptr, Tb, bias_t ? 1 : 0));
+                             (g_attn_headmajor && dim_head % 8 == 0) ? qkv_hm + t0 * 3 * I : nullptr, Tb));
   }
   // 4. to_out + bias + residual
   GemmCall co = linear_call(og, I, w->w_out, I, (int)T, d, (int)I);
@@ -922,12 +826,12 @@ int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned 
   float* maskf = ar.take<float>(T);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_multiply: workspace too small");
 
-  const bool fused_front = g_proj_ctas > 0 && w->w_cat && w->bn == 256 && proj_dim_ok(d) && np8 == N;
+  const bool fused_front = g_proj_ctas > 0 && w->w_cat && w->b_cat && w->bn == 256 && proj_dim_ok(d) && np8 == N;
   if (fused_front) {
     ProjCall pc;
     memset(&pc, 0, sizeof(pc));
     pc.x = x; pc.T = T; pc.d = d;
-    pc.w_cat = w->w_cat; pc.w_ext = w->w_ext; pc.rowmask = mask; pc.nseg = 3;
+    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = mask; pc.nseg = 3;
     const int tl = (d + 127) / 128;
     pc.seg[0] = ProjOut{tl, EK_GATED_CH_SIG, d, Lc, cs_lr};
     pc.seg[1] = ProjOut{tl, EK_GATED_CH_SIG, d, Rc, cs_lr};
@@ -1015,7 +919,7 @@ int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const u
   uint32_t* mwords = ar.take<uint32_t>((long long)((S + 31) / 32) * N);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "outer_mean: workspace too small");
 
-  const bool fused_front = g_proj_ctas > 0 && w->w_cat && proj_dim_ok(d) && np8 == N;
+  const bool fused_front = g_proj_ctas > 0 && w->w_cat && w->b_cat && proj_dim_ok(d) && np8 == N;
   LnParams lp;
   memset(&lp, 0, sizeof(lp));
   lp.x = m; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = mn; lp.T = Tm; lp.d = d; lp.eps = 1e-5f;
@@ -1032,7 +936,7 @@ int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const u
     ProjCall pc;
     memset(&pc, 0, sizeof(pc));
     pc.x = m; pc.T = Tm; pc.d = d;
-    pc.w_cat = w->w_cat; pc.w_ext = w->w_ext; pc.rowmask = msa_mask; pc.nseg = 1;
+    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = msa_mask; pc.nseg = 1;
     pc.seg[0] = ProjOut{(2 * d + 255) / 256, EK_STORE_CH, 2 * d, LRc, cs_lr};
     AF2_TRY(launch_proj(pc, s));
   } else {
@@ -1123,11 +1027,11 @@ int af2_triangle_project(const af2_trimul_weights* w, const float* x, const unsi
   __nv_bfloat16* xn = ar.take<__nv_bfloat16>(tokens * d);
   float* maskf = ar.take<float>(tokens);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_project: workspace too small");
-  if (g_proj_ctas > 0 && w->w_cat && w->bn == 256 && proj_dim_ok(d) && pitch == inner) {
+  if (g_proj_ctas > 0 && w->w_cat && w->b_cat && w->bn == 256 && proj_dim_ok(d) && pitch == inner) {
     ProjCall pc;
     memset(&pc, 0, sizeof(pc));
     pc.x = x; pc.T = tokens; pc.d = d;
-    pc.w_cat = w->w_cat; pc.w_ext = w->w_ext; pc.rowmask = mask; pc.nseg = 3;
+    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = mask; pc.nseg = 3;
     const int tl = (d + 127) / 128;
     pc.seg[0] = ProjOut{tl, EK_GATED_CH_SIG, d, Lc, chan_stride};
     pc.seg[1] = ProjOut{tl, EK_GATED_CH_SIG, d, Rc, chan_stride};
@@ -1259,11 +1163,11 @@ int af2_outer_project(const af2_outer_weights* w, const float* m, const unsigned
   __nv_bfloat16* mn = ar.take<__nv_bfloat16>(tokens * d);
   float* maskf = ar.take<float>(tokens);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "outer_project: workspace too small");
-  if (g_proj_ctas > 0 && w->w_cat && proj_dim_ok(d) && pitch == inner) {
+  if (g_proj_ctas > 0 && w->w_cat && w->b_cat && proj_dim_ok(d) && pitch == inner) {
     ProjCall pc;
     memset(&pc, 0, sizeof(pc));
     pc.x = m; pc.T = tokens; pc.d = d;
-    pc.w_cat = w->w_cat; pc.w_ext = w->w_ext; pc.rowmask = msa_mask; pc.nseg = 1;
+    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = msa_mask; pc.nseg = 1;
     pc.seg[0] = ProjOut{(2 * d + 255) / 256, EK_STORE_CH, 2 * d, LRc, chan_stride};
     return launch_proj(pc, s);
   }

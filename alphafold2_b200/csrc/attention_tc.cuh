@@ -1,30 +1,16 @@
-// Axial self-attention with shared additive pair bias and the reference's two-sided mask, on tcgen05.
+// Axial self-attention with shared additive pair bias and the reference's two-sided mask, on sm_90a wgmma.
 // Replaces Attention.forward (alphafold2.py:125-190) as driven by AxialAttention (alphafold2.py:219-255).
 //
-// Persistent CTAs; a work item = one (folded batch element b', head h, block of 128 queries).  Items are ordered
-// (h, query block, b') and every CTA owns a CONTIGUOUS range of them, so its items share the (h, query block) pair-bias
-// tiles: for n <= 256 those [128 q x n k] bf16 tiles stay RESIDENT in shared memory and are reloaded only when the range
-// crosses into the next (h, query block) (at most twice per CTA at C2).  That removes 64 of the 160 KB that every item
-// used to pull from L2 -- the kernel is bound by the L2 -> SM fill rate, not by the tensor pipe.  Keys/values are
-// streamed in blocks of 128 through a TMA pipeline (2 stages with a bias, 4 without; for n > 256 the bias tile of the
-// block travels with its K/V stage); the producer runs ahead across work items.
-//   S_j = Q K_j^T + I B_j   tcgen05.mma  (M=128, N=128, K=DH, then K=128 against a constant identity tile): the pair bias
-//                           tile B_j [query][key] is the MN-major B operand, so the TENSOR CORE adds the bias and the
-//                           softmax threads never load / unpack / add it  -> TMEM (double buffered, 2 x 128 cols)
-//   softmax warps (16)      four threads per query row (each owns 32 of the 128 keys of the block; the phases of a block
-//                           -- TMEM load, max, exchange, 2^x on the MUFU, pack, TMEM store -- are latency chains, and
-//                           four warps per scheduler overlap them where two could not):
-//                           TMEM -> regs, (+ key mask), online max/sum (row max exchanged through smem),
-//                           P_j -> packed bf16 written back over the S columns it came from (tcgen05.st); O is
-//                           rescaled in TMEM only when the running max moves by more than 2^8
-//   O  += P_j V_j           tcgen05.mma with A = P_j read FROM TENSOR MEMORY (M=128, N=DH, K=128), V consumed MN-major
-//                           straight from its [key][dh] layout.  No P tile in shared memory, no proxy fence per block,
-//                           and P is double buffered with S, so the softmax never waits for the previous P V.
-//   epilogue warps (4)      O is double buffered in TMEM, so the softmax warps hand a finished item over (row sums through
-//                           smem, O through the o_full barrier committed behind the item's last P V) and start the next
-//                           item at once; the epilogue warps compute O / l * sigmoid-gate -> bf16 IN PLACE over the gate
-//                           tile in shared memory and send it to [token, h*DH + e] with one TMA store per 32 rows (a
-//                           thread-per-row STG.128 pattern kept the LSU busy for ~1.5k cycles per item)
+// One CTA per work item = (folded batch element b', head h, block of 128 queries); items are ordered so that the CTAs
+// of one (h, b') pair are launched together and share its K / V tiles in L2.  Three warpgroups:
+//   warpgroup 0     TMA producer: the Q tile once, then K / V tiles of 128 keys through an ATTN_STAGES-deep pipeline
+//   warpgroups 1, 2 64 query rows each, flash-attention style with everything in registers:
+//     S_j = Q K_j^T          wgmma m64n128k16, Q and K from shared memory (K-major)
+//     softmax                + pair bias (bf16, read from global / L2 in the accumulator's fragment layout), key / query
+//                            mask, online max / sum (the four lanes of a row reduce with two shuffles)
+//     O  += P_j V_j          wgmma m64nDHk16 with A = P_j straight from registers (the S fragment of 16 keys IS the
+//                            m64k16 A fragment), V consumed MN-major from its [key][dh] layout
+//     epilogue               O / l * sigmoid-gate -> bf16 [token, h*DH + e]
 // Logits are produced directly in the log2 domain: the host folds dim_head^-0.5 * log2(e) into to_q and
 // log2(e) into edges_to_attn_bias, so the softmax is exp2(v - max) with no per-element scaling.
 //
@@ -32,15 +18,8 @@
 // query that gives probability exactly 0 on masked keys; for a masked query every logit is equal, i.e. a
 // uniform distribution over all n keys (masked ones included).  Keys >= n (tile padding) never count.
 #pragma once
+#include <float.h>
 #include "common.cuh"
-
-// 1: every second softmax exponential by an FMA-pipe polynomial (common.cuh: exp2_poly2) instead of the MUFU.  Measured slower
-// (axial_attention class 4.50 vs 4.04 ms per C2 forward, C4 block 11.8 vs 11.0 ms, profiles/r02h_ab_poly_exp.log): the softmax
-// warps are bound by their own instruction stream (4 warps per scheduler, all in the same phase), not by MUFU throughput, so
-// the ~7 extra instructions per emulated element lengthen the critical path.  Kept as a build option, off.
-#ifndef AF2_ATTN_POLY_EXP
-#define AF2_ATTN_POLY_EXP 0
-#endif
 
 namespace af2 {
 
@@ -49,73 +28,34 @@ struct AttnParams {
   int heads;
   int nbatch;         // folded batch B'
   int has_bias;
+  const __nv_bfloat16* bias;  // [heads][n][npad] (log2 domain), or nullptr
+  int npad;                   // row pitch of the bias (n rounded up to 8; pad columns are zero)
   const uint8_t* mask;        // nullptr or bool mask; element (b', i) at mask[b'*mask_sb + i*mask_si]
   long long mask_sb, mask_si;
   const __nv_bfloat16* gate;  // sigmoid(gating) [token, heads*DH]; token(b', i) = b'*tok_sb + i*tok_si
   __nv_bfloat16* out;         // [token, heads*DH]
   long long tok_sb, tok_si;
   long long ld_gate, ld_out;
-  long long* trace;           // debug (AF2_ATTN_TRACE=1): clock64 stamps of CTA 0, 8 per key block, see tools/attn_trace.py
-  int bias_t;                 // 1: the bias is stored transposed, [h][key][query]: its tile is then a K-major B operand of the bias
-                              //    MMA (full tensor rate; the [query][key] tile is MN-major and runs at about half rate)
-  int ident_tmem;             // 1: the identity operand of the bias MMA lives in tensor memory (AF2_ATTN_IDENT_TMEM)
-  int dbg_skip;               // DEBUG (AF2_ATTN_SKIP): bit 0 skip the V loads, bit 1 the K loads, bit 2 the Q loads, bit 3 the output stores (results wrong; timing experiments only)
-  int k_stages3;              // 1: three K stages in resident-bias mode (AF2_ATTN_K3, default on)
-  int l2_prefetch;            // 1: the K producer prefetches K / V / Q / gate boxes ATTN_PF_DIST key blocks ahead into L2 (AF2_ATTN_L2PF)
 };
 
-constexpr int ATTN_PF_DIST = 4;                    // L2 prefetch distance of the K producer, in key blocks
-constexpr int ATTN_NSPLIT = 4;                      // softmax threads per query row (each owns 128 / NSPLIT keys of a block)
-constexpr int ATTN_SM_WARPS = 4 * ATTN_NSPLIT;      // softmax warps 2 .. 2 + ATTN_SM_WARPS - 1
-constexpr int ATTN_W_KEYMASK = 2 + ATTN_SM_WARPS;   // then: key-mask warp, V TMA warp, 4 epilogue warps
-constexpr int ATTN_W_VPROD = ATTN_W_KEYMASK + 1;
-constexpr int ATTN_W_EPI = ATTN_W_VPROD + 1;        // a multiple of 4, so warp & 3 is the TMEM lane quarter of an epilogue warp
-// 1: a second MMA-issuing warp (the last one) issues P V while warp 1 issues S.  The timeline of the single issuer
-// (AF2_ATTN_TRACE) showed it 100 % busy: ~1150 cycles issuing the 12 S MMAs (they are accepted at the tensor pipe's pace),
-// ~500 for the 8 P V MMAs and ~1500 of mbarrier / fence round trips per key block -- 3300 cycles, the block period, with the
-// softmax warps (1900 cycles of work) waiting for it.  Two issuers run those chains side by side.
-#ifndef AF2_ATTN_SPLIT_MMA
-#define AF2_ATTN_SPLIT_MMA 1
-#endif
-// S / P buffers in tensor memory: three with two MMA issuers (S(g) then only has to wait for P V(g - 3): a whole softmax
-// phase of slack, so the S issue never sits on the critical path), two with one issuer
-constexpr int ATTN_NSB = AF2_ATTN_SPLIT_MMA ? 3 : 2;
-constexpr int ATTN_W_PV = ATTN_W_EPI + 4;           // the P V issuer (AF2_ATTN_SPLIT_MMA)
-constexpr int ATTN_THREADS = (ATTN_W_EPI + 4 + AF2_ATTN_SPLIT_MMA) * 32;
-static_assert(ATTN_W_EPI % 4 == 0, "epilogue warps must start at a multiple of 4");
+constexpr int ATTN_THREADS = 384;
+constexpr int ATTN_STAGES = 3;
+constexpr int ATTN_KB = 128;                        // keys per block
 
 template <int DH>
 struct AttnSmem {
   static constexpr int Q_BYTES = 128 * DH * 2;
-  static constexpr int K_BYTES = 128 * DH * 2;
-  static constexpr int V_BYTES = 128 * DH * 2;
-  static constexpr int BIAS_BYTES = 128 * 128 * 2;      // two 64-key boxes of [128 q rows x 128 B]
-  static constexpr int STAGE_BYTES = K_BYTES + V_BYTES + BIAS_BYTES;
-  // Identity operand of the bias MMA.  K step k needs A_k[r][e] = (r == 16k + e): only the two 8-row groups 2k, 2k+1 are
-  // non-zero and they look the same for every k, so ONE strip of 30 row groups (32-byte swizzle atoms of 8 rows x 16
-  // columns, 256 B each) -- 14 zero groups, the two diagonal groups, 14 zero groups -- serves all eight steps: step k
-  // starts its descriptor (14 - 2k) groups into the strip.
-  static constexpr int IDENT_BYTES = 32 * 256;
-  static constexpr int Q_OFF = 0;                       // [2] Q tiles (slot it & 1)
-  static constexpr int G_OFF = 2 * Q_BYTES;             // [2] sigmoid-gate tiles [128 q x DH] (same layout as Q)
-  // K/V (+ bias) region of 2 * STAGE_BYTES, carved at run time:
-  //   resident bias (n <= 256): [K V] x 2 stages | bias tiles of key blocks 0, 1
-  //   streamed bias (n > 256) : [K V bias] x 2 stages
-  //   no bias                 : [K V] x 4 stages
-  static constexpr int KV_BYTES = K_BYTES + V_BYTES;
-  static constexpr int STAGE_OFF = 4 * Q_BYTES;
-  static constexpr int IDENT_OFF = STAGE_OFF + 2 * STAGE_BYTES;
-  static constexpr int BAR_OFF = IDENT_OFF + IDENT_BYTES;
-  static constexpr int KB_OFF = BAR_OFF + 384;          // float key term (0 / -inf) [2][128]
-  static constexpr int MX_OFF = KB_OFF + 2 * 128 * 4;   // float row-max exchange [2 block parities][NSPLIT][128]
-  static constexpr int L_OFF = MX_OFF + 2 * ATTN_NSPLIT * 128 * 4;   // float row sums handed to the epilogue warps [2 slots][NSPLIT][128]
-  static constexpr int QV_OFF = L_OFF + 2 * ATTN_NSPLIT * 128 * 4;   // query-mask bytes [2][128]
-  static constexpr int KF_OFF = QV_OFF + 2 * 128;       // [2] per-stage flag: some key of the block is masked / padding
-  static constexpr int TOTAL = KF_OFF + 16 + 1024;
+  static constexpr int KV_BYTES = ATTN_KB * DH * 2;
+  static constexpr int STAGE_BYTES = 2 * KV_BYTES;    // K | V
+  static constexpr int STAGE_OFF = Q_BYTES;
+  static constexpr int BAR_OFF = STAGE_OFF + ATTN_STAGES * STAGE_BYTES;
+  static constexpr int KM_OFF = BAR_OFF + 128;        // key codes [nkb * 128]: 0 padding, 1 masked, 2 valid
+  static constexpr int bytes(int n) { return KM_OFF + (n + ATTN_KB - 1) / ATTN_KB * ATTN_KB; }
 };
 
 // tmQ/tmK/tmV: 4-D maps over the projection buffer, dims (e [DH], i [n], h [heads], b' [nbatch]),
-// box (DH, 128, 1, 1), swizzle = DH*2 bytes.  tmBias: 3-D (k [npad], q [n], h), box (64, 128, 1), SW128.
+// box (DH, 128, 1, 1), swizzle = DH*2 bytes.  tmBias / tmG / tmO are not read (bias, gate and output go through the
+// register fragments).
 template <int DH>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -126,682 +66,171 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   constexpr uint32_t SWZ = (DH == 64) ? SWZ_128 : SWZ_64;
   constexpr uint32_t ROWB = DH * 2;                 // bytes per Q/K/V row
   constexpr uint32_t SBO = 8 * ROWB;                // 8-row swizzle atom
-  // 1024-byte aligned by declaration (128B-swizzle atoms); keeping the array symbol (no integer round-up of the pointer)
-  // lets the compiler prove the shared address space and emit LDS/STS instead of generic LD/ST
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* q_full = bars + 0;     // [2] Q tile landed (slot it & 1)
-  uint64_t* g_full = bars + 2;     // [2] gate tile landed (slot it & 1)
-  uint64_t* q_empty = bars + 4;    // [2] Q tile consumed by the item's last QK^T
-  uint64_t* k_full = bars + 6;     // [4] K (+ streamed bias) of a block landed
-  uint64_t* k_empty = bars + 10;   // [4] ... and consumed by the block's S MMAs
-  uint64_t* v_full = bars + 14;    // [4] V of a block landed
-  uint64_t* v_empty = bars + 18;   // [4] ... and consumed by the block's P V
-  uint64_t* s_full = bars + 40;    // [ATTN_NSB]
-  uint64_t* p_full = bars + 43;    // [ATTN_NSB] P of the block is in its S buffer
-  // (bars + 26 unused: the P V retirement is observed through v_empty)
-  uint64_t* kb_full = bars + 27;   // [2] key-mask terms of a block staged
-  uint64_t* kb_empty = bars + 29;  // [2] ... and consumed by the 8 softmax warps
-  uint64_t* g_empty = bars + 31;   // [2] gate / output tile drained by the TMA stores of the 4 row quarters
-  uint64_t* bias_full = bars + 33; // resident bias tiles of the current (h, query block) landed
-  uint64_t* bias_empty = bars + 34;// ... and consumed by the last S MMA of that (h, query block)
-  uint64_t* o_full = bars + 35;    // [2] O accumulator (slot it & 1) complete: committed behind the item's last P V
-  uint64_t* o_empty = bars + 37;   // [2] ... and read (with its row sums) by the 4 epilogue warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 39);
-  float* keyb = reinterpret_cast<float*>(smem + L::KB_OFF);   // [2][128]
-  float* mxbuf = reinterpret_cast<float*>(smem + L::MX_OFF);  // [2][128]
-  float* lbuf = reinterpret_cast<float*>(smem + L::L_OFF);    // [2][2][128]
-  uint8_t* qvbuf = smem + L::QV_OFF;                          // [2][128]
-  uint32_t* kflag = reinterpret_cast<uint32_t*>(smem + L::KF_OFF);   // [2]
+  uint64_t* q_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
+  uint64_t* full_bar = q_bar + 1;
+  uint64_t* empty_bar = full_bar + ATTN_STAGES;
+  uint8_t* kcode = smem + L::KM_OFF;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int nkv = (p.n + 127) / 128;
-  const int nqb = nkv;
-  const int total_items = nqb * p.heads * p.nbatch;
-  // Work split.  With 2..8 query blocks the CTAs form groups of nqb: the CTAs of a group walk the SAME contiguous range of
-  // (h, b') units, one per query block, so they load the same K/V tiles at about the same time and all but the first read
-  // hit L2 instead of HBM (measured at n = 384 / 512 with one item per CTA and (h, qb, b') order: 1.2-2.0 GB of DRAM reads per
-  // launch for 0.6 GB of operands, the kernel was DRAM bound); for n <= 256 each CTA also keeps the bias tiles of its
-  // (h, query block) resident.  Otherwise item id = ((h * nqb + qb) * nbatch + b') and this CTA owns the ids
-  // [item0, item0 + my_items).
-  const bool paired = (nqb >= 2) && (nqb <= 8) && (gridDim.x % nqb == 0);
-  const int n_units = paired ? p.heads * p.nbatch : total_items;
-  const int n_owners = paired ? static_cast<int>(gridDim.x) / nqb : static_cast<int>(gridDim.x);
-  const int owner = paired ? static_cast<int>(blockIdx.x) / nqb : static_cast<int>(blockIdx.x);
-  const int item0 = static_cast<int>(static_cast<long long>(n_units) * owner / n_owners);
-  const int my_items = static_cast<int>(static_cast<long long>(n_units) * (owner + 1) / n_owners) - item0;
-  auto decode = [&](int it, int& qb_, int& h_, int& b_) {
-    const int id = item0 + it;
-    b_ = id % p.nbatch;
-    if (paired) {
-      qb_ = static_cast<int>(blockIdx.x) % nqb;
-      h_ = id / p.nbatch;
-    } else {
-      qb_ = (id / p.nbatch) % nqb;
-      h_ = id / (p.nbatch * nqb);
-    }
-  };
-  auto combo_of = [&](int it) { return (item0 + it) / p.nbatch; };       // changes with (h, query block): selects the bias tiles
-  const bool resident = p.has_bias && nkv <= 2;
-  const int nst = p.has_bias ? 2 : 4;                                    // V pipeline depth (and K's, except below)
-  // Resident-bias mode: THREE K stages.  The timeline (AF2_ATTN_TRACE, profiles/r02m_attn_trace_*.txt) shows a K box landing
-  // ~5400 cycles after its load is issued in steady state (1600 cold), and the load of block g + 2 can only be issued
-  // when block g's S retires: with two stages the block period was (5400 + 900) / 2 -- the whole kernel ran at the pace of
-  // that round trip.  The third stage lives in what used to be the second gate-tile slot (the gate tile is single buffered
-  // in this mode: it is needed one item later, by the epilogue).  V stays at two stages: it is needed a softmax later.
-  const bool k3 = resident && p.k_stages3 != 0;
-  const int nstk = k3 ? 3 : nst;                                         // K pipeline depth
-  const int stage_stride = (p.has_bias && !resident) ? L::STAGE_BYTES : L::KV_BYTES;
-  auto k_off = [&](int kst) { return (k3 && kst == 2) ? (L::G_OFF + L::Q_BYTES) : (L::STAGE_OFF + kst * stage_stride); };
-  auto g_slot = [&](int it) { return k3 ? 0 : (it & 1); };
-  auto g_phase = [&](int it) { return static_cast<uint32_t>(k3 ? (it & 1) : ((it >> 1) & 1)); };
-  const int bias_res_off = L::STAGE_OFF + 2 * L::KV_BYTES;               // resident tiles: + j * BIAS_BYTES
-  constexpr uint32_t TMEM_COLS = 512;
-  constexpr uint32_t S_COL = 0, O_COL = ATTN_NSB * 128;
+  const int n = p.n;
+  const int nqb = (n + 127) / 128;
+  const int nkb = (n + ATTN_KB - 1) / ATTN_KB;
+  const int qb = blockIdx.x % nqb;
+  const int bb = (blockIdx.x / nqb) % p.nbatch;
+  const int hh = blockIdx.x / (nqb * p.nbatch);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV); prefetch_tmap(&tmG);
-    if (p.has_bias) prefetch_tmap(&tmBias);
-    prefetch_tmap(&tmO);
-    mbar_init(bias_full, 1);
-    mbar_init(bias_empty, 1);
-    for (int s = 0; s < 4; ++s) {
-      mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&q_full[s], 1);
-      mbar_init(&q_empty[s], 1);
-      mbar_init(&o_full[s], 1);
-      mbar_init(&o_empty[s], 4);
-      mbar_init(&g_full[s], 1);
-      mbar_init(&g_empty[s], 4);
-      mbar_init(&kb_full[s], 1);
-      mbar_init(&kb_empty[s], ATTN_SM_WARPS);
-    }
-    for (int s = 0; s < ATTN_NSB; ++s) {
-      mbar_init(&s_full[s], 1);
-      mbar_init(&p_full[s], ATTN_SM_WARPS);
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmQ);
+    prefetch_tmap(&tmK);
+    prefetch_tmap(&tmV);
+    mbar_init(q_bar, 1);
+    for (int s = 0; s < ATTN_STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);   // one arrive per softmax warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  if (p.has_bias) {
-    uint4* id4 = reinterpret_cast<uint4*>(smem + L::IDENT_OFF);
-    for (int i = threadIdx.x; i < L::IDENT_BYTES / 16; i += ATTN_THREADS) id4[i] = make_uint4(0u, 0u, 0u, 0u);
-    __syncthreads();
-    if (threadIdx.x < 16) {
-      // diagonal element i of the 16 x 16 block: row group 14 + i / 8, row r = i % 8, column i (16-byte chunk i / 8,
-      // XOR-ed with bit 7 of the byte address = r >> 2 by the 32-byte swizzle)
-      const uint32_t i = threadIdx.x, r = i & 7, c = i >> 3;
-      *reinterpret_cast<__nv_bfloat16*>(smem + L::IDENT_OFF + (14 + c) * 256 + r * 32 + ((c ^ (r >> 2)) << 4) + (i & 7) * 2) =
-          __float2bfloat16(1.0f);
-    }
-    fence_proxy_async_smem();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Identity operand of the bias MMA in TENSOR memory (p.ident_tmem): A[r][k] = (r == k) as packed bf16 pairs in 64 columns
-  // (column k / 2, low half = even k), written once per CTA.  With the identity read from shared memory (32-byte rows,
-  // SW32 strip) the eight K = 16 bias steps took ~1000 cycles per key block -- twice their tensor-pipe time, and the whole S
-  // issue (1300 cycles, AF2_ATTN_TRACE) sits on the kernel's critical path between two softmax phases.
-  constexpr uint32_t IDENT_COL = O_COL + 128;                    // (only with two S buffers: three fill the 512 columns)
-  const bool ident_tmem = p.ident_tmem != 0 && ATTN_NSB == 2;
-  if (p.has_bias && ident_tmem && warp >= ATTN_W_EPI && warp < ATTN_W_EPI + 4) {
-    const uint32_t r = (warp & 3) * 32 + lane;
-    uint32_t v[32];
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-#pragma unroll
-      for (int c = 0; c < 32; ++c) v[c] = (static_cast<uint32_t>(half * 32 + c) == (r >> 1)) ? ((r & 1) ? 0x3f800000u : 0x00003f80u) : 0u;
-      tmem_st32(tmem_base + IDENT_COL + half * 32 + (static_cast<uint32_t>((warp & 3) * 32) << 16), v);
-    }
-    tmem_st_wait();
-    tc_fence_before();
-  }
-  if (p.has_bias && ident_tmem) {
-    __syncthreads();
-    tc_fence_after();
-  }
   pdl_launch_dependents();
   pdl_wait();
-  // debug timeline: slot g * 8 + k of CTA 0 (k: 0/1 S issue begin/end, 2/3 P V issue begin/end [MMA warp], 4 S acquired,
-  // 5 P published [softmax warp 2], 6 K load issued [producer], 7 MMA warp free to issue S of this block)
-  auto stamp = [&](int g, int k) {
-    if (p.trace != nullptr && blockIdx.x == 0 && g < 64) p.trace[g * 16 + k] = clock64();
-  };
+  const uint8_t* mrow = p.mask ? p.mask + static_cast<long long>(bb) * p.mask_sb : nullptr;
+  for (int k = threadIdx.x; k < nkb * ATTN_KB; k += ATTN_THREADS)
+    kcode[k] = k >= n ? 0 : ((mrow && !mrow[static_cast<long long>(k) * p.mask_si]) ? 1 : 2);
+  __syncthreads();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
-      // L2 prefetch ATTN_PF_DIST key blocks ahead of the loads.  The K/V ring is only two stages deep when a bias is present
-      // (the resident bias tiles take the room of two more), so the load of block g + 2 is issued when block g's MMAs
-      // retire: with the operands coming from DRAM (~2 us under load) that round trip, not the tensor pipe or the softmax,
-      // set the block period.  Prefetched, the ring's loads hit L2.
-      auto prefetch_block = [&](int g) {
-        const int it2 = g / nkv, j2 = g - it2 * nkv;
-        if (it2 >= my_items || !p.l2_prefetch) return;
-        int qb2, h2, b2;
-        decode(it2, qb2, h2, b2);
-        tma_prefetch_4d(&tmK, 0, j2 * 128, h2, b2);
-        tma_prefetch_4d(&tmV, 0, j2 * 128, h2, b2);
-        if (j2 == 0) {
-          tma_prefetch_4d(&tmQ, 0, qb2 * 128, h2, b2);
-          tma_prefetch_4d(&tmG, 0, qb2 * 128, h2, b2);
-        }
-      };
-      if (p.l2_prefetch) for (int g = 0; g < ATTN_PF_DIST; ++g) prefetch_block(g);
-      int prev_combo = -1, nc = 0;
-      int kst = 0;                                       // K ring stage / phase of the next block, kept incrementally
-      uint32_t kph = 0;
-      for (int it = 0; it < my_items; ++it) {
-        int qb, h, b;
-        decode(it, qb, h, b);
-        const int gs = it & 1;
-        if (resident && combo_of(it) != prev_combo) {
-          prev_combo = combo_of(it);
-          mbar_wait(bias_empty, (nc & 1) ^ 1);
-          mbar_arrive_expect_tx(bias_full, nkv * L::BIAS_BYTES);
-          for (int j = 0; j < nkv; ++j) {
-            uint8_t* sb = smem + bias_res_off + j * L::BIAS_BYTES;
-            if (p.bias_t) {      // [key rows][query columns]: two 64-query boxes
-              tma_load_3d(sb, &tmBias, bias_full, qb * 128, j * 128, h);
-              tma_load_3d(sb + 16384, &tmBias, bias_full, qb * 128 + 64, j * 128, h);
-            } else {             // [query rows][key columns]: two 64-key boxes
-              tma_load_3d(sb, &tmBias, bias_full, j * 128, qb * 128, h);
-              tma_load_3d(sb + 16384, &tmBias, bias_full, j * 128 + 64, qb * 128, h);
-            }
-          }
-          ++nc;
-        }
-        mbar_wait(&q_empty[gs], ((it >> 1) & 1) ^ 1);
-        if (p.dbg_skip & 4) mbar_arrive(&q_full[gs]);
-        else {
-          mbar_arrive_expect_tx(&q_full[gs], L::Q_BYTES);
-          tma_load_4d(smem + L::Q_OFF + gs * L::Q_BYTES, &tmQ, &q_full[gs], 0, qb * 128, h, b);
-        }
-        // (the gate tile of the item is loaded by the V producer warp: its slot is handed back by the epilogue of item
-        // it - 2, and waiting for that HERE delayed the K loads of the next item -- see the note there)
-        const bool stream_bias = p.has_bias && !resident;
-        for (int j = 0; j < nkv; ++j) {
-          const int g = it * nkv + j;
-          if (p.l2_prefetch) prefetch_block(g + ATTN_PF_DIST);
-          // K is dead as soon as the block's S MMAs retire -- a whole softmax earlier than V -- so its stage refills early
-          const int ks = kst;
-          mbar_wait(&k_empty[ks], kph ^ 1);
-          if (++kst == nstk) { kst = 0; kph ^= 1; }
-          stamp(g, 6);
-          uint8_t* sk = smem + k_off(ks);
-          if ((p.dbg_skip & 2) && !stream_bias) { mbar_arrive(&k_full[ks]); continue; }
-          mbar_arrive_expect_tx(&k_full[ks], L::K_BYTES + (stream_bias ? L::BIAS_BYTES : 0));
-          tma_load_4d(sk, &tmK, &k_full[ks], 0, j * 128, h, b);
-          if (stream_bias) {
-            uint8_t* sbias = sk + L::KV_BYTES;
-            if (p.bias_t) {
-              tma_load_3d(sbias, &tmBias, &k_full[ks], qb * 128, j * 128, h);
-              tma_load_3d(sbias + 16384, &tmBias, &k_full[ks], qb * 128 + 64, j * 128, h);
-            } else {
-              tma_load_3d(sbias, &tmBias, &k_full[ks], j * 128, qb * 128, h);
-              tma_load_3d(sbias + 16384, &tmBias, &k_full[ks], j * 128 + 64, qb * 128, h);
-            }
-          }
-        }
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(q_bar, L::Q_BYTES);
+      tma_load_4d(smem, &tmQ, q_bar, 0, qb * 128, hh, bb);
+      for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % ATTN_STAGES;
+        mbar_wait(&empty_bar[s], ((kb / ATTN_STAGES) & 1) ^ 1);
+        uint8_t* st = smem + L::STAGE_OFF + s * L::STAGE_BYTES;
+        mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
+        tma_load_4d(st, &tmK, &full_bar[s], 0, kb * ATTN_KB, hh, bb);
+        tma_load_4d(st + L::KV_BYTES, &tmV, &full_bar[s], 0, kb * ATTN_KB, hh, bb);
       }
     }
-  } else if (warp == ATTN_W_VPROD) {
-    // ================================ V + gate producer ===========================
-    // The gate tile of item `it` is only needed by the item's epilogue, and its slot (it & 1) is released by the epilogue of
-    // item it - 2.  It used to be loaded by the Q/K producer right after Q: with two key blocks per item that wait sat in
-    // front of the K loads of the NEXT item, so S of every item's first block was issued one TMA round trip late (ncu:
-    // 31 % of the softmax warps' samples on the s_full wait, block period 3800 cycles for ~1000 cycles of tensor work).
-    // Here it follows the item's V loads, where it delays nothing.
-    if (lane == 0) {
-      int vst = 0;                                       // V ring stage / phase of the next block, kept incrementally
-      uint32_t vph = 0;
-      for (int it = 0; it < my_items; ++it) {
-        int qb, h, b;
-        decode(it, qb, h, b);
-        for (int j = 0; j < nkv; ++j) {
-          const int kst = vst;
-          mbar_wait(&v_empty[kst], vph ^ 1);
-          if (++vst == nst) { vst = 0; vph ^= 1; }
-          if (p.dbg_skip & 1) { mbar_arrive(&v_full[kst]); continue; }
-          mbar_arrive_expect_tx(&v_full[kst], L::V_BYTES);
-          tma_load_4d(smem + L::STAGE_OFF + kst * stage_stride + L::K_BYTES, &tmV, &v_full[kst], 0, j * 128, h, b);
-        }
-        if (!k3) {                                   // (k3: the epilogue warps read the gate straight from global memory)
-          const int gs = g_slot(it);
-          mbar_wait(&g_empty[gs], g_phase(it) ^ 1);
-          mbar_arrive_expect_tx(&g_full[gs], L::Q_BYTES);
-          tma_load_4d(smem + L::G_OFF + gs * L::Q_BYTES, &tmG, &g_full[gs], 0, qb * 128, h, b);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ==================================
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);   // S = Q K^T, both K-major
-    constexpr uint32_t idesc_b = umma_idesc_bf16(128, 128, 0, 1);   // S += I B: identity K-major, bias tile MN-major
-    constexpr uint32_t idesc_o = umma_idesc_bf16(128, DH, 0, 1);    // O = P V, P from tensor memory, V MN-major
-    const int total_blocks = my_items * nkv;
-    // Every index of the two block streams this warp walks (S issue runs one block ahead of P V) is kept INCREMENTALLY:
-    // the first version recomputed it = g / nkv, g % stages, (g / stages) & 1 and the bias-tile combo (item / nbatch) with
-    // run-time divisors on every probe -- ~150 cycles of dependent I2F / MUFU.RCP / F2I chain each, 5-8 of them between
-    // "P V issued" and "S of the next block issued" (AF2_ATTN_TRACE showed ~900 cycles there), on the one warp whose latency
-    // every key block waits for.
-    struct Walk { int g, it, j, kst, kph; };             // block g = key block j of item it; ring stage kst, ring phase kph
-    Walk sw = {0, 0, 0, 0, 0};                           // next block whose S is to be issued (K ring, depth nstk)
-    Walk pw = {0, 0, 0, 0, 0};                           // block whose P V is issued next (V ring, depth nst)
-    auto advance = [&](Walk& w, int depth) {
-      ++w.g;
-      if (++w.j == nkv) { w.j = 0; ++w.it; }
-      if (++w.kst == depth) { w.kst = 0; w.kph ^= 1; }
-    };
-    // bias-tile combo (h, query block) of the S stream's item: it changes when (item0 + it) crosses a multiple of nbatch
-    int combo_rem = item0 % p.nbatch;                    // (item0 + sw.it) % nbatch  (one division per kernel)
-    bool combo_new = true;                               // the item sw.it is the first of its combo (or the CTA's first item)
-    int nc = 0;
-    int s_sb = 0;
-    // `probed`: s_ready() has just seen every operand barrier of this block complete (a successful test_wait acquires like a
-    // wait), so the waits -- ~100 cycles of SYNCS round trip each on this latency-bound warp -- are skipped
-    auto issue_s = [&](bool probed) {
-      const int g = sw.g, it = sw.it, j = sw.j, kst = sw.kst;
-      const int st = s_sb;                               // S buffer of this block (g % ATTN_NSB, kept incrementally)
-      if (j == 0) {
-        if (!probed) mbar_wait(&q_full[it & 1], (it >> 1) & 1);
-        if (resident && combo_new) {                       // this CTA's range entered the next (h, query block): new bias tiles
-          if (!probed) mbar_wait(bias_full, nc & 1);
-          ++nc;
-        }
-      }
-      if (lane == 0) stamp(g, 8);                       // entered issue_s (after the Q / bias waits of a first block)
-      if (!probed) mbar_wait(&k_full[kst], sw.kph);
-      if (lane == 0) stamp(g, 9);                       // K landed
-      tc_fence_after();
-      if (lane == 0) stamp(g, 0);
-      const bool last_of_item = (j == nkv - 1);
-      const bool last_of_combo = last_of_item && (it + 1 == my_items || combo_rem == p.nbatch - 1);
-      if (elect_one()) {
-        const uint32_t sq = smem_u32(smem + L::Q_OFF + (it & 1) * L::Q_BYTES);
-        const uint32_t sk = smem_u32(smem + k_off(kst));
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) {
-          const uint64_t ad = umma_smem_desc(sq + k * 32, 16, SBO, SWZ);
-          const uint64_t bd = umma_smem_desc(sk + k * 32, 16, SBO, SWZ);
-          umma_bf16(tmem_base + S_COL + st * 128, ad, bd, idesc_s, k != 0 ? 1u : 0u);
-        }
-        if (p.has_bias) {
-          const uint32_t si = smem_u32(smem + L::IDENT_OFF);
-          // bias tile of key block j: [128 query rows x 128 B] x two 64-key boxes
-          const uint32_t sbz = resident ? smem_u32(smem + bias_res_off + j * L::BIAS_BYTES) : sk + L::KV_BYTES;
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            // B, [query][key] tile: bias rows (the K index) 16k .. 16k+15 with the keys contiguous (MN-major): 8-row atoms
-            //    1024 B apart, the two 64-key boxes 16 KB apart;
-            // B, transposed [key][query] tile: K-major like the K tile of Q K^T -- 128-byte rows of 64 queries, 16 queries
-            //    (32 B) per step, the second 64-query box 16 KB further
-            const uint64_t bd = p.bias_t ? umma_smem_desc(sbz + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024, SWZ_128)
-                                         : umma_smem_desc(sbz + k * 2048, 16384, 1024, SWZ_128);
-            const uint32_t idb = p.bias_t ? idesc_s : idesc_b;
-            if (ident_tmem) {
-              // A: identity columns 16k .. 16k+15 from tensor memory (8 packed columns)
-              umma_bf16_ts(tmem_base + S_COL + st * 128, tmem_base + IDENT_COL + k * 8, bd, idb, 1u);
-            } else {
-              // A: identity columns 16k .. 16k+15 = the diagonal strip entered (14 - 2k) row groups in (see AttnSmem)
-              const uint64_t ad = umma_smem_desc(si + (14 - 2 * k) * 256, 16, 256, SWZ_32);
-              umma_bf16(tmem_base + S_COL + st * 128, ad, bd, idb, 1u);
-            }
-          }
-        }
-        umma_commit(&s_full[st]);
-        umma_commit(&k_empty[kst]);
-        if (last_of_item) {
-          umma_commit(&q_empty[it & 1]);                   // Q slot reusable once the item's last QK^T retires
-          if (resident && last_of_combo) umma_commit(bias_empty);
-        }
-      }
-      __syncwarp();
-      if (lane == 0) stamp(g, 1);
-      if (last_of_item) {                                  // the S stream moves on to the next item
-        combo_new = (combo_rem == p.nbatch - 1);
-        combo_rem = combo_new ? 0 : combo_rem + 1;
-      } else {
-        combo_new = false;
-      }
-      advance(sw, nstk);
-      if (++s_sb == ATTN_NSB) s_sb = 0;
-    };
-    // can S of the next block be issued without blocking?  (Q / bias of a new item and the K stage have landed; the S buffer
-    // itself is free by construction: S(g) is issued after P V(g-2), and the tensor core executes in issue order)
-    auto s_ready = [&]() {
-      if (sw.j == 0) {
-        if (!mbar_test(&q_full[sw.it & 1], (sw.it >> 1) & 1)) return false;
-        if (resident && combo_new && !mbar_test(bias_full, nc & 1)) return false;
-      }
-      return mbar_test(&k_full[sw.kst], sw.kph);
-    };
-#if AF2_ATTN_SPLIT_MMA
-    // S issuer.  S(g) overwrites the TMEM buffer that held P(g - ATTN_NSB): it may only be issued once that P V has RETIRED (the two
-    // issuers are different threads, so program order no longer orders their MMAs; the V stage's v_empty barrier is committed
-    // behind exactly those MMAs).  With three S buffers that is two softmax phases before S(g) is needed.
-    for (int g = 0; g < total_blocks; ++g) {
-      if (g >= ATTN_NSB) {
-        mbar_wait(&v_empty[pw.kst], pw.kph);            // pw walks ATTN_NSB blocks behind here: the stage of P V(g - ATTN_NSB)
-        advance(pw, nst);
-      }
-      issue_s(false);
-    }
-  } else if (warp == ATTN_W_PV) {
-    // ================================ P V issuer ==================================
-    constexpr uint32_t idesc_o = umma_idesc_bf16(128, DH, 0, 1);    // O = P V, P from tensor memory, V MN-major
-    const int total_blocks = my_items * nkv;
-    int it = 0, j = 0, vst = 0, st = 0;
-    uint32_t vph = 0, sph = 0;
-    for (int g = 0; g < total_blocks; ++g) {
-      mbar_wait(&p_full[st], sph);
-      mbar_wait(&v_full[vst], vph);
-      if (j == 0) mbar_wait(&o_empty[it & 1], ((it >> 1) & 1) ^ 1);   // the epilogue has read the item that used this O slot
-      tc_fence_after();
-      if (lane == 0) stamp(g, 2);
-      if (elect_one()) {
-        const uint32_t sv = smem_u32(smem + L::STAGE_OFF + vst * stage_stride + L::K_BYTES);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          // A = P [128 rows x 16 keys] = 8 packed columns of the S / P buffer; B = V [key][dh], MN-major: 16 keys = 2 atoms
-          const uint64_t bd = umma_smem_desc(sv + k * 2 * SBO, 16, SBO, SWZ);
-          umma_bf16_ts(tmem_base + O_COL + (it & 1) * 64, tmem_base + S_COL + st * 128 + k * 8, bd, idesc_o, (j != 0 || k != 0) ? 1u : 0u);
-        }
-        umma_commit(&v_empty[vst]);
-        if (j == nkv - 1) umma_commit(&o_full[it & 1]);
-      }
-      __syncwarp();
-      if (lane == 0) stamp(g, 3);
-      if (++j == nkv) { j = 0; ++it; }
-      if (++vst == nst) { vst = 0; vph ^= 1; }
-      if (++st == ATTN_NSB) { st = 0; sph ^= 1; }
-    }
-#else
-    if (total_blocks > 0) issue_s(false);
-    for (int g = 0; g < total_blocks; ++g) {
-      const int st = g & 1;
-      // S(g+1) goes out as early as its operands allow (it is tried BEFORE the first look at P(g): in steady state P(g) is
-      // still a softmax away), but P V(g) never queues behind a K/V load that is still in flight
-      bool s_issued = g + 1 >= total_blocks;
-      if (lane == 0) stamp(g + 1, 7);                    // the MMA warp starts looking for S(g + 1)'s operands
-      if (!s_issued && s_ready()) { issue_s(true); s_issued = true; }
-      bool first = true;
-      while (!mbar_test(&p_full[st], (g >> 1) & 1)) {
-        if (first && lane == 0) stamp(g + 1, 10);       // first p_full probe came back (not ready)
-        first = false;
-        if (!s_issued && s_ready()) { issue_s(true); s_issued = true; }
-      }
-      mbar_wait(&v_full[pw.kst], pw.kph);
-      const int it = pw.it, j = pw.j;
-      if (j == 0) mbar_wait(&o_empty[it & 1], ((it >> 1) & 1) ^ 1);   // the epilogue has read the item that used this O slot
-      tc_fence_after();
-      if (lane == 0) stamp(g, 2);
-      if (elect_one()) {
-        const uint32_t sv = smem_u32(smem + L::STAGE_OFF + pw.kst * stage_stride + L::K_BYTES);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          // A = P [128 rows x 16 keys] = 8 packed columns of the S / P buffer; B = V [key][dh], MN-major: 16 keys = 2 atoms
-          const uint64_t bd = umma_smem_desc(sv + k * 2 * SBO, 16, SBO, SWZ);
-          umma_bf16_ts(tmem_base + O_COL + (it & 1) * 64, tmem_base + S_COL + st * 128 + k * 8, bd, idesc_o, (j != 0 || k != 0) ? 1u : 0u);
-        }
-        umma_commit(&v_empty[pw.kst]);
-        if (j == nkv - 1) umma_commit(&o_full[it & 1]);
-      }
-      __syncwarp();
-      if (lane == 0) stamp(g, 3);
-      advance(pw, nst);
-      if (!s_issued) issue_s(false);
-    }
-#endif
-  } else if (warp == ATTN_W_KEYMASK) {
-    // ================================ key-mask warp ================================
-    // stages, one block ahead of the softmax warps, the additive key term of every 128-key block:
-    // 0 = usable key, -inf = masked key or tile padding beyond n (hides the mask's global-load latency)
-    const float NEG_INF = -__int_as_float(0x7f800000);
-    for (int it = 0; it < my_items; ++it) {
-      int qb, h, b;
-      decode(it, qb, h, b);
-      for (int j = 0; j < nkv; ++j) {
-        const int g = it * nkv + j;
-        const int st = g & 1;
-        float kb[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int kidx = j * 128 + lane * 4 + i;
-          kb[i] = NEG_INF;
-          if (kidx < p.n) kb[i] = (!p.mask || p.mask[b * p.mask_sb + kidx * p.mask_si]) ? 0.f : NEG_INF;
-        }
-        uint32_t qv = 0x01010101u;
-        if (j == 0 && p.mask) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int qi = qb * 128 + lane * 4 + i;
-            if (qi < p.n && p.mask[b * p.mask_sb + qi * p.mask_si] == 0) qv &= ~(0xffu << (8 * i));
-          }
-        }
-        const bool some_masked = __any_sync(0xffffffffu, (kb[0] != 0.f) | (kb[1] != 0.f) | (kb[2] != 0.f) | (kb[3] != 0.f));
-        mbar_wait(&kb_empty[st], ((g >> 1) & 1) ^ 1);
-        if (lane == 0) kflag[st] = some_masked ? 1u : 0u;
-        *reinterpret_cast<float4*>(keyb + st * 128 + lane * 4) = make_float4(kb[0], kb[1], kb[2], kb[3]);
-        if (j == 0) *reinterpret_cast<uint32_t*>(qvbuf + (it & 1) * 128 + lane * 4) = qv;
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&kb_full[st]);
-      }
-    }
-  } else if (warp >= ATTN_W_EPI) {
-    // ================================ epilogue warps ===============================
-    // O / l * gate -> out for one finished item while the softmax warps are already on the next one
-    const int q = warp & 3;               // TMEM lane quarter
-    const int r = q * 32 + lane;          // query row inside the tile == TMEM lane
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    for (int it = 0; it < my_items; ++it) {
-      int qb, h, b;
-      decode(it, qb, h, b);
-      const int slot = it & 1;
-      // k3 mode (three K stages; the second gate slot holds K stage 2): the gate row of this thread's query comes straight
-      // from global memory into registers BEFORE the wait for the item's O -- the load latency hides behind that wait and the
-      // remaining gate slot is only the staging tile of the TMA store.  A single-buffered TMA-loaded gate tile would put the
-      // ~5000-cycle load behind the previous item's store and throttle the kernel to the old pace.
-      uint4 greg[DH / 8];
-      if (k3) {
-        const int qi = qb * 128 + r;
-        const uint4* grow = reinterpret_cast<const uint4*>(p.gate + (static_cast<long long>(b) * p.tok_sb + static_cast<long long>(qi) * p.tok_si) * p.ld_gate + h * DH);
-#pragma unroll
-        for (int i = 0; i < DH / 8; ++i) greg[i] = (qi < p.n) ? __ldg(grow + i) : make_uint4(0u, 0u, 0u, 0u);
-      }
-      mbar_wait(&o_full[slot], (it >> 1) & 1);
-      tc_fence_after();
-      float lsum = 0.f;
-#pragma unroll
-      for (int i = 0; i < ATTN_NSPLIT; ++i) lsum += lbuf[(slot * ATTN_NSPLIT + i) * 128 + r];
-      const float inv_l = 1.0f / lsum;
-      const int gsl = g_slot(it);
-      if (!k3) mbar_wait(&g_full[gsl], g_phase(it));
-      uint8_t* gt = smem + L::G_OFF + gsl * L::Q_BYTES;
-#pragma unroll
-      for (int half = 0; half < DH / 32; ++half) {
-        uint32_t o[32];
-        tmem_ld32(tmem_base + O_COL + slot * 64 + half * 32 + lane_sel, o);
-        tmem_ld_wait();
-        if (half == DH / 32 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&o_empty[slot]);    // O and the row sums are in registers
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          // gate tile rows are DH*2 bytes with the TMA swizzle of Q (128B for DH = 64, 64B for DH = 32); the gated output
-          // replaces the gate values it was computed from, in the same (swizzled) place
-          const uint32_t goff = (DH == 64) ? swz128_off(r, half * 4 + i) : (r * 64u + ((static_cast<uint32_t>(i) ^ ((r >> 1) & 3u)) << 4));
-          const uint4 gq = k3 ? greg[half * 4 + i] : *reinterpret_cast<const uint4*>(gt + goff);
-          const uint32_t gw[4] = {gq.x, gq.y, gq.z, gq.w};
-          uint32_t ow[4];
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const float a = __uint_as_float(o[8 * i + 2 * t]) * inv_l * bf16lo_to_f32(gw[t]);
-            const float bb = __uint_as_float(o[8 * i + 2 * t + 1]) * inv_l * bf16hi_to_f32(gw[t]);
-            ow[t] = pack_bf16x2(a, bb);
-          }
-          *reinterpret_cast<uint4*>(gt + goff) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-        }
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        // this warp's 32 rows of the tile; rows beyond n are clipped by the tensor map
-        if (!(p.dbg_skip & 8)) tma_store_4d(&tmO, gt + q * 32 * ROWB, 0, qb * 128 + q * 32, h, b);
-        tma_store_commit();
-        tma_store_wait_read<0>();                        // the store has drained the tile: hand the slot back to the producer
-        if (!k3) mbar_arrive(&g_empty[gsl]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ================================ softmax warps ================================
-    constexpr int KPT = 128 / ATTN_NSPLIT;          // keys per thread and block
-    const int q = warp & 3;               // TMEM lane quarter
-    const int hk = (warp - 2) >> 2;       // which KPT-key slice of every 128-key block this thread owns
-    const int r = q * 32 + lane;          // query row inside the tile == TMEM lane
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    const float NEG_INF = -__int_as_float(0x7f800000);
-    // lazy O rescaling (rare): the DH accumulator columns are shared out 16 per slice
-    const bool o_owner = hk * 16 < DH;
-    int sb = 0;                            // S / P buffer of the block (g % ATTN_NSB) and the phase of its barriers, incremental
-    uint32_t sph = 0;
-
-    for (int it = 0; it < my_items; ++it) {
-    bool q_valid = true;
-    const uint32_t o_col = O_COL + (it & 1) * 64 + hk * 16;
-
-    float m_run = NEG_INF, l_run = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      const int g = it * nkv + j;
-      const int st = g & 1;
-      mbar_wait(&kb_full[st], (g >> 1) & 1);      // key terms (and, at j == 0, query-mask bytes) staged by the key-mask warp
-      if (j == 0) q_valid = qvbuf[(it & 1) * 128 + r] != 0;
-      mbar_wait(&s_full[sb], sph);
-      tc_fence_after();
-      if (warp == 2 && lane == 0) stamp(g, 4);
-
-      // logits (log2 domain) = S (pair bias included by the tensor core) + keyterm
-      float s[KPT];
-      {
-        uint32_t u[KPT];
-        tmem_ld32(tmem_base + S_COL + sb * 128 + hk * KPT + lane_sel, u);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < KPT; ++i) s[i] = __uint_as_float(u[i]);
-      }
-      if (kflag[st] != 0u) {                 // block-uniform: most blocks have every key usable
-        const float* kbs = keyb + st * 128 + hk * KPT;
-#pragma unroll
-        for (int c = 0; c < KPT / 4; ++c) {
-          const float4 k4 = *reinterpret_cast<const float4*>(kbs + c * 4);
-          s[c * 4 + 0] += k4.x; s[c * 4 + 1] += k4.y; s[c * 4 + 2] += k4.z; s[c * 4 + 3] += k4.w;
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&kb_empty[st]);
-      if (!q_valid) {                        // rare: masked query row -> uniform over the n real keys
-#pragma unroll
-        for (int k = 0; k < KPT; ++k) s[k] = (j * 128 + hk * KPT + k) < p.n ? 0.f : NEG_INF;
-      }
-      float mx0 = fmaxf(s[0], s[1]), mx1 = fmaxf(s[2], s[3]);
-#pragma unroll
-      for (int k = 4; k < KPT; k += 4) {
-        mx0 = fmaxf(mx0, fmaxf(s[k], s[k + 1]));
-        mx1 = fmaxf(mx1, fmaxf(s[k + 2], s[k + 3]));
-      }
-      // (double buffered by block parity: a warp can only be one named barrier ahead of the slowest reader)
-      float* mxb = mxbuf + st * ATTN_NSPLIT * 128;
-      mxb[hk * 128 + r] = fmaxf(mx0, mx1);
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "n"(32 * ATTN_NSPLIT) : "memory");   // the warps sharing these 32 rows
-      float m_new = m_run;
-#pragma unroll
-      for (int i = 0; i < ATTN_NSPLIT; ++i) m_new = fmaxf(m_new, mxb[i * 128 + r]);
-      // Lazy rescaling: the running maximum only has to be SOME upper bound up to a factor that neither overflows bf16 P nor
-      // the fp32 sums.  While the block maximum exceeds it by <= 2^8 (log2 domain) we keep the stale one and skip the
-      // TMEM round trip of O; the decision is made per warp (all warps sharing these rows see identical values).
-      bool rescale = true;
-      if (j > 0) {
-        rescale = __any_sync(0xffffffffu, m_new > m_run + 8.0f);
-        if (!rescale) m_new = m_run;
-      }
-      const float m_use = (m_new == NEG_INF) ? 0.f : m_new;
-      const float corr = fast_exp2(m_run - m_use);     // m_run = -inf -> 0
-      // packed fp32 pairs: one FADD2 subtracts the maximum from two logits, one FADD2 accumulates two terms of the row sum
-      const f32x2 nm2 = pack2(-m_use, -m_use);
-      f32x2 lsa = pack2(0.f, 0.f), lsb = pack2(0.f, 0.f);
-      uint32_t pk[KPT / 2];
-#pragma unroll
-      for (int k = 0; k < KPT; k += 4) {
-        float a0, a1, b0, b1;
-        unpack2(add2(pack2(s[k], s[k + 1]), nm2), a0, a1);
-        unpack2(add2(pack2(s[k + 2], s[k + 3]), nm2), b0, b1);
-#if AF2_ATTN_POLY_EXP
-        // every second exponential on the FMA pipe (common.cuh: exp2_poly2), the others on the MUFU
-        const float e0 = fast_exp2(a0), e2 = fast_exp2(b0);
-        float e1, e3;
-        unpack2(exp2_poly2(pack2(fmaxf(a1, -126.0f), fmaxf(b1, -126.0f))), e1, e3);
-#else
-        const float e0 = fast_exp2(a0), e1 = fast_exp2(a1), e2 = fast_exp2(b0), e3 = fast_exp2(b1);
-#endif
-        lsa = add2(lsa, pack2(e0, e1));
-        lsb = add2(lsb, pack2(e2, e3));
-        pk[k >> 1] = pack_bf16x2(e0, e1);
-        pk[(k >> 1) + 1] = pack_bf16x2(e2, e3);
-      }
-      float ls0, ls1;
-      unpack2(add2(lsa, lsb), ls0, ls1);
-      l_run = l_run * corr + (ls0 + ls1);
-      m_run = m_new;
-
-      // the previous P V must have retired before O is rescaled (rare: the running maximum moved by more than 2^8).  Its
-      // retirement is the event that frees its V stage, so v_empty of block g - 1 is the barrier to watch: that barrier
-      // cannot complete another phase before this thread has written P(g) (the next P V on the stage needs it).
-      if (j > 0 && rescale) {
-        mbar_wait(&v_empty[(g - 1) % nst], (((g - 1) / nst) & 1));
-        tc_fence_after();
-        if (o_owner) {
-          uint32_t o[16];
-          tmem_ld16(tmem_base + o_col + lane_sel, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * corr);
-          tmem_st16(tmem_base + o_col + lane_sel, o);
-        }
-      }
-      // P_j -> tensor memory: this thread's KPT keys become KPT/2 packed columns of the S buffer.  Those columns held logits
-      // of a lower slice, which its owner loaded before the row-max barrier above.
-      tmem_st16(tmem_base + S_COL + sb * 128 + hk * (KPT / 2) + lane_sel, pk);
-      if (j == nkv - 1) {
-        // hand the item over: its row sums go to the epilogue warps (slot it & 1, free once they have read the item that
-        // used it before); the matching O follows through o_full, committed behind the P V this arrival triggers
-        mbar_wait(&o_empty[it & 1], ((it >> 1) & 1) ^ 1);
-        lbuf[((it & 1) * ATTN_NSPLIT + hk) * 128 + r] = l_run;
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (warp == 2 && lane == 0) stamp(g, 5);
-      if (lane == 0) mbar_arrive(&p_full[sb]);
-      if (++sb == ATTN_NSB) { sb = 0; sph ^= 1; }
-    }
-    }  // work items
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
+  // ========================= softmax warpgroups: 64 query rows each =========================
+  regs_alloc<232>();
+  const int h = wg - 1, wq = warp & 3;
+  int rows[2];
+  bool qvalid[2];
+  const __nv_bfloat16* brow[2];
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    rows[hf] = qb * 128 + h * 64 + wq * 16 + (lane >> 2) + 8 * hf;
+    const bool in = rows[hf] < n;
+    qvalid[hf] = !(in && mrow && !mrow[static_cast<long long>(rows[hf]) * p.mask_si]);
+    brow[hf] = (p.has_bias && in) ? p.bias + (static_cast<long long>(hh) * n + rows[hf]) * p.npad : nullptr;
+  }
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[DH / 2];
+#pragma unroll
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+  float s[ATTN_KB / 2];
+  const uint32_t sq = smem_u32(smem) + h * 64 * ROWB;
+  mbar_wait(q_bar, 0);
+
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int st = kb % ATTN_STAGES;
+    mbar_wait(&full_bar[st], (kb / ATTN_STAGES) & 1);
+    const uint32_t sk = smem_u32(smem + L::STAGE_OFF + st * L::STAGE_BYTES);
+    const uint32_t sv = sk + L::KV_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k)
+      wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc(sq + k * 32, 16, SBO, SWZ), wgmma_desc(sk + k * 32, 16, SBO, SWZ), k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // logits -> probabilities (in place)
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < ATTN_KB / 8; ++j) {
+      const int key = kb * ATTN_KB + 8 * j + 2 * (lane & 3);
+      const uint32_t c0 = kcode[key], c1 = kcode[key + 1];
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        float b0 = 0.f, b1 = 0.f;
+        if (brow[hf] && c0 != 0) {
+          const uint32_t bw = __ldg(reinterpret_cast<const unsigned int*>(brow[hf] + key));
+          b0 = bf16lo_to_f32(bw);
+          b1 = bf16hi_to_f32(bw);
+        }
+        float& v0 = s[4 * j + 2 * hf];
+        float& v1 = s[4 * j + 2 * hf + 1];
+        v0 = c0 == 0 ? -INFINITY : ((c0 == 1 || !qvalid[hf]) ? -FLT_MAX : v0 + b0);
+        v1 = c1 == 0 ? -INFINITY : ((c1 == 1 || !qvalid[hf]) ? -FLT_MAX : v1 + b1);
+        mx[hf] = fmaxf(mx[hf], fmaxf(v0, v1));
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      mx[hf] = fmaxf(mx[hf], __shfl_xor_sync(0xffffffffu, mx[hf], 1));
+      mx[hf] = fmaxf(mx[hf], __shfl_xor_sync(0xffffffffu, mx[hf], 2));
+      const float m_new = fmaxf(m_run[hf], mx[hf]);    // finite: key 0 of block 0 is never padding
+      alpha[hf] = fast_exp2(m_run[hf] - m_new);        // 0 on the first block (m_run = -inf)
+      m_run[hf] = m_new;
+      l_run[hf] *= alpha[hf];
+    }
+    uint32_t pa[ATTN_KB / 16][4];
+#pragma unroll
+    for (int j = 0; j < ATTN_KB / 8; ++j) {
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        const float e0 = fast_exp2(s[4 * j + 2 * hf] - m_run[hf]);
+        const float e1 = fast_exp2(s[4 * j + 2 * hf + 1] - m_run[hf]);
+        l_run[hf] += e0 + e1;
+        // m64k16 A fragment of key chunk j / 2: a0 / a1 = rows lo / hi of keys 2t.., a2 / a3 = the same 8 keys further
+        pa[j >> 1][(j & 1) * 2 + hf] = pack_bf16x2(e0, e1);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) {
+      o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < ATTN_KB / 16; ++kk) {
+      // V tile [key][DH] is the MN-major B operand: 16 keys per step, 8-key groups SBO apart
+      const uint64_t vdesc = wgmma_desc(sv + kk * 16 * ROWB, 8192, SBO, SWZ);
+      if constexpr (DH == 64) wgmma_m64n64k16_rs<1>(o, pa[kk], vdesc, 1u);
+      else wgmma_m64n32k16_rs<1>(o, pa[kk], vdesc, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (lane == 0 && wq == 0) mbar_arrive(&empty_bar[st]);
+  }
+
+  // ------------------------------- epilogue: O / l * gate -> bf16 -------------------------------
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    l_run[hf] += __shfl_xor_sync(0xffffffffu, l_run[hf], 1);
+    l_run[hf] += __shfl_xor_sync(0xffffffffu, l_run[hf], 2);
+    if (rows[hf] >= n) continue;
+    const float inv = 1.0f / l_run[hf];
+    const long long tok = static_cast<long long>(bb) * p.tok_sb + static_cast<long long>(rows[hf]) * p.tok_si;
+    const __nv_bfloat16* g = p.gate + tok * p.ld_gate + hh * DH;
+    __nv_bfloat16* out = p.out + tok * p.ld_out + hh * DH;
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) {
+      const int e = 8 * i + 2 * (lane & 3);
+      const uint32_t gw = __ldg(reinterpret_cast<const unsigned int*>(g + e));
+      *reinterpret_cast<uint32_t*>(out + e) =
+          pack_bf16x2(o[4 * i + 2 * hf] * inv * bf16lo_to_f32(gw), o[4 * i + 2 * hf + 1] * inv * bf16hi_to_f32(gw));
+    }
+  }
 }
 
 }  // namespace af2

@@ -1,7 +1,7 @@
-// sm_100a device primitives shared by every kernel in this library: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (UMMA) descriptors / issue / commit, TMEM alloc / ld / st.
-// Hand-written inline PTX; no CUTLASS dependency.  Bit layouts follow the PTX ISA
-// "tcgen05 matrix descriptors" tables (K-major / MN-major canonical layouts).
+// sm_90a device primitives shared by every kernel in this library: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (warpgroup MMA) shared-memory descriptors / fences / issue.  Hand-written inline PTX; no CUTLASS
+// dependency.  Bit layouts follow the PTX ISA "Matrix Descriptor Format" of wgmma (K-major / MN-major
+// canonical layouts).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -59,20 +59,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
   const float erf_v = copysignf(erf_abs, x);
   return 0.5f * x * (1.0f + erf_v);
 }
-// The same function in 10 instructions for the epilogues that are ALU-issue bound:
-//   gelu(x) = x * Phi(x),  Phi(x) = 0.5 (1 + erf(x / sqrt 2)) ~= 1 / (1 + 2^(x Q(x^2))),  Q minimax-fitted on |x| <= 4.75
-// (tools/fit_gelu.py).  Phi abs err < 1.9e-5; gelu abs err < 5.5e-5 over all x (bf16 rounds the result to 2^-9 relative);
-// the logistic form keeps RELATIVE accuracy in the negative tail (unlike 0.5(1 + tanh)).
-__device__ __forceinline__ float gelu_fast(float x) {
-  const float xc = fminf(fmaxf(x, -7.0f), 7.0f);              // x Q(x^2) is monotone on [-8, 8]
-  const float x2 = xc * xc;
-  float q = fmaf(x2, 0.0009112266168574351f, -0.10617732324431346f);
-  q = fmaf(x2, q, -2.3017271259199106f);
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + fast_exp2(xc * q)));
-  return x * r;
-}
-
 // ------------------------------------------------------------------------------------------
 // mbarrier
 // ------------------------------------------------------------------------------------------
@@ -104,11 +90,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // ------------------------------------------------------------------------------------------
 // fences
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void fence_proxy_async_smem() {   // generic-proxy smem writes -> async proxy (UMMA/TMA)
+__device__ __forceinline__ void fence_proxy_async_smem() {   // generic-proxy smem writes -> async proxy (wgmma/TMA)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
 // TMA loads (tile mode, mbarrier completion)
@@ -120,6 +104,12 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
@@ -161,9 +151,9 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
                : "memory");
 }
 // ------------------------------------------------------------------------------------------
-// L2 eviction-priority hints (experiment AF2_X_EVICT_LAST, DESIGN.md): the fp32 pair stream (67 MB at C2) is read and written
-// by almost every kernel of a block; marking its lines evict_last keeps most of them in the 126 MB L2 between kernels while
-// the bf16 intermediates stream through with normal priority.  The policy operand is always passed (evict_normal = no-op).
+// L2 eviction-priority hints (experiment AF2_X_EVICT_LAST, DESIGN.md): the fp32 pair stream is read and written by almost
+// every kernel of a block; marking its lines evict_last keeps part of it in L2 between kernels while the bf16
+// intermediates stream through with normal priority.  The policy operand is always passed (evict_normal = no-op).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t l2_policy(bool evict_last) {
   uint64_t p;
@@ -199,7 +189,7 @@ __device__ __forceinline__ float2 ldg_f2_hint(const float2* p, uint64_t pol) {
 // cudaLaunchAttributeProgrammaticStreamSerialization and
 //   * signals `launch_dependents` right after its own set-up: the NEXT kernel's CTAs are then scheduled onto an SM the moment
 //     this kernel's CTA leaves it (instead of after the whole grid has drained + a launch latency) and run THEIR set-up
-//     (mbarrier init, TMEM allocation, tensor-map prefetch) in the shadow of this kernel's tail;
+//     (mbarrier init, tensor-map prefetch) in the shadow of this kernel's tail;
 //   * executes `wait` before its first access to global memory that a predecessor may have written (or still reads): the wait
 //     returns only when all prerequisite grids have completed and flushed, so the stream's data dependences are unchanged.
 // Both are no-ops for a launch without the attribute.
@@ -207,320 +197,92 @@ __device__ __forceinline__ float2 ldg_f2_hint(const float2* p, uint64_t pol) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// non-blocking probe of an mbarrier phase
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P1;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
-
-// A operand from tensor memory: D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
 // ------------------------------------------------------------------------------------------
-// packed fp32 pairs (FFMA2 / FADD2 / FMUL2 on sm_100): two IEEE fp32 operations per instruction and lane; the
-// halves round exactly like the scalar instructions
-// ------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-// gelu_fast / sigmoidf_fast on a pair: the polynomial, the +1 and the products run as packed instructions, only the clamp
-// and the two MUFU operations stay scalar (6 instead of 11 instructions per element).  The clamp acts on x^2 (<= 49):
-// beyond |x| = 7 the exponent is -5.3 x, which saturates to the exact limits 0 and x.
-__device__ __forceinline__ f32x2 gelu_fast2(f32x2 x) {
-  float a, b;
-  unpack2(mul2(x, x), a, b);
-  const f32x2 x2 = pack2(fminf(a, 49.0f), fminf(b, 49.0f));
-  f32x2 q = fma2(x2, pack2(0.0009112266168574351f, 0.0009112266168574351f), pack2(-0.10617732324431346f, -0.10617732324431346f));
-  q = fma2(x2, q, pack2(-2.3017271259199106f, -2.3017271259199106f));
-  unpack2(mul2(x, q), a, b);
-  float ra, rb;
-  unpack2(add2(pack2(fast_exp2(a), fast_exp2(b)), pack2(1.0f, 1.0f)), a, b);
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(ra) : "f"(a));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rb) : "f"(b));
-  return mul2(x, pack2(ra, rb));
-}
-__device__ __forceinline__ f32x2 sigmoidf_fast2(f32x2 x) {
-  float a, b, ra, rb;
-  unpack2(mul2(x, pack2(-1.4426950408889634f, -1.4426950408889634f)), a, b);
-  unpack2(add2(pack2(fast_exp2(a), fast_exp2(b)), pack2(1.0f, 1.0f)), a, b);
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(ra) : "f"(a));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rb) : "f"(b));
-  return pack2(ra, rb);
-}
-
-// 2^x for two values on the FMA pipe (no MUFU): round-to-nearest split x = i + f (|f| <= 0.5) by the 1.5 * 2^23 magic
-// constant, degree-4 polynomial for 2^f (max rel. error 4.2e-5 -- the result is rounded to bf16, 2^-9), exponent inserted by
-// an integer add: (as_int(t) << 23) keeps exactly i << 23 because the magic constant's low 9 bits are zero.  Used by the
-// attention softmax for every second element: the 16 softmax warps of a key block all reach their exponentials at the same
-// time, and with one MUFU.EX2 per element that phase alone is 1024 cycles (16 results / clk / SM) of a ~3800-cycle block.
-// x must be >= -126 (the caller clamps; -inf logits of masked keys become 2^-126 ~ 1e-38, i.e. zero after the bf16 pack).
-__device__ __forceinline__ f32x2 exp2_poly2(f32x2 x) {
-  const f32x2 magic = pack2(12582912.0f, 12582912.0f), nmagic = pack2(-12582912.0f, -12582912.0f);
-  const f32x2 t = add2(x, magic);
-  const f32x2 f = fma2(add2(t, nmagic), pack2(-1.0f, -1.0f), x);      // x - round(x), exact
-  f32x2 p = fma2(f, pack2(0.0096181291f, 0.0096181291f), pack2(0.0555041087f, 0.0555041087f));
-  p = fma2(p, f, pack2(0.2402265070f, 0.2402265070f));
-  p = fma2(p, f, pack2(0.6931471806f, 0.6931471806f));
-  p = fma2(p, f, pack2(1.0f, 1.0f));
-  float t0, t1, p0, p1;
-  unpack2(t, t0, t1);
-  unpack2(p, p0, p1);
-  const float r0 = __int_as_float(__float_as_int(p0) + (__float_as_int(t0) << 23));
-  const float r1 = __int_as_float(__float_as_int(p1) + (__float_as_int(t1) << 23));
-  return pack2(r0, r1);
-}
-
-// Four logistic values with ONE reciprocal.  The epilogues that apply sigmoid / GELU to whole accumulator tiles are bound by
-// the MUFU unit (16 results / clk / SM: ex2 + rcp per element = 4096 clk for a 128 x 256 tile against 2176 clk of tensor
-// work).  For a, b, c, d >= 1:  r = 1 / (a b c d)  ->  1/a = r (cd) b, ...: one MUFU.RCP and nine multiplies (five packed
-// instructions) replace four MUFU.RCP, i.e. 1.25 instead of 2 MUFU operations per element.  The exponents are clamped to
-// 2^30 so the product of four stays finite (2^120); beyond the clamp the logistic is < 1e-9, far below bf16 resolution.
-//   in : e01 = (2^y0, 2^y1), e23 = (2^y2, 2^y3) with y <= 30          out: (1/(1+e0), 1/(1+e1)), (1/(1+e2), 1/(1+e3))
-__device__ __forceinline__ void logistic4_from_exp(f32x2 e01, f32x2 e23, f32x2& r01, f32x2& r23) {
-  const f32x2 one = pack2(1.0f, 1.0f);
-  const f32x2 ac = add2(e01, one), bd = add2(e23, one);      // (a, b), (c, d) with a = 1 + e0, b = 1 + e1, c = 1 + e2, d = 1 + e3
-  float a, b, c, d;
-  unpack2(ac, a, b);
-  unpack2(bd, c, d);
-  const float ab = a * b, cd = c * d;
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(ab * cd));
-  const float rab = r * cd, rcd = r * ab;                     // 1 / (ab), 1 / (cd)
-  r01 = mul2(pack2(rab, rab), pack2(b, a));                   // (1/a, 1/b)
-  r23 = mul2(pack2(rcd, rcd), pack2(d, c));                   // (1/c, 1/d)
-}
-__device__ __forceinline__ void sigmoidf_fast4(f32x2 x01, f32x2 x23, f32x2& s01, f32x2& s23) {
-  const f32x2 nl = pack2(-1.4426950408889634f, -1.4426950408889634f);
-  float y0, y1, y2, y3;
-  unpack2(mul2(x01, nl), y0, y1);
-  unpack2(mul2(x23, nl), y2, y3);
-  logistic4_from_exp(pack2(fast_exp2(fminf(y0, 30.0f)), fast_exp2(fminf(y1, 30.0f))),
-                     pack2(fast_exp2(fminf(y2, 30.0f)), fast_exp2(fminf(y3, 30.0f))), s01, s23);
-}
-// gelu_fast on four values (same polynomial as gelu_fast2): x * 1 / (1 + 2^(x Q(x^2)))
-__device__ __forceinline__ void gelu_fast4(f32x2 x01, f32x2 x23, f32x2& g01, f32x2& g23) {
-  const f32x2 c2 = pack2(0.0009112266168574351f, 0.0009112266168574351f), c1 = pack2(-0.10617732324431346f, -0.10617732324431346f),
-              c0 = pack2(-2.3017271259199106f, -2.3017271259199106f);
-  float a, b, c, d;
-  unpack2(mul2(x01, x01), a, b);
-  unpack2(mul2(x23, x23), c, d);
-  const f32x2 q01 = pack2(fminf(a, 49.0f), fminf(b, 49.0f)), q23 = pack2(fminf(c, 49.0f), fminf(d, 49.0f));
-  const f32x2 p01 = fma2(q01, fma2(q01, c2, c1), c0), p23 = fma2(q23, fma2(q23, c2, c1), c0);
-  unpack2(mul2(x01, p01), a, b);
-  unpack2(mul2(x23, p23), c, d);
-  f32x2 r01, r23;
-  logistic4_from_exp(pack2(fast_exp2(fminf(a, 30.0f)), fast_exp2(fminf(b, 30.0f))),
-                     pack2(fast_exp2(fminf(c, 30.0f)), fast_exp2(fminf(d, 30.0f))), r01, r23);
-  g01 = mul2(x01, r01);
-  g23 = mul2(x23, r23);
-}
-
-// ------------------------------------------------------------------------------------------
-// TMEM allocation (one warp, .sync.aligned)
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------
-// UMMA descriptors
+// wgmma (sm_90a warpgroup MMA).  Four warps (one warpgroup) issue each MMA together; the fp32 accumulator of an
+// m64nN tile lives in registers: thread t (warp w = t / 32 % 4, lane l) holds rows 16 w + l / 4 and 16 w + l / 4 + 8,
+// columns 8 j + 2 (l % 4) + {0, 1}, as d[4 j + {0, 1}] (first row) and d[4 j + {2, 3}] (second row).
 // ------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor (64 bit):
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4
-//   [46,48) version (1 on sm_100) | [49,52) base offset | [61,64) layout: 0 none, 2 SW128, 4 SW64, 6 SW32
-enum : uint32_t { SWZ_128 = 2, SWZ_64 = 4, SWZ_32 = 6 };
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout) {
+//   [49,52) base offset (0: every tile is aligned to its swizzle repeat) | [62,64) layout: 1 SW128, 2 SW64, 3 SW32
+// K-major: rows of 16 k-elements' worth of swizzle atom, SBO = stride between 8-row groups (LBO unused).
+// MN-major: LBO = stride between swizzle-atom-wide MN blocks, SBO = stride between 8-row (k) groups.
+enum : uint32_t { SWZ_128 = 1, SWZ_64 = 2, SWZ_32 = 3 };
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
+  d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32:
-//   [4,6) D fmt (1 = f32) | [7,10) A fmt (1 = bf16) | [10,13) B fmt | 15 A major (1 = MN) | 16 B major
-//   [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// register budget per warpgroup: the TMA producer gives registers back, the MMA warpgroups take them
+template <int N>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// D (+)= A * B, A and B from shared memory; TA / TB = 1: operand is MN-major (transposed)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued MMAs of this thread arrive (once) on `bar` when complete.
-// Implicitly performs tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
-// ------------------------------------------------------------------------------------------
-// TMEM <-> registers.  A warp may only touch lanes 32*(warp_id % 4) .. +31; thread t of the warp
-// gets lane (row) 32*(warp_id%4)+t and N consecutive 32-bit columns.
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256k16_ss(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-      "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-      "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// 16-column variants (half the registers of the x32 forms)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+
+// D (+)= A * B, A from registers (the m64k16 bf16 fragment: a[i] = rows / columns of accumulator pairs 2 i, 2 i + 1)
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
+
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+
 
 // byte offset of 16-byte chunk `chunk` of row `row` inside a 128B-swizzled tile whose rows are 128 B
 __device__ __forceinline__ uint32_t swz128_off(uint32_t row, uint32_t chunk) {
   return row * 128u + ((chunk ^ (row & 7u)) << 4);
-}
-
-}  // namespace af2
-
-// ==========================================================================================
-// Thread-block-cluster / CTA-pair (cta_group::2) primitives
-// ==========================================================================================
-namespace af2 {
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier given by a shared::cluster address (possibly in the peer CTA).  Default (CTA-scope release)
-// semantics on purpose: a cluster-scope release compiles to MEMBAR.ALL.GPU and a cluster-scope acquire to CCTL.IVALL
-// (L1 invalidate) per wait, which cost tens of microseconds per work item.  What is ordered through these barriers is
-// either TMEM traffic (ordered by tcgen05.fence) or smem written in the SAME SM that the pair MMA later reads through
-// the async proxy (ordered by fence.proxy.async before the arrive), so CTA scope is sufficient.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
-// 2-D TMA load; CTA-pair variant signals the mbarrier given as a shared::cluster address (the leader's)
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem of both CTAs, 128 rows each] * B[smem, N/2 rows each]; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued cta_group::2 MMAs arrive (once) on the barrier at this smem offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask)
-               : "memory");
 }
 
 }  // namespace af2

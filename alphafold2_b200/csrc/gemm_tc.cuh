@@ -1,5 +1,5 @@
-// Generic batched bf16 GEMM on tcgen05 tensor cores with TMA-staged operands and a programmable epilogue
-// whose results leave the SM through shared memory + TMA stores (coalesced, OOB-clipped by hardware).
+// Generic batched bf16 GEMM on sm_90a warpgroup tensor cores (wgmma) with TMA-staged operands and a programmable
+// epilogue applied to the register accumulators.
 // One kernel serves every dense contraction of the Evoformer block:
 //
 //   K-major mode  : C[b][m][n] = sum_k A[b][m][k] * B[b][n][k]      (Linear layers: B = weight [out,in];
@@ -7,16 +7,12 @@
 //   MN-major mode : C[b][m][n] = sum_k A[b][k][m] * B[b][k][n]      (triangle "ingoing", outer-mean:
 //                                                                    channel-major operands, k = row axis)
 //
-// Tiling: BM = 128 rows (one TMEM lane per row), BN in {64,128,256} accumulator columns, BK = 64.
-// Warp roles (384 threads):
-//   warp 0  TMA producer of A/B stages          warp 1  MMA issuer (one elected lane)
-//   warp 2  TMEM allocator                      warp 3  epilogue staging-buffer producer (residual TMA loads)
-//   warps 4..11  epilogue, two groups of four: TMEM -> registers -> (bias, activation, gate, mask, residual) ->
-//               swizzled smem staging buffer -> TMA store (one leader thread per group issues)
-// Persistent over tiles; the accumulator is double-buffered in TMEM so the epilogue of tile i overlaps the
-// MMAs of tile i+1; four 16 KB staging buffers pipeline the stores.  When the output cannot be described by a
-// TMA tensor (ragged channel-major pitch, unaligned leading dimension, tiny BN) the epilogue falls back to
-// direct (slow, still correct) global stores.
+// Tiling: BM = 128 rows, BN in {64,128,256} accumulator columns, BK = 64.
+// Warp roles (384 threads, three warpgroups):
+//   warpgroup 0     TMA producer of the A/B stages (one thread issues; the warpgroup hands its registers to the others)
+//   warpgroups 1, 2 MMA + epilogue, rows 0..63 / 64..127 of the tile: wgmma m64nBNk16 into registers, then
+//                   (bias, activation, gate, row scale, residual) -> global stores straight from the accumulator fragment
+// Persistent over tiles; the producer runs ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
 #pragma once
 #include "common.cuh"
 
@@ -24,8 +20,6 @@ namespace af2 {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int EPI_BUFS = 4;
-constexpr int EPI_BUF_BYTES = 16384;
 
 enum EpiMode : int { EPI_STORE_BF16 = 0, EPI_GATED_BF16 = 1, EPI_RESID_F32 = 2, EPI_STORE_F32 = 3 };
 enum EpiAct : int { ACT_NONE = 0, ACT_SIGMOID = 1, ACT_GELU = 2 };
@@ -48,7 +42,7 @@ struct GemmParams {
   int M, N, K, batch;          // N = accumulator columns = rows of the B operand
   int num_ntiles;
   int out_cols;                // valid output columns (N, or N/2 for EPI_GATED)
-  int direct;                  // 1: direct global stores (no TMA store)
+  int direct;                  // unused: the epilogue always stores from registers
   const float* rowscale;       // [batch*M] multiplier per row (mask), or nullptr
   const float* resid;          // EPI_RESID_F32: fp32 [M, ld_resid]
   long long ld_resid;
@@ -66,7 +60,7 @@ struct GemmParams {
   // apart.  Rank-4 maps (k | mn, row | k, piece, batch) address them in place -- one launch instead of one per piece.
   //   a_pr / b_pr: rows (K-major) or columns (MN-major) per piece of A / B; 0 = plain rank-3 map.
   int a_pr, b_pr;
-  int x_evict_last;            // 1: residual loads / output stores of the fp32 stream carry an L2 evict_last hint (EK_RESID_F32_W)
+  int x_evict_last;            // 1: residual loads / output stores of the fp32 stream carry an L2 evict_last hint
   NTile tile;
 };
 
@@ -75,9 +69,9 @@ struct GemmSmem {
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KB
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int EPI_OFF = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFF = EPI_OFF + EPI_BUFS * EPI_BUF_BYTES;
-  static constexpr int TOTAL = BAR_OFF + 512 + 1024;       // barriers + 1 KB alignment slack
+  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int TOTAL = BAR_OFF + 256;
+  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA can use");
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -98,7 +92,7 @@ enum EpiKind : int {
   EK_RESID_F32 = 6,       // fp32 token-major, acc + bias + residual                (every output projection)
   EK_STORE_F32 = 7,       // fp32 token-major                                       (per-channel contractions)
   EK_STORE_CH_SIG = 8,    // bf16 channel-major, sigmoid(acc + bias)                (triangle out_gate for the fused tail)
-  EK_RESID_F32_W = 9      // EK_RESID_F32 with warp-autonomous epilogue warps (no block barriers; see the kernel)
+  EK_RESID_F32_W = 9      // EK_RESID_F32 for a single full 256-column tile (same epilogue)
 };
 template <int EK> struct EpiTraits { static constexpr int mode = -1, act = -1, layout = -1; static constexpr bool rowscale = true; };
 template <> struct EpiTraits<EK_STORE_TOK> { static constexpr int mode = EPI_STORE_BF16, act = ACT_NONE, layout = LAYOUT_TOKEN; static constexpr bool rowscale = false; };
@@ -111,51 +105,21 @@ template <> struct EpiTraits<EK_RESID_F32_W> { static constexpr int mode = EPI_R
 template <> struct EpiTraits<EK_STORE_CH_SIG> { static constexpr int mode = EPI_STORE_BF16, act = ACT_SIGMOID, layout = LAYOUT_CHANNEL; static constexpr bool rowscale = false; };
 template <> struct EpiTraits<EK_STORE_F32> { static constexpr int mode = EPI_STORE_F32, act = ACT_NONE, layout = LAYOUT_TOKEN; static constexpr bool rowscale = false; };
 
-__device__ __forceinline__ void load_bias32(const float* b, float (&bv)[32]) {
-  if (b) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 t4 = __ldg(reinterpret_cast<const float4*>(b) + j);
-      bv[4 * j] = t4.x; bv[4 * j + 1] = t4.y; bv[4 * j + 2] = t4.z; bv[4 * j + 3] = t4.w;
-    }
+constexpr int GEMM_THREADS = 384;   // producer warpgroup + two MMA warpgroups
+
+// stores the two values (col, col + 1) of one accumulator row, clipped to the valid columns
+template <bool F32>
+__device__ __forceinline__ void store_pair(void* base, long long off, float v0, float v1, bool two, bool vec) {
+  if constexpr (F32) {
+    float* o = reinterpret_cast<float*>(base) + off;
+    if (two && vec) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+    else { o[0] = v0; if (two) o[1] = v1; }
   } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) bv[j] = 0.f;
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(base) + off;
+    if (two && vec) *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(v0, v1);
+    else { o[0] = __float2bfloat16(v0); if (two) o[1] = __float2bfloat16(v1); }
   }
 }
-
-// 32 accumulator columns starting at tile-local column c -> finished values (bias, activation / gate, row scale)
-template <int BN, int EK>
-__device__ __forceinline__ void epi_values(uint32_t t_acc, int c, int mode, int act, const float* bias_tile, float rs,
-                                           float (&v)[32]) {
-  uint32_t u[32];
-  tmem_ld32(t_acc + c, u);
-  if (mode == EPI_GATED_BF16) {
-    uint32_t g[32];
-    tmem_ld32(t_acc + BN / 2 + c, g);
-    float bu[32], bg[32];
-    load_bias32(bias_tile ? bias_tile + c : nullptr, bu);
-    load_bias32(bias_tile ? bias_tile + BN / 2 + c : nullptr, bg);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const float uu = __uint_as_float(u[j]) + bu[j], gg = __uint_as_float(g[j]) + bg[j];
-      v[j] = uu * apply_act(gg, act);
-      if (EpiTraits<EK>::rowscale) v[j] *= rs;
-    }
-  } else {
-    float bu[32];
-    load_bias32(bias_tile ? bias_tile + c : nullptr, bu);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      v[j] = apply_act(__uint_as_float(u[j]) + bu[j], act);
-      if (EpiTraits<EK>::rowscale) v[j] *= rs;
-    }
-  }
-}
-
-constexpr int GEMM_THREADS = 384;   // 4 control warps + 8 epilogue warps
 
 template <int BN, int STAGES, bool MN_MAJOR, int EK>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -169,43 +133,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;     // [2] accumulator ready
-  uint64_t* tempty_bar = tfull_bar + 2;         // [2] accumulator drained
-  uint64_t* efull_bar = tempty_bar + 2;         // [EPI_BUFS] staging buffer free (+ residual landed)
-  uint64_t* eempty_bar = efull_bar + EPI_BUFS;  // [EPI_BUFS] staging buffer released by its TMA store
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(eempty_bar + EPI_BUFS);
-  uint64_t* wres_bar = eempty_bar + EPI_BUFS + 1;   // [8 warps][2] residual box landed (EK_RESID_F32_W)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr uint32_t TMEM_COLS = 2 * BN;
+  const int wg = warp >> 2;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    if (!p.direct) prefetch_tmap(&tmC);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);     // one arrive per MMA warpgroup
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 8);   // one arrive per epilogue warp
-    }
-    for (int s = 0; s < EPI_BUFS; ++s) {
-      mbar_init(&efull_bar[s], 1);
-      mbar_init(&eempty_bar[s], 1);
-    }
-    for (int s = 0; s < 16; ++s) mbar_init(&wres_bar[s], 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();
 
@@ -214,26 +156,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int total_tiles = p.batch * m_tiles * n_tiles;
   const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
   const int nseg = p.nseg > 1 ? p.nseg : 1;
-  const int num_kk = num_kb * nseg;                 // k-blocks the MMA warp consumes per tile
+  const int num_kk = num_kb * nseg;                 // k-blocks consumed per tile
 
-  // epilogue geometry shared by the staging producer (warp 3) and the epilogue warps
-  const int e_mode = (EK == EK_GENERIC) ? p.tile.mode : EpiTraits<EK>::mode;
-  const int e_act = (EK == EK_GENERIC) ? p.tile.act : EpiTraits<EK>::act;
-  const int e_layout = (EK == EK_GENERIC) ? p.tile.layout : EpiTraits<EK>::layout;
-  const int W = (e_mode == EPI_GATED_BF16) ? BN / 2 : BN;                      // output columns per tile
-  const bool out_f32 = (e_mode == EPI_RESID_F32) || (e_mode == EPI_STORE_F32);
-  const int CW = out_f32 ? 32 : 64;                                            // output columns per staging chunk
-
-  if (warp == 0) {
+  if (wg == 0) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = tile % n_tiles;
         const int mt = (tile / n_tiles) % m_tiles;
         const int b = tile / (n_tiles * m_tiles);
-        for (int kk = 0; kk < num_kb * nseg; ++kk) {
+        for (int kk = 0; kk < num_kk; ++kk) {
           const int seg = kk / num_kb, kb = kk - seg * num_kb;
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * L::STAGE_BYTES;
@@ -286,270 +221,117 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ==================================
-    constexpr uint32_t idesc = umma_idesc_bf16(GEMM_BM, BN, MN_MAJOR ? 1 : 0, MN_MAJOR ? 1 : 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kk; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            uint64_t adesc, bdesc;
-            if constexpr (!MN_MAJOR) {
-              // rows of 128 B (64 bf16 of K); 8-row swizzle atoms 1024 B apart; K step = 32 B
-              adesc = umma_smem_desc(sa + k * 32, 16, 1024, SWZ_128);
-              bdesc = umma_smem_desc(sb + k * 32, 16, 1024, SWZ_128);
-            } else {
-              // k-rows of 128 B (64 bf16 of M/N); 8 k-rows = 1024 B (SBO); next 64-wide mn group 8 KB (LBO)
-              adesc = umma_smem_desc(sa + k * 2048, 8192, 1024, SWZ_128);
-              bdesc = umma_smem_desc(sb + k * 2048, 8192, 1024, SWZ_128);
-            }
-            umma_bf16(d_tmem, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);                       // smem slot free once these MMAs retire
-          if (kb == num_kk - 1) umma_commit(&tfull_bar[acc]);   // accumulator complete
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 3) {
-    // ===================== staging-buffer producer (residual prefetch) ==================
-    if (lane == 0 && !p.direct && EK != EK_RESID_F32_W) {
-      uint32_t ec = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int nt = tile % n_tiles;
-        const int mt = (tile / n_tiles) % m_tiles;
-        const int b = tile / (n_tiles * m_tiles);
-        const int ncols = min(W, p.out_cols - nt * W);
-        const int nchunks = (ncols + CW - 1) / CW;
-        for (int cc = 0; cc < nchunks; ++cc, ++ec) {
-          const int buf = ec % EPI_BUFS;
-          mbar_wait(&eempty_bar[buf], ((ec / EPI_BUFS) & 1) ^ 1);
-          if (e_mode == EPI_RESID_F32) {
-            mbar_arrive_expect_tx(&efull_bar[buf], EPI_BUF_BYTES);
-            tma_load_3d(smem + L::EPI_OFF + buf * EPI_BUF_BYTES, &tmR, &efull_bar[buf], nt * W + cc * CW,
-                        mt * GEMM_BM, b);
-          } else {
-            mbar_arrive(&efull_bar[buf]);
-          }
-        }
-      }
-    }
-  } else if (warp >= 4 && EK == EK_RESID_F32_W) {
-    // ============ epilogue, warp-autonomous (out = acc + bias + residual, fp32, BN = 256, TMA-describable) ============
-    // Every warp owns the 32 accumulator rows of its TMEM lane quarter and every second 32-column chunk of them, two
-    // private 4 KB staging buffers ([32 rows][128 B], 128B swizzle), prefetches its own residual boxes with TMA one
-    // chunk ahead (across tiles), adds in place and stores with its own TMA store: no block barriers, no helper warp.
-    const int q = warp & 3;
-    const int grp = (warp - 4) >> 2;
-    uint8_t* wbuf = smem + L::EPI_OFF + (warp - 4) * 8192;
-    uint64_t* rbar = wres_bar + (warp - 4) * 2;
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    const NTile tl = p.tile;
-    const uint64_t xpol = l2_policy(p.x_evict_last != 0);
-    const int my_tiles = (total_tiles > static_cast<int>(blockIdx.x)) ? (total_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1 : 0;
-    constexpr int CPW = 4;                                   // chunks per warp and tile (256 columns / 32 / 2 warps)
-    const int total_chunks = my_tiles * CPW;
-    auto chunk_coords = [&](int k, int& m0w, int& colc) {    // k-th chunk of this warp's stream
-      const int mt = blockIdx.x + (k / CPW) * gridDim.x;    // = the tile index: EK_RESID_F32_W launches have batch 1 and ONE column
-                                                             // tile (no run-time divisions on this path: it runs per 32-column chunk)
-      m0w = mt * GEMM_BM + q * 32;
-      colc = (grp + 2 * (k % CPW)) * 32;
-    };
-    auto prefetch = [&](int k) {                             // lane 0: residual box of chunk k -> buffer k & 1
-      int m0w, colc;
-      chunk_coords(k, m0w, colc);
-      tma_store_wait_read<0>();                              // the store that used this buffer (chunk k - 2) has read it
-      mbar_arrive_expect_tx(&rbar[k & 1], 4096);
-      tma_load_3d_hint(wbuf + (k & 1) * 4096, &tmR, &rbar[k & 1], colc, m0w, 0, xpol);
-    };
-    if (lane == 0 && total_chunks > 0) prefetch(0);
-    for (int k = 0; k < total_chunks; ++k) {
-      const int ti = k / CPW, ci = k % CPW;
-      const int acc = ti & 1;
-      int m0w, colc;
-      chunk_coords(k, m0w, colc);
-      if (ci == 0) {
-        mbar_wait(&tfull_bar[acc], (ti >> 1) & 1);
-        tc_fence_after();
-      }
-      uint32_t u[32];
-      tmem_ld32(tmem_base + acc * BN + lane_sel + colc, u);
-      float bv[32];
-      load_bias32(tl.bias ? tl.bias + colc : nullptr, bv);
-      // residual box of the next chunk into the other buffer: its last user, the store of chunk k - 1, was issued a whole
-      // chunk ago, so waiting for its smem read here is normally free
-      if (lane == 0 && k + 1 < total_chunks) prefetch(k + 1);
-      tmem_ld_wait();
-      if (ci == CPW - 1) {                                   // this warp's loads of the tile have landed: release the stage
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      }
-      mbar_wait(&rbar[k & 1], (k >> 1) & 1);
-      uint8_t* eb = wbuf + (k & 1) * 4096;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4* sp = reinterpret_cast<float4*>(eb + swz128_off(lane, j));
-        const float4 r4 = *sp;
-        *sp = make_float4(__uint_as_float(u[4 * j]) + bv[4 * j] + r4.x, __uint_as_float(u[4 * j + 1]) + bv[4 * j + 1] + r4.y,
-                          __uint_as_float(u[4 * j + 2]) + bv[4 * j + 2] + r4.z, __uint_as_float(u[4 * j + 3]) + bv[4 * j + 3] + r4.w);
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_3d_hint(&tmC, eb, colc, m0w, 0, xpol);
-        tma_store_commit();
-      }
-    }
-    if (lane == 0) tma_store_wait_read<0>();
-  } else if (warp >= 4) {
-    // ================================ epilogue ====================================
-    // Two groups of four warps (4..7 and 8..11); warp w may touch TMEM lanes 32*(w%4)..+31, so each group covers
-    // all 128 rows; the groups take alternating staging chunks (group g owns chunks with ec % 2 == g).
-    const int q = warp & 3;                   // TMEM lane quarter this warp may access
-    const int grp = (warp - 4) >> 2;          // 0 / 1
-    const int row_in_tile = q * 32 + lane;
-    const bool leader = (threadIdx.x == 128 + grp * 128);
-    const NTile t = p.tile;
-    int it = 0;
-    uint32_t ec = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int nt = tile % n_tiles;
-      const int mt = (tile / n_tiles) % m_tiles;
-      const int b = tile / (n_tiles * m_tiles);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int col0 = nt * W;
-      const int ncols = min(W, p.out_cols - col0);
-      const float* bias_tile = t.bias ? t.bias + nt * BN : nullptr;
-      const int row = mt * GEMM_BM + row_in_tile;
-      const bool row_ok = row < p.M;
-      float rs = 1.0f;
-      if (t.use_rowscale && row_ok) rs = __ldg(p.rowscale + static_cast<long long>(b) * p.M + row);
-
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_acc = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16);
-
-      if (!p.direct) {
-        const int nchunks = (ncols + CW - 1) / CW;
-        for (int cc = 0; cc < nchunks; ++cc, ++ec) {
-          if ((ec & 1) != static_cast<uint32_t>(grp)) continue;
-          const int buf = ec % EPI_BUFS;
-          uint8_t* eb = smem + L::EPI_OFF + buf * EPI_BUF_BYTES;
-          mbar_wait(&efull_bar[buf], (ec / EPI_BUFS) & 1);
-          if (out_f32) {
-            float v[32];
-            epi_values<BN, EK>(t_acc, cc * 32, e_mode, e_act, bias_tile, rs, v);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4* sp = reinterpret_cast<float4*>(eb + swz128_off(row_in_tile, j));
-              float4 o = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              if (e_mode == EPI_RESID_F32) {
-                const float4 r4 = *sp;
-                o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
-              }
-              *sp = o;
-            }
-          } else {
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-              float v[32];
-              epi_values<BN, EK>(t_acc, cc * 64 + half * 32, e_mode, e_act, bias_tile, rs, v);
-              if (e_layout == LAYOUT_TOKEN) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const uint4 pk = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                                              pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-                  *reinterpret_cast<uint4*>(eb + swz128_off(row_in_tile, half * 4 + j)) = pk;
-                }
-              } else {
-                // staging holds [64 channels][128 tokens] as two 64-token boxes of 64 rows x 128 B
-                uint8_t* bx = eb + (row_in_tile >> 6) * 8192;
-                const uint32_t tl = row_in_tile & 63;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  const uint32_t c = half * 32 + j;
-                  *reinterpret_cast<__nv_bfloat16*>(bx + c * 128 + ((((tl >> 3) ^ (c & 7)) << 4) | ((tl & 7) << 1))) =
-                      __float2bfloat16(v[j]);
-                }
-              }
-            }
-          }
-          fence_proxy_async_smem();
-          if (grp == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-          else asm volatile("bar.sync 2, 128;" ::: "memory");
-          if (leader) {
-            if (e_layout == LAYOUT_TOKEN) {
-              tma_store_3d(&tmC, eb, col0 + cc * CW, mt * GEMM_BM, b);
-            } else {
-              tma_store_3d(&tmC, eb, mt * GEMM_BM, col0 + cc * 64, b);
-              tma_store_3d(&tmC, eb + 8192, mt * GEMM_BM + 64, col0 + cc * 64, b);
-            }
-            tma_store_commit();
-            tma_store_wait_read<1>();                       // this group's previous store (chunk ec-2) has drained its buffer
-            if (ec >= 2) mbar_arrive(&eempty_bar[(ec - 2) % EPI_BUFS]);
-          }
-        }
-      } else if (grp == 0) {
-        // ------------------------- direct global stores (fallback, one group) -------------------------
-        long long cm_off = 0;
-        if (e_layout == LAYOUT_CHANNEL) cm_off = static_cast<long long>(row / p.cm_inner) * p.cm_pitch + row % p.cm_inner;
-#pragma unroll 1
-        for (int c0 = 0; c0 < W; c0 += 32) {
-          if (c0 >= ncols) break;           // warp-uniform
-          float v[32];
-          epi_values<BN, EK>(t_acc, c0, e_mode, e_act, bias_tile, rs, v);
-          if (!row_ok) continue;
-          if (!out_f32) {
-            __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(t.out) + b * p.out_batch_stride;
-            if (e_layout == LAYOUT_TOKEN) {
-              __nv_bfloat16* dst = out + static_cast<long long>(row) * t.ld + col0 + c0;
-              for (int j = 0; j < 32; ++j)
-                if (c0 + j < ncols) dst[j] = __float2bfloat16(v[j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (c0 + j < ncols) out[static_cast<long long>(col0 + c0 + j) * t.ld + cm_off] = __float2bfloat16(v[j]);
-            }
-          } else {
-            float* dst = reinterpret_cast<float*>(t.out) + b * p.out_batch_stride + static_cast<long long>(row) * t.ld + col0 + c0;
-            if (e_mode == EPI_RESID_F32) {
-              const float* rsd = p.resid + static_cast<long long>(row) * p.ld_resid + col0 + c0;
-              for (int j = 0; j < 32; ++j)
-                if (c0 + j < ncols) dst[j] = v[j] + rsd[j];
-            } else {
-              for (int j = 0; j < 32; ++j)
-                if (c0 + j < ncols) dst[j] = v[j];
-            }
-          }
-        }
-      }
-      // accumulator drained: hand the TMEM stage back to the MMA warp (8 warps arrive)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-    }
-    if (!p.direct && leader) tma_store_wait_read<0>();   // smem must outlive the last TMA store's reads
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, TMEM_COLS);
+  // ===================== MMA + epilogue (warpgroup 1: rows 0..63, warpgroup 2: rows 64..127) =====================
+  regs_alloc<232>();
+  const int h = wg - 1;
+  const int wq = warp & 3;
+  const int e_mode = (EK == EK_GENERIC) ? p.tile.mode : EpiTraits<EK>::mode;
+  const int e_act = (EK == EK_GENERIC) ? p.tile.act : EpiTraits<EK>::act;
+  const int e_layout = (EK == EK_GENERIC) ? p.tile.layout : EpiTraits<EK>::layout;
+  const bool gated = e_mode == EPI_GATED_BF16;
+  const bool out_f32 = (e_mode == EPI_RESID_F32) || (e_mode == EPI_STORE_F32);
+  const int W = gated ? BN / 2 : BN;                                           // output columns per tile
+  const NTile t = p.tile;
+  // paired (8-byte fp32 / 4-byte bf16) stores need an even row pitch and an aligned base
+  const bool vec_out = (t.ld % 2 == 0) && (p.out_batch_stride % 2 == 0) &&
+                       (reinterpret_cast<uintptr_t>(t.out) & (out_f32 ? 7 : 3)) == 0;
+  const bool vec_res = (p.ld_resid % 2 == 0) && (reinterpret_cast<uintptr_t>(p.resid) & 7) == 0;
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int nt = tile % n_tiles;
+    const int mt = (tile / n_tiles) % m_tiles;
+    const int b = tile / (n_tiles * m_tiles);
+    int prev = -1;
+    for (int kk = 0; kk < num_kk; ++kk) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
+      const uint32_t sb = sa + L::A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BK / 16; ++k) {
+        uint64_t adesc, bdesc;
+        if constexpr (!MN_MAJOR) {
+          // rows of 128 B (64 bf16 of K); 8-row swizzle atoms 1024 B apart; K step = 32 B; this warpgroup's 64 rows 8 KB in
+          adesc = wgmma_desc(sa + h * 8192 + k * 32, 16, 1024, SWZ_128);
+          bdesc = wgmma_desc(sb + k * 32, 16, 1024, SWZ_128);
+        } else {
+          // k-rows of 128 B (64 bf16 of M/N); 8 k-rows = 1024 B (SBO); next 64-wide mn block 8 KB (LBO); this warpgroup's
+          // 64 rows are the h-th 64-wide box of A
+          adesc = wgmma_desc(sa + h * 8192 + k * 2048, 8192, 1024, SWZ_128);
+          bdesc = wgmma_desc(sb + k * 2048, 8192, 1024, SWZ_128);
+        }
+        const uint32_t scale_d = (kk | k) != 0 ? 1u : 0u;
+        if constexpr (BN == 256) wgmma_m64n256k16_ss<MN_MAJOR ? 1 : 0, MN_MAJOR ? 1 : 0>(acc, adesc, bdesc, scale_d);
+        else if constexpr (BN == 128) wgmma_m64n128k16_ss<MN_MAJOR ? 1 : 0, MN_MAJOR ? 1 : 0>(acc, adesc, bdesc, scale_d);
+        else wgmma_m64n64k16_ss<MN_MAJOR ? 1 : 0, MN_MAJOR ? 1 : 0>(acc, adesc, bdesc, scale_d);
+      }
+      wgmma_commit();
+      // keep one k-block in flight: the previous one has retired, so its stage goes back to the producer
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0 && wq == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (prev >= 0 && lane == 0 && wq == 0) mbar_arrive(&empty_bar[prev]);
+
+    // ------------------------------- epilogue from registers -------------------------------
+    const int col0 = nt * W;
+    const int ncols = min(W, p.out_cols - col0);
+    const float* bias_tile = t.bias ? t.bias + nt * BN : nullptr;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int row = mt * GEMM_BM + h * 64 + wq * 16 + (lane >> 2) + half * 8;
+      if (row >= p.M) continue;
+      float rs = 1.0f;
+      if (EpiTraits<EK>::rowscale && t.use_rowscale) rs = __ldg(p.rowscale + static_cast<long long>(b) * p.M + row);
+      long long cm_off = 0;
+      if (e_layout == LAYOUT_CHANNEL) cm_off = static_cast<long long>(row / p.cm_inner) * p.cm_pitch + row % p.cm_inner;
+      const long long obase = static_cast<long long>(b) * p.out_batch_stride;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {                    // fully unrolled: the accumulator stays in registers
+        const int c = 8 * j + 2 * (lane & 3);                // tile-local output column of the pair
+        if ((gated && j >= BN / 16) || c >= ncols) continue;
+        const bool two = c + 1 < ncols;
+        float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+        if (bias_tile) { v0 += __ldg(bias_tile + c); v1 += __ldg(bias_tile + c + 1); }
+        if (gated) {
+          // gate columns of the packed tile sit BN / 2 columns (BN / 16 fragment steps) to the right of their values
+          constexpr int JM = BN / 8 - 1;
+          const int jg = (j + BN / 16) & JM;
+          float g0 = acc[4 * jg + 2 * half], g1 = acc[4 * jg + 2 * half + 1];
+          if (bias_tile) { g0 += __ldg(bias_tile + BN / 2 + c); g1 += __ldg(bias_tile + BN / 2 + c + 1); }
+          v0 *= apply_act(g0, e_act);
+          v1 *= apply_act(g1, e_act);
+        } else {
+          v0 = apply_act(v0, e_act);
+          v1 = apply_act(v1, e_act);
+        }
+        if (EpiTraits<EK>::rowscale && t.use_rowscale) { v0 *= rs; v1 *= rs; }
+        const int col = col0 + c;
+        if (e_layout == LAYOUT_CHANNEL) {
+          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(t.out) + obase + cm_off;
+          o[static_cast<long long>(col) * t.ld] = __float2bfloat16(v0);
+          if (two) o[static_cast<long long>(col + 1) * t.ld] = __float2bfloat16(v1);
+        } else if (out_f32) {
+          if (e_mode == EPI_RESID_F32) {
+            const float* r = p.resid + static_cast<long long>(row) * p.ld_resid + col;
+            if (two && vec_res) { const float2 r2 = *reinterpret_cast<const float2*>(r); v0 += r2.x; v1 += r2.y; }
+            else { v0 += r[0]; if (two) v1 += r[1]; }
+          }
+          store_pair<true>(t.out, obase + static_cast<long long>(row) * t.ld + col, v0, v1, two, vec_out);
+        } else {
+          store_pair<false>(t.out, obase + static_cast<long long>(row) * t.ld + col, v0, v1, two, vec_out);
+        }
+      }
+    }
+  }
 }
 
 }  // namespace af2

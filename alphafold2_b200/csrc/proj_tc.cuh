@@ -1,717 +1,223 @@
-// Fused  LayerNorm -> multi-segment projection GEMM  for K = d <= 256 on tcgen05, CTA-pair (cta_group::2) MMA.
+// Fused  LayerNorm -> multi-segment projection GEMM  for K = d in {128, 192, 256} on sm_90a wgmma.
 //
 //   out_seg = epilogue_seg( LN(x)[T, d] * Wcat[tiles of 256 rows, d]^T + bcat )
 // x is the fp32 token-major residual stream; the LayerNorm affine is folded into the packed operands on the host
-// (W' = W diag(gamma), b' = W beta + b), so the kernel's producer computes (x - mean) * rstd only.  This is every
-// LN -> Linear cluster of the reference: alphafold2.py:82-85, 210-217 + 114-118, 269-276 + 297-311, 330-340.
+// (W' = W diag(gamma), b' = W beta + b, alphafold2_b200/ops.py _cat_segments), so the kernel computes (x - mean) * rstd
+// only.  This is every LN -> Linear cluster of the reference: alphafold2.py:82-85, 210-217 + 114-118, 269-276 + 297-311,
+// 330-340.  Against the unfused LayerNorm kernel + GEMM it saves the bf16 round trip of the normalised activations through
+// HBM, and one launch serves several outputs with different epilogue programs (q|k|v + gate; left + right + out-gate ...).
 //
-// Why this shape: the K = 256 projections of the Evoformer are L2->SM bandwidth bound when tiled 128 x 256 with
-// both operands streamed (192 KB of operand per 16.8 MFLOP; the L2 caps near 6300 B/clk chip-wide).  Here
-//   * the A tile (128 rows x d, bf16, 64 KB) is produced once per work item by SIMT warps straight from the fp32
-//     residual stream (no LayerNorm kernel, no bf16 round trip through HBM) and stays resident (double buffered)
-//     while ALL column tiles of the item stream past it;
-//   * two CTAs of a cluster form a pair: one tcgen05.mma.cta_group::2 covers M = 256 rows (128 per CTA) x N = 256,
-//     each CTA stages only its half of the weight tile (TMA, 16 KB per k-block), halving weight traffic per FLOP;
-//   * one launch serves several outputs with different epilogue programs (q|k|v + gate; left + right + out-gate ...)
-//     so the normalised activations are never re-read;
-//   * the bias enters through the tensor core: every column tile starts with one extra K = 16 MMA step
-//     ones[128 x 16] x Bext[256 x 16]^T  (Bext columns 0 / 1 = bf16 hi / lo split of the fp32 bias), so the epilogue
-//     neither loads nor adds biases and hands the accumulator stage back as soon as its TMEM loads have landed.
-// The kernel is specialised at compile time on (pair / single CTA, set of epilogue kinds) so each instantiation carries
-// only the code it runs (the all-in-one version was instruction-cache bound).
-// Warp roles per CTA (512 threads): 0 weight-tile TMA producer | 1 MMA issuer (leader CTA only) | 2 TMEM allocator |
-// 3 idle | 4..11 epilogue: each warp autonomous (its 32 TMEM lanes, every second 64-column block -- 32-column chunk when
-// a segment's width is not a multiple of 64 --, a private 4 KB staging area, its own TMA stores; no block barriers) |
-// 12..15 LayerNorm producers (8 lanes per row, packed fp32 math).
-// Accumulators are double buffered in TMEM (2 x 256 columns per CTA).
-// Work split: the flat sequence of (row unit of 256 rows, column tile) pairs is cut into one contiguous range per cluster.
-// A debug timeline of one CTA is available (ProjParams::trace, AF2_PROJ_TRACE=1, tools/proj_trace.py); DESIGN.md 10b
-// reads it: the steady state is bound by the epilogue's fixed per-step latencies, the q|k|v+gate launch additionally by
-// the rate at which HBM absorbs its 268 MB of output.
+// Work item = 128 rows.  The MMA warpgroups (1, 2) normalise the item's rows straight into the 128B-swizzled A tile in
+// shared memory (one warp per row, one 16-byte chunk of 8 channels per lane); the tile then stays resident while EVERY
+// 256-column weight tile of every segment streams past it through a TMA ring fed by warpgroup 0.  Each MMA warpgroup
+// runs wgmma m64n256k16 on its 64 rows and applies the segment's epilogue from the register fragment (the same
+// programs as gemm_tc.cuh: bias, sigmoid / erf-GELU, GEGLU gate, row mask, token- or channel-major bf16 store).
+// Persistent CTAs; the producer runs ahead into the next item's weight tiles while the A tile is being rebuilt.
 #pragma once
 #include "gemm_tc.cuh"
-#include "simt_kernels.cuh"
 
 namespace af2 {
 
-constexpr int PROJ_THREADS = 512;
-constexpr int PROJ_MAX_SEG = 4;
-constexpr int PROJ_NPROD = 4;             // producer warps per CTA (12..15, one per SM sub-partition: adding warps 2 / 3 slowed the
-                                          // epilogue warps of their sub-partitions by more than it gained)
-constexpr int PROJ_A_BUF = 65536;          // 128 rows x 256 K bf16 (4 k-blocks of 16 KB)
-
-__host__ __device__ constexpr int KBIT(int ek) { return 1 << ek; }
-// epilogue-kind sets of the instantiations
-constexpr int PK_ATTN = KBIT(EK_STORE_TOK) | KBIT(EK_STORE_TOK_SIG);      // [q|k|v] + sigmoid(gating)
-constexpr int PK_TRI = KBIT(EK_GATED_CH_SIG) | KBIT(EK_STORE_TOK_SIG);    // left, right (gated, masked, channel-major) + out gate
-constexpr int PK_TRI_CH = KBIT(EK_GATED_CH_SIG) | KBIT(EK_STORE_CH_SIG);  // ... with a channel-major out gate (fused tail)
-constexpr int PK_FF = KBIT(EK_GATED_TOK_GELU);                            // GEGLU
-constexpr int PK_OUTER = KBIT(EK_STORE_CH);                               // left | right (masked, channel-major)
+constexpr int PROJ_THREADS = 384;
+constexpr int PROJ_MAX_SEG = 3;
+constexpr int PROJ_BN = 256;               // accumulator columns per weight tile
+constexpr int PROJ_STAGES = 4;
 
 struct ProjSeg {
-  int tile0, ntiles;     // accumulator-column tiles (256 columns each) [tile0, tile0 + ntiles)
-  int kind;              // EpiKind
+  int tile0, ntiles;     // weight tiles (256 accumulator columns each) [tile0, tile0 + ntiles)
+  int kind;              // EpiKind: EK_STORE_TOK, EK_STORE_TOK_SIG, EK_STORE_CH, EK_GATED_TOK_GELU, EK_GATED_CH_SIG
   int out_cols;          // valid output columns of the segment
-  int map;               // output tensor map index (0..2)
-  int wide;              // 1: out_cols % 64 == 0 -> 64-column epilogue steps (tensor map box 64 x 32 / 32 x 64)
+  void* out;
+  long long ld;          // token layout: row stride (elements); channel layout: channel stride (elements)
 };
 
 struct ProjParams {
   const float* x;                // [T, d] fp32 token-major residual stream
   long long T;
   int d;
-  float inv_d;
-  float eps;
-  const unsigned char* rowmask;  // [T] bool row scale or nullptr (kinds with rowscale)
+  float inv_d, eps;
+  const unsigned char* rowmask;  // [T] bool row scale (channel-major kinds) or nullptr
+  const float* bcat;             // fp32 bias per accumulator column of Wcat (LayerNorm shift folded in)
   int nseg;
   ProjSeg seg[PROJ_MAX_SEG];
   int n_tiles_total;
-  int nsplit;                    // column chunks per row unit (balance == 0)
-  int balance;                   // 1: every cluster owns a contiguous range of the flat (row unit, column tile) sequence
-  long long* trace;              // debug (AF2_PROJ_TRACE=1): clock64 stamps of cluster 0's leader CTA, see tools/proj_trace.py
   int m_tiles;                   // ceil(T / 128)
-  int l2_prefetch;               // 1: producers prefetch the next item's rows into L2 (AF2_PROJ_L2PF)
-  int x_evict_last;              // 1: loads of x carry an L2 evict_last hint (AF2_X_EVICT_LAST)
 };
 
-template <int CTAS>
 struct ProjSmem {
-  static constexpr int STAGES = CTAS == 2 ? 4 : 1;      // (the single-CTA variant is a debugging aid only)
-  static constexpr int B_ROWS = 256 / CTAS;
-  static constexpr int B_STAGE = B_ROWS * GEMM_BK * 2;               // 16 KB (pair) / 32 KB
-  static constexpr int EPI_BUFS = 16;                                 // two private staging buffers per epilogue warp
-  static constexpr int EPI_BYTES = 2048;                              // 32 rows x 64 B (32 bf16 columns)
-  static constexpr int A_OFF = 0;
-  static constexpr int B_OFF = 2 * PROJ_A_BUF;
-  static constexpr int EPI_OFF = B_OFF + STAGES * B_STAGE;
-  static constexpr int AEXT_OFF = EPI_OFF + EPI_BUFS * EPI_BYTES;      // ones block of the bias K-step: 128 rows x 32 B
-  static constexpr int BEXT_BYTES = B_ROWS * 32;                       // bias block of a column tile: rows x 16 bf16
-  // every row of the ones block is identical, so ONE 8-row atom (256 B) is stored and the descriptor's stride between
-  // 8-row groups is 0 (the 4 KB it saves buy the fourth weight stage)
-  static constexpr int AEXT_BYTES = 256;
-  static constexpr int BAR_OFF = AEXT_OFF + AEXT_BYTES;
-  static constexpr int TOTAL = BAR_OFF + 512;
+  static constexpr int A_BYTES = 128 * 256 * 2;                 // 128 rows x d <= 256, four 16 KB k-blocks
+  static constexpr int B_STAGE = PROJ_BN * GEMM_BK * 2;          // 32 KB
+  static constexpr int B_OFF = A_BYTES;
+  static constexpr int BAR_OFF = B_OFF + PROJ_STAGES * B_STAGE;
+  static constexpr int TOTAL = BAR_OFF + 128;
   static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA can use");
 };
 
-// byte offset of 16-byte chunk `chunk` (0..3) of row `row` inside a 64B-swizzled tile whose rows are 64 B
-__device__ __forceinline__ uint32_t swz64_off(uint32_t row, uint32_t chunk) {
-  return row * 64u + ((chunk ^ ((row >> 1) & 3u)) << 4);
-}
+__device__ __forceinline__ void proj_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the two MMA warpgroups
 
-// Finish 32 output columns held in registers (u [, g]): activation / gate, row scale, pack to bf16x2.
+// epilogue of one 256-column weight tile of segment sg, specialised on its kind (EpiTraits: mode, activation, layout)
 template <int EK>
-__device__ __forceinline__ void proj_finish32(const uint32_t* u, const uint32_t* g, float rs, uint32_t (&pk)[16]) {
-  constexpr int mode = EpiTraits<EK>::mode, act = EpiTraits<EK>::act;
-  const f32x2 rs2 = pack2(rs, rs);
-#ifndef AF2_RCP_SHARE
-#define AF2_RCP_SHARE 1
-#endif
-#if !AF2_RCP_SHARE
+__device__ __forceinline__ void proj_epilogue(const float (&acc)[PROJ_BN / 2], const ProjParams& p, const ProjSeg& sg, int mt, int nt,
+                                              int h, int wq, int lane) {
+  constexpr bool gated = EpiTraits<EK>::mode == EPI_GATED_BF16;
+  constexpr bool chan = EpiTraits<EK>::layout == LAYOUT_CHANNEL;
+  constexpr int act = EpiTraits<EK>::act;
+  constexpr int W = gated ? PROJ_BN / 2 : PROJ_BN;
+  const int col0 = (nt - sg.tile0) * W;
+  const int ncols = min(W, sg.out_cols - col0);
+  const float* bias = p.bcat + static_cast<long long>(nt) * PROJ_BN;
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {      // A/B reference: one MUFU.RCP per element (round-1 epilogue)
-    f32x2 a = pack2(__uint_as_float(u[2 * j]), __uint_as_float(u[2 * j + 1]));
-    if constexpr (mode == EPI_GATED_BF16) {
-      const f32x2 gg = pack2(__uint_as_float(g[2 * j]), __uint_as_float(g[2 * j + 1]));
-      if constexpr (act == ACT_GELU) a = mul2(a, gelu_fast2(gg));
-      else a = mul2(a, sigmoidf_fast2(gg));
-    } else {
-      if constexpr (act == ACT_SIGMOID) a = sigmoidf_fast2(a);
-    }
-    if constexpr (EpiTraits<EK>::rowscale) a = mul2(a, rs2);
-    float lo, hi;
-    unpack2(a, lo, hi);
-    pk[j] = pack_bf16x2(lo, hi);
-  }
-  return;
-#endif
-  // four columns per step: the sigmoid / GELU forms share one MUFU reciprocal between four values (common.cuh)
+  for (int half = 0; half < 2; ++half) {
+    const long long row = static_cast<long long>(mt) * 128 + h * 64 + wq * 16 + (lane >> 2) + half * 8;
+    if (row >= p.T) continue;
+    const float rs = (chan && p.rowmask) ? (p.rowmask[row] ? 1.0f : 0.0f) : 1.0f;
 #pragma unroll
-  for (int j = 0; j < 16; j += 2) {
-    f32x2 a = pack2(__uint_as_float(u[2 * j]), __uint_as_float(u[2 * j + 1]));
-    f32x2 b = pack2(__uint_as_float(u[2 * j + 2]), __uint_as_float(u[2 * j + 3]));
-    if constexpr (mode == EPI_GATED_BF16) {
-      const f32x2 ga = pack2(__uint_as_float(g[2 * j]), __uint_as_float(g[2 * j + 1]));
-      const f32x2 gb = pack2(__uint_as_float(g[2 * j + 2]), __uint_as_float(g[2 * j + 3]));
-      f32x2 fa, fb;
-      if constexpr (act == ACT_GELU) gelu_fast4(ga, gb, fa, fb);
-      else sigmoidf_fast4(ga, gb, fa, fb);
-      a = mul2(a, fa);
-      b = mul2(b, fb);
-    } else {
-      if constexpr (act == ACT_SIGMOID) {
-        f32x2 fa, fb;
-        sigmoidf_fast4(a, b, fa, fb);
-        a = fa;
-        b = fb;
-      }
-    }
-    if constexpr (EpiTraits<EK>::rowscale) {
-      a = mul2(a, rs2);
-      b = mul2(b, rs2);
-    }
-    float lo, hi;
-    unpack2(a, lo, hi);
-    pk[j] = pack_bf16x2(lo, hi);
-    unpack2(b, lo, hi);
-    pk[j + 1] = pack_bf16x2(lo, hi);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// epilogue of one 128 x 256 accumulator tile (one CTA's rows), kind fixed at compile time.
-// Every epilogue warp is autonomous: it owns the 32 accumulator rows of its TMEM lane quarter, every second 32-column
-// chunk of them (the other chunks belong to the warp of the other group on the same quarter), two private 2 KB staging
-// buffers and its own TMA stores (box 32 columns x 32 rows) -- no block barriers anywhere in the epilogue.  The TMEM load
-// of the next chunk is in flight while the current one is converted, staged and stored.  `release` is called right
-// after the loads of the warp's LAST chunk of the tile have landed: the accumulator stage goes back to the MMA warp
-// before that chunk is converted.
-// ---------------------------------------------------------------------------------------------------
-template <int EK, class Release>
-__device__ __forceinline__ void proj_epilogue_tile(uint8_t* wbuf, uint32_t& ec, uint32_t& gc, int grp, int lane, uint32_t t_acc,
-                                                   const CUtensorMap* tmc, float rs, int m0w, int col0, int ncols,
-                                                   Release release, long long* ctrace) {
-  // ctrace (debug, warp 4 of the traced CTA only): 5 stamps per chunk from slot 1024 + 5 * gc
-  auto cst = [&](int k) { if (ctrace && lane == 0 && gc < 200) ctrace[1024 + 5 * gc + k] = clock64(); };
-  constexpr int mode = EpiTraits<EK>::mode, layout = EpiTraits<EK>::layout;
-  constexpr bool gated = (mode == EPI_GATED_BF16);
-  const int nchunks = (ncols + 31) / 32;
-  const int first = ((ec & 1) == static_cast<uint32_t>(grp)) ? 0 : 1;     // this warp's chunks: first, first + 2, ...
-  ec += nchunks;
-  if (first >= nchunks) { release(); return; }
-  uint32_t u[32], g[gated ? 32 : 1];
-  tmem_ld32(t_acc + first * 32, u);
-  if constexpr (gated) tmem_ld32(t_acc + 128 + first * 32, g);
-  for (int cc = first; cc < nchunks; cc += 2) {
-    uint32_t pk[16];
-    tmem_ld_wait();
-    cst(0);
-    if (cc + 2 >= nchunks) release();
-    proj_finish32<EK>(u, g, rs, pk);
-    cst(1);
-    if (cc + 2 < nchunks) {                         // next chunk's loads overlap staging + store of this one
-      tmem_ld32(t_acc + (cc + 2) * 32, u);
-      if constexpr (gated) tmem_ld32(t_acc + 128 + (cc + 2) * 32, g);
-    }
-    uint8_t* eb = wbuf + (gc & 1) * 2048;
-    // the store that used this buffer two chunks ago must have read it (one newer store may still be in flight)
-    if (lane == 0) tma_store_wait_read<1>();
-    __syncwarp();
-    cst(2);
-    if constexpr (layout == LAYOUT_TOKEN) {
-      // [32 rows][64 B], 64B swizzle
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4*>(eb + swz64_off(lane, j)) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-    } else {
-      // [32 channels][32 tokens x 2 B], 64B swizzle; lane = token
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const uint32_t c0 = 2 * j, c1 = c0 + 1;
-        *reinterpret_cast<uint16_t*>(eb + c0 * 64 + ((((lane >> 3) ^ ((c0 >> 1) & 3)) << 4) | ((lane & 7) << 1))) = static_cast<uint16_t>(pk[j] & 0xffffu);
-        *reinterpret_cast<uint16_t*>(eb + c1 * 64 + ((((lane >> 3) ^ ((c1 >> 1) & 3)) << 4) | ((lane & 7) << 1))) = static_cast<uint16_t>(pk[j] >> 16);
-      }
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    cst(3);
-    if (lane == 0) {
-      if constexpr (layout == LAYOUT_TOKEN) tma_store_3d(tmc, eb, col0 + cc * 32, m0w, 0);
-      else tma_store_3d(tmc, eb, m0w, col0 + cc * 32, 0);
-      tma_store_commit();
-    }
-    cst(4);
-    ++gc;
-  }
-}
-
-// Same tile, 64 output columns per step (segments whose width is a multiple of 64).  Tracing the 32-column version showed
-// ~650 cycles per chunk for ~50 instructions: the buffer-free wait, the proxy fence, the elected-thread TMA issue and the
-// loop turn-around each cost 100+ cycles regardless of the data they cover.  Here two 32-column halves are converted and
-// staged back to back into ONE 4 KB block (32 rows x 128 B, or 64 channels x 64 B) and leave with one fence and one store.
-template <int EK, class Release>
-__device__ __forceinline__ void proj_epilogue_tile_wide(uint8_t* wbuf, uint32_t& ec, uint32_t& gc, int grp, int lane, uint32_t t_acc,
-                                                        const CUtensorMap* tmc, float rs, int m0w, int col0, int ncols,
-                                                        Release release, long long* ctrace) {
-  constexpr int mode = EpiTraits<EK>::mode, layout = EpiTraits<EK>::layout;
-  constexpr bool gated = (mode == EPI_GATED_BF16);
-  auto cst = [&](int k) { if (ctrace && lane == 0 && gc < 200) ctrace[1024 + 5 * gc + k] = clock64(); };
-  const int nblk = ncols >> 6;
-  const int first = ((ec & 1) == static_cast<uint32_t>(grp)) ? 0 : 1;     // this warp's 64-column blocks: first, first + 2, ...
-  ec += nblk;
-  if (first >= nblk) { release(); return; }
-  uint32_t u[32], g[32];
-  tmem_ld32(t_acc + first * 64, u);
-  if constexpr (gated) tmem_ld32(t_acc + 128 + first * 64, g);
-  for (int b = first; b < nblk; b += 2) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t pk[16];
-      tmem_ld_wait();
-      if (h == 0) cst(0);
-      if (h == 1 && b + 2 >= nblk) release();
-      proj_finish32<EK>(u, g, rs, pk);
-      if (h == 0) {                                   // the other half of this block
-        tmem_ld32(t_acc + b * 64 + 32, u);
-        if constexpr (gated) tmem_ld32(t_acc + 128 + b * 64 + 32, g);
-      } else if (b + 2 < nblk) {                      // first half of the warp's next block
-        tmem_ld32(t_acc + (b + 2) * 64, u);
-        if constexpr (gated) tmem_ld32(t_acc + 128 + (b + 2) * 64, g);
-      }
-      if (h == 0) {
-        cst(1);
-        if (lane == 0) tma_store_wait_read<0>();      // the previous store has drained the staging block
-        __syncwarp();
-        cst(2);
-      }
-      if constexpr (layout == LAYOUT_TOKEN) {
-        // [32 rows][128 B], 128B swizzle; this half fills 16-byte chunks 4h .. 4h+3 of the lane's row
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          *reinterpret_cast<uint4*>(wbuf + lane * 128 + (((4 * h + j) ^ (lane & 7)) << 4)) =
-              make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+    for (int j = 0; j < W / 8; ++j) {                      // fully unrolled: the accumulator stays in registers
+      const int c = 8 * j + 2 * (lane & 3);
+      if (c >= ncols) continue;
+      const bool two = c + 1 < ncols;
+      float v0 = acc[4 * j + 2 * half] + __ldg(bias + c), v1 = acc[4 * j + 2 * half + 1] + __ldg(bias + c + 1);
+      if constexpr (gated) {
+        // gate columns of the packed tile sit 128 columns (16 fragment steps) to the right of their values
+        v0 *= apply_act(acc[4 * (j + PROJ_BN / 16) + 2 * half] + __ldg(bias + PROJ_BN / 2 + c), act);
+        v1 *= apply_act(acc[4 * (j + PROJ_BN / 16) + 2 * half + 1] + __ldg(bias + PROJ_BN / 2 + c + 1), act);
       } else {
-        // [64 channels][32 tokens x 2 B], 64B swizzle; lane = token; this half fills channels 32h .. 32h+31
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const uint32_t c0 = 32 * h + 2 * j, c1 = c0 + 1;
-          *reinterpret_cast<uint16_t*>(wbuf + c0 * 64 + ((((lane >> 3) ^ ((c0 >> 1) & 3)) << 4) | ((lane & 7) << 1))) = static_cast<uint16_t>(pk[j] & 0xffffu);
-          *reinterpret_cast<uint16_t*>(wbuf + c1 * 64 + ((((lane >> 3) ^ ((c1 >> 1) & 3)) << 4) | ((lane & 7) << 1))) = static_cast<uint16_t>(pk[j] >> 16);
-        }
+        v0 = apply_act(v0, act);
+        v1 = apply_act(v1, act);
+      }
+      if constexpr (chan) { v0 *= rs; v1 *= rs; }
+      const long long col = col0 + c;
+      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(sg.out);
+      if constexpr (chan) {
+        o[col * sg.ld + row] = __float2bfloat16(v0);
+        if (two) o[(col + 1) * sg.ld + row] = __float2bfloat16(v1);
+      } else {
+        store_pair<false>(o, row * sg.ld + col, v0, v1, two, true);
       }
     }
-    fence_proxy_async_smem();
-    __syncwarp();
-    cst(3);
-    if (lane == 0) {
-      if constexpr (layout == LAYOUT_TOKEN) tma_store_3d(tmc, wbuf, col0 + b * 64, m0w, 0);
-      else tma_store_3d(tmc, wbuf, m0w, col0 + b * 64, 0);
-      tma_store_commit();
-    }
-    cst(4);
-    ++gc;
   }
 }
 
-__device__ __forceinline__ int proj_tile_width(int kind) {
-  return (kind == EK_GATED_TOK_GELU || kind == EK_GATED_CH_SIG) ? 128 : 256;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// mode-0 producer helpers.  Eight lanes share a row (4 rows per warp instruction): lane l of a row group owns float4
-// chunks l, l + 8, ... of the row, so a load instruction reads 128 contiguous bytes per row, the two row reductions
-// need 3 shuffle levels instead of 5, and ~50 warp instructions produce one normalised row (one-warp-per-row: ~270).
-// ---------------------------------------------------------------------------------------------------
-struct RowQuad { float4 v[8]; };     // this lane's 32 values of its row (d <= 256)
-
-// streaming 16-byte load that does not allocate in L1 (the activations are read once; L1 is left to the small hot data)
-__device__ __forceinline__ float4 ldg_stream(const float4* p) {
-  float4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-  return v;
-}
-
-template <int NJ>
-__device__ __forceinline__ void proj_load_quad(RowQuad& b, const float4* xr, bool live, uint64_t pol) {
-#pragma unroll
-  for (int j = 0; j < NJ; ++j) b.v[j] = live ? ldg_stream_hint(xr + j * 8, pol) : make_float4(0.f, 0.f, 0.f, 0.f);
-}
-
-template <int NJ>
-__device__ __forceinline__ void proj_process_quad(const RowQuad& b, uint8_t* abuf, int r, bool live, float inv_d, float eps, int sub) {
-  // all vector math on packed fp32 pairs (FADD2 / FFMA2): the producer warps are bound by instruction latency, not by memory
-  f32x2 lo[NJ], hi[NJ];
-#pragma unroll
-  for (int j = 0; j < NJ; ++j) {
-    lo[j] = pack2(b.v[j].x, b.v[j].y);
-    hi[j] = pack2(b.v[j].z, b.v[j].w);
-  }
-  f32x2 sa = lo[0], sb = hi[0];
-#pragma unroll
-  for (int j = 1; j < NJ; ++j) {
-    sa = add2(sa, lo[j]);
-    sb = add2(sb, hi[j]);
-  }
-  float s0, s1;
-  unpack2(add2(sa, sb), s0, s1);
-  float s = s0 + s1;
-  s += __shfl_xor_sync(0xffffffffu, s, 1);
-  s += __shfl_xor_sync(0xffffffffu, s, 2);
-  s += __shfl_xor_sync(0xffffffffu, s, 4);
-  const float mean = s * inv_d;
-  const f32x2 nm = pack2(-mean, -mean);
-  f32x2 qa = pack2(0.f, 0.f), qb = pack2(0.f, 0.f);
-#pragma unroll
-  for (int j = 0; j < NJ; ++j) {
-    const f32x2 da = add2(lo[j], nm), db = add2(hi[j], nm);
-    qa = fma2(da, da, qa);
-    qb = fma2(db, db, qb);
-  }
-  float q0, q1;
-  unpack2(add2(qa, qb), q0, q1);
-  float sq = q0 + q1;
-  sq += __shfl_xor_sync(0xffffffffu, sq, 1);
-  sq += __shfl_xor_sync(0xffffffffu, sq, 2);
-  sq += __shfl_xor_sync(0xffffffffu, sq, 4);
-  const float rs = live ? rsqrtf(sq * inv_d + eps) : 0.f;      // dead rows (beyond T) become zeros
-  const float sh = -mean * rs;
-  const f32x2 rs2 = pack2(rs, rs), sh2 = pack2(sh, sh);
-  // float4 chunk idx = j*8 + sub covers columns 4*idx..: k-block idx/16 = j/2, 16-byte chunk (idx%16)/2, half idx&1
-  uint8_t* rowp = abuf + r * 128;
-  const uint32_t sw = static_cast<uint32_t>(r & 7);
-#pragma unroll
-  for (int j = 0; j < NJ; ++j) {
-    const uint32_t chunk = static_cast<uint32_t>(((j & 1) * 8 + sub) >> 1);
-    float o0, o1, o2, o3;
-    unpack2(fma2(lo[j], rs2, sh2), o0, o1);
-    unpack2(fma2(hi[j], rs2, sh2), o2, o3);
-    const uint2 o = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
-    *reinterpret_cast<uint2*>(rowp + (j >> 1) * 16384 + ((chunk ^ sw) << 4) + (sub & 1) * 8) = o;
-  }
-}
-
-// One producer warp's share of the A tiles: steps (4 rows each) pi, pi + NP, ... of every item of this CTA.
-//   item_row0(it) -> first row of the CTA's tile of item `it`;  wait_empty(it) / signal_full(it): A buffer hand-off
-template <int NJ, int NP, class ItemRow, class WaitEmpty, class SignalFull>
-__device__ __forceinline__ void proj_producer_loop(const float* x, long long T, int d, float inv_d, float eps, uint8_t* a_base,
-                                                   int my_items, int pi, int lane, ItemRow item_row0, WaitEmpty wait_empty,
-                                                   SignalFull signal_full, bool l2_prefetch, bool x_evict_last) {
-  const int sub = lane & 7, rg = lane >> 3;
-  const uint64_t pol = l2_policy(x_evict_last);
-  constexpr int STEPS = 32;                       // 128 rows / 4
-  auto row_ptr = [&](long long row) { return reinterpret_cast<const float4*>(x + row * d) + sub; };
-  RowQuad qa, qb;
-  if (my_items > 0) {
-    const long long row = item_row0(0) + pi * 4 + rg;
-    proj_load_quad<NJ>(qa, row_ptr(row), row < T, pol);
-  }
-  for (int it = 0; it < my_items; ++it) {
-    const long long m0 = item_row0(it);
-    uint8_t* abuf = a_base + (it & 1) * PROJ_A_BUF;
-    wait_empty(it);
-    const long long m_next = (it + 1 < my_items) ? item_row0(it + 1) : -1;
-    if (m_next >= 0 && l2_prefetch) {
-      // pull the next item's tile (128 rows) into L2: one 128-byte line per lane and round, shared by the NP producer warps
-      const char* nb = reinterpret_cast<const char*>(x + m_next * d);
-      const long long nrows = (m_next + 128 <= T) ? 128 : (T > m_next ? T - m_next : 0);
-      const long long nbytes = nrows * d * 4;
-      for (long long o = (pi * 32 + lane) * 128LL; o < nbytes; o += NP * 32 * 128LL)
-        if (x_evict_last) asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(nb + o));
-        else asm volatile("prefetch.global.L2 [%0];" ::"l"(nb + o));
-    }
-    // steps pi, pi + NP, ...: process qa while qb's loads are in flight and vice versa
-    int st = pi;
-#pragma unroll 1
-    while (st < STEPS) {
-      const int st1 = st + NP, st2 = st + 2 * NP;
-      {
-        long long row; bool any = true;
-        if (st1 < STEPS) row = m0 + st1 * 4 + rg;
-        else if (m_next >= 0) row = m_next + pi * 4 + rg;           // first step of the next item
-        else { row = 0; any = false; }
-        proj_load_quad<NJ>(qb, row_ptr(row), any && row < T, pol);
-      }
-      proj_process_quad<NJ>(qa, abuf, st * 4 + rg, (m0 + st * 4 + rg) < T, inv_d, eps, sub);
-      if (st1 >= STEPS) { qa = qb; break; }
-      {
-        long long row; bool any = true;
-        if (st2 < STEPS) row = m0 + st2 * 4 + rg;
-        else if (m_next >= 0) row = m_next + pi * 4 + rg;
-        else { row = 0; any = false; }
-        proj_load_quad<NJ>(qa, row_ptr(row), any && row < T, pol);
-      }
-      proj_process_quad<NJ>(qb, abuf, st1 * 4 + rg, (m0 + st1 * 4 + rg) < T, inv_d, eps, sub);
-      st = st2;
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) signal_full(it);
-  }
-}
-
-template <int CTAS, int KINDS>
+// tmB: 2-D map over Wcat (k = d contiguous, rows), box (64, 256), 128B swizzle
 __global__ void __launch_bounds__(PROJ_THREADS, 1)
-proj_tc_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC0,
-               const __grid_constant__ CUtensorMap tmC1, const __grid_constant__ CUtensorMap tmC2,
-               const __grid_constant__ CUtensorMap tmX, const __grid_constant__ ProjParams p) {
-  using L = ProjSmem<CTAS>;
-  constexpr int STAGES = L::STAGES;
-  // 1024-byte aligned by declaration (128B-swizzle atoms); keeping the array symbol (no integer round-up of the pointer)
-  // lets the compiler prove the shared address space and emit LDS/STS instead of generic LD/ST
+proj_tc_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ProjParams p) {
+  using L = ProjSmem;
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);   // [STAGES] weight stage landed (leader's)
-  uint64_t* empty_bar = full_bar + STAGES;                                // [STAGES] weight stage consumed
-  uint64_t* tfull_bar = empty_bar + STAGES;                               // [2] accumulator ready
-  uint64_t* tempty_bar = tfull_bar + 2;                                   // [2] accumulator drained (leader's)
-  uint64_t* afull_bar = tempty_bar + 2;                                   // [2] A buffer produced (leader's)
-  uint64_t* aempty_bar = afull_bar + 2;                                   // [2] A buffer consumed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(aempty_bar + 2);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
+  uint64_t* empty_bar = full_bar + PROJ_STAGES;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const int num_kb = p.d / GEMM_BK;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = (CTAS == 2) ? cluster_ctarank() : 0u;
-  const bool is_leader = rank == 0;
-  const int cluster_id = blockIdx.x / CTAS;
-  const int nclusters = gridDim.x / CTAS;
-  constexpr uint32_t TMEM_COLS = 512;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmB);
-    prefetch_tmap(&tmX);
-    prefetch_tmap(&tmC0);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
+    for (int s = 0; s < PROJ_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 8 * CTAS);
-      mbar_init(&afull_bar[s], PROJ_NPROD * CTAS);
-      mbar_init(&aempty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);     // one arrive per MMA warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (CTAS == 2) tmem_alloc_pair(tmem_slot, TMEM_COLS);
-    else tmem_alloc(tmem_slot, TMEM_COLS);
-  }
-  // ones block of the bias K-step (SW32 rows of 32 B; both 16-byte chunks identical, so the chunk swizzle is irrelevant):
-  // A_ext[r][k] = 1 for k in {0, 1, 8, 9}; the bias block has data in columns 0 / 1 only
-  for (int i = threadIdx.x; i < L::AEXT_BYTES / 16; i += PROJ_THREADS)
-    *reinterpret_cast<uint4*>(smem + L::AEXT_OFF + i * 16) = make_uint4(0x3f803f80u, 0u, 0u, 0u);
-  fence_proxy_async_smem();
-  tc_fence_before();
-  if constexpr (CTAS == 2) cluster_sync_all();
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   pdl_launch_dependents();
   pdl_wait();
 
-  // ---- work decomposition: item = (row unit of 128*CTAS rows, column chunk) ----
-  const int m_units = (p.m_tiles + CTAS - 1) / CTAS;
-  // balance == 0: items (row unit, column chunk) are dealt round-robin; a cluster's load is a whole number of items.
-  // balance == 1: the flat sequence of (row unit, column tile) pairs is cut into nclusters equal ranges; a range becomes a
-  //               partial first unit, whole units and a partial last unit.  Every cluster then runs the same number of
-  //               tiles (+-1) at the price of producing at most one extra A tile.
-  const int ntt = p.n_tiles_total;
-  const long long flat = static_cast<long long>(m_units) * ntt;
-  const long long f0 = flat * cluster_id / nclusters, f1 = flat * (cluster_id + 1) / nclusters;
-  const int total_items = m_units * p.nsplit;
-  const int tiles_per_chunk = (ntt + p.nsplit - 1) / p.nsplit;
-  const int my_items = p.balance ? (f1 > f0 ? static_cast<int>((f1 - 1) / ntt - f0 / ntt) + 1 : 0)
-                                 : ((total_items > cluster_id) ? (total_items - 1 - cluster_id) / nclusters + 1 : 0);
-  const int nkb = p.d / GEMM_BK;
-  // (the 64-bit divisions of the balanced split are done ONCE here: these lambdas are called per item by every warp role,
-  // several times per item by the latency-bound producer warps)
-  const int unit_first = static_cast<int>(f0 / ntt);
-  const int t0_first = static_cast<int>(f0 - static_cast<long long>(unit_first) * ntt);
-  const int t1_last = (f1 > f0) ? static_cast<int>((f1 - 1) % ntt) + 1 : 0;
-  auto item_unit = [&](int it) { return p.balance ? unit_first + it : (cluster_id + it * nclusters) / p.nsplit; };
-  auto item_t0 = [&](int it) {
-    if (p.balance) return it == 0 ? t0_first : 0;
-    return ((cluster_id + it * nclusters) % p.nsplit) * tiles_per_chunk;
-  };
-  auto item_t1 = [&](int it) {
-    if (p.balance) return it == my_items - 1 ? t1_last : ntt;
-    return min(((cluster_id + it * nclusters) % p.nsplit + 1) * tiles_per_chunk, ntt);
-  };
-  auto seg_of = [&](int nt) {
-    int s = 0;
-#pragma unroll
-    for (int i = 1; i < PROJ_MAX_SEG; ++i)
-      if (i < p.nseg && nt >= p.seg[i].tile0) s = i;
-    return s;
-  };
-
-  const bool tr = p.trace != nullptr && cluster_id == 0 && rank == 0;
-  auto stamp = [&](int idx) { if (tr && lane == 0 && idx < 1023) p.trace[idx] = clock64(); };
-  if (tr && threadIdx.x == 0) p.trace[1023] = clock64();
-
-  if (warp == 0) {
+  if (wg == 0) {
     // ================================ weight-tile TMA producer ================================
-    if (lane == 0) {
-      uint32_t full_remote[STAGES];
-#pragma unroll
-      for (int s = 0; s < STAGES; ++s) full_remote[s] = (CTAS == 2) ? mapa_u32(smem_u32(&full_bar[s]), 0) : 0u;
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int it = 0; it < my_items; ++it) {
-        const int t1 = item_t1(it);
-        for (int nt = item_t0(it); nt < t1; ++nt) {
-          for (int kb = -1; kb < nkb; ++kb) {                 // kb = -1: the tile's bias block (rows x 16 bf16)
+      for (int mt = blockIdx.x; mt < p.m_tiles; mt += gridDim.x)
+        for (int nt = 0; nt < p.n_tiles_total; ++nt)
+          for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sb = smem + L::B_OFF + stage * L::B_STAGE;
-            const CUtensorMap* tm = kb < 0 ? &tmX : &tmB;
-            const int bytes = kb < 0 ? L::BEXT_BYTES : L::B_STAGE;
-            const int c0 = kb < 0 ? 0 : kb * GEMM_BK;
-            if constexpr (CTAS == 2) {
-              if (is_leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * bytes);
-              tma_load_2d_pair(sb, tm, full_remote[stage], c0, nt * 256 + static_cast<int>(rank) * L::B_ROWS);
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], bytes);
-              tma_load_2d(sb, tm, &full_bar[stage], c0, nt * 256);
-            }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            mbar_arrive_expect_tx(&full_bar[stage], L::B_STAGE);
+            tma_load_2d(smem + L::B_OFF + stage * L::B_STAGE, &tmB, &full_bar[stage], kb * GEMM_BK, nt * PROJ_BN);
+            if (++stage == PROJ_STAGES) { stage = 0; phase ^= 1; }
           }
-        }
-      }
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer (leader CTA) =================================
-    if (is_leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128 * CTAS, 256, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t tcnt = 0;
-      for (int it = 0; it < my_items; ++it) {
-        const int ab = it & 1;
-        mbar_wait(&afull_bar[ab], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t sa0 = smem_u32(smem + L::A_OFF + ab * PROJ_A_BUF);
-        const int t1 = item_t1(it);
-        for (int nt = item_t0(it); nt < t1; ++nt, ++tcnt) {
-          const int acc = tcnt & 1;
-          mbar_wait(&tempty_bar[acc], ((tcnt >> 1) & 1) ^ 1);
-          tc_fence_after();
-          stamp(3 * static_cast<int>(tcnt));
-          const uint32_t d_tmem = tmem_base + acc * 256;
-          for (int kb = -1; kb < nkb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            if (kb < 0) stamp(3 * static_cast<int>(tcnt) + 1);
-            if (kb == nkb - 1) stamp(3 * static_cast<int>(tcnt) + 2);
-            if (elect_one()) {
-              const uint32_t sb = smem_u32(smem + L::B_OFF + stage * L::B_STAGE);
-              if (kb < 0) {
-                // accumulator = ones x bias block (SW32 operands: 32-byte rows, 8-row atoms 256 B apart)
-                const uint64_t adesc = umma_smem_desc(smem_u32(smem + L::AEXT_OFF), 16, 0, SWZ_32);   // SBO 0: rows aliased
-                const uint64_t bdesc = umma_smem_desc(sb, 16, 256, SWZ_32);
-                if constexpr (CTAS == 2) umma_bf16_pair(d_tmem, adesc, bdesc, idesc, 0u);
-                else umma_bf16(d_tmem, adesc, bdesc, idesc, 0u);
-              } else {
-                const uint32_t sa = sa0 + kb * 16384;
-#pragma unroll
-                for (int k = 0; k < GEMM_BK / 16; ++k) {
-                  const uint64_t adesc = umma_smem_desc(sa + k * 32, 16, 1024, SWZ_128);
-                  const uint64_t bdesc = umma_smem_desc(sb + k * 32, 16, 1024, SWZ_128);
-                  if constexpr (CTAS == 2) umma_bf16_pair(d_tmem, adesc, bdesc, idesc, 1u);
-                  else umma_bf16(d_tmem, adesc, bdesc, idesc, 1u);
-                }
-              }
-              if constexpr (CTAS == 2) {
-                umma_commit_pair(&empty_bar[stage], 3);
-                if (kb == nkb - 1) {
-                  umma_commit_pair(&tfull_bar[acc], 3);
-                  if (nt == t1 - 1) umma_commit_pair(&aempty_bar[ab], 3);
-                }
-              } else {
-                umma_commit(&empty_bar[stage]);
-                if (kb == nkb - 1) {
-                  umma_commit(&tfull_bar[acc]);
-                  if (nt == t1 - 1) umma_commit(&aempty_bar[ab]);
-                }
-              }
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp >= 4 && warp < 12) {
-    // ================================ epilogue ====================================
-    const int q = warp & 3;                   // TMEM lane quarter = rows 32q .. 32q+31 of the tile
-    const int grp = (warp - 4) >> 2;          // chunk parity this warp takes
-    uint32_t tempty_remote[2];
-    tempty_remote[0] = (CTAS == 2) ? mapa_u32(smem_u32(&tempty_bar[0]), 0) : 0u;
-    tempty_remote[1] = (CTAS == 2) ? mapa_u32(smem_u32(&tempty_bar[1]), 0) : 0u;
-    uint8_t* wbuf = smem + L::EPI_OFF + (warp - 4) * 4096;     // two private 2 KB staging buffers
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    uint32_t ec = 0, gc = 0, tcnt = 0;
-    for (int it = 0; it < my_items; ++it) {
-      const int unit = item_unit(it), t1 = item_t1(it);
-      const int m0w = (unit * CTAS + static_cast<int>(rank)) * 128 + q * 32;
-      const long long row = static_cast<long long>(m0w) + lane;
-      float rs = 1.0f;
-      if (p.rowmask && row < p.T) rs = p.rowmask[row] ? 1.0f : 0.0f;
-      for (int nt = item_t0(it); nt < t1; ++nt, ++tcnt) {
-        const ProjSeg& sg = p.seg[seg_of(nt)];
-        const int acc = tcnt & 1;
-        const int W = proj_tile_width(sg.kind);
-        const int col0 = (nt - sg.tile0) * W;
-        const int ncols = min(W, sg.out_cols - col0);
-        const CUtensorMap* tmc = sg.map == 0 ? &tmC0 : (sg.map == 1 ? &tmC1 : &tmC2);
-        const int tbase = (warp == 4) ? 256 : (warp == 8 ? 512 : 4096);
-        stamp(tbase + 3 * static_cast<int>(tcnt));
-        mbar_wait(&tfull_bar[acc], (tcnt >> 1) & 1);
-        tc_fence_after();
-        stamp(tbase + 3 * static_cast<int>(tcnt) + 1);
-        const uint32_t t_acc = tmem_base + acc * 256 + lane_sel;
-        // hand the accumulator stage back: this warp's TMEM loads of the tile have landed (8 * CTAS warps arrive)
-        auto release = [&]() {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (CTAS == 2) mbar_arrive_cluster(tempty_remote[acc]);
-            else mbar_arrive(&tempty_bar[acc]);
-          }
-        };
-#define AF2_PROJ_CASE(EKV)                                                                                               \
-  if constexpr ((KINDS & KBIT(EKV)) != 0) {                                                                              \
-    if (sg.kind == EKV) {                                                                                                \
-      if (sg.wide)                                                                                                       \
-        proj_epilogue_tile_wide<EKV>(wbuf, ec, gc, grp, lane, t_acc, tmc, rs, m0w, col0, ncols > 0 ? ncols : 0, release, \
-                                     (tr && warp == 4) ? p.trace : nullptr);                                             \
-      else                                                                                                               \
-        proj_epilogue_tile<EKV>(wbuf, ec, gc, grp, lane, t_acc, tmc, rs, m0w, col0, ncols > 0 ? ncols : 0, release,      \
-                                (tr && warp == 4) ? p.trace : nullptr);                                                  \
-    }                                                                                                                    \
-  }
-        AF2_PROJ_CASE(EK_STORE_TOK)
-        AF2_PROJ_CASE(EK_STORE_TOK_SIG)
-        AF2_PROJ_CASE(EK_STORE_CH)
-        AF2_PROJ_CASE(EK_STORE_CH_SIG)
-        AF2_PROJ_CASE(EK_GATED_TOK_GELU)
-        AF2_PROJ_CASE(EK_GATED_CH_SIG)
-#undef AF2_PROJ_CASE
-        stamp(tbase + 3 * static_cast<int>(tcnt) + 2);
-      }
-    }
-    if (lane == 0) tma_store_wait_read<0>();
-  } else if (warp >= 12) {
-    // ================================ LayerNorm producers (warps 12..15) ====================================
-    const int pi = warp - 12;
-    uint32_t afull_remote[2];
-    afull_remote[0] = (CTAS == 2) ? mapa_u32(smem_u32(&afull_bar[0]), 0) : 0u;
-    afull_remote[1] = (CTAS == 2) ? mapa_u32(smem_u32(&afull_bar[1]), 0) : 0u;
-    auto item_row0 = [&](int it) { return static_cast<long long>(item_unit(it) * CTAS + static_cast<int>(rank)) * 128; };
-    auto wait_empty = [&](int it) {
-      mbar_wait(&aempty_bar[it & 1], ((it >> 1) & 1) ^ 1);
-      if (warp == 12) stamp(768 + 2 * it);
-    };
-    auto signal_full = [&](int it) {
-      if (warp == 12) stamp(768 + 2 * it + 1);
-      if constexpr (CTAS == 2) mbar_arrive_cluster(afull_remote[it & 1]);
-      else mbar_arrive(&afull_bar[it & 1]);
-    };
-    uint8_t* a_base = smem + L::A_OFF;
-    const int nj = p.d >> 5;                     // float4 chunks per lane (d / 32)
-    if (nj == 8) proj_producer_loop<8, PROJ_NPROD>(p.x, p.T, p.d, p.inv_d, p.eps, a_base, my_items, pi, lane, item_row0, wait_empty, signal_full, p.l2_prefetch != 0, p.x_evict_last != 0);
-    else if (nj == 4) proj_producer_loop<4, PROJ_NPROD>(p.x, p.T, p.d, p.inv_d, p.eps, a_base, my_items, pi, lane, item_row0, wait_empty, signal_full, p.l2_prefetch != 0, p.x_evict_last != 0);
-    else proj_producer_loop<6, PROJ_NPROD>(p.x, p.T, p.d, p.inv_d, p.eps, a_base, my_items, pi, lane, item_row0, wait_empty, signal_full, p.l2_prefetch != 0, p.x_evict_last != 0);
+    return;
   }
 
-  __syncwarp();
-  tc_fence_before();
-  if constexpr (CTAS == 2) cluster_sync_all();
-  else __syncthreads();
-  if (warp == 2) {
-    if constexpr (CTAS == 2) tmem_dealloc_pair(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
+  regs_alloc<232>();
+  const int h = wg - 1, wq = warp & 3;
+  const int cw = warp - 4;                  // 0..7: LayerNorm row owner
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[PROJ_BN / 2];
+  for (int mt = blockIdx.x; mt < p.m_tiles; mt += gridDim.x) {
+    // ---------------- LayerNorm of the item's 128 rows -> bf16 A tile (128B swizzle, 16 KB per 64 channels) ----------------
+#pragma unroll 4                            // four rows' loads in flight per warp
+    for (int r = cw; r < 128; r += 8) {
+      const long long row = static_cast<long long>(mt) * 128 + r;
+      const bool live = lane * 8 < p.d && row < p.T;
+      float v[8];
+      float s = 0.f;
+      if (live) {
+        const float4* src = reinterpret_cast<const float4*>(p.x + row * p.d + lane * 8);
+        const float4 a = __ldg(src), b = __ldg(src + 1);
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) s += v[i];
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = 0.f;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      const float mean = s * p.inv_d;
+      float q = 0.f;
+      if (live) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { v[i] -= mean; q += v[i] * v[i]; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+      const float rstd = rsqrtf(q * p.inv_d + p.eps);
+      if (lane * 8 < p.d) {
+        const uint4 pk = live ? make_uint4(pack_bf16x2(v[0] * rstd, v[1] * rstd), pack_bf16x2(v[2] * rstd, v[3] * rstd),
+                                           pack_bf16x2(v[4] * rstd, v[5] * rstd), pack_bf16x2(v[6] * rstd, v[7] * rstd))
+                              : make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(smem + (lane >> 3) * 16384 + swz128_off(r, lane & 7)) = pk;
+      }
+    }
+    fence_proxy_async_smem();               // generic-proxy stores of the A tile -> wgmma (async proxy) reads
+    proj_bar_sync();
+
+    for (int nt = 0; nt < p.n_tiles_total; ++nt) {
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem) + kb * 16384 + h * 8192;
+        const uint32_t sb = smem_u32(smem + L::B_OFF + stage * L::B_STAGE);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k)
+          wgmma_m64n256k16_ss<0, 0>(acc, wgmma_desc(sa + k * 32, 16, 1024, SWZ_128), wgmma_desc(sb + k * 32, 16, 1024, SWZ_128),
+                                    (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0 && wq == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == PROJ_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (lane == 0 && wq == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ------------------------------- epilogue of weight tile nt -------------------------------
+      int si = 0;
+      while (si + 1 < p.nseg && nt >= p.seg[si + 1].tile0) ++si;
+      const ProjSeg& sg = p.seg[si];
+      switch (sg.kind) {
+        case EK_STORE_TOK: proj_epilogue<EK_STORE_TOK>(acc, p, sg, mt, nt, h, wq, lane); break;
+        case EK_STORE_TOK_SIG: proj_epilogue<EK_STORE_TOK_SIG>(acc, p, sg, mt, nt, h, wq, lane); break;
+        case EK_STORE_CH: proj_epilogue<EK_STORE_CH>(acc, p, sg, mt, nt, h, wq, lane); break;
+        case EK_GATED_TOK_GELU: proj_epilogue<EK_GATED_TOK_GELU>(acc, p, sg, mt, nt, h, wq, lane); break;
+        default: proj_epilogue<EK_GATED_CH_SIG>(acc, p, sg, mt, nt, h, wq, lane); break;
+      }
+    }
+    proj_bar_sync();                         // both warpgroups are done with the A tile before it is rebuilt
   }
 }
 

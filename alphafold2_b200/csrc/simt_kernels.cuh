@@ -1,6 +1,6 @@
 // Bandwidth-bound helper kernels (no tensor-core work): row LayerNorm with optional fused pair-bias
 // projection, channel-major -> token-major LayerNorm*gate, pair-mask counts, rotary embedding.
-// All are coalesced / vectorised and sized as grid-stride loops over 148 x k CTAs.
+// All are coalesced / vectorised and sized as grid-stride loops over (SM count) x k CTAs.
 #pragma once
 #include "common.cuh"
 

@@ -167,18 +167,6 @@ def _cat_segments(ws, bs, gamma, beta):
     return _bf16(w * g[None, :]), (b + w @ be).contiguous()
 
 
-def _bias_block(b: torch.Tensor) -> torch.Tensor:
-    """bf16 [rows pad256][16] operand of the fused kernel's bias K-step: column 0 = bf16(b), column 1 = bf16(b - col0)
-    (hi / lo split, ~2^-17 relative), other columns zero.  The tensor core adds hi + lo to the fp32 accumulator."""
-    b = _pad_rows(b.detach().float().reshape(-1))
-    hi = b.to(torch.bfloat16)
-    lo = (b - hi.float()).to(torch.bfloat16)
-    out = torch.zeros(b.shape[0], 16, dtype=torch.bfloat16, device=b.device)
-    out[:, 0] = hi
-    out[:, 1] = lo
-    return out.contiguous()
-
-
 def _p(t):
     return None if t is None else t.data_ptr()
 
@@ -201,10 +189,8 @@ def pack_feed_forward(norm_w, norm_b, w1, b1, w2, b2) -> Packed:
     t = dict(g=_f32(norm_w), b=_f32(norm_b), w1=_bf16(w1f), b1=b1p, w2=_bf16(w2), b2=_f32(b2))
     if half == 128:                                         # the fused kernel works on 256-column accumulator tiles
         t["wcat"], t["bcat"] = _cat_segments([w1f], [b1p], norm_w, norm_b)
-        t["wext"] = _bias_block(t["bcat"])
     s = _lib.FFWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["w1"].data_ptr(), t["b1"].data_ptr(),
-                       t["w2"].data_ptr(), t["b2"].data_ptr(), 2 * half, _p(t.get("wcat")), _p(t.get("bcat")),
-                       _p(t.get("wext")))
+                       t["w2"].data_ptr(), t["b2"].data_ptr(), 2 * half, _p(t.get("wcat")), _p(t.get("bcat")), None)
     return Packed(s, t)
 
 
@@ -218,11 +204,9 @@ def pack_attention(norm_w, norm_b, wq, wkv, wg, bg, wo, bo, w_edge, dim_head: in
     if w_edge is not None:
         t["we"] = _f32(w_edge.detach().float() * log2e)
     t["wcat"], t["bcat"] = _cat_segments([wqkv, wg], [torch.zeros(wqkv.shape[0], device=wqkv.device), bg], norm_w, norm_b)
-    t["wext"] = _bias_block(t["bcat"])
     s = _lib.AttnWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["wqkv"].data_ptr(), t["wg"].data_ptr(),
                          t["bg"].data_ptr(), t["wo"].data_ptr(), t["bo"].data_ptr(),
-                         t["we"].data_ptr() if w_edge is not None else None, t["wcat"].data_ptr(), t["bcat"].data_ptr(),
-                         t["wext"].data_ptr())
+                         t["we"].data_ptr() if w_edge is not None else None, t["wcat"].data_ptr(), t["bcat"].data_ptr(), None)
     return Packed(s, t)
 
 
@@ -236,12 +220,10 @@ def pack_triangle_multiply(norm_w, norm_b, wl, bl, wr, br, wlg, blg, wrg, brg, w
              ong=_f32(onw), onb=_f32(onb), wo=_bf16(wo), bo=_f32(bo))
     if half == 128:
         t["wcat"], t["bcat"] = _cat_segments([wlp, wrp, wog], [blp, brp, bog], norm_w, norm_b)
-        t["wext"] = _bias_block(t["bcat"])
-    t["wexto"] = _bias_block(bo)
     s = _lib.TriMulWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["wl"].data_ptr(), t["bl"].data_ptr(),
                            t["wr"].data_ptr(), t["br"].data_ptr(), t["wog"].data_ptr(), t["bog"].data_ptr(),
                            t["ong"].data_ptr(), t["onb"].data_ptr(), t["wo"].data_ptr(), t["bo"].data_ptr(), 2 * half,
-                           _p(t.get("wcat")), _p(t.get("bcat")), _p(t.get("wext")), t["wexto"].data_ptr())
+                           _p(t.get("wcat")), _p(t.get("bcat")), None, None)
     return Packed(s, t)
 
 
@@ -249,11 +231,9 @@ def pack_outer_mean(norm_w, norm_b, wl, bl, wr, br, wo, bo) -> Packed:
     t = dict(g=_f32(norm_w), b=_f32(norm_b), wlr=_bf16(torch.cat([wl.detach(), wr.detach()], 0)),
              blr=_f32(torch.cat([bl.detach(), br.detach()], 0)), wo=_bf16(wo), bo=_f32(bo))
     t["wcat"], t["bcat"] = _cat_segments([torch.cat([wl.detach(), wr.detach()], 0)], [t["blr"]], norm_w, norm_b)
-    t["wext"] = _bias_block(t["bcat"])
-    t["wexto"] = _bias_block(bo)
     s = _lib.OuterWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["wlr"].data_ptr(), t["blr"].data_ptr(),
                           t["wo"].data_ptr(), t["bo"].data_ptr(), t["wcat"].data_ptr(), t["bcat"].data_ptr(),
-                          t["wext"].data_ptr(), t["wexto"].data_ptr())
+                          None, None)
     return Packed(s, t)
 
 

@@ -1,6 +1,6 @@
 """Axis-sharded Evoformer trunk over the GPUs of one node (one process per GPU, torch.distributed / NCCL).
 
-The reference has no multi-device path (SURVEY.md §2.2); this is the B200-native addition named by the north
+The reference has no multi-device path (SURVEY.md §2.2); this is the GPU-native addition named by the north
 star: one sequence's forward is split over the MSA-row and pair-row axes (FastFold-DAP style).  At block entry
 rank r owns pair rows x[r*N/P:(r+1)*N/P, :, :] and MSA rows m[r*S/P:(r+1)*S/P, :, :]; weights are replicated.
 Every sub-op is embarrassingly parallel along ONE axis, so the schedule switches the sharded axis with
@@ -10,7 +10,7 @@ all-to-alls and all-gathers the one operand a contraction needs in full (SURVEY.
   right x2; bf16 channel-major), 2 all-to-alls of m, 4 all-to-alls of x (fp32 residual stream).
 
 "A single all-gather per block" (north star) is not dependency-feasible with exact semantics; the real count is
-stated above and measured by bench.py --gpus N.  The compute between collectives is the same sm_100a kernels as
+stated above and measured by bench.py --gpus N.  The compute between collectives is the same sm_90a kernels as
 the single-GPU path (stage-level C ABI: af2_pair_bias / *_project / *_contract / af2_axial_attention_prebias).
 
 `ops` is the stage-op provider: CudaStageOps (product, C ABI).  tests/ plug in a CPU oracle provider to check the
@@ -304,7 +304,7 @@ def release_peer_arenas() -> None:
 # stage ops on the GPU (C ABI)
 # ------------------------------------------------------------------------------------------------------------
 class CudaStageOps:
-    """Every method launches hand-written sm_100a kernels through libaf2b200.so; tensors are CUDA tensors."""
+    """Every method launches hand-written sm_90a kernels through libaf2b200.so; tensors are CUDA tensors."""
 
     def pair_bias(self, ax, x_rows: torch.Tensor) -> torch.Tensor:
         """bf16 [H, rows, align8(n)] = edges_to_attn_bias of a band of pair rows (raw, un-normalised x)."""

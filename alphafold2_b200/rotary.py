@@ -1,5 +1,5 @@
 """Mirror of alphafold2_pytorch/rotary.py (dead code at the reference HEAD, named in the north star).
-``apply_rotary_pos_emb`` runs the sm_100a kernel; the sin/cos table builders are host-side setup."""
+``apply_rotary_pos_emb`` runs the sm_90a kernel; the sin/cos table builders are host-side setup."""
 import torch
 from torch import nn
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Evoformer trunk forward benchmark (BASELINE.json: residue-pairs/sec at N_res=256, depth=12; fwd ms/block).
 
-    python bench.py --gpus 1 --steps 10 --warmup 3                      # B200 arm (this repo)
+    python bench.py --gpus 1 --steps 10 --warmup 3                      # GPU arm (this repo, H100 / sm_90a)
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1      # CPU arm: oracle port of the reference
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...    # one rank per GPU
 
@@ -13,6 +13,8 @@ tensors randomised so no path is an identity).
           (pinned) inputs: H2D of the token ids / masks and D2H of the distogram logits inside the timed region.
 Timing: CUDA events per step on the launching stream, L2 flushed (256 MiB write) between steps outside the
 event pairs, barrier + synchronize around the loop, max over ranks.  Prints ONE JSON line on rank 0.
+--dump-outputs DIR writes what the last timed step returned (the trunk's pair and MSA tracks) as float32 .npy files;
+the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -61,7 +63,8 @@ def measured_peaks():
         return dict(tflops=float(p["bf16_tflops_sustained"]), tflops_burst=float(p["bf16_tflops"]),
                     hbm_gbs=float(p["hbm_gbs"]), source="MEASURED_PEAKS.json (measured)")
     except Exception:
-        return dict(tflops=1400.0, tflops_burst=1590.0, hbm_gbs=6650.0, source="B200_PROFILING.md fallback")
+        # NVIDIA H100 SXM data sheet (700 W card): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- not measured
+        return dict(tflops=989.0, tflops_burst=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet (not measured)")
 
 
 class ClockSampler:
@@ -135,7 +138,7 @@ def exchange_transport():
 def host_threads():
     """All the host CORES the CPU arm can use.  torchrun exports OMP_NUM_THREADS=1 to its workers (round 1's N>1 CPU arm ran
     on one thread), so the count is set explicitly -- to the PHYSICAL cores: with one thread per hyper-thread (128 on the
-    pool's 64-core hosts) MKL / OpenMP oversubscribe and the block takes 131 s instead of 6.9 s (measured, profiles/r02a)."""
+    pool's 64-core hosts) MKL / OpenMP oversubscribe and the block takes many times longer."""
     n = None
     try:
         import psutil
@@ -283,13 +286,28 @@ def gpu_torch_baseline(dev, x0, m0, x_mask, msa_mask, model):
             out[name] = {"ms_per_step": ms, "value": N_RES * N_RES / (ms * 1e-3), "unit": UNIT}
     finally:
         torch.backends.cuda.matmul.allow_tf32 = prev
-    out["what"] = "oracle port of the reference trunk (einsum OuterMean) executed by stock PyTorch eager on the same B200; not part of any timed region"
+    out["what"] = "oracle port of the reference trunk (einsum OuterMean) executed by stock PyTorch eager on the same GPU; not part of any timed region"
     return out
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 22          # elements kept per dumped output (16 MB of float32); larger outputs are sampled
+
+
+def dump_outputs(outdir, named):
+    """Writes each output as DIR/<name>.npy (float32).  An output larger than DUMP_SAMPLE elements is replaced by a fixed
+    sample of its flattened elements: the sorted first DUMP_SAMPLE entries of torch.randperm(numel) under seed 0."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    for name, t in named.items():
+        flat = t.detach().float().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(outdir, f"{name}.npy"), flat.cpu().numpy().astype(np.float32))
 def run_ours(args, rank, world, local_rank):
     import torch.distributed as dist
     import alphafold2_b200 as A
@@ -342,6 +360,8 @@ def run_ours(args, rank, world, local_rank):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(fn, steps):
         total = 0.0
         barrier()
@@ -349,7 +369,7 @@ def run_ours(args, rank, world, local_rank):
             flush.zero_()
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            fn()
+            last[fn] = fn()
             b.record()
             b.synchronize()
             total += a.elapsed_time(b)
@@ -374,6 +394,9 @@ def run_ours(args, rank, world, local_rank):
     if graphed is not None and graphed.graph is not None:
         launches = graphed.launches_per_replay * args.steps      # the sharded forward is replayed as a CUDA graph
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        x_out, m_out = last[trunk_step]
+        dump_outputs(args.dump_outputs, {"pair": x_out, "msa": m_out})
     ms_e2e = timed(e2e_step, args.steps)
 
     # secondary, labelled number at N > 1 (SURVEY.md 8e fallback statement): N independent replicas, one unsharded sequence
@@ -395,7 +418,7 @@ def run_ours(args, rank, world, local_rank):
     e2e_value = pairs / (ms_e2e / args.steps * 1e-3)
 
     # per-kernel-class device time of 2 more steps (CUDA events around every launch; not part of `value`)
-    names = ["gemm_linear(tcgen05)", "gemm_per_channel(tcgen05)", "axial_attention(tcgen05)", "layernorm",
+    names = ["gemm_linear(wgmma)", "gemm_per_channel(wgmma)", "axial_attention(wgmma)", "layernorm",
              "channel_to_token", "misc"]
     lib.af2_profile_enable(1)
     prof_steps = 2
@@ -415,37 +438,10 @@ def run_ours(args, rank, world, local_rank):
     peaks = measured_peaks()
     tot_ms = sum(c["ms"] for c in classes) or 1.0
     dom = max(classes, key=lambda c: c["ms"])
-    # DRAM traffic per launch of the dominant class from the committed `ncu --set full` capture of one C2 block
-    traffic, traffic_src = None, None
-    try:
-        import glob
-        cand = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_traffic.json")))
-        if cand:
-            tj = json.load(open(cand[-1]))
-            if dom["name"] in tj:
-                traffic = tj[dom["name"]]["dram_bytes_per_launch"]
-                traffic_src = os.path.relpath(cand[-1], ROOT)
-    except Exception:
-        pass
-    # whole-block DRAM traffic of the committed `ncu --set full` capture of one C2 block, next to SURVEY.md 8(d)'s
-    # ideal-fusion minimum (0.69 GB with bf16 activations; ~1.0 GB with the fp32 residual stream kept here)
-    block_dram, block_src = None, None
-    try:
-        import csv
-        import glob
-        cand = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_block_C2_ncu_full_summary.csv")))
-        if cand and N_RES == 256:
-            rows = list(csv.DictReader(open(cand[-1])))
-            rk = [k for k in rows[0] if k.startswith("dram_read_MB")][0]
-            wk = [k for k in rows[0] if k.startswith("dram_write_MB")][0]
-            block_dram = sum(float(r[rk]) + float(r[wk]) for r in rows) * 1e6
-            block_src = os.path.relpath(cand[-1], ROOT)
-    except Exception:
-        pass
     if dom["flops"] > 0:
         ach = dom["flops"] / (dom["ms"] * 1e-3) / 1e12
         roof = {"bound": "tensor", "kernel": dom["name"], "achieved": ach, "peak": peaks["tflops"], "unit": "TFLOP/s",
-                "frac": ach / peaks["tflops"], "traffic": traffic, "traffic_source": traffic_src,
+                "frac": ach / peaks["tflops"],
                 "algorithmic_bytes_per_launch": dom["bytes"] / max(dom["launches"], 1),
                 "peak_source": peaks["source"] + ", sustained bf16",
                 "share_of_step": dom["ms"] / tot_ms, "avg_launch_ms": dom["ms"] / max(dom["launches"], 1),
@@ -453,7 +449,7 @@ def run_ours(args, rank, world, local_rank):
     else:
         ach = dom["bytes"] / (dom["ms"] * 1e-3) / 1e9
         roof = {"bound": "hbm", "kernel": dom["name"], "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": ach / peaks["hbm_gbs"], "traffic": traffic, "traffic_source": traffic_src, "peak_source": peaks["source"],
+                "frac": ach / peaks["hbm_gbs"], "peak_source": peaks["source"],
                 "share_of_step": dom["ms"] / tot_ms, "avg_launch_ms": dom["ms"] / max(dom["launches"], 1)}
     step_flops = flops_per_block(N_RES, N_SEQ, CFG["dim"], CFG["heads"], CFG["dim_head"]) * CFG["depth"]
     step_tf = step_flops / (ms_step * 1e-3) / 1e12
@@ -475,9 +471,7 @@ def run_ours(args, rank, world, local_rank):
         "roofline": roof,
         "roofline_whole_step": {"bound": "tensor", "achieved": step_tf, "peak": peaks["tflops"], "unit": "TFLOP/s",
                                 "frac": step_tf / peaks["tflops"], "frac_of_burst_peak": step_tf / peaks["tflops_burst"],
-                                "flops_per_step": step_flops, "block_dram_bytes": block_dram,
-                                "block_dram_bytes_source": block_src, "block_algorithmic_min_bytes": 0.69e9 if N_RES == 256 else None,
-                                "block_dram_over_min": (block_dram / 0.69e9) if block_dram else None},
+                                "flops_per_step": step_flops},
         "kernel_classes": [dict(name=c["name"], launches_per_step=c["launches"] // prof_steps,
                                 ms_per_step=c["ms"] / prof_steps, share=c["ms"] / tot_ms,
                                 tflops=(c["flops"] / (c["ms"] * 1e-3) / 1e12 if c["ms"] > 0 else 0.0),
@@ -507,6 +501,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     ap.add_argument("--workload", default="C2", choices=list(WORKLOADS),
                     help="BASELINE.json config shape (default C2 = the configuration the metric is quoted on)")
     args = ap.parse_args()

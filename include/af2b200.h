@@ -1,4 +1,4 @@
-/* libaf2b200.so — C ABI of the B200-native Evoformer trunk hot path.
+/* libaf2b200.so — C ABI of the H100-native Evoformer trunk hot path.
  *
  * The reference (lucidrains/alphafold2 @ 931466e) is 100 % Python and has no FFI: its boundary for this
  * path is the nn.Module API (alphafold2_pytorch/alphafold2.py).  Each entry point below therefore replaces
@@ -6,7 +6,7 @@
  * INTEGRATION.md shows the stub a reference maintainer would add.
  *
  * Conventions
- *   - every pointer is a DEVICE pointer on the current CUDA device (sm_100a only); nothing is allocated
+ *   - every pointer is a DEVICE pointer on the current CUDA device (sm_90a only); nothing is allocated
  *     or retained by the library: outputs and workspace are caller-owned;
  *   - activations x / m are fp32, channel-last, contiguous; weights are packed bf16 (see packing.py) with
  *     fp32 biases / LayerNorm affine parameters; masks are 1-byte bools (torch.bool);
@@ -30,15 +30,14 @@ typedef void* af2_stream_t; /* cudaStream_t */
 
 const char* af2_last_error(void);
 int af2_abi_version(void);
-/* 0 if the current device is compute capability 10.x, AF2_ERR_UNSUPPORTED_DEVICE otherwise */
+/* 0 if the current device is compute capability 9.0 (H100, sm_90a), AF2_ERR_UNSUPPORTED_DEVICE otherwise */
 int af2_check_device(void);
-/* 2 (default): LN->projection clusters run on the fused CTA-pair kernel; 1: its single-CTA variant; 0: unfused
- * LayerNorm + GEMM launches (also selectable with the environment variable AF2_PROJ_CTAS, read by af2_check_device) */
+/* nonzero: LN->projection clusters run on the fused LayerNorm->projection kernel (1 and 2 select the same kernel);
+ * 0 (default): LayerNorm kernel + GEMM launches.  Also selectable with the environment variable AF2_PROJ_CTAS, read by
+ * af2_check_device */
 void af2_set_proj_mode(int ctas);
-/* debug aid: with AF2_PROJ_TRACE=1 in the environment the fused projection kernel records clock64 stamps of one CTA
- * (MMA issue, epilogue and producer progress per tile); this copies the 2048 stamps of the last launch to `out` */
+/* kept for ABI compatibility: no kernel of this build records a timeline; both return AF2_ERR_BAD_ARG */
 int af2_debug_proj_trace(long long* out);
-/* same for the attention kernel (AF2_ATTN_TRACE=1): 8 stamps per key block of CTA 0 (tools/attn_trace.py), 1024 entries */
 int af2_debug_attn_trace(long long* out);
 
 /* Kernel launches issued by this library since load (bench.py's gpu_launches). */
@@ -62,7 +61,7 @@ typedef struct {
    * each segment zero-padded to a multiple of 256 accumulator columns; b_cat is the matching fp32 bias (zeros where none).
    * NULL -> the unfused LayerNorm + GEMM launches are used.  FeedForward: w_cat == w1, b_cat == b1 (bn must be 256). */
   const void* w_cat; const float* b_cat;
-  const void* w_ext;   /* bias block of the fused kernel: bf16 [rows(w_cat)][16], columns 0 / 1 = hi / lo bf16 split of b_cat */
+  const void* w_ext;   /* unused (NULL); kept for the struct layout -- the fused kernel reads b_cat */
 } af2_ff_weights;
 int af2_feed_forward(const af2_ff_weights* w, float* x, long long tokens, int d, int hidden,
                      void* workspace, long long workspace_bytes, af2_stream_t stream);
@@ -105,7 +104,7 @@ typedef struct {
   const void* w_out; const float* b_out;              /* to_out                    [d, d], [d]      */
   int bn;
   const void* w_cat; const float* b_cat;              /* [w_left packed | w_right packed | pad256(d) rows w_ogate]  */
-  const void* w_ext; const void* w_ext_out;           /* bias blocks of w_cat and (fused tail) of w_out              */
+  const void* w_ext; const void* w_ext_out;           /* unused (NULL); kept for the struct layout                   */
 } af2_trimul_weights;
 int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned char* mask, int B, int N, int d,
                           int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);

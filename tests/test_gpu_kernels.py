@@ -1,4 +1,4 @@
-"""-m gpu: building-block kernels (tcgen05 GEMM in both operand layouts, LayerNorm, rotary) against fp64 math."""
+"""-m gpu: building-block kernels (wgmma GEMM in both operand layouts, LayerNorm, rotary) against fp64 math."""
 import pytest
 import torch
 

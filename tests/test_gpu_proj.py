@@ -1,5 +1,5 @@
-"""-m gpu: the fused LayerNorm -> multi-segment projection kernel (csrc/proj_tc.cuh; CTA-pair and single-CTA variants)
-against (a) the unfused LayerNorm + GEMM launches of the same library and (b) the fp64 oracle."""
+"""-m gpu: the fused LayerNorm -> multi-segment projection kernel (csrc/proj_tc.cuh; af2_set_proj_mode 1 or 2) against
+(a) the unfused LayerNorm + GEMM launches of the same library (mode 0) and (b) the fp64 oracle."""
 import pytest
 import torch
 
@@ -31,7 +31,7 @@ def _set_mode(mode):
 @pytest.fixture(autouse=True)
 def _restore_mode():
     yield
-    _set_mode(2)
+    _set_mode(0)                                   # the library default
 
 
 def _both(fn, mode):

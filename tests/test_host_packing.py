@@ -8,18 +8,6 @@ import torch
 from alphafold2_b200 import ops
 
 
-def test_bias_block_hi_lo_split_reconstructs_bias():
-    g = torch.Generator().manual_seed(0)
-    b = torch.randn(300, generator=g) * 3.0
-    blk = ops._bias_block(b)
-    assert blk.shape == (512, 16) and blk.dtype == torch.bfloat16          # padded to 256-row tiles, 16 bf16 columns
-    rec = blk[:, 0].float() + blk[:, 1].float()
-    assert torch.all(blk[:, 2:] == 0)
-    assert torch.all(rec[300:] == 0)
-    err = (rec[:300] - b).abs() / b.abs().clamp_min(1e-6)
-    assert err.max() < 2.0 ** -15                                           # two bf16 terms: ~2^-17 relative
-
-
 def test_cat_segments_folds_layernorm_affine():
     """W' = W diag(gamma), b' = W beta + b: (x_hat W'^T + b') == Linear(LayerNorm(x)) up to the bf16 rounding of W'."""
     g = torch.Generator().manual_seed(1)

@@ -22,11 +22,11 @@ WANT = [
 
 def kernel_class(name):
     if "proj_tc_kernel" in name:
-        return "gemm_linear(tcgen05)"
+        return "gemm_linear(wgmma)"
     if "gemm_tc_kernel" in name:
-        return "gemm_per_channel(tcgen05)" if name.rstrip(">").endswith(", 7") else "gemm_linear(tcgen05)"
+        return "gemm_per_channel(wgmma)" if name.rstrip(">").endswith(", 7") else "gemm_linear(wgmma)"
     if "attention_tc_kernel" in name:
-        return "axial_attention(tcgen05)"
+        return "axial_attention(wgmma)"
     if "layernorm" in name or "pair_bias" in name:
         return "layernorm"
     if "chan_to_token" in name:

@@ -35,6 +35,12 @@ class OuterWeights(C.Structure):
                 ("w_cat", vp), ("b_cat", vp), ("w_ext", vp), ("w_ext_out", vp)]
 
 
+class GemmEpilogue(C.Structure):
+    _fields_ = [("bn", ci), ("mode", ci), ("act", ci), ("layout", ci), ("use_rowscale", ci), ("bias", vp), ("rowscale", vp),
+                ("resid", vp), ("ld_resid", ll), ("out", vp), ("ld_out", ll), ("out_batch", ll), ("cm_inner", ci),
+                ("cm_pitch", ci), ("out_cols", ci)]
+
+
 class FFWeightsStrict(C.Structure):
     _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w1", vp), ("b1", vp), ("w2", vp), ("b2", vp)]
 
@@ -84,6 +90,8 @@ _SIGNATURES = {
     "af2_rotary": (ci, [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
     "af2_layernorm_bf16": (ci, [vp, vp, vp, vp, ll, ci, cf, vp]),
     "af2_gemm_bf16_f32": (ci, [vp, ll, ll, vp, ll, ll, vp, ll, ll, ci, ci, ci, ci, ci, vp]),
+    "af2_gemm_bf16_epilogue": (ci, [vp, ll, ll, vp, ll, ll, ci, ci, ci, ci, ci, C.POINTER(GemmEpilogue), vp]),
+    "af2_attention_bf16": (ci, [vp, vp, vp, vp, vp, ci, ci, ci, ci, ll, ll, vp]),
     # strict precision mode (split-bf16 x3 operands)
     "af2_feed_forward_strict": (ci, [C.POINTER(FFWeightsStrict), vp, ll, ci, ci, vp, ll, vp]),
     "af2_feed_forward_strict_workspace": (ll, [ll, ci, ci]),

@@ -219,6 +219,8 @@ int launch_gemm_inst(const CUtensorMap& ta, const CUtensorMap& tb, const CUtenso
 
 int launch_gemm(const GemmCall& c, cudaStream_t s) {
   if (c.M <= 0 || c.N <= 0 || c.K <= 0 || c.batch <= 0) return AF2_OK;
+  // the residual is read at [row][col] of batch 0 whatever the batch index: a batched residual GEMM would add the wrong rows
+  if (c.mode == EPI_RESID_F32 && c.batch > 1) return fail(AF2_ERR_BAD_ARG, "gemm: residual epilogue with batch %d (needs 1)", c.batch);
   CUtensorMap ta, tb;
   const int BN = c.bn;
   if (c.nseg > 1) {
@@ -1265,15 +1267,47 @@ int af2_layernorm_bf16(const float* x, const float* gamma, const float* beta, vo
   return launch_layernorm(lp, static_cast<cudaStream_t>(stream));
 }
 
-int af2_gemm_bf16_f32(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,
-                      float* C, long long ldc, long long c_batch, int M, int N, int K, int batch, int mn_major,
-                      af2_stream_t stream) {
+int af2_gemm_bf16_epilogue(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,
+                           int M, int N, int K, int batch, int mn_major, const af2_gemm_epilogue* epi, af2_stream_t stream) {
+  if (!A || !Bm || !epi || !epi->out) return fail(AF2_ERR_BAD_ARG, "gemm: null argument");
+  if (epi->bn != 64 && epi->bn != 128 && epi->bn != 256) return fail(AF2_ERR_BAD_ARG, "gemm: bn %d (64, 128 or 256)", epi->bn);
+  if (epi->mode < EPI_STORE_BF16 || epi->mode > EPI_STORE_F32 || epi->act < ACT_NONE || epi->act > ACT_GELU ||
+      epi->layout < LAYOUT_TOKEN || epi->layout > LAYOUT_CHANNEL)
+    return fail(AF2_ERR_BAD_ARG, "gemm: epilogue mode %d / act %d / layout %d", epi->mode, epi->act, epi->layout);
+  const bool f32 = epi->mode == EPI_RESID_F32 || epi->mode == EPI_STORE_F32;
+  if (f32 && (epi->layout != LAYOUT_TOKEN || epi->use_rowscale))
+    return fail(AF2_ERR_BAD_ARG, "gemm: fp32 epilogues store token-major without a row scale");
+  if (epi->use_rowscale && !epi->rowscale) return fail(AF2_ERR_BAD_ARG, "gemm: use_rowscale without rowscale");
+  if (epi->mode == EPI_RESID_F32 && !epi->resid) return fail(AF2_ERR_BAD_ARG, "gemm: residual epilogue without resid");
+  if (epi->mode == EPI_GATED_BF16 && N % epi->bn) return fail(AF2_ERR_BAD_ARG, "gemm: gated N %d not a multiple of bn %d", N, epi->bn);
   GemmCall c;
   memset(&c, 0, sizeof(c));
   c.A = A; c.lda = lda; c.a_batch = a_batch; c.Bm = Bm; c.ldb = ldb; c.b_batch = b_batch;
-  c.M = M; c.N = N; c.K = K; c.batch = batch; c.mn_major = mn_major != 0; c.bn = pick_bn(N);
-  c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = C; c.ld_out = ldc; c.out_batch = c_batch;
+  c.M = M; c.N = N; c.K = K; c.batch = batch; c.mn_major = mn_major != 0; c.bn = epi->bn;
+  c.mode = epi->mode; c.act = epi->act; c.layout = epi->layout; c.use_rowscale = epi->use_rowscale;
+  c.bias = epi->bias; c.rowscale = epi->rowscale; c.resid = epi->resid; c.ld_resid = epi->ld_resid;
+  c.out = epi->out; c.ld_out = epi->ld_out; c.out_batch = epi->out_batch;
+  c.cm_inner = epi->cm_inner; c.cm_pitch = epi->cm_pitch; c.out_cols = epi->out_cols;
   return launch_gemm(c, static_cast<cudaStream_t>(stream));
+}
+
+int af2_gemm_bf16_f32(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,
+                      float* C, long long ldc, long long c_batch, int M, int N, int K, int batch, int mn_major,
+                      af2_stream_t stream) {
+  af2_gemm_epilogue e;
+  memset(&e, 0, sizeof(e));
+  e.bn = pick_bn(N); e.mode = EPI_STORE_F32; e.layout = LAYOUT_TOKEN; e.out = C; e.ld_out = ldc; e.out_batch = c_batch;
+  return af2_gemm_bf16_epilogue(A, lda, a_batch, Bm, ldb, b_batch, M, N, K, batch, mn_major, &e, stream);
+}
+
+int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, const unsigned char* mask, void* out, int n,
+                       int nbatch, int heads, int dim_head, long long tok_sb, long long tok_si, af2_stream_t stream) {
+  if (!qkv || !gate || !out) return fail(AF2_ERR_BAD_ARG, "attention: null argument");
+  if (n <= 0 || nbatch <= 0 || heads <= 0) return AF2_OK;
+  return launch_attention(static_cast<const __nv_bfloat16*>(qkv), heads, dim_head, n, nbatch, tok_sb, tok_si,
+                          static_cast<const __nv_bfloat16*>(bias), (int)align_up(n, 8), mask,
+                          static_cast<const __nv_bfloat16*>(gate), static_cast<__nv_bfloat16*>(out),
+                          static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

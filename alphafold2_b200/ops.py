@@ -529,3 +529,63 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, mn_major: bool = False) -> torch
                                              b.shape[1] * b.shape[2], c.data_ptr(), ldc, M * ldc, M, N, K, batch,
                                              int(mn_major), _stream_ptr()))
     return c[:, :, :N]
+
+
+# epilogue of af2_gemm_bf16_epilogue (include/af2b200.h)
+EPI_STORE_BF16, EPI_GATED_BF16, EPI_RESID_F32, EPI_STORE_F32 = 0, 1, 2, 3
+ACT_NONE, ACT_SIGMOID, ACT_GELU = 0, 1, 2
+LAYOUT_TOKEN, LAYOUT_CHANNEL = 0, 1
+
+
+def gemm_bf16_epilogue(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, bn: int, mode: int, act: int = ACT_NONE,
+                       layout: int = LAYOUT_TOKEN, mn_major: bool = False, bias: Optional[torch.Tensor] = None,
+                       rowscale: Optional[torch.Tensor] = None, resid: Optional[torch.Tensor] = None, ld_resid: int = 0,
+                       ld_out: int, out_batch: int = 0, cm_inner: int = 0, cm_pitch: int = 0,
+                       out_cols: int = 0) -> torch.Tensor:
+    """a [batch, M, K] x b [batch, N, K] (mn_major: a [batch, K, M], b [batch, K, N]) through the GEMM epilogue `mode` / `act` /
+    `layout` with an accumulator column tile of `bn`; the output is written into the flat buffer `out` (bf16 or fp32 by
+    mode) with the pitches given (include/af2b200.h, af2_gemm_epilogue).  `resid` (mode EPI_RESID_F32) may be `out` itself.
+    Returns `out`."""
+    _require(a, torch.bfloat16, "a")
+    _require(b, torch.bfloat16, "b")
+    _require(out, torch.float32 if mode in (EPI_RESID_F32, EPI_STORE_F32) else torch.bfloat16, "out")
+    if mn_major:
+        batch, K, M = a.shape
+        N = b.shape[2]
+        lda, ldb = M, N
+    else:
+        batch, M, K = a.shape
+        N = b.shape[1]
+        lda, ldb = K, K
+    for t, name in ((bias, "bias"), (rowscale, "rowscale"), (resid, "resid")):
+        if t is not None:
+            _require(t, torch.float32, name)
+    e = _lib.GemmEpilogue(bn=bn, mode=mode, act=act, layout=layout, use_rowscale=int(rowscale is not None), bias=_ptr(bias),
+                          rowscale=_ptr(rowscale), resid=_ptr(resid), ld_resid=ld_resid,
+                          out=out.data_ptr(), ld_out=ld_out, out_batch=out_batch,
+                          cm_inner=cm_inner, cm_pitch=cm_pitch, out_cols=out_cols)
+    _lib.check(_lib.load().af2_gemm_bf16_epilogue(a.data_ptr(), lda, a.shape[1] * a.shape[2], b.data_ptr(), ldb,
+                                                  b.shape[1] * b.shape[2], M, N, K, batch, int(mn_major), C.byref(e),
+                                                  _stream_ptr()))
+    return out
+
+
+def attention_bf16(qkv: torch.Tensor, gate: torch.Tensor, n: int, nbatch: int, heads: int, dim_head: int, tok_sb: int,
+                   tok_si: int, bias: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The attention kernel alone: qkv bf16 [tokens, 3 * heads * dim_head], gate bf16 [tokens, heads * dim_head] (sigmoid
+    applied), bias bf16 [heads, n, align8(n)] in the log2 domain, mask bool [tokens]; token (b, i) = b * tok_sb + i * tok_si.
+    Returns bf16 [tokens, heads * dim_head]."""
+    _require(qkv, torch.bfloat16, "qkv")
+    _require(gate, torch.bfloat16, "gate")
+    I = heads * dim_head
+    if qkv.dim() != 2 or qkv.shape[1] != 3 * I or tuple(gate.shape) != (qkv.shape[0], I):
+        raise ValueError(f"qkv must be [tokens, {3 * I}] and gate [tokens, {I}]")
+    if bias is not None:
+        _require(bias, torch.bfloat16, "bias")
+        if tuple(bias.shape) != (heads, n, (n + 7) // 8 * 8):
+            raise ValueError(f"bias must have shape {(heads, n, (n + 7) // 8 * 8)}, got {tuple(bias.shape)}")
+    mask = _mask_u8(mask, (qkv.shape[0],), "mask")
+    out = torch.empty(qkv.shape[0], I, dtype=torch.bfloat16, device=qkv.device)
+    _lib.check(_lib.load().af2_attention_bf16(qkv.data_ptr(), gate.data_ptr(), _ptr(bias), _ptr(mask), out.data_ptr(), n,
+                                              nbatch, heads, dim_head, tok_sb, tok_si, _stream_ptr()))
+    return out

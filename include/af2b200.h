@@ -175,6 +175,31 @@ int af2_layernorm_bf16(const float* x, const float* gamma, const float* beta, vo
 int af2_gemm_bf16_f32(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb,
                       long long b_batch, float* C, long long ldc, long long c_batch, int M, int N, int K,
                       int batch, int mn_major, af2_stream_t stream);
+/* The same GEMM with the epilogue the module launches use, applied per accumulator column tile of `bn` (64 / 128 / 256,
+ * used as given) columns.  mode: 0 bf16 store, 1 gated bf16 (B rows packed per tile as [bn/2 value rows | bn/2 gate rows],
+ * out = (u + b_u) * act(g + b_g)), 2 fp32 acc + bias + resid (batch 1 only), 3 fp32 store.  act: 0 none, 1 sigmoid,
+ * 2 erf-GELU (applied to the value, or to the gate when gated).  layout: 0 token-major out[b][row][col] (row pitch ld_out),
+ * 1 channel-major bf16 out[b][col * ld_out + (row / cm_inner) * cm_pitch + row % cm_inner].  rowscale: fp32 [batch * M]
+ * multiplier of every output row when use_rowscale (bf16 modes only).  bias: fp32 per accumulator column (N rounded up
+ * to even) or NULL.
+ * out_cols: valid output columns (0: N, or N / 2 when gated).  out_batch: element stride between batches of out. */
+typedef struct {
+  int bn, mode, act, layout, use_rowscale;
+  const float* bias; const float* rowscale;
+  const float* resid; long long ld_resid;
+  void* out; long long ld_out; long long out_batch;
+  int cm_inner, cm_pitch, out_cols;
+} af2_gemm_epilogue;
+int af2_gemm_bf16_epilogue(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,
+                           int M, int N, int K, int batch, int mn_major, const af2_gemm_epilogue* epi, af2_stream_t stream);
+/* out[tok, h*dh + e] = gate[tok, h*dh + e] * sum_j softmax_j(q_i . k_j + bias[h][i][j]) v_j[e]  (all in the log2 domain:
+ * the softmax is exp2 based, fold dim_head^-0.5 * log2(e) into q and log2(e) into the bias) over the n tokens
+ * tok = b * tok_sb + i * tok_si of each of the nbatch folded rows / columns.  qkv bf16 [tokens, 3 * heads * dim_head]
+ * (q | k | v), gate bf16 [tokens, heads * dim_head] (sigmoid already applied), bias bf16 [heads][n][align8(n)] or NULL,
+ * mask bool indexed like the tokens or NULL: logits where !(mask[i] & mask[j]) are replaced by -FLT_MAX (a fully masked
+ * query averages all n values).  dim_head 32 or 64. */
+int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, const unsigned char* mask, void* out, int n,
+                       int nbatch, int heads, int dim_head, long long tok_sb, long long tok_si, af2_stream_t stream);
 
 /* ======================================================================================================================
  * STRICT precision mode (alphafold2_b200.set_precision(model, "strict")): the same modules with fp32 activations between

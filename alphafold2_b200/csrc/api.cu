@@ -217,6 +217,22 @@ int launch_gemm_inst(const CUtensorMap& ta, const CUtensorMap& tb, const CUtenso
   return AF2_OK;
 }
 
+// Whether the call's output (and residual) can go through TMA: 16-byte aligned bases and pitches, and for the channel-major
+// layout whole 64-row boxes inside each cm_inner block.  Otherwise the epilogue stores from registers.  A token-major row
+// must also end on a 16-byte boundary: a TMA store clipped inside a 16-byte segment writes the rest of the segment.
+bool gemm_epi_tma_ok(const GemmCall& c, int out_cols) {
+  const bool f32 = c.mode == EPI_RESID_F32 || c.mode == EPI_STORE_F32;
+  const long long es = f32 ? 4 : 2;
+  if (!aligned16(c.out) || (c.batch > 1 && (c.out_batch * es) % 16)) return false;
+  if (c.layout == LAYOUT_CHANNEL) {
+    if (f32 || c.cm_inner <= 0 || c.cm_inner % GEMM_BM || c.M % c.cm_inner || (c.cm_pitch * 2) % 16 || (c.ld_out * 2) % 16) return false;
+  } else if ((c.ld_out * es) % 16 || (out_cols * es) % 16) {
+    return false;
+  }
+  if (c.mode == EPI_RESID_F32 && (!aligned16(c.resid) || (c.ld_resid * 4) % 16)) return false;
+  return true;
+}
+
 int launch_gemm(const GemmCall& c, cudaStream_t s) {
   if (c.M <= 0 || c.N <= 0 || c.K <= 0 || c.batch <= 0) return AF2_OK;
   // the residual is read at [row][col] of batch 0 whatever the batch index: a batched residual GEMM would add the wrong rows
@@ -230,7 +246,7 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
     if (!c.mn_major) {
       unsigned long long da[4] = {(unsigned long long)c.K, (unsigned long long)c.M, npl, (unsigned long long)c.batch};
       unsigned long long sa[3] = {(unsigned long long)c.lda * 2, (unsigned long long)c.a_half * 2, ab ? ab : (unsigned long long)c.a_half * 8};
-      unsigned ba[4] = {64, 128, 1, 1};
+      unsigned ba[4] = {64, GEMM_BM, 1, 1};
       AF2_TRY(make_tmap(&ta, c.A, 4, da, sa, ba, CU_TENSOR_MAP_SWIZZLE_128B));
       unsigned long long db[4] = {(unsigned long long)c.K, (unsigned long long)c.N, npl, (unsigned long long)c.batch};
       unsigned long long sb[3] = {(unsigned long long)c.ldb * 2, (unsigned long long)c.b_half * 2, bb_ ? bb_ : (unsigned long long)c.b_half * 8};
@@ -248,7 +264,7 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
   } else if (!c.mn_major) {
     unsigned long long da[3] = {(unsigned long long)c.K, (unsigned long long)c.M, (unsigned long long)c.batch};
     unsigned long long sa[2] = {(unsigned long long)c.lda * 2, (unsigned long long)(c.batch > 1 ? c.a_batch : c.lda * c.M) * 2};
-    unsigned ba[3] = {64, 128, 1};
+    unsigned ba[3] = {64, GEMM_BM, 1};
     AF2_TRY(make_tmap(&ta, c.A, 3, da, sa, ba, CU_TENSOR_MAP_SWIZZLE_128B));
     unsigned long long db[3] = {(unsigned long long)c.K, (unsigned long long)c.N, (unsigned long long)c.batch};
     unsigned long long sb[2] = {(unsigned long long)c.ldb * 2, (unsigned long long)(c.batch > 1 && c.b_batch ? c.b_batch : c.ldb * c.N) * 2};
@@ -271,7 +287,7 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
         if (c.a_pr % 128 != 0) return fail(AF2_ERR_BAD_ARG, "gemm: gathered A pieces of %d rows (need a multiple of 128)", c.a_pr);
         unsigned long long da[4] = {(unsigned long long)c.K, (unsigned long long)c.a_pr, (unsigned long long)((c.M + c.a_pr - 1) / c.a_pr), (unsigned long long)c.batch};
         unsigned long long sa[3] = {(unsigned long long)c.lda * 2, (unsigned long long)c.a_piece * 2, bsa};
-        unsigned ba[4] = {64, 128, 1, 1};
+        unsigned ba[4] = {64, GEMM_BM, 1, 1};
         AF2_TRY(make_tmap(&ta, c.A, 4, da, sa, ba, CU_TENSOR_MAP_SWIZZLE_128B));
       }
       if (c.b_pr > 0) {
@@ -309,9 +325,6 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
   p.cm_inner = c.cm_inner > 0 ? c.cm_inner : 1; p.cm_pitch = c.cm_pitch > 0 ? c.cm_pitch : 1;
   p.tile.mode = c.mode; p.tile.act = c.act; p.tile.layout = c.layout; p.tile.use_rowscale = c.use_rowscale;
   p.tile.out = c.out; p.tile.bias = c.bias; p.tile.ld = c.ld_out;
-  // the epilogue stores straight from the accumulator registers: no output / residual tensor maps
-  const CUtensorMap& tc = ta;
-  const CUtensorMap& tr = ta;
   // compile-time epilogue specialisation for the big-tile instantiation
   int ek = EK_GENERIC;
   if (BN == 256) {
@@ -323,28 +336,56 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
     else if (c.mode == EPI_RESID_F32) ek = EK_RESID_F32;
     else if (c.mode == EPI_STORE_F32) ek = EK_STORE_F32;
   }
+  if (c.mn_major && ek != EK_STORE_F32) ek = EK_GENERIC;
+  // output (and residual) tensor maps of the TMA epilogue; the register epilogue needs none
+  CUtensorMap tc = ta, tr = ta;
+  p.epi_tma = ek != EK_GENERIC && gemm_epi_tma_ok(c, p.out_cols) ? 1 : 0;
+  if (p.epi_tma) {
+    const bool f32 = c.mode == EPI_RESID_F32 || c.mode == EPI_STORE_F32;
+    const unsigned long long es = f32 ? 4 : 2;
+    const unsigned long long bstride = (unsigned long long)(c.batch > 1 ? c.out_batch : c.ld_out * c.M) * es;
+    if (c.layout == LAYOUT_CHANNEL) {
+      // [batch][col][row block][row in block]: 64-row x 64-column boxes written from a [col][row] stage
+      unsigned long long dc[4] = {(unsigned long long)p.cm_inner, (unsigned long long)(c.M / p.cm_inner), (unsigned long long)p.out_cols, (unsigned long long)c.batch};
+      unsigned long long sc[3] = {(unsigned long long)p.cm_pitch * 2, (unsigned long long)c.ld_out * 2, bstride};
+      unsigned bc[4] = {64, 1, 64, 1};
+      AF2_TRY(make_tmap(&tc, c.out, 4, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B));
+    } else {
+      unsigned long long dc[3] = {(unsigned long long)p.out_cols, (unsigned long long)c.M, (unsigned long long)c.batch};
+      unsigned long long sc[2] = {(unsigned long long)c.ld_out * es, bstride};
+      unsigned bc[3] = {f32 ? 32u : 64u, (unsigned)GEMM_BM, 1};
+      AF2_TRY(make_tmap(&tc, c.out, 3, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B,
+                        f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16));
+    }
+    if (c.mode == EPI_RESID_F32) {
+      unsigned long long dr[2] = {(unsigned long long)p.out_cols, (unsigned long long)c.M};
+      unsigned long long sr[1] = {(unsigned long long)c.ld_resid * 4};
+      unsigned br[2] = {32, (unsigned)GEMM_BM};
+      AF2_TRY(make_tmap(&tr, c.resid, 2, dr, sr, br, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_FLOAT32));
+    }
+  }
   if (c.mn_major) {
     if (BN == 256) {
-      if (ek == EK_STORE_F32) return launch_gemm_inst<256, 3, true, EK_STORE_F32>(ta, tb, tc, tr, p, s);
-      return launch_gemm_inst<256, 3, true, EK_GENERIC>(ta, tb, tc, tr, p, s);
+      if (ek == EK_STORE_F32) return launch_gemm_inst<256, 4, true, EK_STORE_F32>(ta, tb, tc, tr, p, s);
+      return launch_gemm_inst<256, 4, true, EK_GENERIC>(ta, tb, tc, tr, p, s);
     }
-    if (BN == 128) return launch_gemm_inst<128, 4, true, EK_GENERIC>(ta, tb, tc, tr, p, s);
-    return launch_gemm_inst<64, 6, true, EK_GENERIC>(ta, tb, tc, tr, p, s);
+    if (BN == 128) return launch_gemm_inst<128, 6, true, EK_GENERIC>(ta, tb, tc, tr, p, s);
+    return launch_gemm_inst<64, 8, true, EK_GENERIC>(ta, tb, tc, tr, p, s);
   }
   if (BN == 256) {
     switch (ek) {
-      case EK_STORE_TOK: return launch_gemm_inst<256, 3, false, EK_STORE_TOK>(ta, tb, tc, tr, p, s);
-      case EK_STORE_TOK_SIG: return launch_gemm_inst<256, 3, false, EK_STORE_TOK_SIG>(ta, tb, tc, tr, p, s);
-      case EK_STORE_CH: return launch_gemm_inst<256, 3, false, EK_STORE_CH>(ta, tb, tc, tr, p, s);
-      case EK_GATED_TOK_GELU: return launch_gemm_inst<256, 3, false, EK_GATED_TOK_GELU>(ta, tb, tc, tr, p, s);
-      case EK_GATED_CH_SIG: return launch_gemm_inst<256, 3, false, EK_GATED_CH_SIG>(ta, tb, tc, tr, p, s);
-      case EK_RESID_F32: return launch_gemm_inst<256, 3, false, EK_RESID_F32>(ta, tb, tc, tr, p, s);
-      case EK_STORE_F32: return launch_gemm_inst<256, 3, false, EK_STORE_F32>(ta, tb, tc, tr, p, s);
-      default: return launch_gemm_inst<256, 3, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
+      case EK_STORE_TOK: return launch_gemm_inst<256, 4, false, EK_STORE_TOK>(ta, tb, tc, tr, p, s);
+      case EK_STORE_TOK_SIG: return launch_gemm_inst<256, 4, false, EK_STORE_TOK_SIG>(ta, tb, tc, tr, p, s);
+      case EK_STORE_CH: return launch_gemm_inst<256, 4, false, EK_STORE_CH>(ta, tb, tc, tr, p, s);
+      case EK_GATED_TOK_GELU: return launch_gemm_inst<256, 4, false, EK_GATED_TOK_GELU>(ta, tb, tc, tr, p, s);
+      case EK_GATED_CH_SIG: return launch_gemm_inst<256, 4, false, EK_GATED_CH_SIG>(ta, tb, tc, tr, p, s);
+      case EK_RESID_F32: return launch_gemm_inst<256, 4, false, EK_RESID_F32>(ta, tb, tc, tr, p, s);
+      case EK_STORE_F32: return launch_gemm_inst<256, 4, false, EK_STORE_F32>(ta, tb, tc, tr, p, s);
+      default: return launch_gemm_inst<256, 4, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
     }
   }
-  if (BN == 128) return launch_gemm_inst<128, 4, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
-  return launch_gemm_inst<64, 6, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
+  if (BN == 128) return launch_gemm_inst<128, 6, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
+  return launch_gemm_inst<64, 8, false, EK_GENERIC>(ta, tb, tc, tr, p, s);
 }
 
 int pick_bn(int n) { return n > 128 ? 256 : (n > 64 ? 128 : 64); }

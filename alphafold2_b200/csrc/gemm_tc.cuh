@@ -7,19 +7,29 @@
 //   MN-major mode : C[b][m][n] = sum_k A[b][k][m] * B[b][k][n]      (triangle "ingoing", outer-mean:
 //                                                                    channel-major operands, k = row axis)
 //
-// Tiling: BM = 128 rows, BN in {64,128,256} accumulator columns, BK = 64.
+// Tiling: BM = 64 rows, BN in {64,128,256} accumulator columns, BK = 64.
 // Warp roles (384 threads, three warpgroups):
-//   warpgroup 0     TMA producer of the A/B stages (one thread issues; the warpgroup hands its registers to the others)
-//   warpgroups 1, 2 MMA + epilogue, rows 0..63 / 64..127 of the tile: wgmma m64nBNk16 into registers, then
-//                   (bias, activation, gate, row scale, residual) -> global stores straight from the accumulator fragment
-// Persistent over tiles; the producer runs ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
+//   warpgroup 0     TMA producers (the warpgroup hands its registers to the others):
+//                     warp 0  A/B stages of every tile, in tile order
+//                     warps 1, 2  residual sub-tiles of the tiles of MMA warpgroup 1 / 2 (EPI_RESID_F32 through TMA)
+//   warpgroups 1, 2 "ping-pong" MMA + epilogue: the CTA's tiles alternate between them, each owns whole 64 x BN tiles.
+//                   An ordered hand-off (named barriers 1, 2) lets one warpgroup issue its k loop only after the other
+//                   has issued its own, so one warpgroup's epilogue runs while the other keeps the tensor cores busy.
+// Epilogue (bias, activation, gate, row scale, residual): the fragment goes into 8 KB 128B-swizzled shared chunks (a ring
+// per warpgroup) and leaves through TMA stores -- token-major [row][col] boxes, or channel-major [col][row] boxes (the
+// transposing stage).  The residual arrives in the same chunks by TMA and is added in place.  Layouts TMA cannot express
+// (odd pitches, unaligned bases, channel-major blocks that are not whole 64-row boxes) and the EK_GENERIC
+// instantiations store straight from registers instead; the host chooses per call (GemmParams::epi_tma).
+// The per-element k order is the same in both epilogues and for any tile size: results do not depend on the path.
 #pragma once
 #include "common.cuh"
 
 namespace af2 {
 
-constexpr int GEMM_BM = 128;
+constexpr int GEMM_BM = 64;
 constexpr int GEMM_BK = 64;
+constexpr int GEMM_EPI_BUFS = 4;          // epilogue chunks per MMA warpgroup
+constexpr int GEMM_EPI_CHUNK = 8192;      // 64 rows x 128 B
 
 enum EpiMode : int { EPI_STORE_BF16 = 0, EPI_GATED_BF16 = 1, EPI_RESID_F32 = 2, EPI_STORE_F32 = 3 };
 enum EpiAct : int { ACT_NONE = 0, ACT_SIGMOID = 1, ACT_GELU = 2 };
@@ -42,7 +52,7 @@ struct GemmParams {
   int M, N, K, batch;          // N = accumulator columns = rows of the B operand
   int num_ntiles;
   int out_cols;                // valid output columns (N, or N/2 for EPI_GATED)
-  int direct;                  // unused: the epilogue always stores from registers
+  int epi_tma;                 // 1: epilogue through shared memory + TMA (tmC, and tmR for the residual); 0: register stores
   const float* rowscale;       // [batch*M] multiplier per row (mask), or nullptr
   const float* resid;          // EPI_RESID_F32: fp32 [M, ld_resid]
   long long ld_resid;
@@ -66,11 +76,14 @@ struct GemmParams {
 
 template <int BN, int STAGES>
 struct GemmSmem {
-  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KB
+  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;   // 8 KB
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int EPI_OFF = STAGES * STAGE_BYTES;                        // [2][GEMM_EPI_BUFS] chunks
+  static constexpr int BIAS_OFF = EPI_OFF + 2 * GEMM_EPI_BUFS * GEMM_EPI_CHUNK;  // [2][BN] fp32
+  static constexpr int BAR_OFF = BIAS_OFF + 2 * BN * 4;
   static constexpr int TOTAL = BAR_OFF + 256;
+  static_assert(2 * STAGES + 4 * GEMM_EPI_BUFS <= 32, "mbarriers exceed their 256-byte region");
   static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA can use");
 };
 
@@ -133,17 +146,30 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* efull_bar = empty_bar + STAGES;                 // [2][GEMM_EPI_BUFS] residual chunk landed
+  uint64_t* eempty_bar = efull_bar + 2 * GEMM_EPI_BUFS;     // [2][GEMM_EPI_BUFS] chunk read out by its TMA store
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;
 
+  const int e_mode = (EK == EK_GENERIC) ? p.tile.mode : EpiTraits<EK>::mode;
+  const int e_act = (EK == EK_GENERIC) ? p.tile.act : EpiTraits<EK>::act;
+  const int e_layout = (EK == EK_GENERIC) ? p.tile.layout : EpiTraits<EK>::layout;
+  const bool epi_tma = EK != EK_GENERIC && p.epi_tma;
+
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
+    if (epi_tma) prefetch_tmap(&tmC);
+    if (epi_tma && e_mode == EPI_RESID_F32) prefetch_tmap(&tmR);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);     // one arrive per MMA warpgroup
+      mbar_init(&empty_bar[s], 1);     // the one MMA warpgroup that consumed the stage
+    }
+    for (int s = 0; s < 2 * GEMM_EPI_BUFS; ++s) {
+      mbar_init(&efull_bar[s], 1);
+      mbar_init(&eempty_bar[s], 1);    // the storing thread, once the TMA store has read the chunk
     }
     fence_barrier_init();
   }
@@ -157,9 +183,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
   const int nseg = p.nseg > 1 ? p.nseg : 1;
   const int num_kk = num_kb * nseg;                 // k-blocks consumed per tile
+  const bool gated = e_mode == EPI_GATED_BF16;
+  const int W = gated ? BN / 2 : BN;                // output columns per tile
 
   if (wg == 0) {
-    // ================================ TMA producer ================================
+    // ================================ TMA producers ================================
     regs_dealloc<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
@@ -168,6 +196,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int nt = tile % n_tiles;
         const int mt = (tile / n_tiles) % m_tiles;
         const int b = tile / (n_tiles * m_tiles);
+        const int m0 = mt * GEMM_BM;
         for (int kk = 0; kk < num_kk; ++kk) {
           const int seg = kk / num_kb, kb = kk - seg * num_kb;
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -180,72 +209,84 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (nseg == 3) { ha = (seg == 1) ? 1 : 0; hb = (seg == 0) ? 1 : 0; }
             else { ha = (0x021010 >> (4 * (5 - seg))) & 0xf; hb = (0x201100 >> (4 * (5 - seg))) & 0xf; }
             if constexpr (!MN_MAJOR) {
-              tma_load_4d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, mt * GEMM_BM, ha, b);
+              tma_load_4d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, m0, ha, b);
               tma_load_4d(sb, &tmB, &full_bar[stage], kb * GEMM_BK, nt * BN, hb, b);
             } else {
-#pragma unroll
-              for (int h = 0; h < GEMM_BM / 64; ++h)
-                tma_load_4d(sa + h * 8192, &tmA, &full_bar[stage], mt * GEMM_BM + h * 64, kb * GEMM_BK, ha, b);
+              tma_load_4d(sa, &tmA, &full_bar[stage], m0, kb * GEMM_BK, ha, b);
 #pragma unroll
               for (int h = 0; h < BN / 64; ++h)
                 tma_load_4d(sb + h * 8192, &tmB, &full_bar[stage], nt * BN + h * 64, kb * GEMM_BK, hb, b);
             }
           } else if constexpr (!MN_MAJOR) {
-            if (p.a_pr > 0) tma_load_4d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, (mt * GEMM_BM) % p.a_pr, (mt * GEMM_BM) / p.a_pr, b);
-            else tma_load_3d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, mt * GEMM_BM, b);
+            if (p.a_pr > 0) tma_load_4d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, m0 % p.a_pr, m0 / p.a_pr, b);
+            else tma_load_3d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, m0, b);
             if (p.b_pr > 0) tma_load_4d(sb, &tmB, &full_bar[stage], kb * GEMM_BK, (nt * BN) % p.b_pr, (nt * BN) / p.b_pr, b);
             else tma_load_3d(sb, &tmB, &full_bar[stage], kb * GEMM_BK, nt * BN, b);
-          } else if (p.a_pr > 0 || p.b_pr > 0) {
-#pragma unroll
-            for (int h = 0; h < GEMM_BM / 64; ++h) {
-              const int m = mt * GEMM_BM + h * 64;
-              if (p.a_pr > 0) tma_load_4d(sa + h * 8192, &tmA, &full_bar[stage], m % p.a_pr, kb * GEMM_BK, m / p.a_pr, b);
-              else tma_load_3d(sa + h * 8192, &tmA, &full_bar[stage], m, kb * GEMM_BK, b);
-            }
+          } else {
+            // operand stored [k][mn]: 64-wide mn boxes, each 64 k-rows x 128 B = 8 KB
+            if (p.a_pr > 0) tma_load_4d(sa, &tmA, &full_bar[stage], m0 % p.a_pr, kb * GEMM_BK, m0 / p.a_pr, b);
+            else tma_load_3d(sa, &tmA, &full_bar[stage], m0, kb * GEMM_BK, b);
 #pragma unroll
             for (int h = 0; h < BN / 64; ++h) {
               const int n = nt * BN + h * 64;
               if (p.b_pr > 0) tma_load_4d(sb + h * 8192, &tmB, &full_bar[stage], n % p.b_pr, kb * GEMM_BK, n / p.b_pr, b);
               else tma_load_3d(sb + h * 8192, &tmB, &full_bar[stage], n, kb * GEMM_BK, b);
             }
-          } else {
-            // operand stored [k][mn]: 64-wide mn boxes, each 64 k-rows x 128 B = 8 KB
-#pragma unroll
-            for (int h = 0; h < GEMM_BM / 64; ++h)
-              tma_load_3d(sa + h * 8192, &tmA, &full_bar[stage], mt * GEMM_BM + h * 64, kb * GEMM_BK, b);
-#pragma unroll
-            for (int h = 0; h < BN / 64; ++h)
-              tma_load_3d(sb + h * 8192, &tmB, &full_bar[stage], nt * BN + h * 64, kb * GEMM_BK, b);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    } else if ((warp == 1 || warp == 2) && lane == 0 && epi_tma && e_mode == EPI_RESID_F32) {
+      // residual of MMA warpgroup (warp - 1)'s tiles, 64 x 32 fp32 chunks in the order its epilogue adds them; runs ahead
+      // by up to GEMM_EPI_BUFS chunks, independently of the A/B stages
+      const int hh = warp - 1;
+      int e = 0;
+      for (int i = hh; blockIdx.x + i * gridDim.x < total_tiles; i += 2) {
+        const int tile = blockIdx.x + i * gridDim.x;
+        const int nt = tile % n_tiles;
+        const int mt = (tile / n_tiles) % m_tiles;
+        for (int ch = 0; ch < BN / 32; ++ch, ++e) {
+          const int buf = hh * GEMM_EPI_BUFS + e % GEMM_EPI_BUFS;
+          mbar_wait(&eempty_bar[buf], ((e / GEMM_EPI_BUFS) & 1) ^ 1);
+          mbar_arrive_expect_tx(&efull_bar[buf], GEMM_EPI_CHUNK);
+          tma_load_2d(smem + L::EPI_OFF + buf * GEMM_EPI_CHUNK, &tmR, &efull_bar[buf], nt * W + ch * 32, mt * GEMM_BM);
         }
       }
     }
     return;
   }
 
-  // ===================== MMA + epilogue (warpgroup 1: rows 0..63, warpgroup 2: rows 64..127) =====================
+  // ============== MMA + epilogue: warpgroup hh = wg - 1 owns the CTA's tiles i = hh, hh + 2, hh + 4, ... ==============
   regs_alloc<232>();
-  const int h = wg - 1;
+  const int hh = wg - 1;
   const int wq = warp & 3;
-  const int e_mode = (EK == EK_GENERIC) ? p.tile.mode : EpiTraits<EK>::mode;
-  const int e_act = (EK == EK_GENERIC) ? p.tile.act : EpiTraits<EK>::act;
-  const int e_layout = (EK == EK_GENERIC) ? p.tile.layout : EpiTraits<EK>::layout;
-  const bool gated = e_mode == EPI_GATED_BF16;
+  const int tid = threadIdx.x & 127;
   const bool out_f32 = (e_mode == EPI_RESID_F32) || (e_mode == EPI_STORE_F32);
-  const int W = gated ? BN / 2 : BN;                                           // output columns per tile
   const NTile t = p.tile;
   // paired (8-byte fp32 / 4-byte bf16) stores need an even row pitch and an aligned base
   const bool vec_out = (t.ld % 2 == 0) && (p.out_batch_stride % 2 == 0) &&
                        (reinterpret_cast<uintptr_t>(t.out) & (out_f32 ? 7 : 3)) == 0;
   const bool vec_res = (p.ld_resid % 2 == 0) && (reinterpret_cast<uintptr_t>(p.resid) & 7) == 0;
-  int stage = 0;
-  uint32_t phase = 0;
+  float* sbias = reinterpret_cast<float*>(smem + L::BIAS_OFF) + hh * BN;
+  uint8_t* sepi = smem + L::EPI_OFF + hh * GEMM_EPI_BUFS * GEMM_EPI_CHUNK;
+  const int bar_self = 3 + hh;                       // this warpgroup's 128 threads
+  int e = 0;                                         // epilogue chunks this warpgroup has used
   float acc[BN / 2];
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+  for (int i = hh; blockIdx.x + i * gridDim.x < total_tiles; i += 2) {
+    const int tile = blockIdx.x + i * gridDim.x;
     const int nt = tile % n_tiles;
     const int mt = (tile / n_tiles) % m_tiles;
     const int b = tile / (n_tiles * m_tiles);
+    // the bias of the tile goes to shared memory once (the previous epilogue has finished reading it)
+    named_bar_sync(bar_self, 128);
+    if (t.bias)
+      for (int c = tid; c < BN; c += 128) sbias[c] = nt * BN + c < p.N ? __ldg(t.bias + nt * BN + c) : 0.0f;
+
+    // k loop; stage ring position = k-blocks the producer issued for the CTA's tiles 0 .. i-1
+    const int g0 = i * num_kk;
+    int stage = g0 % STAGES;
+    uint32_t phase = (g0 / STAGES) & 1;
+    if (i > 0) named_bar_sync(1 + hh, 256);          // tile i - 1 (other warpgroup) has issued its k loop
     int prev = -1;
     for (int kk = 0; kk < num_kk; ++kk) {
       mbar_wait(&full_bar[stage], phase);
@@ -256,13 +297,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int k = 0; k < GEMM_BK / 16; ++k) {
         uint64_t adesc, bdesc;
         if constexpr (!MN_MAJOR) {
-          // rows of 128 B (64 bf16 of K); 8-row swizzle atoms 1024 B apart; K step = 32 B; this warpgroup's 64 rows 8 KB in
-          adesc = wgmma_desc(sa + h * 8192 + k * 32, 16, 1024, SWZ_128);
+          // rows of 128 B (64 bf16 of K); 8-row swizzle atoms 1024 B apart; K step = 32 B
+          adesc = wgmma_desc(sa + k * 32, 16, 1024, SWZ_128);
           bdesc = wgmma_desc(sb + k * 32, 16, 1024, SWZ_128);
         } else {
-          // k-rows of 128 B (64 bf16 of M/N); 8 k-rows = 1024 B (SBO); next 64-wide mn block 8 KB (LBO); this warpgroup's
-          // 64 rows are the h-th 64-wide box of A
-          adesc = wgmma_desc(sa + h * 8192 + k * 2048, 8192, 1024, SWZ_128);
+          // k-rows of 128 B (64 bf16 of M/N); 8 k-rows = 1024 B (SBO); next 64-wide mn block 8 KB (LBO)
+          adesc = wgmma_desc(sa + k * 2048, 8192, 1024, SWZ_128);
           bdesc = wgmma_desc(sb + k * 2048, 8192, 1024, SWZ_128);
         }
         const uint32_t scale_d = (kk | k) != 0 ? 1u : 0u;
@@ -277,61 +317,148 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
+    if (blockIdx.x + (i + 1) * gridDim.x < total_tiles) named_bar_arrive(2 - hh, 256);   // tile i + 1 may start
     wgmma_wait<0>();
     reg_fence(acc);
     if (prev >= 0 && lane == 0 && wq == 0) mbar_arrive(&empty_bar[prev]);
+    named_bar_sync(bar_self, 128);                   // bias of the tile visible
 
-    // ------------------------------- epilogue from registers -------------------------------
     const int col0 = nt * W;
-    const int ncols = min(W, p.out_cols - col0);
-    const float* bias_tile = t.bias ? t.bias + nt * BN : nullptr;
+    const int r_lo = wq * 16 + (lane >> 2);          // tile-local rows r_lo, r_lo + 8 of this thread
+    if (epi_tma) {
+      // ---------------- epilogue through 8 KB swizzled chunks + TMA stores (compile-time EK) ----------------
+      constexpr int MODE = EpiTraits<EK>::mode, ACT = EpiTraits<EK>::act, LAYOUT = EpiTraits<EK>::layout;
+      constexpr bool F32 = MODE == EPI_RESID_F32 || MODE == EPI_STORE_F32;
+      constexpr bool GATED = MODE == EPI_GATED_BF16;
+      constexpr int CJ = F32 ? 4 : 8;                // fragment column steps (8 columns) per chunk
+      constexpr int NJ = GATED ? BN / 16 : BN / 8;
+      constexpr int NCH = NJ / CJ >= 1 ? NJ / CJ : 1;
+      float rs[2] = {1.0f, 1.0f};
+      if (EpiTraits<EK>::rowscale && t.use_rowscale) {
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      const int row = mt * GEMM_BM + h * 64 + wq * 16 + (lane >> 2) + half * 8;
-      if (row >= p.M) continue;
-      float rs = 1.0f;
-      if (EpiTraits<EK>::rowscale && t.use_rowscale) rs = __ldg(p.rowscale + static_cast<long long>(b) * p.M + row);
-      long long cm_off = 0;
-      if (e_layout == LAYOUT_CHANNEL) cm_off = static_cast<long long>(row / p.cm_inner) * p.cm_pitch + row % p.cm_inner;
-      const long long obase = static_cast<long long>(b) * p.out_batch_stride;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {                    // fully unrolled: the accumulator stays in registers
-        const int c = 8 * j + 2 * (lane & 3);                // tile-local output column of the pair
-        if ((gated && j >= BN / 16) || c >= ncols) continue;
-        const bool two = c + 1 < ncols;
-        float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
-        if (bias_tile) { v0 += __ldg(bias_tile + c); v1 += __ldg(bias_tile + c + 1); }
-        if (gated) {
-          // gate columns of the packed tile sit BN / 2 columns (BN / 16 fragment steps) to the right of their values
-          constexpr int JM = BN / 8 - 1;
-          const int jg = (j + BN / 16) & JM;
-          float g0 = acc[4 * jg + 2 * half], g1 = acc[4 * jg + 2 * half + 1];
-          if (bias_tile) { g0 += __ldg(bias_tile + BN / 2 + c); g1 += __ldg(bias_tile + BN / 2 + c + 1); }
-          v0 *= apply_act(g0, e_act);
-          v1 *= apply_act(g1, e_act);
-        } else {
-          v0 = apply_act(v0, e_act);
-          v1 = apply_act(v1, e_act);
+        for (int half = 0; half < 2; ++half) {
+          const int row = mt * GEMM_BM + r_lo + half * 8;
+          if (row < p.M) rs[half] = __ldg(p.rowscale + static_cast<long long>(b) * p.M + row);
         }
-        if (EpiTraits<EK>::rowscale && t.use_rowscale) { v0 *= rs; v1 *= rs; }
-        const int col = col0 + c;
-        if (e_layout == LAYOUT_CHANNEL) {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(t.out) + obase + cm_off;
-          o[static_cast<long long>(col) * t.ld] = __float2bfloat16(v0);
-          if (two) o[static_cast<long long>(col + 1) * t.ld] = __float2bfloat16(v1);
-        } else if (out_f32) {
-          if (e_mode == EPI_RESID_F32) {
-            const float* r = p.resid + static_cast<long long>(row) * p.ld_resid + col;
-            if (two && vec_res) { const float2 r2 = *reinterpret_cast<const float2*>(r); v0 += r2.x; v1 += r2.y; }
-            else { v0 += r[0]; if (two) v1 += r[1]; }
+      }
+      const int q2 = 2 * (lane & 3);
+#pragma unroll
+      for (int ch = 0; ch < NCH; ++ch, ++e) {
+        const int buf = e % GEMM_EPI_BUFS;
+        const uint32_t par = (e / GEMM_EPI_BUFS) & 1;
+        if (MODE == EPI_RESID_F32) mbar_wait(&efull_bar[hh * GEMM_EPI_BUFS + buf], par);
+        else mbar_wait(&eempty_bar[hh * GEMM_EPI_BUFS + buf], par ^ 1);
+        uint8_t* sc = sepi + buf * GEMM_EPI_CHUNK;
+#pragma unroll
+        for (int jj = 0; jj < CJ; ++jj) {
+          const int j = ch * CJ + jj;
+          if (j >= NJ) break;
+          const int c = 8 * j + q2;                  // tile-local output column of the pair
+          const int cl = 8 * jj + q2;                // chunk-local
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int r = r_lo + half * 8;
+            float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+            if (t.bias) { v0 += sbias[c]; v1 += sbias[c + 1]; }
+            if constexpr (GATED) {
+              const int jg = j + BN / 16;
+              float g0 = acc[4 * jg + 2 * half], g1 = acc[4 * jg + 2 * half + 1];
+              if (t.bias) { g0 += sbias[BN / 2 + c]; g1 += sbias[BN / 2 + c + 1]; }
+              v0 *= apply_act(g0, ACT);
+              v1 *= apply_act(g1, ACT);
+            } else {
+              v0 = apply_act(v0, ACT);
+              v1 = apply_act(v1, ACT);
+            }
+            if (EpiTraits<EK>::rowscale && t.use_rowscale) { v0 *= rs[half]; v1 *= rs[half]; }
+            if constexpr (LAYOUT == LAYOUT_CHANNEL) {
+              // [col][row] box: 128-byte lines of 64 rows, 16-byte chunk (r / 8) swizzled by col % 8
+              __nv_bfloat16* o0 = reinterpret_cast<__nv_bfloat16*>(sc + cl * 128 + (((r >> 3) ^ (cl & 7)) << 4)) + (r & 7);
+              __nv_bfloat16* o1 = reinterpret_cast<__nv_bfloat16*>(sc + (cl + 1) * 128 + (((r >> 3) ^ ((cl + 1) & 7)) << 4)) + (r & 7);
+              *o0 = __float2bfloat16(v0);
+              *o1 = __float2bfloat16(v1);
+            } else if constexpr (F32) {
+              // [row][32 fp32] box
+              float2* o = reinterpret_cast<float2*>(sc + r * 128 + (((cl >> 2) ^ (r & 7)) << 4) + (cl & 3) * 4);
+              if constexpr (MODE == EPI_RESID_F32) { const float2 rv = *o; v0 += rv.x; v1 += rv.y; }
+              *o = make_float2(v0, v1);
+            } else {
+              // [row][64 bf16] box
+              *reinterpret_cast<uint32_t*>(sc + r * 128 + (((cl >> 3) ^ (r & 7)) << 4) + (cl & 7) * 2) = pack_bf16x2(v0, v1);
+            }
           }
-          store_pair<true>(t.out, obase + static_cast<long long>(row) * t.ld + col, v0, v1, two, vec_out);
-        } else {
-          store_pair<false>(t.out, obase + static_cast<long long>(row) * t.ld + col, v0, v1, two, vec_out);
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(bar_self, 128);
+        if (tid == 0) {
+          const int m0 = mt * GEMM_BM;
+          if constexpr (LAYOUT == LAYOUT_CHANNEL)
+            tma_store_4d(&tmC, sc, m0 % p.cm_inner, m0 / p.cm_inner, col0 + ch * 64, b);
+          else
+            tma_store_3d(&tmC, sc, col0 + ch * (F32 ? 32 : 64), m0, b);
+          tma_store_commit();
+          if (ch > 0) {
+            tma_store_wait_read<1>();
+            mbar_arrive(&eempty_bar[hh * GEMM_EPI_BUFS + (e - 1) % GEMM_EPI_BUFS]);
+          }
+        }
+      }
+      if (tid == 0) {
+        tma_store_wait_read<0>();
+        mbar_arrive(&eempty_bar[hh * GEMM_EPI_BUFS + (e - 1) % GEMM_EPI_BUFS]);
+      }
+    } else {
+      // ------------------------------- epilogue from registers -------------------------------
+      const int ncols = min(W, p.out_cols - col0);
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int row = mt * GEMM_BM + r_lo + half * 8;
+        if (row >= p.M) continue;
+        float rs = 1.0f;
+        if (EpiTraits<EK>::rowscale && t.use_rowscale) rs = __ldg(p.rowscale + static_cast<long long>(b) * p.M + row);
+        long long cm_off = 0;
+        if (e_layout == LAYOUT_CHANNEL) cm_off = static_cast<long long>(row / p.cm_inner) * p.cm_pitch + row % p.cm_inner;
+        const long long obase = static_cast<long long>(b) * p.out_batch_stride;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {                    // fully unrolled: the accumulator stays in registers
+          const int c = 8 * j + 2 * (lane & 3);                // tile-local output column of the pair
+          if ((gated && j >= BN / 16) || c >= ncols) continue;
+          const bool two = c + 1 < ncols;
+          float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+          if (t.bias) { v0 += sbias[c]; v1 += sbias[c + 1]; }
+          if (gated) {
+            // gate columns of the packed tile sit BN / 2 columns (BN / 16 fragment steps) to the right of their values
+            constexpr int JM = BN / 8 - 1;
+            const int jg = (j + BN / 16) & JM;
+            float g0 = acc[4 * jg + 2 * half], g1 = acc[4 * jg + 2 * half + 1];
+            if (t.bias) { g0 += sbias[BN / 2 + c]; g1 += sbias[BN / 2 + c + 1]; }
+            v0 *= apply_act(g0, e_act);
+            v1 *= apply_act(g1, e_act);
+          } else {
+            v0 = apply_act(v0, e_act);
+            v1 = apply_act(v1, e_act);
+          }
+          if (EpiTraits<EK>::rowscale && t.use_rowscale) { v0 *= rs; v1 *= rs; }
+          const int col = col0 + c;
+          if (e_layout == LAYOUT_CHANNEL) {
+            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(t.out) + obase + cm_off;
+            o[static_cast<long long>(col) * t.ld] = __float2bfloat16(v0);
+            if (two) o[static_cast<long long>(col + 1) * t.ld] = __float2bfloat16(v1);
+          } else if (out_f32) {
+            if (e_mode == EPI_RESID_F32) {
+              const float* r = p.resid + static_cast<long long>(row) * p.ld_resid + col;
+              if (two && vec_res) { const float2 r2 = *reinterpret_cast<const float2*>(r); v0 += r2.x; v1 += r2.y; }
+              else { v0 += r[0]; if (two) v1 += r[1]; }
+            }
+            store_pair<true>(t.out, obase + static_cast<long long>(row) * t.ld + col, v0, v1, two, vec_out);
+          } else {
+            store_pair<false>(t.out, obase + static_cast<long long>(row) * t.ld + col, v0, v1, two, vec_out);
+          }
         }
       }
     }
   }
+  if (epi_tma && tid == 0) tma_store_wait<0>();
 }
 
 }  // namespace af2

@@ -482,14 +482,52 @@ int g_c2t_tma = 1;   // 0: tile-per-CTA kernel (AF2_C2T_TMA=0)
 int g_attn_headmajor = 0;  // EXPERIMENT: attention reads a head-major copy of q|k|v (AF2_ATTN_HEADMAJOR=1)
 int g_gather_fused = 1;   // 1: contractions over all-gathered operand pieces in ONE launch (AF2_GATHER_FUSED=0: one launch per piece)
 
-int launch_chan_to_token(const ChanLnParams& p, cudaStream_t s) {
+// channel -> token kernels (af2_chan_to_token numbers them the same way)
+enum C2tVariant { C2T_AUTO = 0, C2T_SIMT = 1, C2T_TILE = 2, C2T_TMA = 3 };
+
+// What each kernel needs of the call.  Both dense-grid kernels read src[c][t] at t = row * n + j, so the rows must be
+// unpadded (pitch == n).  TMA: 16-byte aligned bases and a 16-byte channel stride for the tensor maps, int token
+// coordinates.  Tile: 16-byte loads of src (at c * chan_stride) and stores of y, in mode 0 also of gate, gamma and beta,
+// and whole float4 token groups (T % 4 == 0).  SIMT: one block row per token row (grid.y), d * 33 floats of shared memory.
+bool c2t_variant_ok(const ChanLnParams& p, int v) {
   const long long T = (long long)p.rows * p.n;
-  if (g_c2t_tma && p.pitch == p.n && (p.d == 256 || p.d == 128) && (p.chan_stride % 4) == 0 && T > 0 && T < (1ll << 31) &&
-      aligned16(p.src) && aligned16(p.y) && (p.mode != 0 || aligned16(p.gate))) {
+  switch (v) {
+    case C2T_TMA:
+      return p.pitch == p.n && (p.d == 256 || p.d == 128) && (p.chan_stride % 4) == 0 && T > 0 && T < (1ll << 31) &&
+             aligned16(p.src) && aligned16(p.y) && (p.mode != 0 || aligned16(p.gate));
+    case C2T_TILE:
+      return p.pitch == p.n && p.d % 64 == 0 && p.d <= 256 && (T % 4) == 0 && (p.chan_stride % 4) == 0 &&
+             aligned16(p.src) && aligned16(p.y) && (p.mode != 0 || (aligned16(p.gate) && aligned16(p.gamma) && aligned16(p.beta)));
+    case C2T_SIMT:
+      return p.rows <= 65535 && p.d > 0 && (size_t)p.d * 33 * sizeof(float) <= 227 * 1024;
+    default:
+      return false;
+  }
+}
+
+// the kernel launch_chan_to_token runs for this call: the TMA kernel where it applies (unless AF2_C2T_TMA=0), else the tile
+// kernel, else the SIMT kernel; 0 if none can take it
+int c2t_select(const ChanLnParams& p) {
+  if (g_c2t_tma && c2t_variant_ok(p, C2T_TMA)) return C2T_TMA;
+  if (c2t_variant_ok(p, C2T_TILE)) return C2T_TILE;
+  return c2t_variant_ok(p, C2T_SIMT) ? C2T_SIMT : 0;
+}
+
+// variant: C2T_AUTO (c2t_select) or a forced kernel, which must satisfy c2t_variant_ok; *ran <- the kernel launched (0: none)
+int launch_chan_to_token(const ChanLnParams& p, cudaStream_t s, int variant = C2T_AUTO, int* ran = nullptr) {
+  if (ran) *ran = 0;
+  const long long T = (long long)p.rows * p.n;
+  if (T <= 0) return AF2_OK;
+  const int v = variant == C2T_AUTO ? c2t_select(p) : variant;
+  if (v == 0 || !c2t_variant_ok(p, v))
+    return fail(AF2_ERR_BAD_ARG, "chan_to_token: variant %d cannot run d=%d rows=%d n=%d pitch=%d chan_stride=%lld mode=%d",
+                variant, p.d, p.rows, p.n, p.pitch, p.chan_stride, p.mode);
+  if (ran) *ran = v;
+  if (v == C2T_TMA) {
     // dense token grid: persistent TMA-pipelined kernel
     return p.d == 256 ? launch_chan_to_token_tma<256>(p, T, s) : launch_chan_to_token_tma<128>(p, T, s);
   }
-  if (p.pitch == p.n && p.d % 64 == 0 && p.d <= 256 && (T % 4) == 0) {
+  if (v == C2T_TILE) {
     // dense token grid: 64-token tiles, fully coalesced
     const size_t smem = (size_t)p.d * 64 * sizeof(float) + 8 * 64 * 2 * sizeof(float);
     static bool configured[MAX_DEVICES] = {false};
@@ -592,7 +630,10 @@ int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nba
 
 // OuterMean normaliser of pair rows [row0, row0 + rows) of one batch element (quirk Q3): bit-packed kernel when the packed
 // mask fits in shared memory, else the byte-loop kernel
-int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int row0, int rows, int S, int N, float eps, cudaStream_t s);
+// variant: 0 the choice above, 1 the byte-loop kernel, 2 the bit-packed pair (needs `words` and the shared-memory fit);
+// *ran <- the variant launched (0: none)
+int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int row0, int rows, int S, int N, float eps, cudaStream_t s,
+                       int variant = 0, int* ran = nullptr);
 
 int ew_grid(long long n) {
   long long b = (n + 255) / 256;
@@ -600,13 +641,20 @@ int ew_grid(long long n) {
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
-int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int row0, int rows, int S, int N, float eps, cudaStream_t s) {
+int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int row0, int rows, int S, int N, float eps, cudaStream_t s,
+                       int variant, int* ran) {
+  if (ran) *ran = 0;
   const long long T = (long long)rows * N;
   if (T <= 0) return AF2_OK;
   const int nw = (S + 31) / 32;
   const size_t smem = (size_t)nw * N * 4;
+  const bool bits_ok = words && smem <= 160 * 1024;
+  if (variant == 2 && !bits_ok)
+    return fail(AF2_ERR_BAD_ARG, "outer_scale: bit-packed kernel needs the words workspace and %zu <= %d bytes of shared memory", smem, 160 * 1024);
+  const bool bits = variant == 2 || (variant == 0 && bits_ok);
+  if (ran) *ran = bits ? 2 : 1;
   ProfScope ps(s, KC_MISC, 0.0, 0.0);
-  if (words && smem <= 160 * 1024) {
+  if (bits) {
     static size_t configured[MAX_DEVICES] = {0};
     if (smem > 48 * 1024 && smem > configured[cur_dev()]) {
       CUDA_OK(cudaFuncSetAttribute(outer_scale_bits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1349,6 +1397,70 @@ int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, cons
                           static_cast<const __nv_bfloat16*>(bias), (int)align_up(n, 8), mask,
                           static_cast<const __nv_bfloat16*>(gate), static_cast<__nv_bfloat16*>(out),
                           static_cast<cudaStream_t>(stream));
+}
+
+int af2_gemm_bf16_f32_gathered(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,
+                               float* C, long long ldc, long long c_batch, int M, int N, int K, int batch, int mn_major, int bn,
+                               int a_pr, long long a_piece, int b_pr, long long b_piece, af2_stream_t stream) {
+  if (!A || !Bm || !C) return fail(AF2_ERR_BAD_ARG, "gemm: null argument");
+  if (bn != 64 && bn != 128 && bn != 256) return fail(AF2_ERR_BAD_ARG, "gemm: bn %d (64, 128 or 256)", bn);
+  if (a_pr < 0 || b_pr < 0) return fail(AF2_ERR_BAD_ARG, "gemm: negative piece size");
+  GemmCall c;
+  memset(&c, 0, sizeof(c));
+  c.A = A; c.lda = lda; c.a_batch = a_batch; c.Bm = Bm; c.ldb = ldb; c.b_batch = b_batch;
+  c.M = M; c.N = N; c.K = K; c.batch = batch; c.mn_major = mn_major != 0; c.bn = bn;
+  c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = C; c.ld_out = ldc; c.out_batch = c_batch;
+  c.a_pr = a_pr; c.a_piece = a_piece; c.b_pr = b_pr; c.b_piece = b_piece;
+  return launch_gemm(c, static_cast<cudaStream_t>(stream));
+}
+
+static ChanLnParams chan_ln_params(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode,
+                                   const float* gamma, const float* beta, const void* gate, const float* scale,
+                                   float scale_const, float eps, void* y) {
+  ChanLnParams p;
+  memset(&p, 0, sizeof(p));
+  p.src = src; p.chan_stride = chan_stride; p.pitch = pitch; p.rows = rows; p.n = n; p.d = d; p.mode = mode;
+  p.gamma = gamma; p.beta = beta; p.gate = static_cast<const __nv_bfloat16*>(gate); p.scale = scale;
+  p.scale_const = scale_const; p.eps = eps; p.y = static_cast<__nv_bfloat16*>(y);
+  return p;
+}
+
+static int chan_ln_check(const ChanLnParams& p) {
+  if (!p.src || !p.y || (p.mode == 0 && (!p.gamma || !p.beta || !p.gate))) return fail(AF2_ERR_BAD_ARG, "chan_to_token: null argument");
+  if (p.mode != 0 && p.mode != 1) return fail(AF2_ERR_BAD_ARG, "chan_to_token: mode %d (0 or 1)", p.mode);
+  if (p.rows < 0 || p.n < 0 || p.d <= 0 || p.pitch < p.n || p.chan_stride < (long long)p.rows * p.pitch)
+    return fail(AF2_ERR_BAD_ARG, "chan_to_token: rows=%d n=%d pitch=%d d=%d chan_stride=%lld", p.rows, p.n, p.pitch, p.d, p.chan_stride);
+  return AF2_OK;
+}
+
+int af2_chan_to_token_select(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode,
+                             const float* gamma, const float* beta, const void* gate, const float* scale, float scale_const,
+                             float eps, void* y) {
+  const ChanLnParams p = chan_ln_params(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y);
+  AF2_TRY(chan_ln_check(p));
+  const int v = c2t_select(p);
+  return v ? v : fail(AF2_ERR_BAD_ARG, "chan_to_token: no kernel takes d=%d rows=%d", d, rows);
+}
+
+int af2_chan_to_token(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode, const float* gamma,
+                      const float* beta, const void* gate, const float* scale, float scale_const, float eps, void* y, int variant,
+                      int* ran, af2_stream_t stream) {
+  if (ran) *ran = 0;
+  const ChanLnParams p = chan_ln_params(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y);
+  AF2_TRY(chan_ln_check(p));
+  if (variant < C2T_AUTO || variant > C2T_TMA) return fail(AF2_ERR_BAD_ARG, "chan_to_token: variant %d (0..3)", variant);
+  return launch_chan_to_token(p, static_cast<cudaStream_t>(stream), variant, ran);
+}
+
+int af2_outer_scale(const unsigned char* mask, float* scale, void* words, int row0, int rows, int S, int N, float eps, int variant,
+                    int* ran, af2_stream_t stream) {
+  if (ran) *ran = 0;
+  if (!mask || !scale) return fail(AF2_ERR_BAD_ARG, "outer_scale: null argument");
+  if (S < 1 || N < 1 || row0 < 0 || rows < 0 || row0 + rows > N)
+    return fail(AF2_ERR_BAD_ARG, "outer_scale: S=%d N=%d rows [%d, %d)", S, N, row0, row0 + rows);
+  if (variant < 0 || variant > 2) return fail(AF2_ERR_BAD_ARG, "outer_scale: variant %d (0..2)", variant);
+  return launch_outer_scale(mask, scale, static_cast<uint32_t*>(words), row0, rows, S, N, eps, static_cast<cudaStream_t>(stream),
+                            variant, ran);
 }
 
 }  // extern "C"

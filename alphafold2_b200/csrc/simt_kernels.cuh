@@ -426,23 +426,8 @@ __global__ void __launch_bounds__(512) chan_to_token_tile_kernel(const ChanLnPar
 // ------------------------------------------------------------------------------------------------
 // OuterMean normaliser (quirk Q3, alphafold2.py:345-347):
 //   scale[b][i][j] = 1 / (S * (sum_s mask[b,s,i] * mask[b,s,j] + eps))      (fp32, like the reference)
+// computed for a band of pair rows [row0, row0 + rows) of one batch element: scale[(i - row0) * N + j]
 // ------------------------------------------------------------------------------------------------
-__global__ void outer_scale_kernel(const uint8_t* __restrict__ mask, float* __restrict__ scale, int B, int S, int N,
-                                   float eps) {
-  const long long total = static_cast<long long>(B) * N * N;
-  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
-       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int j = idx % N;
-    const int i = (idx / N) % N;
-    const int b = idx / (static_cast<long long>(N) * N);
-    const uint8_t* mb = mask + static_cast<long long>(b) * S * N;
-    int cnt = 0;
-    for (int s = 0; s < S; ++s) cnt += (mb[s * N + i] != 0) & (mb[s * N + j] != 0);
-    scale[idx] = 1.0f / (static_cast<float>(S) * (static_cast<float>(cnt) + eps));
-  }
-}
-
-// same for a band of pair rows [row0, row0 + rows) (sharded outer mean): scale[(i - row0) * N + j]
 __global__ void outer_scale_rows_kernel(const uint8_t* __restrict__ mask, float* __restrict__ scale, int row0, int rows,
                                         int S, int N, float eps) {
   const long long total = static_cast<long long>(rows) * N;
@@ -456,7 +441,7 @@ __global__ void outer_scale_rows_kernel(const uint8_t* __restrict__ mask, float*
   }
 }
 
-// Bit-packed version of both kernels above: count[i][j] = popc(bits_i & bits_j) with bits_i = the S mask bits of residue i.
+// Bit-packed version of the kernel above: count[i][j] = popc(bits_i & bits_j) with bits_i = the S mask bits of residue i.
 //   mask_pack_bits_kernel: words[w][i] (w = s / 32) <- the [S][N] byte mask, once per call (coalesced byte reads over i);
 //   outer_scale_bits_kernel: every block copies the packed words (S/32 * N * 4 bytes, L2 resident) into shared memory and
 //   walks its (i, j) pairs: the i-word is a broadcast, the j-words are consecutive -> conflict-free.  S / 32 AND+POPC steps

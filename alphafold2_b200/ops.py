@@ -589,3 +589,83 @@ def attention_bf16(qkv: torch.Tensor, gate: torch.Tensor, n: int, nbatch: int, h
     _lib.check(_lib.load().af2_attention_bf16(qkv.data_ptr(), gate.data_ptr(), _ptr(bias), _ptr(mask), out.data_ptr(), n,
                                               nbatch, heads, dim_head, tok_sb, tok_si, _stream_ptr()))
     return out
+
+
+def _addr(t: torch.Tensor, offset: int = 0) -> int:
+    """device address of element `offset` of the flat buffer t"""
+    return t.data_ptr() + offset * t.element_size()
+
+
+def gemm_bf16_f32_strided(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, *, M: int, N: int, K: int, batch: int,
+                          mn_major: bool, bn: int, lda: int, a_batch: int, ldb: int, b_batch: int, ldc: int, c_batch: int,
+                          a_off: int = 0, b_off: int = 0, c_off: int = 0, a_pr: int = 0, a_piece: int = 0, b_pr: int = 0,
+                          b_piece: int = 0) -> torch.Tensor:
+    """af2_gemm_bf16_f32_gathered on flat buffers with explicit strides, as the contractions issue it: operand A (B) starts
+    at element a_off (b_off) of a (b), C at element c_off of the fp32 buffer c.  a_pr / b_pr > 0 address the operand as
+    gathered pieces a_piece / b_piece elements apart (include/af2b200.h).  Returns c."""
+    _require(a, torch.bfloat16, "a")
+    _require(b, torch.bfloat16, "b")
+    _require(c, torch.float32, "c")
+    _lib.check(_lib.load().af2_gemm_bf16_f32_gathered(_addr(a, a_off), lda, a_batch, _addr(b, b_off), ldb, b_batch,
+                                                      _addr(c, c_off), ldc, c_batch, M, N, K, batch, int(mn_major), bn,
+                                                      a_pr, a_piece, b_pr, b_piece, _stream_ptr()))
+    return c
+
+
+C2T_AUTO, C2T_SIMT, C2T_TILE, C2T_TMA = 0, 1, 2, 3
+
+
+def _c2t_args(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y, src_off, gate_off, y_off):
+    _require(src, torch.float32, "src")
+    _require(y, torch.bfloat16, "y")
+    if mode == 0:
+        _require(gate, torch.bfloat16, "gate")
+    for t, name in ((gamma, "gamma"), (beta, "beta"), (scale, "scale")):
+        if t is not None:
+            _require(t, torch.float32, name)
+    return (_addr(src, src_off), chan_stride, pitch, rows, n, d, mode, _ptr(gamma), _ptr(beta),
+            None if gate is None else _addr(gate, gate_off), _ptr(scale), float(scale_const), float(eps), _addr(y, y_off))
+
+
+def chan_to_token(src: torch.Tensor, y: torch.Tensor, *, chan_stride: int, pitch: int, rows: int, n: int, d: int, mode: int,
+                  gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None,
+                  gate: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None, scale_const: float = 1.0,
+                  eps: float = 1e-5, variant: int = C2T_AUTO, src_off: int = 0, gate_off: int = 0, y_off: int = 0) -> int:
+    """af2_chan_to_token on flat buffers (src fp32, gate / y bf16; *_off in elements): channel-major src -> token-major y,
+    mode 0 LayerNorm over channels * gate, mode 1 * scale.  Returns the kernel variant that ran (C2T_*)."""
+    ran = C.c_int(0)
+    args = _c2t_args(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y, src_off,
+                     gate_off, y_off)
+    _lib.check(_lib.load().af2_chan_to_token(*args, variant, C.byref(ran), _stream_ptr()))
+    return ran.value
+
+
+def chan_to_token_select(src: torch.Tensor, y: torch.Tensor, *, chan_stride: int, pitch: int, rows: int, n: int, d: int,
+                         mode: int, gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None,
+                         gate: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None, scale_const: float = 1.0,
+                         eps: float = 1e-5, src_off: int = 0, gate_off: int = 0, y_off: int = 0) -> int:
+    """the kernel variant chan_to_token(variant=C2T_AUTO) would run for these arguments; launches nothing"""
+    args = _c2t_args(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y, src_off,
+                     gate_off, y_off)
+    v = _lib.load().af2_chan_to_token_select(*args)
+    if v < 0:
+        _lib.check(v)
+    return v
+
+
+OUTER_SCALE_AUTO, OUTER_SCALE_BYTES, OUTER_SCALE_BITS = 0, 1, 2
+
+
+def outer_scale(mask: torch.Tensor, scale: torch.Tensor, *, row0: int, rows: int, eps: float, variant: int = OUTER_SCALE_AUTO,
+                words: Optional[torch.Tensor] = None) -> int:
+    """af2_outer_scale: scale fp32 [rows * N] (flat) <- 1 / (S (count_ij + eps)) for pair rows [row0, row0 + rows) of the bool
+    mask [S, N]; words: uint32-sized workspace of ceil(S / 32) * N elements or None.  Returns the variant that ran."""
+    S, N = mask.shape
+    m = _mask_u8(mask, (S, N), "mask")
+    _require(scale, torch.float32, "scale")
+    if words is not None and words.numel() * words.element_size() < (S + 31) // 32 * N * 4:
+        raise ValueError("outer_scale: words workspace too small")
+    ran = C.c_int(0)
+    _lib.check(_lib.load().af2_outer_scale(m.data_ptr(), scale.data_ptr(), _ptr(words), row0, rows, S, N, float(eps), variant,
+                                           C.byref(ran), _stream_ptr()))
+    return ran.value

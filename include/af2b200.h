@@ -200,6 +200,32 @@ int af2_gemm_bf16_epilogue(const void* A, long long lda, long long a_batch, cons
  * query averages all n values).  dim_head 32 or 64. */
 int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, const unsigned char* mask, void* out, int n,
                        int nbatch, int heads, int dim_head, long long tok_sb, long long tok_si, af2_stream_t stream);
+/* af2_gemm_bf16_f32 with the tile width `bn` (64 / 128 / 256) as given and gathered operands, as the sharded contractions
+ * issue it: a_pr > 0 makes A `a_pr`-row (K-major) or -column (MN-major) pieces `a_piece` elements apart, row / column
+ * r = p * a_pr + rr of piece p; b_pr / b_piece likewise for B.  0 = a plain operand.  K-major A pieces must be a multiple
+ * of 128 rows and B pieces a multiple of 8 rows that divides or is divided by bn; MN-major pieces a multiple of 64 columns. */
+int af2_gemm_bf16_f32_gathered(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,
+                               float* C, long long ldc, long long c_batch, int M, int N, int K, int batch, int mn_major, int bn,
+                               int a_pr, long long a_piece, int b_pr, long long b_piece, af2_stream_t stream);
+/* The tail of the triangle / outer-product contractions: channel-major fp32 src[c * chan_stride + row * pitch + j] (c < d,
+ * row < rows, j < n) -> token-major bf16 y[t][c], t = row * n + j:
+ *   mode 0: y = (LayerNorm_c(src) * gamma + beta) * gate[t][c]      (gate bf16 [tokens][d])
+ *   mode 1: y = src * scale[t]                                       (scale fp32 [tokens], or scale_const when NULL)
+ * variant: 0 the kernel the modules get, 1 SIMT, 2 tile, 3 TMA; a forced kernel whose preconditions the call does not meet
+ * returns AF2_ERR_BAD_ARG and launches nothing.  *ran (may be NULL) receives the kernel launched (0: none, T = 0).
+ * af2_chan_to_token_select returns the kernel variant 0 would launch for these arguments, without launching. */
+int af2_chan_to_token(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode, const float* gamma,
+                      const float* beta, const void* gate, const float* scale, float scale_const, float eps, void* y, int variant,
+                      int* ran, af2_stream_t stream);
+int af2_chan_to_token_select(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode,
+                             const float* gamma, const float* beta, const void* gate, const float* scale, float scale_const,
+                             float eps, void* y);
+/* OuterMean normaliser of pair rows [row0, row0 + rows): scale[(i - row0) * N + j] = 1 / (S * (count_ij + eps)), count_ij =
+ * sum_s (mask[s][i] & mask[s][j]), mask bool [S][N].  words: workspace of ceil(S / 32) * N uint32 for the bit-packed
+ * kernel, or NULL.  variant: 0 the modules' choice (bit-packed when words is given and ceil(S / 32) * N * 4 <= 160 KB),
+ * 1 byte loop, 2 bit-packed (AF2_ERR_BAD_ARG when it does not apply).  *ran (may be NULL) receives the variant launched. */
+int af2_outer_scale(const unsigned char* mask, float* scale, void* words, int row0, int rows, int S, int N, float eps, int variant,
+                    int* ran, af2_stream_t stream);
 
 /* ======================================================================================================================
  * STRICT precision mode (alphafold2_b200.set_precision(model, "strict")): the same modules with fp32 activations between

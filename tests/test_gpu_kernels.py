@@ -12,7 +12,8 @@ GEMM (bf16 operands, fp32 accumulation in the tensor cores, K-term accumulation 
     error of the kernel's approximations (common.cuh): sigmoid ~1e-6 relative, erf-GELU 1.5e-7 absolute on erf, i.e.
     eps_gelu(x) = 1.5e-7 |x| + 1e-6 |gelu(x)|.
   gated:         |out - ref| <= 2^-8 |ref| + |rs| * (|act(g)| E_u + |u| (A' E_g + eps_act(g))),  ref = u act(g) rs
-  fp32 stores:   |out - ref| <= E + 2^-23 |ref| + 2^-24 |resid|  (two fp32 roundings: + bias, + residual)
+  fp32 stores:   |out - ref| <= E + 2^-23 |ref| + 2^-24 |resid|  (two fp32 roundings: + bias, + residual; E + 2^-23 |ref| is
+                 gpu_util.gemm_f32_bound, shared with test_gpu_contractions.py)
   Activations and gates are applied in fp64 in the reference; 2^-8 is the unit roundoff of the bf16 store.  Rows whose row
   scale is 0 must come out exactly 0.  C_GEMM = 1 holds on an H100 80GB HBM3 (700 W power limit): worst err / bound 0.28 on the fp32
   outputs, 0.99 on the bf16 ones, where the rounding term alone reaches ~1 for outputs that round by nearly half an ulp.
@@ -27,12 +28,9 @@ import pytest
 import torch
 
 from conftest import load_golden
-from gpu_util import check_bound
+from gpu_util import C_GEMM, U32 as U, check_bound, gemm_f32_bound
 
 pytestmark = pytest.mark.gpu
-
-C_GEMM = 1.0
-U = 2.0 ** -24
 
 
 def _ops():
@@ -143,15 +141,16 @@ def gemm_case(name, *, M, K, nout, batch, bn, mn_major, mode, act, layout, rowsc
     else:
         w64 = w.double()[:, :nout]
         x = a64 @ w64.transpose(1, 2)
-        e = C_GEMM * K * U * (a64.abs() @ w64.abs().transpose(1, 2))
+        absdot = a64.abs() @ w64.abs().transpose(1, 2)
+        e = C_GEMM * K * U * absdot
         if bias:
             x = x + bvec[:nout].to(dev).double()
         if mode == ops.EPI_RESID_F32:
             ref = x + resid.double()
-            bound = e + 2 * U * ref.abs() + U * resid.double().abs()
+            bound = gemm_f32_bound(absdot, K, ref) + U * resid.double().abs()
         elif mode == ops.EPI_STORE_F32:
             ref = x
-            bound = e + 2 * U * ref.abs()
+            bound = gemm_f32_bound(absdot, K, ref)
         else:
             ref = _act(x, act) * rs64
             bound = 2.0 ** -8 * ref.abs() + rs64.abs() * (ACT_D[act] * e + _act_eps(x, act))
@@ -258,7 +257,7 @@ def _gemm_store_f32(mn_major, M, N, K, batch):
     b = torch.randn(batch, N, K, device="cuda").bfloat16()
     c = ops.gemm_bf16(_operand(a, mn_major), _operand(b, mn_major), mn_major=mn_major)
     ref = a.double() @ b.double().transpose(1, 2)
-    bound = C_GEMM * K * U * (a.double().abs() @ b.double().abs().transpose(1, 2)) + 2 * U * ref.abs()
+    bound = gemm_f32_bound(a.double().abs() @ b.double().abs().transpose(1, 2), K, ref)
     check_bound(f"gemm_f32 {'mn' if mn_major else 'k'} M{M} N{N} K{K} b{batch}", c, ref, bound)
 
 

@@ -58,6 +58,21 @@ class OuterWeightsStrict(C.Structure):
     _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w_lr", vp), ("b_lr", vp), ("w_out", vp), ("b_out", vp)]
 
 
+class TemplateAttnWeights(C.Structure):
+    _fields_ = [("w_q", vp), ("w_gate", vp), ("b_gate", vp), ("w_kv", vp), ("w_out", vp), ("b_out", vp)]
+
+
+class TemplateAttnWeightsStrict(C.Structure):
+    _fields_ = [("w_qg", vp), ("b_qg", vp), ("w_kv", vp), ("w_out", vp), ("b_out", vp)]
+
+
+class TemplateAngleWeights(C.Structure):
+    _fields_ = [("w1", vp), ("b1", vp), ("w2", vp), ("b2", vp)]
+
+
+TemplateAngleWeightsStrict = TemplateAngleWeights      # same layout, split-bf16 weights
+
+
 _SIGNATURES = {
     "af2_last_error": (C.c_char_p, []),
     "af2_abi_version": (ci, []),
@@ -111,6 +126,22 @@ _SIGNATURES = {
     "af2_l2_persist": (ci, [vp, ll, cf, vp]),
     "af2_split_bf16": (ci, [vp, vp, ll, ci, vp]),
     "af2_gemm_split_f32": (ci, [vp, vp, vp, ll, ci, ci, ci, ci, vp]),
+    # template embedder (alphafold2.py:743-792)
+    "af2_template_pointwise_attention": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_template_pointwise_attention_workspace": (ll, [ci, ci, ci, ci, ci, ci]),
+    "af2_template_pointwise_attention_strict": (ci, [C.POINTER(TemplateAttnWeightsStrict), vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, ll,
+                                                     vp]),
+    "af2_template_pointwise_attention_strict_workspace": (ll, [ci, ci, ci, ci, ci, ci]),
+    "af2_template_pointwise_bf16": (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, ll, ci, ci, vp]),
+    "af2_template_pointwise_f32": (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, ll, ci, ci, vp]),
+    "af2_template_embed": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),
+    "af2_template_embed_workspace": (ll, [ll, ci]),
+    "af2_template_embed_strict": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),
+    "af2_template_embed_strict_workspace": (ll, [ll, ci]),
+    "af2_template_angles": (ci, [C.POINTER(TemplateAngleWeights), vp, vp, ci, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_template_angles_workspace": (ll, [ci, ci, ci, ci, ci]),
+    "af2_template_angles_strict": (ci, [C.POINTER(TemplateAngleWeightsStrict), vp, vp, ci, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_template_angles_strict_workspace": (ll, [ci, ci, ci, ci, ci]),
     # peer-memory exchange of the sharded trunk
     "af2_peer_ctrl_bytes": (ci, []),
     "af2_peer_can_access": (ci, [ci, ci]),

@@ -174,8 +174,9 @@ class FeedForward(_Packable):
 # ------------------------------------------------------------------------------------------------------
 # Attention / AxialAttention (alphafold2.py:98-255)
 # ------------------------------------------------------------------------------------------------------
-class Attention(nn.Module):
-    """Parameter container with the reference's layout; the math runs inside AxialAttention's kernel call."""
+class Attention(_Packable):
+    """Parameters with the reference's layout.  Self-attention runs inside AxialAttention's kernel call; the packed weights of
+    this module itself serve the pointwise template attention (Attention with `context`, alphafold2.py:764-777)."""
 
     def __init__(self, dim, seq_len=None, heads=8, dim_head=64, dropout=0., gating=True):
         super().__init__()
@@ -194,10 +195,41 @@ class Attention(nn.Module):
         nn.init.zeros_(self.to_out.weight)           # alphafold2.py:123
         nn.init.zeros_(self.to_out.bias)
 
+    def _pack(self):
+        fn = ops.pack_template_attention_strict if ops.precision_of(self) == "strict" else ops.pack_template_attention
+        return fn(self.to_q.weight, self.to_kv.weight, self.gating.weight, self.gating.bias, self.to_out.weight, self.to_out.bias,
+                  self.dim_head)
+
+    def add_context_(self, x, t, x_mask, t_mask):
+        """x [b, n, n, d] <- x + pooled * Attention(x, context=t, mask=x_mask, context_mask=t_mask) per pair position, in place:
+        the pointwise template attention of alphafold2.py:764-785 (t [b * T, n, n, d], t_mask [b * T, n, n] crossed)."""
+        return ops.template_pointwise_attention_(self.packed(), x, t, x_mask, t_mask, self.heads, self.dim_head)
+
     def forward(self, x, mask=None, attn_bias=None, context=None, context_mask=None, tie_dim=None):
         raise NotImplementedError(
-            "alphafold2_b200.Attention is only executed through AxialAttention (fused sm_90a kernel); "
-            "cross-attention / tied-row attention (templates, extra-MSA stack) are outside the hot path, see DESIGN.md")
+            "alphafold2_b200.Attention runs through AxialAttention (self-attention) or Alphafold2's template branch "
+            "(pointwise attention over the templates, Attention.add_context_); a standalone call is not on the hot path")
+
+
+class _TemplateEmbed(_Packable, nn.Linear):
+    """to_template_embed (alphafold2.py:751): nn.Linear whose packed weight feeds af2_template_embed."""
+
+    def _pack(self):
+        return ops.pack_linear(self.weight, self.bias, strict=ops.precision_of(self) == "strict")
+
+    def embed(self, feats):
+        return ops.template_embed(self.packed(), feats)
+
+
+class _TemplateAngleMLP(_Packable, nn.Sequential):
+    """template_angle_mlp (alphafold2.py:789): Linear -> GELU -> Linear, one C-ABI call writing into rows of m."""
+
+    def _pack(self):
+        return ops.pack_template_angles(self[0].weight, self[0].bias, self[2].weight, self[2].bias,
+                                        strict=ops.precision_of(self) == "strict")
+
+    def write_(self, angles, m, row0):
+        return ops.template_angle_features(self.packed(), angles, m, row0)
 
 
 class AxialAttention(_Packable):
@@ -450,11 +482,11 @@ class Alphafold2(nn.Module):
         self.extra_msa_evoformer = Evoformer(dim=dim, depth=extra_msa_evoformer_layers, seq_len=max_seq_len, heads=heads,
                                              dim_head=dim_head, attn_dropout=attn_dropout, ff_dropout=ff_dropout,
                                              global_column_attn=True)
-        self.to_template_embed = nn.Linear(templates_dim, dim)
+        self.to_template_embed = _TemplateEmbed(templates_dim, dim)
         self.templates_embed_layers = templates_embed_layers
         self.template_pairwise_embedder = PairwiseAttentionBlock(dim=dim, dim_head=dim_head, heads=heads, seq_len=max_seq_len)
         self.template_pointwise_attn = Attention(dim=dim, dim_head=dim_head, heads=heads, dropout=attn_dropout)
-        self.template_angle_mlp = nn.Sequential(nn.Linear(templates_angles_feats_dim, dim), nn.GELU(), nn.Linear(dim, dim))
+        self.template_angle_mlp = _TemplateAngleMLP(nn.Linear(templates_angles_feats_dim, dim), nn.GELU(), nn.Linear(dim, dim))
 
         self.predict_angles = predict_angles
         self.symmetrize_omega = symmetrize_omega
@@ -484,6 +516,47 @@ class Alphafold2(nn.Module):
         self.recycling_distance_buckets = recycling_distance_buckets
         self._warned_training = False
 
+    def _check_templates(self, seq, mask, templates_feats, templates_mask, templates_angles):
+        """The template inputs the reference cannot handle crash it inside einops / torch.cat; here they raise ValueError up
+        front, before any device work."""
+        b, n = seq.shape[:2]
+        if exists(templates_feats):
+            if not exists(mask):
+                raise ValueError("templates_feats needs `mask`: the pointwise template attention masks with the pair mask "
+                                 "(alphafold2.py:767; the reference fails in einops without it)")
+            if not exists(templates_mask):
+                raise ValueError("templates_feats needs templates_mask [b, T, n] (alphafold2.py:752)")
+            if templates_feats.dim() != 5 or templates_feats.shape[0] != b or tuple(templates_feats.shape[2:4]) != (n, n):
+                raise ValueError(f"templates_feats must be [{b}, T, {n}, {n}, templates_dim], got {tuple(templates_feats.shape)}")
+            if tuple(templates_mask.shape) != tuple(templates_feats.shape[:3]):
+                raise ValueError(f"templates_mask must be {tuple(templates_feats.shape[:3])}, got {tuple(templates_mask.shape)}")
+        if exists(templates_angles):
+            if not exists(templates_mask):
+                raise ValueError("templates_angles needs templates_mask [b, T, n]: it is appended to msa_mask (alphafold2.py:792)")
+            if templates_angles.dim() != 4 or templates_angles.shape[0] != b or templates_angles.shape[2] != n:
+                raise ValueError(f"templates_angles must be [{b}, T, {n}, angle_feats], got {tuple(templates_angles.shape)}")
+            if tuple(templates_mask.shape) != tuple(templates_angles.shape[:3]):
+                raise ValueError(f"templates_mask must be {tuple(templates_angles.shape[:3])}, got {tuple(templates_mask.shape)}")
+
+    def template_pair_stack(self, templates_feats, templates_mask):
+        """alphafold2.py:751-760: t = to_template_embed(feats) -> [b * T, n, n, d] fp32, then templates_embed_layers passes of
+        the SAME template_pairwise_embedder (shared weights, no OuterMean) under the crossed mask.  Returns (t, crossed mask)."""
+        b, T, n = templates_feats.shape[:3]
+        tm = templates_mask.bool()
+        tm2 = (tm[:, :, :, None] & tm[:, :, None, :]).reshape(b * T, n, n).contiguous()
+        t = self.to_template_embed.embed(templates_feats.detach().float().contiguous()).reshape(b * T, n, n, -1)
+        for _ in range(self.templates_embed_layers):
+            self.template_pairwise_embedder.update_(t, tm2)
+        return t, tm2
+
+    def embed_templates_(self, x, x_mask, templates_feats, templates_mask):
+        """alphafold2.py:743-785 in place on the fp32 pair tensor x [b, n, n, d]: template pair stack, then the pointwise
+        attention of every pair over its T templates, scaled by `any template valid` and added to x.  Under shard_evoformer
+        every rank computes this whole (it runs before the sharded trunk)."""
+        t, tm2 = self.template_pair_stack(templates_feats, templates_mask)
+        self.template_pointwise_attn.add_context_(x, t, x_mask, tm2)
+        return x
+
     def forward(
         self, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None, seq_index=None,
         seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None, templates_angles=None,
@@ -492,10 +565,10 @@ class Alphafold2(nn.Module):
     ):
         assert not (self.disable_token_embed and not exists(seq_embed)), 'sequence embedding must be supplied if one has disabled token embedding'
         assert not (self.disable_token_embed and not exists(msa_embed)), 'msa embedding must be supplied if one has disabled token embedding'
-        _forward_only(seq_embed, msa_embed, embedds)
-        for name, val in (("templates_feats", templates_feats), ("templates_angles", templates_angles), ("recyclables", recyclables)):
-            if exists(val):
-                raise NotImplementedError(f"{name}: templates / recycling are outside the trunk hot path (SURVEY.md §8f n3 / n4)")
+        _forward_only(seq_embed, msa_embed, embedds, templates_feats, templates_angles)
+        if exists(recyclables):
+            raise NotImplementedError("recyclables: recycling is outside the trunk hot path (SURVEY.md §8f n4)")
+        self._check_templates(seq, mask, templates_feats, templates_mask, templates_angles)
         if self.training and not self._warned_training:
             warnings.warn("alphafold2_b200 is forward-only: running inference semantics (no MLM noising, no autograd)")
             self._warned_training = True
@@ -513,8 +586,10 @@ class Alphafold2(nn.Module):
                 # alphafold2.py:676-726 as fused kernels (SURVEY.md 8f n1): embedding gather, m = emb[msa] + emb[seq], pair init
                 if not exists(msa_mask):
                     msa_mask = torch.ones_like(msa).bool()
+                # with template angles, m gets the T angle rows after the S MSA rows (alphafold2.py:789-790): allocated here at once
+                m_rows = msa.shape[1] + (templates_angles.shape[1] if exists(templates_angles) else 0)
                 x, m = ops.embed_pair_init(seq, msa, self.token_emb.weight, self.to_pairwise_repr.weight, self.to_pairwise_repr.bias,
-                                           self.pos_emb.weight, self.max_rel_dist, seq_embed, msa_embed, seq_index)
+                                           self.pos_emb.weight, self.max_rel_dist, seq_embed, msa_embed, seq_index, m_rows=m_rows)
             else:
                 x = self.token_emb(seq) if not self.disable_token_embed else 0
                 if exists(seq_embed):
@@ -537,7 +612,16 @@ class Alphafold2(nn.Module):
                 rel = (seq_index[None, :, None] - seq_index[None, None, :]).clamp(-self.max_rel_dist, self.max_rel_dist) + self.max_rel_dist
                 x = x + self.pos_emb(rel)
                 x, m = x.float().contiguous(), m.float().contiguous()
+                if exists(templates_angles):
+                    m = torch.cat((m, m.new_empty(m.shape[0], templates_angles.shape[1], *m.shape[2:])), dim=1)
             x_mask = (mask[:, :, None] & mask[:, None, :]) if exists(mask) else None
+
+            if exists(templates_feats):                                # alphafold2.py:743-785
+                self.embed_templates_(x, x_mask, templates_feats, templates_mask)
+            if exists(templates_angles):                               # alphafold2.py:787-792
+                S = m.shape[1] - templates_angles.shape[1]
+                self.template_angle_mlp.write_(templates_angles.detach().float().contiguous(), m, S)
+                msa_mask = torch.cat((msa_mask.bool(), templates_mask.bool()), dim=1)
 
             if exists(extra_msa):
                 # alphafold2.py:789-798, reproduced WITH its quirks (SURVEY.md Q11, do not "fix"): the stack embeds `msa`, not

@@ -19,6 +19,7 @@
 #include "simt_kernels.cuh"
 #include "strict_kernels.cuh"
 #include "glue_kernels.cuh"
+#include "template_attn.cuh"
 
 using namespace af2;
 
@@ -333,7 +334,7 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
     else if (c.mode == EPI_STORE_BF16 && c.layout == LAYOUT_CHANNEL && c.act == ACT_NONE) ek = EK_STORE_CH;
     else if (c.mode == EPI_GATED_BF16 && c.layout == LAYOUT_TOKEN && c.act == ACT_GELU && !c.use_rowscale) ek = EK_GATED_TOK_GELU;
     else if (c.mode == EPI_GATED_BF16 && c.layout == LAYOUT_CHANNEL && c.act == ACT_SIGMOID) ek = EK_GATED_CH_SIG;
-    else if (c.mode == EPI_RESID_F32) ek = EK_RESID_F32;
+    else if (c.mode == EPI_RESID_F32 && !c.use_rowscale) ek = EK_RESID_F32;
     else if (c.mode == EPI_STORE_F32) ek = EK_STORE_F32;
   }
   if (c.mn_major && ek != EK_STORE_F32) ek = EK_GENERIC;
@@ -1467,3 +1468,4 @@ int af2_outer_scale(const unsigned char* mask, float* scale, void* words, int ro
 
 #include "strict_api.inl"
 #include "peer_api.inl"
+#include "template_api.inl"

@@ -439,8 +439,10 @@ def _w32(t: torch.Tensor) -> torch.Tensor:
     return t if (t.dtype == torch.float32 and t.is_contiguous()) else t.to(torch.float32).contiguous()
 
 
-def embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: int, seq_embed=None, msa_embed=None, seq_index=None):
-    """alphafold2.py:676-726 in three fused kernels: returns (x [b,n,n,d], m [b,s,n,d]) fp32."""
+def embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: int, seq_embed=None, msa_embed=None, seq_index=None,
+                    m_rows: Optional[int] = None):
+    """alphafold2.py:676-726 in three fused kernels: returns (x [b,n,n,d], m [b,m_rows,n,d]) fp32.  m_rows > s leaves rows s..
+    m_rows - 1 of m unwritten (the template angle features go there)."""
     if not seq.is_cuda:
         raise RuntimeError("seq must be a CUDA tensor (alphafold2_b200 has no CPU fallback)")
     emb = _w32(token_emb)
@@ -451,13 +453,24 @@ def embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: 
     seq = seq.to(torch.int64).contiguous()
     msa = msa.to(torch.int64).contiguous()
     x = torch.empty(B, n, n, d, dtype=torch.float32, device=seq.device)
-    m = torch.empty(B, S, n, d, dtype=torch.float32, device=seq.device)
+    R = S if m_rows is None else int(m_rows)
+    if R < S:
+        raise ValueError(f"m_rows {R} < {S} MSA rows")
+    m = torch.empty(B, R, n, d, dtype=torch.float32, device=seq.device)
     se = None if seq_embed is None else _w32(seq_embed)
     me = None if msa_embed is None else _w32(msa_embed)
     si = None if seq_index is None else seq_index.to(device=seq.device, dtype=torch.int64).contiguous()
     lib = _lib.load()
     ws = workspace(lib.af2_embed_pair_init_workspace(B, n, d), seq.device)
     wp, bp, pe = _w32(w_pair), _w32(b_pair), _w32(pos_emb)
+    if R != S and B > 1:
+        # the kernels write S contiguous rows per batch element: one call per element into its slice of m
+        for b in range(B):
+            pick = lambda t: None if t is None else t[b]  # noqa: E731
+            _lib.check(lib.af2_embed_pair_init(seq[b].data_ptr(), msa[b].data_ptr(), emb.data_ptr(), emb.shape[0], _ptr(pick(se)),
+                                               _ptr(pick(me)), wp.data_ptr(), bp.data_ptr(), pe.data_ptr(), int(max_rel_dist), _ptr(si),
+                                               x[b].data_ptr(), m[b].data_ptr(), 1, S, n, d, ws.data_ptr(), ws.numel(), _stream_ptr()))
+        return x, m
     _lib.check(lib.af2_embed_pair_init(seq.data_ptr(), msa.data_ptr(), emb.data_ptr(), emb.shape[0], _ptr(se), _ptr(me), wp.data_ptr(),
                                        bp.data_ptr(), pe.data_ptr(), int(max_rel_dist), _ptr(si), x.data_ptr(), m.data_ptr(), B, S, n, d,
                                        ws.data_ptr(), ws.numel(), _stream_ptr()))
@@ -669,3 +682,151 @@ def outer_scale(mask: torch.Tensor, scale: torch.Tensor, *, row0: int, rows: int
     _lib.check(_lib.load().af2_outer_scale(m.data_ptr(), scale.data_ptr(), _ptr(words), row0, rows, S, N, float(eps), variant,
                                            C.byref(ran), _stream_ptr()))
     return ran.value
+
+
+# --------------------------------------------------------------------------------------------------
+# template embedder (alphafold2.py:743-792, SURVEY.md 8f n3)
+# --------------------------------------------------------------------------------------------------
+def _pad_cols(w: torch.Tensor) -> torch.Tensor:
+    """fp32 [rows, K] zero-padded to align8(K) columns: bf16 operand rows must be 16-byte multiples for TMA."""
+    w = w.detach().float()
+    r = (-w.shape[1]) % 8
+    return w if r == 0 else torch.cat([w, torch.zeros(w.shape[0], r, dtype=w.dtype, device=w.device)], 1)
+
+
+def pack_template_attention(wq, wkv, wg, bg, wo, bo, dim_head: int) -> Packed:
+    """Attention(context=...) weights of the pointwise template attention; dim_head^-0.5 * log2(e) folded into to_q."""
+    scale = dim_head ** -0.5 * 1.4426950408889634
+    t = dict(wq=_bf16(wq.detach().float() * scale), wg=_bf16(wg), bg=_f32(bg), wkv=_bf16(wkv), wo=_bf16(wo), bo=_f32(bo))
+    s = _lib.TemplateAttnWeights(*(t[k].data_ptr() for k in ("wq", "wg", "bg", "wkv", "wo", "bo")))
+    return Packed(s, t)
+
+
+def pack_template_attention_strict(wq, wkv, wg, bg, wo, bo, dim_head: int) -> Packed:
+    wqg = torch.cat([wq.detach().float() * dim_head ** -0.5, wg.detach().float()], 0)
+    bqg = torch.cat([torch.zeros(wq.shape[0], device=wq.device), bg.detach().float()], 0)
+    t = dict(wqg=split_weight(wqg), bqg=_f32(bqg), wkv=split_weight(wkv), wo=split_weight(wo), bo=_f32(bo))
+    s = _lib.TemplateAttnWeightsStrict(*(t[k].data_ptr() for k in ("wqg", "bqg", "wkv", "wo", "bo")))
+    return Packed(s, t, "strict")
+
+
+def pack_linear(w, b, strict: bool = False) -> Packed:
+    """nn.Linear for af2_template_embed: bf16 [out, align8(in)] (zero pad columns), or split-bf16 in strict mode."""
+    t = dict(w=split_weight(w) if strict else _bf16(_pad_cols(w)), b=_f32(b))
+    pk = Packed(None, t, "strict" if strict else "bf16")
+    pk.k_in = int(w.shape[1])
+    return pk
+
+
+def pack_template_angles(w1, b1, w2, b2, strict: bool = False) -> Packed:
+    """template_angle_mlp = Linear(K, d) -> GELU -> Linear(d, d); K zero-padded to a multiple of 8."""
+    if strict:
+        t = dict(w1=split_weight(w1), b1=_f32(b1), w2=split_weight(w2), b2=_f32(b2))
+    else:
+        t = dict(w1=_bf16(_pad_cols(w1)), b1=_f32(b1), w2=_bf16(w2), b2=_f32(b2))
+    cls = _lib.TemplateAngleWeightsStrict if strict else _lib.TemplateAngleWeights
+    pk = Packed(cls(*(t[k].data_ptr() for k in ("w1", "b1", "w2", "b2"))), t, "strict" if strict else "bf16")
+    pk.k_in = int(w1.shape[1])
+    return pk
+
+
+def template_embed(pk: Packed, feats: torch.Tensor) -> torch.Tensor:
+    """to_template_embed (alphafold2.py:751): feats [..., K] fp32 -> t [..., d] fp32."""
+    _require(feats, torch.float32, "templates_feats")
+    K = feats.shape[-1]
+    if K != pk.k_in:
+        raise ValueError(f"templates_feats has {K} features, to_template_embed expects {pk.k_in}")
+    d = pk.tensors["w"].shape[0]
+    rows = feats.numel() // K
+    t = torch.empty(*feats.shape[:-1], d, dtype=torch.float32, device=feats.device)
+    lib = _lib.load()
+    if pk.kind == "strict":
+        ws = workspace(lib.af2_template_embed_strict_workspace(rows, K), feats.device)
+        fn = lib.af2_template_embed_strict
+    else:
+        ws = workspace(lib.af2_template_embed_workspace(rows, K), feats.device)
+        fn = lib.af2_template_embed
+    _lib.check(fn(pk.tensors["w"].data_ptr(), pk.tensors["b"].data_ptr(), feats.data_ptr(), t.data_ptr(), rows, K, d, ws.data_ptr(),
+                  ws.numel(), _stream_ptr()))
+    return t
+
+
+def template_pointwise_attention_(pk: Packed, x: torch.Tensor, t: torch.Tensor, x_mask: Optional[torch.Tensor],
+                                  t_mask: Optional[torch.Tensor], heads: int, dim_head: int) -> torch.Tensor:
+    """x [B, n, n, d] fp32 <- x + pooled * Attention(x, context=t, mask=x_mask, context_mask=t_mask) at every pair position
+    (alphafold2.py:764-785).  t [B * T, n, n, d] fp32 (template-major: row b * T + t), t_mask [B * T, n, n] (the crossed
+    template mask), x_mask [B, n, n] or None; pooled = any template valid at the pair."""
+    _require(x, torch.float32, "x")
+    _require(t, torch.float32, "t")
+    if x.dim() != 4 or x.shape[1] != x.shape[2]:
+        raise ValueError(f"x must be [B, n, n, d], got {tuple(x.shape)}")
+    B, n, _, d = x.shape
+    if t.dim() != 4 or B == 0 or t.shape[0] % B or tuple(t.shape[1:]) != (n, n, d):
+        raise ValueError(f"t must be [B * T, {n}, {n}, {d}], got {tuple(t.shape)}")
+    T = t.shape[0] // B
+    xm = _mask_u8(x_mask, (B, n, n), "x_mask")
+    tm = _mask_u8(t_mask, (B * T, n, n), "t_mask")
+    lib = _lib.load()
+    if pk.kind == "strict":
+        ws = workspace(lib.af2_template_pointwise_attention_strict_workspace(B, T, n, d, heads, dim_head), x.device)
+        fn = lib.af2_template_pointwise_attention_strict
+    else:
+        ws = workspace(lib.af2_template_pointwise_attention_workspace(B, T, n, d, heads, dim_head), x.device)
+        fn = lib.af2_template_pointwise_attention
+    _lib.check(fn(C.byref(pk.struct), x.data_ptr(), t.data_ptr(), _ptr(xm), _ptr(tm), B, T, n, d, heads, dim_head, ws.data_ptr(),
+                  ws.numel(), _stream_ptr()))
+    return x
+
+
+def template_angle_features(pk: Packed, angles: torch.Tensor, m: torch.Tensor, row0: int) -> torch.Tensor:
+    """template_angle_mlp (alphafold2.py:789-790): angles [B, T, n, K] fp32 -> rows row0 .. row0 + T - 1 of m [B, R, n, d] fp32
+    (the reference concatenates them after the S MSA rows: row0 = S).  Returns m."""
+    _require(angles, torch.float32, "templates_angles")
+    _require(m, torch.float32, "m")
+    B, T, n, K = angles.shape
+    if K != pk.k_in:
+        raise ValueError(f"templates_angles has {K} features, template_angle_mlp expects {pk.k_in}")
+    if m.dim() != 4 or m.shape[0] != B or m.shape[2] != n:
+        raise ValueError(f"m must be [{B}, rows, {n}, d], got {tuple(m.shape)}")
+    d, R = m.shape[3], m.shape[1]
+    lib = _lib.load()
+    if pk.kind == "strict":
+        ws = workspace(lib.af2_template_angles_strict_workspace(B, T, n, K, d), m.device)
+        fn = lib.af2_template_angles_strict
+    else:
+        ws = workspace(lib.af2_template_angles_workspace(B, T, n, K, d), m.device)
+        fn = lib.af2_template_angles
+    _lib.check(fn(C.byref(pk.struct), angles.data_ptr(), m.data_ptr(), B, T, n, K, d, R, int(row0), ws.data_ptr(), ws.numel(),
+                  _stream_ptr()))
+    return m
+
+
+def template_pointwise(q: torch.Tensor, gate: torch.Tensor, kv: torch.Tensor, B: int, T: int, heads: int, dim_head: int,
+                       x_mask: Optional[torch.Tensor] = None, t_mask: Optional[torch.Tensor] = None,
+                       out: Optional[torch.Tensor] = None, pooled: Optional[torch.Tensor] = None):
+    """The pointwise template-attention kernel alone (include/af2b200.h, af2_template_pointwise_bf16 / _f32): q, gate [P, I],
+    kv [B * T * pairs, 2I] with P = B * pairs; bf16 operands (q in the log2 domain, gate after the sigmoid) or fp32 operands
+    (the strict instantiation: natural-log domain, gate logits).  x_mask bool [P], t_mask bool [B * T * pairs].
+    out / pooled: caller-given output buffers (flat views of at least P * I / P elements) or None.
+    Returns (out [P, I] in the operand dtype, pooled fp32 [P])."""
+    dt = q.dtype
+    if dt not in (torch.bfloat16, torch.float32):
+        raise TypeError(f"q must be bfloat16 or float32, got {dt}")
+    for t, name in ((q, "q"), (gate, "gate"), (kv, "kv")):
+        _require(t, dt, name)
+    I = heads * dim_head
+    P = q.shape[0]
+    if B <= 0 or P % B or tuple(q.shape) != (P, I) or tuple(gate.shape) != (P, I) or tuple(kv.shape) != (P * T, 2 * I):
+        raise ValueError(f"q / gate must be [P, {I}] and kv [P * T, {2 * I}] with P a multiple of B")
+    xm = _mask_u8(x_mask, (P,), "x_mask")
+    tm = _mask_u8(t_mask, (P * T,), "t_mask")
+    out = torch.empty(P, I, dtype=dt, device=q.device) if out is None else out
+    pooled = torch.empty(P, dtype=torch.float32, device=q.device) if pooled is None else pooled
+    _require(out, dt, "out")
+    _require(pooled, torch.float32, "pooled")
+    if out.numel() < P * I or pooled.numel() < P:
+        raise ValueError("out / pooled too small")
+    fn = _lib.load().af2_template_pointwise_bf16 if dt == torch.bfloat16 else _lib.load().af2_template_pointwise_f32
+    _lib.check(fn(q.data_ptr(), gate.data_ptr(), kv.data_ptr(), _ptr(xm), _ptr(tm), out.data_ptr(), pooled.data_ptr(), B, T, P // B,
+                  heads, dim_head, _stream_ptr()))
+    return out, pooled

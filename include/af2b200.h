@@ -180,7 +180,7 @@ int af2_gemm_bf16_f32(const void* A, long long lda, long long a_batch, const voi
  * out = (u + b_u) * act(g + b_g)), 2 fp32 acc + bias + resid (batch 1 only), 3 fp32 store.  act: 0 none, 1 sigmoid,
  * 2 erf-GELU (applied to the value, or to the gate when gated).  layout: 0 token-major out[b][row][col] (row pitch ld_out),
  * 1 channel-major bf16 out[b][col * ld_out + (row / cm_inner) * cm_pitch + row % cm_inner].  rowscale: fp32 [batch * M]
- * multiplier of every output row when use_rowscale (bf16 modes only).  bias: fp32 per accumulator column (N rounded up
+ * multiplier of every output row when use_rowscale (bf16 modes; mode 2 scales acc + bias before the residual add).  bias: fp32 per accumulator column (N rounded up
  * to even) or NULL.
  * out_cols: valid output columns (0: N, or N / 2 when gated).  out_batch: element stride between batches of out. */
 typedef struct {
@@ -290,6 +290,73 @@ int af2_embed_pair_init(const long long* seq, const long long* msa, const float*
                         long long workspace_bytes, af2_stream_t stream);
 int af2_distogram_head(const float* x, const float* gamma, const float* beta, const float* w, const float* bias, float* out, int B,
                        int n, int d, int buckets, af2_stream_t stream);
+
+/* ---------------- template embedder: alphafold2.py:743-785 (SURVEY.md 8f n3) ---------------------------------------------
+ * The template pair stack is af2_triangle_multiply / af2_axial_attention with batch B * T.  The rest:
+ *
+ * af2_template_pointwise_attention: Attention(x, context = t, mask = x_mask, context_mask = t_mask) at every pair position, in
+ *   place on x [B][n][n][d], multiplied by the pooled mask and added (alphafold2.py:764-785):
+ *     q = to_q(x) * dim_head^-0.5, [k | v] = to_kv(t), no LayerNorm on either side; template t of pair p = (b, i, j) is row
+ *     (b T + t) n^2 + i n + j of t [B T][n][n][d] and of the crossed template mask t_mask [B T][n][n] (NULL: all valid);
+ *     logits where !(x_mask[p] & t_mask[...]) are -FLT_MAX, so a pair masked by x_mask, or with every template masked, gets
+ *     the uniform mean over all T templates;  x[p] += pooled[p] * (to_out(softmax_t(q k_t) v_t * sigmoid(gating(x[p]))) + b_out)
+ *     with pooled[p] = any_t t_mask (NOT x_mask).  x_mask [B][n][n] or NULL.  dim_head / 8 a power of two <= 32 (8..256),
+ *     any heads, any T >= 1, d % 8 == 0.  The strict twin: dim_head / 4 a power of two <= 32, fp32 attention with expf. */
+typedef struct {
+  const void* w_q;                                    /* to_q * dim_head^-0.5 * log2(e)  bf16 [I][d]      */
+  const void* w_gate; const float* b_gate;            /* gating                          bf16 [I][d], [I] */
+  const void* w_kv;                                   /* to_kv                           bf16 [2I][d]     */
+  const void* w_out; const float* b_out;              /* to_out                          bf16 [d][I], [d] */
+} af2_template_attn_weights;
+long long af2_template_pointwise_attention_workspace(int B, int T, int n, int d, int heads, int dim_head);
+int af2_template_pointwise_attention(const af2_template_attn_weights* w, float* x, const float* t, const unsigned char* x_mask,
+                                     const unsigned char* t_mask, int B, int T, int n, int d, int heads, int dim_head,
+                                     void* workspace, long long workspace_bytes, af2_stream_t stream);
+typedef struct {
+  const void* w_qg; const float* b_qg;                /* [to_q * dim_head^-0.5 ; gating] split [2I][3][align8(d)], fp32 [2I] (zeros | gating.bias) */
+  const void* w_kv;                                   /* to_kv split [2I][3][align8(d)]                                        */
+  const void* w_out; const float* b_out;              /* to_out split [d][3][align8(I)], fp32 [d]                              */
+} af2_template_attn_weights_strict;
+long long af2_template_pointwise_attention_strict_workspace(int B, int T, int n, int d, int heads, int dim_head);
+int af2_template_pointwise_attention_strict(const af2_template_attn_weights_strict* w, float* x, const float* t,
+                                            const unsigned char* x_mask, const unsigned char* t_mask, int B, int T, int n, int d,
+                                            int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
+/* The pointwise kernel alone, on P = B * pairs pair positions:  out[p] = gate[p] * sum_t softmax_t(q[p] . k) v,  k | v = kv row
+ * (b T + t) * pairs + (p % pairs), kv [B T pairs][2I] (k | v); pooled fp32 [P] = any_t t_mask; masks as above (t_mask indexed
+ * like the kv rows).  _bf16: q [P][I] pre-scaled by dim_head^-0.5 * log2(e) (exp2-domain softmax), gate [P][I] with the sigmoid
+ * applied, out bf16 [P][I].  _f32 (the strict instantiation): q pre-scaled by dim_head^-0.5, gate_logits BEFORE the sigmoid,
+ * out fp32.  q, gate, kv and out 16-byte aligned.  A shape the kernel does not support returns AF2_ERR_BAD_ARG and launches
+ * nothing. */
+int af2_template_pointwise_bf16(const void* q, const void* gate, const void* kv, const unsigned char* x_mask,
+                                const unsigned char* t_mask, void* out, float* pooled, int B, int T, long long pairs, int heads,
+                                int dim_head, af2_stream_t stream);
+int af2_template_pointwise_f32(const float* q, const float* gate_logits, const float* kv, const unsigned char* x_mask,
+                               const unsigned char* t_mask, float* out, float* pooled, int B, int T, long long pairs, int heads,
+                               int dim_head, af2_stream_t stream);
+/* to_template_embed (alphafold2.py:751): t fp32 [rows][d] = feats fp32 [rows][K] W^T + bias.  w bf16 [d][align8(K)] (zero pad
+ * columns); _strict: w split [d][3][align8(K)]. */
+long long af2_template_embed_workspace(long long rows, int K);
+int af2_template_embed(const void* w, const float* bias, const float* feats, float* t, long long rows, int K, int d, void* workspace,
+                       long long workspace_bytes, af2_stream_t stream);
+long long af2_template_embed_strict_workspace(long long rows, int K);
+int af2_template_embed_strict(const void* w_split, const float* bias, const float* feats, float* t, long long rows, int K, int d,
+                              void* workspace, long long workspace_bytes, af2_stream_t stream);
+/* template_angle_mlp (alphafold2.py:789-792): Linear(K -> d), exact-erf GELU, Linear(d -> d) of angles fp32 [B][T][n][K], written
+ * as fp32 rows row0 .. row0 + T - 1 of m [B][m_rows][n][d] (the reference appends them after the S MSA rows: row0 = S). */
+typedef struct {
+  const void* w1; const float* b1;                    /* template_angle_mlp.0  bf16 [d][align8(K)] (zero pad columns), [d] */
+  const void* w2; const float* b2;                    /* template_angle_mlp.2  bf16 [d][d], [d]                            */
+} af2_template_angle_weights;
+long long af2_template_angles_workspace(int B, int T, int n, int K, int d);
+int af2_template_angles(const af2_template_angle_weights* w, const float* angles, float* m, int B, int T, int n, int K, int d,
+                        int m_rows, int row0, void* workspace, long long workspace_bytes, af2_stream_t stream);
+typedef struct {
+  const void* w1; const float* b1;                    /* split [d][3][align8(K)], fp32 [d] */
+  const void* w2; const float* b2;                    /* split [d][3][align8(d)], fp32 [d] */
+} af2_template_angle_weights_strict;
+long long af2_template_angles_strict_workspace(int B, int T, int n, int K, int d);
+int af2_template_angles_strict(const af2_template_angle_weights_strict* w, const float* angles, float* m, int B, int T, int n, int K,
+                               int d, int m_rows, int row0, void* workspace, long long workspace_bytes, af2_stream_t stream);
 
 /* L2 residency hint for the fp32 pair stream: every kernel launched on `stream` afterwards treats [ptr, ptr + bytes) as
  * persisting in L2 (cudaAccessPolicyWindow; clipped to the device's set-aside / window limits).  ptr == NULL clears it. */

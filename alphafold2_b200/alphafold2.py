@@ -557,6 +557,38 @@ class Alphafold2(nn.Module):
         self.template_pointwise_attn.add_context_(x, t, x_mask, tm2)
         return x
 
+    def _check_recyclables(self, b, n, device, recyclables):
+        """Duck-typed like the reference (alphafold2.py:730-739 reads three attributes): its Recyclables and ours are both
+        accepted.  Returns (coords, single_msa_repr_row, pairwise_repr); raises before any device work."""
+        fields = ("coords", "single_msa_repr_row", "pairwise_repr")
+        ts = tuple(getattr(recyclables, f, None) for f in fields)
+        if not all(torch.is_tensor(t) for t in ts):
+            raise NotImplementedError(f"recyclables must carry tensors {', '.join(fields)} (alphafold2.py:24-28); "
+                                      f"got {type(recyclables).__name__}")
+        coords, single, pair = ts
+        expect = {"coords": (coords, 3, (b, n)), "single_msa_repr_row": (single, 3, (b, n, self.dim)),
+                  "pairwise_repr": (pair, 4, (b, n, n, self.dim))}
+        for name, (t, rank, lead) in expect.items():
+            if t.dim() != rank or tuple(t.shape[:len(lead)]) != lead or (name == "coords" and t.shape[-1] < 1):
+                want = f"[{b}, {n}, c]" if name == "coords" else str(list(lead))
+                raise ValueError(f"recyclables.{name} must be {want}, got {tuple(t.shape)}")
+            if not torch.is_floating_point(t):
+                raise ValueError(f"recyclables.{name} must be a floating tensor, got {t.dtype}")
+            if t.device != device:
+                raise ValueError(f"recyclables.{name} is on {t.device}, seq on {device}")
+        return ts
+
+    def embed_recyclables_(self, x, m, recyclables):
+        """alphafold2.py:730-739 in place on the fp32 pair tensor x [b, n, n, d] and row 0 of m [b, rows, n, d], one kernel:
+        x += LN(pairwise_repr), then += recycling_distance_embed[bucket(|coords_i - coords_j|)]; m[:, 0] += LN(single_msa_repr_row).
+        Masks do not gate it (as in the reference).  Under shard_evoformer every rank computes it whole (it runs before the trunk)."""
+        ts = self._check_recyclables(x.shape[0], x.shape[1], x.device, recyclables)
+        coords, single, pair = (t.detach().to(torch.float32).contiguous() for t in ts)
+        ops.recycle_embed_(x, m, coords, single, pair, self.recycling_msa_norm.weight, self.recycling_msa_norm.bias,
+                           self.recycling_pairwise_norm.weight, self.recycling_pairwise_norm.bias,
+                           self.recycling_distance_embed.weight, eps=self.recycling_pairwise_norm.eps)
+        return x, m
+
     def forward(
         self, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None, seq_index=None,
         seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None, templates_angles=None,
@@ -567,7 +599,7 @@ class Alphafold2(nn.Module):
         assert not (self.disable_token_embed and not exists(msa_embed)), 'msa embedding must be supplied if one has disabled token embedding'
         _forward_only(seq_embed, msa_embed, embedds, templates_feats, templates_angles)
         if exists(recyclables):
-            raise NotImplementedError("recyclables: recycling is outside the trunk hot path (SURVEY.md §8f n4)")
+            _forward_only(*self._check_recyclables(seq.shape[0], seq.shape[1], seq.device, recyclables))
         self._check_templates(seq, mask, templates_feats, templates_mask, templates_angles)
         if self.training and not self._warned_training:
             warnings.warn("alphafold2_b200 is forward-only: running inference semantics (no MLM noising, no autograd)")
@@ -616,6 +648,8 @@ class Alphafold2(nn.Module):
                     m = torch.cat((m, m.new_empty(m.shape[0], templates_angles.shape[1], *m.shape[2:])), dim=1)
             x_mask = (mask[:, :, None] & mask[:, None, :]) if exists(mask) else None
 
+            if exists(recyclables):                                    # alphafold2.py:730-739, before the templates read x
+                self.embed_recyclables_(x, m, recyclables)
             if exists(templates_feats):                                # alphafold2.py:743-785
                 self.embed_templates_(x, x_mask, templates_feats, templates_mask)
             if exists(templates_angles):                               # alphafold2.py:787-792

@@ -148,4 +148,112 @@ __global__ void __launch_bounds__(256) glue_distogram_kernel(const float* __rest
   }
 }
 
+// recycling embedder (alphafold2.py:730-739), in place, one warp per token of one grid:
+//   pair tokens t < B n^2, t = (b, i, j):  x[t] = (x[t] + LN_pair(p[t])) + table[bucket(|coords[b][i] - coords[b][j]|)]
+//   MSA-row tokens (b, j) after them:      m[b][0][j] = m[b][0][j] + LN_msa(s[b][j])   (m's batch stride m_bstride elements)
+// LayerNorm is fp32 and two-pass (mean, then the centred biased variance), 1 / sqrtf (IEEE).  The distance is the direct one:
+// coordinate differences in fp32, squares summed by fmaf over the c coordinates in order, IEEE sqrtf.  bucket = lower bound of
+// the distance in bnd[0 .. nb-2] under !(bnd >= v) (torch.bucketize, right=False): NaN -> nb - 1, nb == 1 -> 0.
+// Lane owns the float4 chunks lane, lane + 32, ... (NCH of them, d4 = d / 4 <= 32 NCH); every row 16-byte aligned.
+template <int NCH>
+__device__ __forceinline__ void recycle_ln_row(const float* __restrict__ src, const float* __restrict__ g, const float* __restrict__ be,
+                                               int d, int lane, float eps, float (&y)[4 * NCH]) {
+  const int d4 = d >> 2;
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < NCH; ++k) {
+    const int c4 = lane + 32 * k;
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (c4 < d4) a = __ldcs(reinterpret_cast<const float4*>(src) + c4);
+    y[4 * k] = a.x; y[4 * k + 1] = a.y; y[4 * k + 2] = a.z; y[4 * k + 3] = a.w;
+    s += (a.x + a.y) + (a.z + a.w);
+  }
+  const float mean = warp_sum(s) / static_cast<float>(d);
+  float q = 0.f;
+#pragma unroll
+  for (int k = 0; k < NCH; ++k) {
+    if (lane + 32 * k < d4) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) { const float a = y[4 * k + e] - mean; q = fmaf(a, a, q); }
+    }
+  }
+  const float rstd = 1.0f / sqrtf(warp_sum(q) / static_cast<float>(d) + eps);
+#pragma unroll
+  for (int k = 0; k < NCH; ++k) {
+    const int c4 = lane + 32 * k;
+    if (c4 < d4) {
+      const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + c4), b4 = __ldg(reinterpret_cast<const float4*>(be) + c4);
+      y[4 * k] = fmaf((y[4 * k] - mean) * rstd, g4.x, b4.x);
+      y[4 * k + 1] = fmaf((y[4 * k + 1] - mean) * rstd, g4.y, b4.y);
+      y[4 * k + 2] = fmaf((y[4 * k + 2] - mean) * rstd, g4.z, b4.z);
+      y[4 * k + 3] = fmaf((y[4 * k + 3] - mean) * rstd, g4.w, b4.w);
+    }
+  }
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(256) glue_recycle_kernel(const float* __restrict__ coords, int c, const float* __restrict__ srow,
+                                                           const float* __restrict__ pprev, const float* __restrict__ msa_g,
+                                                           const float* __restrict__ msa_b, const float* __restrict__ pair_g,
+                                                           const float* __restrict__ pair_b, const float* __restrict__ table,
+                                                           const float* __restrict__ bnd, int nb, float* __restrict__ x,
+                                                           float* __restrict__ m, long long m_bstride, int B, int n, int d, float eps) {
+  const int lane = threadIdx.x & 31;
+  const int d4 = d >> 2;
+  const long long warp_global = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const long long nwarps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
+  const long long T1 = static_cast<long long>(B) * n * n;
+  const long long T = T1 + static_cast<long long>(B) * n;
+  float y[4 * NCH];
+  for (long long t = warp_global; t < T; t += nwarps) {
+    if (t < T1) {
+      const int j = static_cast<int>(t % n);
+      const int i = static_cast<int>((t / n) % n);
+      const long long b = t / (static_cast<long long>(n) * n);
+      float4 xv[NCH];
+#pragma unroll
+      for (int k = 0; k < NCH; ++k)
+        if (lane + 32 * k < d4) xv[k] = reinterpret_cast<const float4*>(x + t * d)[lane + 32 * k];
+      recycle_ln_row<NCH>(pprev + t * d, pair_g, pair_b, d, lane, eps, y);
+      const float* ci = coords + (b * n + i) * c;
+      const float* cj = coords + (b * n + j) * c;
+      float s2 = 0.f;
+      for (int e = 0; e < c; ++e) { const float dl = __ldg(ci + e) - __ldg(cj + e); s2 = fmaf(dl, dl, s2); }
+      const float dist = sqrtf(s2);
+      int lo = 0, hi = nb - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (!(__ldg(bnd + mid) >= dist)) lo = mid + 1; else hi = mid;
+      }
+      const float4* er = reinterpret_cast<const float4*>(table + static_cast<long long>(lo) * d);
+#pragma unroll
+      for (int k = 0; k < NCH; ++k) {
+        const int c4 = lane + 32 * k;
+        if (c4 < d4) {
+          const float4 e4 = __ldg(er + c4);
+          float4 o;
+          o.x = (xv[k].x + y[4 * k]) + e4.x; o.y = (xv[k].y + y[4 * k + 1]) + e4.y;
+          o.z = (xv[k].z + y[4 * k + 2]) + e4.z; o.w = (xv[k].w + y[4 * k + 3]) + e4.w;
+          reinterpret_cast<float4*>(x + t * d)[c4] = o;
+        }
+      }
+    } else {
+      const long long r = t - T1;                  // (b, j)
+      const long long b = r / n;
+      const int j = static_cast<int>(r - b * n);
+      recycle_ln_row<NCH>(srow + r * d, msa_g, msa_b, d, lane, eps, y);
+      float4* mr = reinterpret_cast<float4*>(m + b * m_bstride + static_cast<long long>(j) * d);
+#pragma unroll
+      for (int k = 0; k < NCH; ++k) {
+        const int c4 = lane + 32 * k;
+        if (c4 < d4) {
+          float4 o = mr[c4];
+          o.x += y[4 * k]; o.y += y[4 * k + 1]; o.z += y[4 * k + 2]; o.w += y[4 * k + 3];
+          mr[c4] = o;
+        }
+      }
+    }
+  }
+}
+
 }  // namespace af2

@@ -493,6 +493,55 @@ def distogram_head(x, ln_w, ln_b, w, b) -> torch.Tensor:
     return out
 
 
+_RECYCLE_BOUNDARIES: Dict[tuple, torch.Tensor] = {}
+
+
+def recycling_boundaries(nb: int, device) -> torch.Tensor:
+    """torch.linspace(2, 20, steps=nb) on `device` (alphafold2.py:736), cached per (nb, device): built by the same torch call as
+    the reference's, so the bucket edges are bitwise its own.  The kernel searches the first nb - 1 of them."""
+    device = torch.device(device)
+    key = (int(nb), device)
+    t = _RECYCLE_BOUNDARIES.get(key)
+    if t is None:
+        t = torch.linspace(2, 20, steps=int(nb), device=device, dtype=torch.float32)
+        _RECYCLE_BOUNDARIES[key] = t
+    return t
+
+
+def recycle_embed_(x, m, coords, single_row, prev_pair, msa_gamma, msa_beta, pair_gamma, pair_beta, table, eps: float = 1e-5,
+                   boundaries: Optional[torch.Tensor] = None):
+    """alphafold2.py:730-739 in one kernel, in place: x [b,n,n,d] += LN_pair(prev_pair), then += table[bucket(dist)]; row 0 of
+    m [b,rows,n,d] += LN_msa(single_row).  coords [b,n,c], single_row [b,n,d], prev_pair [b,n,n,d]; every tensor fp32 on x's
+    device.  `boundaries` defaults to recycling_boundaries(table rows)."""
+    _require(x, torch.float32, "x")
+    _require(m, torch.float32, "m")
+    B, n, _, d = x.shape
+    if m.dim() != 4 or m.shape[0] != B or m.shape[2] != n or m.shape[3] != d or m.shape[1] < 1:
+        raise ValueError(f"m must be [{B}, rows, {n}, {d}], got {tuple(m.shape)}")
+    nb = table.shape[0]
+    bnd = recycling_boundaries(nb, x.device) if boundaries is None else boundaries
+    ts = {"coords": coords, "single_row": single_row, "prev_pair": prev_pair, "msa_gamma": msa_gamma, "msa_beta": msa_beta,
+          "pair_gamma": pair_gamma, "pair_beta": pair_beta, "table": table, "boundaries": bnd}
+    ts = {k: _w32(v) for k, v in ts.items()}
+    for k, v in ts.items():
+        _require(v, torch.float32, k)
+        if v.device != x.device:
+            raise ValueError(f"{k} is on {v.device}, x on {x.device}")
+    if ts["boundaries"].numel() < nb:
+        raise ValueError(f"boundaries must hold {nb} values, got {ts['boundaries'].numel()}")
+    c = ts["coords"].shape[-1]
+    want = {"coords": (B, n, c), "single_row": (B, n, d), "prev_pair": (B, n, n, d), "msa_gamma": (d,), "msa_beta": (d,),
+            "pair_gamma": (d,), "pair_beta": (d,), "table": (nb, d)}
+    for k, shape in want.items():
+        if tuple(ts[k].shape) != shape:
+            raise ValueError(f"{k} must be {shape}, got {tuple(ts[k].shape)}")
+    _lib.check(_lib.load().af2_recycle_embed(
+        ts["coords"].data_ptr(), c, ts["single_row"].data_ptr(), ts["prev_pair"].data_ptr(), ts["msa_gamma"].data_ptr(),
+        ts["msa_beta"].data_ptr(), ts["pair_gamma"].data_ptr(), ts["pair_beta"].data_ptr(), ts["table"].data_ptr(),
+        ts["boundaries"].data_ptr(), nb, x.data_ptr(), m.data_ptr(), m.stride(0), B, n, d, float(eps), _stream_ptr()))
+    return x, m
+
+
 # --------------------------------------------------------------------------------------------------
 # building blocks exported for the parity tests
 # --------------------------------------------------------------------------------------------------

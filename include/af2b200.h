@@ -290,6 +290,20 @@ int af2_embed_pair_init(const long long* seq, const long long* msa, const float*
                         long long workspace_bytes, af2_stream_t stream);
 int af2_distogram_head(const float* x, const float* gamma, const float* beta, const float* w, const float* bias, float* out, int B,
                        int n, int d, int buckets, af2_stream_t stream);
+/* af2_recycle_embed: alphafold2.py:730-739 -- the recycling embedder, in place, one launch:
+ *   x[b][i][j] = (x[b][i][j] + LN_pair(prev_pair[b][i][j])) + table[k(b, i, j)]        x, prev_pair [B][n][n][d]
+ *   m[b][0][j] = m[b][0][j] + LN_msa(single_row[b][j])                                 single_row [B][n][d]; no other row of m changes
+ *   k = lower bound of dist in boundaries[0 .. nb-2] under !(boundary >= dist), i.e. torch.bucketize(right=False): NaN -> nb - 1,
+ *   and nb == 1 -> 0.  dist = sqrtf(sum_e (coords[b][i][e] - coords[b][j][e])^2) over coords [B][n][c] fp32, summed in order
+ *   (the direct distance; torch.cdist switches to a less exact formula for n > 25).  boundaries [nb] as built by the caller
+ *   (torch.linspace(2, 20, nb)); table [nb][d]; LayerNorm fp32, two-pass, biased variance, eps.
+ *   m is addressed as m + b * m_bstride + j * d (elements): m may hold more rows than the S MSA rows (template angles).
+ *   Rows (x, m, prev_pair, single_row, table, gammas, betas) 16-byte aligned, d % 4 == 0, d <= 1024, c >= 1, nb >= 1; otherwise
+ *   AF2_ERR_BAD_ARG and nothing is launched.  All fp32: strict mode uses the same kernel. */
+int af2_recycle_embed(const float* coords, int c, const float* single_row, const float* prev_pair, const float* msa_gamma,
+                      const float* msa_beta, const float* pair_gamma, const float* pair_beta, const float* table,
+                      const float* boundaries, int nb, float* x, float* m, long long m_bstride, int B, int n, int d, float eps,
+                      af2_stream_t stream);
 
 /* ---------------- template embedder: alphafold2.py:743-785 (SURVEY.md 8f n3) ---------------------------------------------
  * The template pair stack is af2_triangle_multiply / af2_axial_attention with batch B * T.  The rest:

@@ -480,7 +480,6 @@ int launch_chan_to_token_tma(const ChanLnParams& p, long long T, cudaStream_t s)
 }
 
 int g_c2t_tma = 1;   // 0: tile-per-CTA kernel (AF2_C2T_TMA=0)
-int g_attn_headmajor = 0;  // EXPERIMENT: attention reads a head-major copy of q|k|v (AF2_ATTN_HEADMAJOR=1)
 int g_gather_fused = 1;   // 1: contractions over all-gathered operand pieces in ONE launch (AF2_GATHER_FUSED=0: one launch per piece)
 
 // channel -> token kernels (af2_chan_to_token numbers them the same way)
@@ -565,7 +564,8 @@ int launch_chan_to_token(const ChanLnParams& p, cudaStream_t s, int variant = C2
 // attention launch (one folded batch group)
 // -------------------------------------------------------------------------------------------------
 template <int DH>
-int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p, cudaStream_t s) {
+int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tg,
+                          const AttnParams& p, cudaStream_t s) {
   using L = AttnSmem<DH>;
   static int configured[MAX_DEVICES] = {0};
   auto kern = attention_tc_kernel<DH>;
@@ -578,52 +578,44 @@ int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CU
   const int nqb = (p.n + 127) / 128;
   const long long items = (long long)nqb * p.heads * p.nbatch;
   if (items <= 0) return AF2_OK;
-  if (items > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "attention: too many work items");
+  const int grid = (int)(items < sm_count() ? items : sm_count());   // persistent: one CTA per SM, items strided over them
+  if (items > 0x7fffffffLL - grid) return fail(AF2_ERR_BAD_ARG, "attention: too many work items");
   const double tokens = (double)p.n * p.nbatch;
   ProfScope ps(s, KC_ATTENTION, 4.0 * tokens * p.n * p.heads * DH,
                tokens * p.heads * DH * 2.0 * 5 + (p.has_bias ? (double)p.heads * p.n * p.n * 2 : 0));
-  CUDA_OK(launch_pdl(kern, dim3((unsigned)items), dim3(ATTN_THREADS), smem, s, tq, tk, tv, tq, tq, tq, p));
+  CUDA_OK(launch_pdl(kern, dim3(grid), dim3(ATTN_THREADS), smem, s, tq, tk, tv, tg, p));
   return AF2_OK;
 }
 
-// qkv: bf16 [tokens, 3I] (q | k | v), token(b', i) = b' * tok_sb + i * tok_si
+// qkv: bf16 [tokens, 3I] (q | k | v), gate: bf16 [tokens, I], token(b', i) = b' * tok_sb + i * tok_si
 int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nbatch, long long tok_sb, long long tok_si,
                      const __nv_bfloat16* bias, int npad, const uint8_t* mask, const __nv_bfloat16* gate,
-                     __nv_bfloat16* out, cudaStream_t s, const __nv_bfloat16* qkv_hm = nullptr, long long hm_tokens = 0) {
+                     __nv_bfloat16* out, cudaStream_t s) {
+  if (dh != 32 && dh != 64) return fail(AF2_ERR_BAD_ARG, "attention: dim_head %d unsupported (32 or 64)", dh);
   const long long I = (long long)heads * dh;
   const long long ld = 3 * I;
-  CUtensorMap tq, tk, tv;
+  CUtensorMap tq, tk, tv, tg;
   unsigned long long dims[4] = {(unsigned long long)dh, (unsigned long long)n, (unsigned long long)heads, (unsigned long long)nbatch};
   unsigned long long str[3] = {(unsigned long long)(tok_si * ld * 2), (unsigned long long)(dh * 2), (unsigned long long)(tok_sb * ld * 2)};
-  if (qkv_hm) {   // head-major q|k|v [3H][hm_tokens][dh] (experiment AF2_ATTN_HEADMAJOR)
-    str[0] = (unsigned long long)(tok_si * dh * 2); str[1] = (unsigned long long)(hm_tokens * dh * 2); str[2] = (unsigned long long)(tok_sb * dh * 2);
-  }
+  unsigned long long gstr[3] = {(unsigned long long)(tok_si * I * 2), (unsigned long long)(dh * 2), (unsigned long long)(tok_sb * I * 2)};
   unsigned box[4] = {(unsigned)dh, 128, 1, 1};
   const CUtensorMapSwizzle swz = (dh == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  // A box row is ONE head's slice of a token (dh * 2 bytes); the bytes next to it belong to other heads, which other CTAs
-  // read at other times, so the L2 fill granularity must not exceed the row (256B promotion doubled the DRAM reads).
+  // A box row is ONE head's slice of a token (dh * 2 bytes); the CTAs resident together read all heads of the same tokens
+  // (head-innermost item order).  256B promotion measured no faster than promotion to the row size under that order (one
+  // H100, C2 shapes, tools/time_attention.py), so the L2 fill stays at the row size.
   const CUtensorMapL2promotion promo = (dh == 64) ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_64B;
   const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  if (qkv_hm) {
-    const long long part = (long long)heads * hm_tokens * dh;
-    AF2_TRY(make_tmap(&tq, qkv_hm, 4, dims, str, box, swz, bf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    AF2_TRY(make_tmap(&tk, qkv_hm + part, 4, dims, str, box, swz, bf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    AF2_TRY(make_tmap(&tv, qkv_hm + 2 * part, 4, dims, str, box, swz, bf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-  } else {
-    AF2_TRY(make_tmap(&tq, qkv, 4, dims, str, box, swz, bf, promo));
-    AF2_TRY(make_tmap(&tk, qkv + I, 4, dims, str, box, swz, bf, promo));
-    AF2_TRY(make_tmap(&tv, qkv + 2 * I, 4, dims, str, box, swz, bf, promo));
-  }
+  AF2_TRY(make_tmap(&tq, qkv, 4, dims, str, box, swz, bf, promo));
+  AF2_TRY(make_tmap(&tk, qkv + I, 4, dims, str, box, swz, bf, promo));
+  AF2_TRY(make_tmap(&tv, qkv + 2 * I, 4, dims, str, box, swz, bf, promo));
+  AF2_TRY(make_tmap(&tg, gate, 4, dims, gstr, box, swz, bf, promo));
   if (bias && npad % 2 != 0) return fail(AF2_ERR_BAD_ARG, "attention: bias pitch %d must be even", npad);
-  if (I % 2 != 0) return fail(AF2_ERR_BAD_ARG, "attention: heads * dim_head must be even");
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.n = n; p.heads = heads; p.nbatch = nbatch; p.has_bias = bias != nullptr; p.bias = bias; p.npad = npad;
   p.mask = mask; p.mask_sb = tok_sb; p.mask_si = tok_si;
-  p.gate = gate; p.out = out; p.tok_sb = tok_sb; p.tok_si = tok_si; p.ld_gate = I; p.ld_out = I;
-  if (dh == 64) return launch_attention_inst<64>(tq, tk, tv, p, s);
-  if (dh == 32) return launch_attention_inst<32>(tq, tk, tv, p, s);
-  return fail(AF2_ERR_BAD_ARG, "attention: dim_head %d unsupported (32 or 64)", dh);
+  p.out = out; p.tok_sb = tok_sb; p.tok_si = tok_si; p.ld_out = I;
+  return dh == 64 ? launch_attention_inst<64>(tq, tk, tv, tg, p, s) : launch_attention_inst<32>(tq, tk, tv, tg, p, s);
 }
 
 
@@ -721,7 +713,6 @@ int af2_check_device(void) {
   if (const char* e = getenv("AF2_C2T_TMA")) g_c2t_tma = atoi(e) != 0;
   if (const char* e = getenv("AF2_GATHER_FUSED")) g_gather_fused = atoi(e) != 0;
   if (const char* e = getenv("AF2_PROJ_CTAS")) af2_set_proj_mode(atoi(e));
-  if (const char* e = getenv("AF2_ATTN_HEADMAJOR")) g_attn_headmajor = atoi(e) != 0;
   if (const char* e = getenv("AF2_X_EVICT_LAST")) g_x_evict_last = atoi(e) != 0;
   if (const char* e = getenv("AF2_PDL")) g_pdl = atoi(e) != 0;
   int dev = 0;
@@ -783,7 +774,7 @@ long long af2_axial_attention_workspace(int B, int h, int wdim, int d, int heads
   const long long T = (long long)B * h * wdim, I = (long long)heads * dim_head;
   const int n = row_attn ? wdim : h;
   const long long npad = align_up(n, 8);
-  return align_up(T * d * 2, 256) + 2 * align_up(T * 3 * I * 2, 256) + 2 * align_up(T * I * 2, 256) +
+  return align_up(T * d * 2, 256) + align_up(T * 3 * I * 2, 256) + 2 * align_up(T * I * 2, 256) +
          align_up((long long)B * heads * n * npad * 2, 256) + 1024;
 }
 
@@ -807,7 +798,6 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   __nv_bfloat16* gate = ar.take<__nv_bfloat16>(T * I);
   __nv_bfloat16* og = ar.take<__nv_bfloat16>(T * I);
   __nv_bfloat16* bias = ar.take<__nv_bfloat16>((long long)B * heads * n * npad);
-  __nv_bfloat16* qkv_hm = ar.take<__nv_bfloat16>(T * 3 * I);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "axial_attention: workspace too small");
   if (pre_bias) bias = const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(pre_bias));   // [B][H][n][npad], zero padded
 
@@ -868,17 +858,9 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
       tie_queries_kernel<__nv_bfloat16><<<ew_grid((long long)n * I), 256, 0, s>>>(qkv + t0 * 3 * I, 3 * I, (int)I, n, nb, tok_sb, tok_si);
       CUDA_OK(cudaGetLastError());
     }
-    const long long Tb = (long long)h * wdim;
-    if (g_attn_headmajor && dim_head % 8 == 0) {
-      ProfScope ps(s, KC_MISC, 0.0, 0.0);
-      qkv_to_headmajor_kernel<<<ew_grid(Tb * 3 * I / 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(qkv + t0 * 3 * I),
-                                                                        reinterpret_cast<uint4*>(qkv_hm + t0 * 3 * I), Tb, (int)(3 * I), dim_head);
-      CUDA_OK(cudaGetLastError());
-    }
     AF2_TRY(launch_attention(qkv + t0 * 3 * I, heads, dim_head, n, nb, tok_sb, tok_si,
                              has_bias ? bias + (long long)b * heads * n * npad : nullptr, npad,
-                             mask ? mask + t0 : nullptr, gate + t0 * I, og + t0 * I, s,
-                             (g_attn_headmajor && dim_head % 8 == 0) ? qkv_hm + t0 * 3 * I : nullptr, Tb));
+                             mask ? mask + t0 : nullptr, gate + t0 * I, og + t0 * I, s));
   }
   // 4. to_out + bias + residual
   GemmCall co = linear_call(og, I, w->w_out, I, (int)T, d, (int)I);

@@ -502,20 +502,6 @@ __global__ void __launch_bounds__(256) tie_queries_kernel(T* __restrict__ buf, l
   }
 }
 
-// EXPERIMENT (AF2_ATTN_HEADMAJOR=1): token-major q|k|v [T][3I] -> head-major [3H][T][dh], so that the 128-row K / V / Q boxes
-// of the attention kernel are 16 KB of contiguous memory instead of 128 pieces of 128 B at a 3 KB stride
-__global__ void __launch_bounds__(256) qkv_to_headmajor_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, long long T, int I3, int dh) {
-  const int c8n = I3 >> 3, d8 = dh >> 3;
-  const long long total = T * c8n;
-  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
-       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const long long t = idx / c8n;
-    const int c8 = static_cast<int>(idx - t * c8n);
-    const int hc = c8 / d8, e8 = c8 - hc * d8;
-    out[(static_cast<long long>(hc) * T + t) * d8 + e8] = in[idx];
-  }
-}
-
 // bool mask -> float 0/1 row scale
 __global__ void mask_to_float_kernel(const uint8_t* __restrict__ mask, float* __restrict__ out, long long n) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;

@@ -127,6 +127,18 @@ _SIGNATURES = {
     "af2_l2_persist": (ci, [vp, ll, cf, vp]),
     "af2_split_bf16": (ci, [vp, vp, ll, ci, vp]),
     "af2_gemm_split_f32": (ci, [vp, vp, vp, ll, ci, ci, ci, ci, vp]),
+    "af2_gemm_split_epilogue": (ci, [vp, ll, ll, ll, vp, ll, ll, ll, ci, ci, ci, ci, ci, C.POINTER(GemmEpilogue), vp]),
+    "af2_strict_ln_split": (ci, [vp, vp, vp, vp, ll, ci, vp]),
+    "af2_strict_geglu_split": (ci, [vp, vp, ll, ci, vp]),
+    "af2_strict_gelu_split": (ci, [vp, vp, ll, ci, vp]),
+    "af2_strict_qkv_split": (ci, [vp, vp, vp, vp, ci, ci, ci, ci, ci, ll, ll, vp]),
+    "af2_strict_pair_bias": (ci, [vp, vp, vp, ll, ci, ci, vp]),
+    "af2_strict_softmax_split": (ci, [vp, ll, vp, vp, vp, ci, ci, ci, ci, ll, ll, vp]),
+    "af2_strict_gate_split": (ci, [vp, ll, vp, vp, ci, ci, ci, ci, ci, ll, ll, vp]),
+    "af2_strict_tok2chan_split": (ci, [vp, ll, ci, ci, vp, vp, ci, ci, ci, ll, ll, ll, vp]),
+    "af2_strict_chan_to_token": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, ll, ci, vp, cf, cf, vp, vp]),
+    "af2_tie_queries_f32": (ci, [vp, ll, ci, ci, ci, ll, ll, vp]),
+    "af2_tie_queries_bf16": (ci, [vp, ll, ci, ci, ci, ll, ll, vp]),
     # template embedder (alphafold2.py:743-792)
     "af2_template_pointwise_attention": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
     "af2_template_pointwise_attention_workspace": (ll, [ci, ci, ci, ci, ci, ci]),

@@ -189,7 +189,7 @@ struct GemmCall {
   const float* bias; const float* rowscale; const float* resid; long long ld_resid;
   int cm_inner, cm_pitch;
   int out_cols;           // 0: N (N/2 for GATED); else explicit number of valid output columns
-  // split-bf16 operands (strict precision, GemmParams::nseg): nseg = 3 (2 planes) or 6 (3 planes); a_half / b_half = element stride between planes
+  // split-bf16 operands (strict precision, GemmParams::nseg): nseg = SPL_NSEG (3 planes); a_half / b_half = element stride between planes
   int nseg; long long a_half, b_half;
   // gathered operands (GemmParams::a_pr / b_pr): rows (K-major) or columns (MN-major) per piece, element stride between pieces
   int a_pr, b_pr; long long a_piece, b_piece;
@@ -241,8 +241,9 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
   CUtensorMap ta, tb;
   const int BN = c.bn;
   if (c.nseg > 1) {
-    // rank-4 maps (k | mn, row | k, plane, batch) over split-bf16 operands: 2 planes for nseg 3, 3 planes for nseg 6
-    const unsigned long long npl = c.nseg == 6 ? 3ull : 2ull;
+    // rank-4 maps (k | mn, row | k, plane, batch) over the SPL planes of split-bf16 operands
+    if (c.nseg != SPL_NSEG) return fail(AF2_ERR_BAD_ARG, "gemm: %d split passes (needs %d)", c.nseg, SPL_NSEG);
+    const unsigned long long npl = SPL;
     const unsigned long long ab = (unsigned long long)(c.batch > 1 ? c.a_batch : 0) * 2, bb_ = (unsigned long long)(c.batch > 1 ? c.b_batch : 0) * 2;
     if (!c.mn_major) {
       unsigned long long da[4] = {(unsigned long long)c.K, (unsigned long long)c.M, npl, (unsigned long long)c.batch};
@@ -634,6 +635,16 @@ int ew_grid(long long n) {
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
+// tied queries (alphafold2.py:142-151): q <- mean over the nbatch folded rows / columns, in place in the projection
+// buf [tokens][ld] (its first `cols` columns); T = bf16 (default path) or float (strict mode)
+template <class T>
+int tie_queries(T* buf, long long ld, int cols, int n, int nbatch, long long tok_sb, long long tok_si, cudaStream_t s) {
+  ProfScope ps(s, KC_MISC, 0.0, 0.0);
+  tie_queries_kernel<T><<<ew_grid((long long)n * cols), 256, 0, s>>>(buf, ld, cols, n, nbatch, tok_sb, tok_si);
+  CUDA_OK(cudaGetLastError());
+  return AF2_OK;
+}
+
 int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int row0, int rows, int S, int N, float eps, cudaStream_t s,
                        int variant, int* ran) {
   if (ran) *ran = 0;
@@ -853,11 +864,8 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   const long long tok_sb = row_attn ? wdim : 1, tok_si = row_attn ? 1 : wdim;
   for (int b = 0; b < B; ++b) {
     const long long t0 = (long long)b * h * wdim;
-    if (tied) {   // MSAColumnGlobalAttention-style tied queries (alphafold2.py:142-151): q <- mean over the folded batch
-      ProfScope ps(s, KC_MISC, 0.0, 0.0);
-      tie_queries_kernel<__nv_bfloat16><<<ew_grid((long long)n * I), 256, 0, s>>>(qkv + t0 * 3 * I, 3 * I, (int)I, n, nb, tok_sb, tok_si);
-      CUDA_OK(cudaGetLastError());
-    }
+    // MSAColumnGlobalAttention-style tied queries (alphafold2.py:142-151): q <- mean over the folded batch
+    if (tied) AF2_TRY(tie_queries<__nv_bfloat16>(qkv + t0 * 3 * I, 3 * I, (int)I, n, nb, tok_sb, tok_si, s));
     AF2_TRY(launch_attention(qkv + t0 * 3 * I, heads, dim_head, n, nb, tok_sb, tok_si,
                              has_bias ? bias + (long long)b * heads * n * npad : nullptr, npad,
                              mask ? mask + t0 : nullptr, gate + t0 * I, og + t0 * I, s));

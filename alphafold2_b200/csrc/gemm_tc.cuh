@@ -59,10 +59,9 @@ struct GemmParams {
   long long out_batch_stride;  // elements
   int cm_inner, cm_pitch;      // channel-major: row r -> (r / cm_inner) * cm_pitch + r % cm_inner
   // Split-bf16 (strict precision) operands: every fp32 operand value v is stored as bf16 planes p0 = bf16(v),
-  // p1 = bf16(v - p0) [, p2 = bf16(v - p0 - p1)] (tensor maps of rank 4: k, row, plane, batch) and the k loop makes nseg passes
-  // over K, one per plane pair (A plane, B plane), smallest products first, all into the same fp32 accumulator:
-  //   nseg = 3 (two planes,   ~16 mantissa bits): (0,1) (1,0) (0,0)
-  //   nseg = 6 (three planes,  24 mantissa bits): (0,2) (2,0) (1,1) (0,1) (1,0) (0,0)      <- strict mode
+  // p1 = bf16(v - p0), p2 = bf16(v - p0 - p1) (tensor maps of rank 4: k, row, plane, batch) and the k loop makes nseg = 6
+  // passes over K, one per plane pair (A plane, B plane), smallest products first, all into the same fp32 accumulator:
+  //   (0,2) (2,0) (1,1) (0,1) (1,0) (0,0)     (24 mantissa bits; (1,2) (2,1) (2,2) lie below 2^-24 and are dropped)
   // nseg = 1: plain bf16 operands, rank-3 maps.
   int nseg;
   // Operands gathered from several ranks ("pieces", alphafold2_b200/parallel.py): an all-gather concatenates the per-rank
@@ -205,9 +204,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
           if (nseg > 1) {
             // split operands (rank-4 maps): plane pair of this pass, small cross terms first, p0 x p0 last
-            int ha, hb;
-            if (nseg == 3) { ha = (seg == 1) ? 1 : 0; hb = (seg == 0) ? 1 : 0; }
-            else { ha = (0x021010 >> (4 * (5 - seg))) & 0xf; hb = (0x201100 >> (4 * (5 - seg))) & 0xf; }
+            const int ha = (0x021010 >> (4 * (5 - seg))) & 0xf, hb = (0x201100 >> (4 * (5 - seg))) & 0xf;
             if constexpr (!MN_MAJOR) {
               tma_load_4d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, m0, ha, b);
               tma_load_4d(sb, &tmB, &full_bar[stage], kb * GEMM_BK, nt * BN, hb, b);

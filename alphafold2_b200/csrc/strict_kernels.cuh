@@ -1,6 +1,6 @@
 // SIMT kernels of the STRICT precision mode (alphafold2_b200.set_precision(model, "strict")).
 //
-// Strict mode keeps every activation in fp32 between kernels and feeds the wgmma GEMM (gemm_tc.cuh, GemmParams::nseg = 3)
+// Strict mode keeps every activation in fp32 between kernels and feeds the wgmma GEMM (gemm_tc.cuh, GemmParams::nseg = 6)
 // with SPLIT-bf16 operands: v = p0 + p1 + p2 with p0 = bf16(v), p1 = bf16(v - p0), p2 = bf16(v - p0 - p1) (24 mantissa bits),
 // and the six products p0*p2 + p2*p0 + p1*p1 + p0*p1 + p1*p0 + p0*p0 accumulated in fp32 (everything below 2^-24 relative is
 // dropped), so the trunk output matches the reference's fp32 path inside the north star's rtol 1e-3 / atol 1e-4 band even

@@ -273,10 +273,58 @@ long long af2_outer_mean_strict_workspace(int B, int S, int N, int d);
 int af2_outer_mean_strict(const af2_outer_weights_strict* w, float* x, const float* m, const unsigned char* msa_mask, int B, int S,
                           int N, int d, float eps, void* workspace, long long workspace_bytes, af2_stream_t stream);   /* alphafold2.py:321-351 */
 
-/* building blocks exported for the parity tests of the split-operand GEMM */
+/* building blocks exported for the parity tests: the launches the strict modules make, one entry point per kernel.  A split
+ * operand row holds its 3 bf16 planes `half` elements apart; every SIMT kernel below writes p0 = bf16(v), p1 = bf16(v - p0),
+ * p2 = bf16(v - p0 - p1).  Token-major split rows are [rows][3][align8(cols)] with the pad columns [cols, align8(cols))
+ * zeroed, except where noted.
+ * af2_split_bf16: y split of x fp32 [rows][K] (af2_strict_ln_split without the LayerNorm).
+ * af2_gemm_split_f32: C[b] fp32 [M][ldc] = A[b] B[b]^T on split A [batch][M][3][align8(K)], B [batch][N][3][align8(K)].
+ * af2_gemm_split_epilogue: the split GEMM as the modules issue it.  mn_major = 0: A row m at A + b * a_batch + m * lda,
+ *   plane p at + p * a_half, k contiguous; mn_major = 1: A element (k, m) of plane p at A + b * a_batch + p * a_half + k * lda
+ *   + m; B likewise.  Six tensor-core passes (A plane, B plane) = (0,2) (2,0) (1,1) (0,1) (1,0) (0,0) into one fp32
+ *   accumulator.  epi: bn (64 / 128 / 256) used as given; mode 3 (fp32 store, bias or NULL) or 2 (fp32 acc + bias + resid,
+ *   batch 1) only, act 0, layout 0, no row scale; anything else returns AF2_ERR_BAD_ARG and launches nothing.
+ * af2_strict_ln_split: y split [T][3][align8(d)] = LayerNorm(x) * gamma + beta (eps 1e-5), or x when gamma = beta = NULL.
+ * af2_strict_geglu_split: y split [T][3][align8(hidden)] = a * gelu_erf(g), h fp32 [T][2 * hidden] = (a | g).
+ * af2_strict_gelu_split: y split [rows][3][align8(d)] = gelu_erf(h), h fp32 [rows][d].
+ * af2_strict_qkv_split: from p1 fp32 [tokens][4I] = (q | k | v | gate logits), I = heads * dim_head, token(b', i) =
+ *   (b0 + b') * tok_sb + i * tok_si for the folded batch elements b' < nb: Q, K split [nb * heads][n][3][align8(dim_head)],
+ *   Vt split [nb * heads][dim_head][3][align8(n)].
+ * af2_strict_pair_bias: bias fp32 [heads][T] = x fp32 [T][d] . w_edge fp32 [heads][d].
+ * af2_strict_softmax_split: P split [nb * heads][n][3][align8(n)] = softmax_j(S[r][j] + bias[h][i][j]) of the logits S fp32
+ *   [nb * heads][n][lds]; bias fp32 [heads][n][n] or NULL; mask bool or NULL, key j of folded batch element b' at
+ *   mask[(b0 + b') * mask_sb + j * mask_si]: where !(mask[i] & mask[j]) the logit is replaced by -FLT_MAX.
+ * af2_strict_gate_split: og split rows of the tokens of b' < nb, [tokens][3][align8(I)] = O[(b' heads + h) n + i][e] (row
+ *   pitch ldo) * sigmoid(p1[token][3I + h dim_head + e]).
+ * af2_strict_tok2chan_split: out[c * cs + plane * hs + r * rs + k] = src[t][val_off + c] * sigmoid(src[t][gate_off + c])
+ *   (no gate when gate_off < 0) * mask[t] (mask bool or NULL), t = r * inner + k, src row pitch ld; writes no pad.
+ * af2_strict_chan_to_token: y split [rows * n][3][align8(d)] of src fp32 [c * chan_stride + row * pitch + j]: mode 0
+ *   (LayerNorm_c(src) * gamma + beta) * sigmoid(gate_src[t][gate_off + c]) (row pitch gate_ld), mode 1 src * (scale[t] or
+ *   scale_const when scale is NULL).
+ * af2_tie_queries_f32 / _bf16: buf[(b tok_sb + i tok_si) * ld + c] <- mean over b < nbatch, for i < n and c < cols. */
 int af2_split_bf16(const float* x, void* y_split, long long rows, int K, af2_stream_t stream);
 int af2_gemm_split_f32(const void* A_split, const void* B_split, float* C, long long ldc, int M, int N, int K, int batch,
                        af2_stream_t stream);
+int af2_gemm_split_epilogue(const void* A, long long lda, long long a_half, long long a_batch, const void* Bm, long long ldb,
+                            long long b_half, long long b_batch, int M, int N, int K, int batch, int mn_major,
+                            const af2_gemm_epilogue* epi, af2_stream_t stream);
+int af2_strict_ln_split(const float* x, const float* gamma, const float* beta, void* y, long long T, int d, af2_stream_t stream);
+int af2_strict_geglu_split(const float* h, void* y, long long T, int hidden, af2_stream_t stream);
+int af2_strict_gelu_split(const float* h, void* y, long long rows, int d, af2_stream_t stream);
+int af2_strict_qkv_split(const float* p1, void* Q, void* K, void* Vt, int b0, int nb, int heads, int n, int dim_head,
+                         long long tok_sb, long long tok_si, af2_stream_t stream);
+int af2_strict_pair_bias(const float* x, const float* w_edge, float* bias, long long T, int d, int heads, af2_stream_t stream);
+int af2_strict_softmax_split(const float* S, long long lds, const float* bias, const unsigned char* mask, void* P, int b0, int nb,
+                             int heads, int n, long long mask_sb, long long mask_si, af2_stream_t stream);
+int af2_strict_gate_split(const float* O, long long ldo, const float* p1, void* og, int b0, int nb, int heads, int n, int dim_head,
+                          long long tok_sb, long long tok_si, af2_stream_t stream);
+int af2_strict_tok2chan_split(const float* src, long long ld, int val_off, int gate_off, const unsigned char* mask, void* out, int C,
+                              int rows, int inner, long long cs, long long hs, long long rs, af2_stream_t stream);
+int af2_strict_chan_to_token(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode, const float* gamma,
+                             const float* beta, const float* gate_src, long long gate_ld, int gate_off, const float* scale,
+                             float scale_const, float eps, void* y, af2_stream_t stream);
+int af2_tie_queries_f32(float* buf, long long ld, int cols, int n, int nbatch, long long tok_sb, long long tok_si, af2_stream_t stream);
+int af2_tie_queries_bf16(void* buf, long long ld, int cols, int n, int nbatch, long long tok_sb, long long tok_si, af2_stream_t stream);
 
 /* ---------------- pre- / post-trunk glue as fused kernels (SURVEY.md 8f n1) -------------------------------------------
  * af2_embed_pair_init: alphafold2.py:676-726 -- token embedding gather, m = (emb[msa] + msa_embed) + emb[seq],

@@ -61,6 +61,25 @@ def test_gelu_fast_matches_erf_gelu():
     assert abs(float(_gelu_fast(torch.tensor([20.0], dtype=torch.float64))) - 20.0) < 1e-9
 
 
+def test_split_weight_planes_sum_exactly():
+    """strict-mode weights: bf16 [rows, 3, align8(K)] planes p0 = bf16(w), p1 = bf16(w - p0), p2 = bf16(w - p0 - p1) sum to w
+    exactly in fp64 (24 mantissa bits over three 8-bit planes, |w| >= 2^-110), ties and negatives included; pads are zero."""
+    g = torch.Generator().manual_seed(3)
+    rows, K = 41, 29
+    mant = 1.0 + torch.randint(0, 1 << 23, (rows, K), generator=g).double() / (1 << 23)
+    expo = torch.randint(-100, 100, (rows, K), generator=g).double()
+    w = (torch.where(torch.rand(rows, K, generator=g) < 0.5, -1.0, 1.0) * mant * torch.exp2(expo)).float()
+    w[0, :4] = torch.tensor([1 + 2.0 ** -8, -(1 + 2.0 ** -7 + 2.0 ** -8), 1 + 2.0 ** -8 + 2.0 ** -16 + 2.0 ** -17, 0.0])
+    w[1, :3] = torch.tensor([-(2.0 ** -110) * (2 - 2.0 ** -23), 2.0 ** 127 * (2 - 2.0 ** -8 - 2.0 ** -23), -3.0])
+    s = ops.split_weight(w)
+    P = (K + 7) // 8 * 8
+    assert s.dtype == torch.bfloat16 and tuple(s.shape) == (rows, ops.SPLIT_PLANES, P)
+    p = s.double()
+    assert torch.equal(p[..., 0, :] + p[..., 1, :] + p[..., 2, :], torch.nn.functional.pad(w.double(), (0, P - K)))
+    assert torch.equal(s[..., 0, :K], w.to(torch.bfloat16))
+    assert torch.all(s[..., K:] == 0)
+
+
 def test_ops_refuse_cpu_tensors():
     with pytest.raises(RuntimeError):
         ops._require(torch.zeros(4), torch.float32, "x")

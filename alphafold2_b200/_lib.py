@@ -14,25 +14,22 @@ vp, ll, ci, cf = C.c_void_p, C.c_longlong, C.c_int, C.c_float
 
 
 class FFWeights(C.Structure):
-    _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w1", vp), ("b1", vp), ("w2", vp), ("b2", vp), ("bn", ci),
-                ("w_cat", vp), ("b_cat", vp), ("w_ext", vp)]
+    _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w1", vp), ("b1", vp), ("w2", vp), ("b2", vp), ("bn", ci)]
 
 
 class AttnWeights(C.Structure):
     _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w_qkv", vp), ("w_gate", vp), ("b_gate", vp),
-                ("w_out", vp), ("b_out", vp), ("w_edge", vp), ("w_cat", vp), ("b_cat", vp), ("w_ext", vp)]
+                ("w_out", vp), ("b_out", vp), ("w_edge", vp)]
 
 
 class TriMulWeights(C.Structure):
     _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w_left", vp), ("b_left", vp), ("w_right", vp),
                 ("b_right", vp), ("w_ogate", vp), ("b_ogate", vp), ("on_gamma", vp), ("on_beta", vp),
-                ("w_out", vp), ("b_out", vp), ("bn", ci), ("w_cat", vp), ("b_cat", vp),
-                ("w_ext", vp), ("w_ext_out", vp)]
+                ("w_out", vp), ("b_out", vp), ("bn", ci)]
 
 
 class OuterWeights(C.Structure):
-    _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w_lr", vp), ("b_lr", vp), ("w_out", vp), ("b_out", vp),
-                ("w_cat", vp), ("b_cat", vp), ("w_ext", vp), ("w_ext_out", vp)]
+    _fields_ = [("ln_gamma", vp), ("ln_beta", vp), ("w_lr", vp), ("b_lr", vp), ("w_out", vp), ("b_out", vp)]
 
 
 class GemmEpilogue(C.Structure):
@@ -77,9 +74,6 @@ _SIGNATURES = {
     "af2_last_error": (C.c_char_p, []),
     "af2_abi_version": (ci, []),
     "af2_check_device": (ci, []),
-    "af2_set_proj_mode": (None, [ci]),
-    "af2_debug_proj_trace": (ci, [C.POINTER(C.c_longlong)]),
-    "af2_debug_attn_trace": (ci, [C.POINTER(C.c_longlong)]),
     "af2_launch_count": (C.c_ulonglong, []),
     "af2_profile_enable": (None, [ci]),
     "af2_profile_read": (ll, [ci, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
@@ -124,7 +118,6 @@ _SIGNATURES = {
     "af2_embed_pair_init": (ci, [vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, vp, ll, vp]),
     "af2_distogram_head": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]),
     "af2_recycle_embed": (ci, [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, ll, ci, ci, ci, cf, vp]),
-    "af2_l2_persist": (ci, [vp, ll, cf, vp]),
     "af2_split_bf16": (ci, [vp, vp, ll, ci, vp]),
     "af2_gemm_split_f32": (ci, [vp, vp, vp, ll, ci, ci, ci, ci, vp]),
     "af2_gemm_split_epilogue": (ci, [vp, ll, ll, ll, vp, ll, ll, ll, ci, ci, ci, ci, ci, C.POINTER(GemmEpilogue), vp]),

@@ -430,9 +430,8 @@ class Evoformer(nn.Module):
             xo, mo = _f32c(x), _f32c(m)
             mk = mask.bool().contiguous() if exists(mask) else None
             mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
-            with ops.l2_resident(xo):
-                for layer in self.layers:
-                    layer.update_(xo, mo, mk, mmk)
+            for layer in self.layers:
+                layer.update_(xo, mo, mk, mmk)
         return xo.to(x.dtype), mo.to(m.dtype)
 
     def run_(self, x, m, mask=None, msa_mask=None):
@@ -443,9 +442,8 @@ class Evoformer(nn.Module):
         with torch.no_grad():
             mk = mask.bool().contiguous() if exists(mask) else None
             mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
-            with ops.l2_resident(x):
-                for layer in self.layers:
-                    layer.update_(x, m, mk, mmk)
+            for layer in self.layers:
+                layer.update_(x, m, mk, mmk)
         return x, m
 
 

@@ -15,7 +15,6 @@
 #include "attention_tc.cuh"
 #include "chan2tok_tma.cuh"
 #include "gemm_tc.cuh"
-#include "proj_tc.cuh"
 #include "simt_kernels.cuh"
 #include "strict_kernels.cuh"
 #include "glue_kernels.cuh"
@@ -64,16 +63,7 @@ int sm_count() {
   return n[dev];
 }
 
-// AF2_X_EVICT_LAST=1: accesses to a fp32 residual stream whose size suits the L2 (48..100 MB: the pair tensor at C2) carry an
-// evict_last hint, so most of it stays L2-resident from kernel to kernel (experiment, DESIGN.md)
-int g_x_evict_last = 0;
-inline int x_hint(long long tokens, int d) {
-  const double mb = (double)tokens * d * 4 / 1e6;
-  return (g_x_evict_last && mb >= 48.0 && mb <= 100.0) ? 1 : 0;
-}
-
-// Programmatic dependent launch (common.cuh): AF2_PDL=0 launches without the attribute (then wait / launch_dependents are no-ops)
-int g_pdl = 1;
+// Programmatic dependent launch (common.cuh)
 template <class... KArgs, class... Args>
 cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
   cudaLaunchConfig_t cfg;
@@ -82,7 +72,7 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = g_pdl ? 1 : 0;
+  cfg.attrs = at; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
@@ -319,7 +309,6 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
   memset(&p, 0, sizeof(p));
   p.M = c.M; p.N = c.N; p.K = c.K; p.batch = c.batch; p.nseg = c.nseg > 1 ? c.nseg : 1;
   if (c.nseg <= 1) { p.a_pr = c.a_pr; p.b_pr = c.b_pr; }
-  p.x_evict_last = (c.mode == EPI_RESID_F32) ? x_hint(c.M, c.N) : 0;
   p.num_ntiles = (c.N + BN - 1) / BN;
   p.out_cols = c.out_cols > 0 ? c.out_cols : ((c.mode == EPI_GATED_BF16) ? c.N / 2 : c.N);
   p.rowscale = c.rowscale; p.resid = c.resid; p.ld_resid = c.ld_resid;
@@ -425,7 +414,6 @@ int launch_pair_bias(const float* x, long long T, int d, const float* wb, __nv_b
   if (T <= 0) return AF2_OK;
   PairBiasParams p;
   p.x = x; p.T = T; p.d = d; p.wb = wb; p.bias_out = bias_out; p.heads = heads; p.bias_hs = bias_hs; p.n_inner = n_inner; p.pitch = pitch;
-  p.x_evict_last = x_hint(T, d);
   p.transpose = transpose;
   if (T > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "pair_bias: too many tokens");
   const bool mma = (d == 256 || d == 128);
@@ -480,9 +468,6 @@ int launch_chan_to_token_tma(const ChanLnParams& p, long long T, cudaStream_t s)
   return AF2_OK;
 }
 
-int g_c2t_tma = 1;   // 0: tile-per-CTA kernel (AF2_C2T_TMA=0)
-int g_gather_fused = 1;   // 1: contractions over all-gathered operand pieces in ONE launch (AF2_GATHER_FUSED=0: one launch per piece)
-
 // channel -> token kernels (af2_chan_to_token numbers them the same way)
 enum C2tVariant { C2T_AUTO = 0, C2T_SIMT = 1, C2T_TILE = 2, C2T_TMA = 3 };
 
@@ -506,10 +491,10 @@ bool c2t_variant_ok(const ChanLnParams& p, int v) {
   }
 }
 
-// the kernel launch_chan_to_token runs for this call: the TMA kernel where it applies (unless AF2_C2T_TMA=0), else the tile
-// kernel, else the SIMT kernel; 0 if none can take it
+// the kernel launch_chan_to_token runs for this call: the TMA kernel where it applies, else the tile kernel, else the SIMT
+// kernel; 0 if none can take it
 int c2t_select(const ChanLnParams& p) {
-  if (g_c2t_tma && c2t_variant_ok(p, C2T_TMA)) return C2T_TMA;
+  if (c2t_variant_ok(p, C2T_TMA)) return C2T_TMA;
   if (c2t_variant_ok(p, C2T_TILE)) return C2T_TILE;
   return c2t_variant_ok(p, C2T_SIMT) ? C2T_SIMT : 0;
 }
@@ -619,9 +604,6 @@ int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nba
   return dh == 64 ? launch_attention_inst<64>(tq, tk, tv, tg, p, s) : launch_attention_inst<32>(tq, tk, tv, tg, p, s);
 }
 
-
-#include "proj_launch.inl"
-
 // OuterMean normaliser of pair rows [row0, row0 + rows) of one batch element (quirk Q3): bit-packed kernel when the packed
 // mask fits in shared memory, else the byte-loop kernel
 // variant: 0 the choice above, 1 the byte-loop kernel, 2 the bit-packed pair (needs `words` and the shared-memory fit);
@@ -676,6 +658,80 @@ int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int r
   return AF2_OK;
 }
 
+// -------------------------------------------------------------------------------------------------
+// module stages shared by the whole-module and the stage-level entry points
+// -------------------------------------------------------------------------------------------------
+// TriangleMultiply front of `tokens` tokens of x (a grid of rows x inner): LN(x) -> xn; left / right = (proj + b) * mask *
+// sigmoid(gate + b) -> channel-major Lc, Rc [c][chan_stride] (token t at (t / inner) * pitch + t % inner, pad columns zeroed);
+// sigmoid(out_gate) -> gate [tokens][d].  xn [tokens][d] and maskf [tokens] are workspace.
+int triangle_front(const af2_trimul_weights* w, const float* x, const unsigned char* mask, long long tokens, int inner, int pitch,
+                   int d, __nv_bfloat16* xn, float* maskf, void* Lc, void* Rc, long long chan_stride, void* gate, cudaStream_t s) {
+  LnParams lp;
+  memset(&lp, 0, sizeof(lp));
+  lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
+  AF2_TRY(launch_layernorm(lp, s));
+  if (mask) {
+    { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(tokens), 256, 0, s>>>(mask, maskf, tokens); }
+    CUDA_OK(cudaGetLastError());
+  }
+  if (pitch != inner) {   // pad columns of the channel-major operands are read by TMA as K / MN padding: keep them zero
+    CUDA_OK(cudaMemsetAsync(Lc, 0, (size_t)d * chan_stride * 2, s));
+    CUDA_OK(cudaMemsetAsync(Rc, 0, (size_t)d * chan_stride * 2, s));
+  }
+  const int half = w->bn / 2;
+  const int npk = (d + half - 1) / half * w->bn;
+  for (int side = 0; side < 2; ++side) {
+    GemmCall c = linear_call(xn, d, side ? w->w_right : w->w_left, d, (int)tokens, npk, d);
+    c.bn = w->bn; c.mode = EPI_GATED_BF16; c.act = ACT_SIGMOID; c.layout = LAYOUT_CHANNEL;
+    c.out = side ? Rc : Lc; c.ld_out = chan_stride; c.bias = side ? w->b_right : w->b_left;
+    c.use_rowscale = mask != nullptr; c.rowscale = maskf; c.cm_inner = inner; c.cm_pitch = pitch; c.out_cols = d;
+    AF2_TRY(launch_gemm(c, s));
+  }
+  GemmCall cg = linear_call(xn, d, w->w_ogate, d, (int)tokens, d, d);
+  cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = d; cg.bias = w->b_ogate;
+  return launch_gemm(cg, s);
+}
+
+// OuterMean front of `tokens` MSA tokens of m (a grid of rows x inner): [left | right] = (LN(m) W^T + b) * mask ->
+// channel-major LRc [2d][chan_stride] (layout as in triangle_front).  mn [tokens][d] and maskf [tokens] are workspace.
+int outer_front(const af2_outer_weights* w, const float* m, const unsigned char* msa_mask, long long tokens, int inner, int pitch,
+                int d, __nv_bfloat16* mn, float* maskf, void* LRc, long long chan_stride, cudaStream_t s) {
+  LnParams lp;
+  memset(&lp, 0, sizeof(lp));
+  lp.x = m; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = mn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
+  AF2_TRY(launch_layernorm(lp, s));
+  if (msa_mask) {
+    { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(tokens), 256, 0, s>>>(msa_mask, maskf, tokens); }
+    CUDA_OK(cudaGetLastError());
+  }
+  if (pitch != inner) CUDA_OK(cudaMemsetAsync(LRc, 0, (size_t)2 * d * chan_stride * 2, s));
+  GemmCall c = linear_call(mn, d, w->w_lr, d, (int)tokens, 2 * d, d);
+  c.mode = EPI_STORE_BF16; c.layout = LAYOUT_CHANNEL; c.out = LRc; c.ld_out = chan_stride; c.bias = w->b_lr;
+  c.use_rowscale = msa_mask != nullptr; c.rowscale = maskf; c.cm_inner = inner; c.cm_pitch = pitch;
+  return launch_gemm(c, s);
+}
+
+ChanLnParams chan_ln_params(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode,
+                            const float* gamma, const float* beta, const void* gate, const float* scale,
+                            float scale_const, float eps, void* y) {
+  ChanLnParams p;
+  memset(&p, 0, sizeof(p));
+  p.src = src; p.chan_stride = chan_stride; p.pitch = pitch; p.rows = rows; p.n = n; p.d = d; p.mode = mode;
+  p.gamma = gamma; p.beta = beta; p.gate = static_cast<const __nv_bfloat16*>(gate); p.scale = scale;
+  p.scale_const = scale_const; p.eps = eps; p.y = static_cast<__nv_bfloat16*>(y);
+  return p;
+}
+
+// tail of the triangle / outer-product contractions: channel-major O -> token-major bf16 cp.y (launch_chan_to_token), then
+// x [rows * n][d] += cp.y w_out^T + b_out
+int contract_tail(const ChanLnParams& cp, const void* w_out, const float* b_out, float* x, cudaStream_t s) {
+  AF2_TRY(launch_chan_to_token(cp, s));
+  const int d = cp.d;
+  GemmCall co = linear_call(cp.y, d, w_out, d, (int)((long long)cp.rows * cp.n), d, d);
+  co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = b_out; co.resid = x; co.ld_resid = d;
+  return launch_gemm(co, s);
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -684,7 +740,7 @@ int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int r
 extern "C" {
 
 const char* af2_last_error(void) { return g_err; }
-int af2_abi_version(void) { return 2; }
+int af2_abi_version(void) { return 3; }
 
 unsigned long long af2_launch_count(void) { return g_launches; }
 
@@ -713,19 +769,7 @@ long long af2_profile_read(int cls, double* ms, double* flops, double* bytes) {
   return n;
 }
 
-// debug entry points kept for ABI compatibility: no kernel of this build records a timeline
-int af2_debug_proj_trace(long long*) { return fail(AF2_ERR_BAD_ARG, "no projection trace in this build"); }
-int af2_debug_attn_trace(long long*) { return fail(AF2_ERR_BAD_ARG, "no attention trace in this build"); }
-
-// 0: every LN -> Linear cluster runs as LayerNorm kernel + GEMM; nonzero: on the fused projection kernel
-void af2_set_proj_mode(int ctas) { g_proj_ctas = ctas != 0 ? 2 : 0; }
-
 int af2_check_device(void) {
-  if (const char* e = getenv("AF2_C2T_TMA")) g_c2t_tma = atoi(e) != 0;
-  if (const char* e = getenv("AF2_GATHER_FUSED")) g_gather_fused = atoi(e) != 0;
-  if (const char* e = getenv("AF2_PROJ_CTAS")) af2_set_proj_mode(atoi(e));
-  if (const char* e = getenv("AF2_X_EVICT_LAST")) g_x_evict_last = atoi(e) != 0;
-  if (const char* e = getenv("AF2_PDL")) g_pdl = atoi(e) != 0;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return fail(AF2_ERR_CUDA, "no CUDA device");
   int major = 0;
@@ -756,24 +800,14 @@ int af2_feed_forward(const af2_ff_weights* w, float* x, long long tokens, int d,
   // h = a * gelu(g)
   const int half = w->bn / 2;
   const int n1p = (hidden + half - 1) / half * w->bn;   // packed accumulator columns
-  if (g_proj_ctas > 0 && w->w_cat && w->b_cat && w->bn == 256 && proj_dim_ok(d)) {
-    // fused LayerNorm -> Linear -> GEGLU
-    ProjCall pc;
-    memset(&pc, 0, sizeof(pc));
-    pc.x = x; pc.T = tokens; pc.d = d;
-    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.nseg = 1;
-    pc.seg[0] = ProjOut{n1p / 256, EK_GATED_TOK_GELU, hidden, hbuf, hidden};
-    AF2_TRY(launch_proj(pc, s));
-  } else {
-    LnParams lp;
-    memset(&lp, 0, sizeof(lp));
-    lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
-    AF2_TRY(launch_layernorm(lp, s));
-    GemmCall c1 = linear_call(xn, d, w->w1, d, (int)tokens, n1p, d);
-    c1.bn = w->bn; c1.mode = EPI_GATED_BF16; c1.act = ACT_GELU; c1.layout = LAYOUT_TOKEN;
-    c1.out = hbuf; c1.ld_out = hidden; c1.bias = w->b1; c1.out_cols = hidden;
-    AF2_TRY(launch_gemm(c1, s));
-  }
+  LnParams lp;
+  memset(&lp, 0, sizeof(lp));
+  lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
+  AF2_TRY(launch_layernorm(lp, s));
+  GemmCall c1 = linear_call(xn, d, w->w1, d, (int)tokens, n1p, d);
+  c1.bn = w->bn; c1.mode = EPI_GATED_BF16; c1.act = ACT_GELU; c1.layout = LAYOUT_TOKEN;
+  c1.out = hbuf; c1.ld_out = hidden; c1.bias = w->b1; c1.out_cols = hidden;
+  AF2_TRY(launch_gemm(c1, s));
   GemmCall c2 = linear_call(hbuf, hidden, w->w2, hidden, (int)tokens, d, hidden);
   c2.mode = EPI_RESID_F32; c2.out = x; c2.ld_out = d; c2.bias = w->b2; c2.resid = x; c2.ld_resid = d;
   AF2_TRY(launch_gemm(c2, s));
@@ -813,7 +847,6 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   if (pre_bias) bias = const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(pre_bias));   // [B][H][n][npad], zero padded
 
   // 1. LayerNorm (+ pair bias from the RAW edges; fused when the edges are x itself)
-  const bool fused_proj = g_proj_ctas > 0 && w->w_cat && w->b_cat && proj_dim_ok(d) && (I % 8) == 0;
   LnParams lp;
   memset(&lp, 0, sizeof(lp));
   lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = T; lp.d = d; lp.eps = 1e-5f;
@@ -826,8 +859,7 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   } else if (fuse_bias) {
     lp.wb = w->w_edge; lp.bias_out = bias; lp.heads = heads; lp.bias_hs = (long long)n * npad; lp.n_inner = n; lp.pitch = npad;
   }
-  if (fused_proj) lp.y = nullptr;          // the fused projection normalises x itself
-  if (lp.y || lp.wb) AF2_TRY(launch_layernorm(lp, s));
+  AF2_TRY(launch_layernorm(lp, s));
   if (has_bias && !fuse_bias && !pre_bias && pair_bias_fast_ok(d, heads)) {
     for (int b = 0; b < B; ++b)
       AF2_TRY(launch_pair_bias(edges + (long long)b * n * n * d, (long long)n * n, d, w->w_edge, bias + (long long)b * heads * n * npad,
@@ -843,23 +875,12 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
     }
   }
   // 2. projections
-  if (fused_proj) {
-    // one launch: LayerNorm -> [q | k | v] and sigmoid(gating)
-    ProjCall pc;
-    memset(&pc, 0, sizeof(pc));
-    pc.x = x; pc.T = T; pc.d = d;
-    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.nseg = 2;
-    pc.seg[0] = ProjOut{(int)((3 * I + 255) / 256), EK_STORE_TOK, (int)(3 * I), qkv, 3 * I};
-    pc.seg[1] = ProjOut{(int)((I + 255) / 256), EK_STORE_TOK_SIG, (int)I, gate, I};
-    AF2_TRY(launch_proj(pc, s));
-  } else {
-    GemmCall cq = linear_call(xn, d, w->w_qkv, d, (int)T, (int)(3 * I), d);
-    cq.mode = EPI_STORE_BF16; cq.layout = LAYOUT_TOKEN; cq.out = qkv; cq.ld_out = 3 * I;
-    AF2_TRY(launch_gemm(cq, s));
-    GemmCall cg = linear_call(xn, d, w->w_gate, d, (int)T, (int)I, d);
-    cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = I; cg.bias = w->b_gate;
-    AF2_TRY(launch_gemm(cg, s));
-  }
+  GemmCall cq = linear_call(xn, d, w->w_qkv, d, (int)T, (int)(3 * I), d);
+  cq.mode = EPI_STORE_BF16; cq.layout = LAYOUT_TOKEN; cq.out = qkv; cq.ld_out = 3 * I;
+  AF2_TRY(launch_gemm(cq, s));
+  GemmCall cg = linear_call(xn, d, w->w_gate, d, (int)T, (int)I, d);
+  cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = I; cg.bias = w->b_gate;
+  AF2_TRY(launch_gemm(cg, s));
   // 3. attention per batch element
   const long long tok_sb = row_attn ? wdim : 1, tok_si = row_attn ? 1 : wdim;
   for (int b = 0; b < B; ++b) {
@@ -908,43 +929,7 @@ int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned 
   float* maskf = ar.take<float>(T);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_multiply: workspace too small");
 
-  const bool fused_front = g_proj_ctas > 0 && w->w_cat && w->b_cat && w->bn == 256 && proj_dim_ok(d) && np8 == N;
-  if (fused_front) {
-    ProjCall pc;
-    memset(&pc, 0, sizeof(pc));
-    pc.x = x; pc.T = T; pc.d = d;
-    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = mask; pc.nseg = 3;
-    const int tl = (d + 127) / 128;
-    pc.seg[0] = ProjOut{tl, EK_GATED_CH_SIG, d, Lc, cs_lr};
-    pc.seg[1] = ProjOut{tl, EK_GATED_CH_SIG, d, Rc, cs_lr};
-    pc.seg[2] = ProjOut{(d + 255) / 256, EK_STORE_TOK_SIG, d, gate, (long long)d};
-    AF2_TRY(launch_proj(pc, s));
-  }
-  LnParams lp;
-  memset(&lp, 0, sizeof(lp));
-  lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = T; lp.d = d; lp.eps = 1e-5f;
-  if (!fused_front) AF2_TRY(launch_layernorm(lp, s));
-  if (mask && !fused_front) {
-    { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(T), 256, 0, s>>>(mask, maskf, T); }
-    CUDA_OK(cudaGetLastError());
-  }
-  if (np8 != N) {   // pad columns of the channel-major operands are read by TMA as K / MN padding: keep them zero
-    CUDA_OK(cudaMemsetAsync(Lc, 0, (size_t)d * cs_lr * 2, s));
-    CUDA_OK(cudaMemsetAsync(Rc, 0, (size_t)d * cs_lr * 2, s));
-  }
-  // left / right: (proj + b) * mask * sigmoid(gate + b)  -> channel-major [c][b*N + i][k]
-  const int half = w->bn / 2;
-  const int npk = (d + half - 1) / half * w->bn;
-  for (int side = 0; side < 2 && !fused_front; ++side) {
-    GemmCall c = linear_call(xn, d, side ? w->w_right : w->w_left, d, (int)T, npk, d);
-    c.bn = w->bn; c.mode = EPI_GATED_BF16; c.act = ACT_SIGMOID; c.layout = LAYOUT_CHANNEL;
-    c.out = side ? Rc : Lc; c.ld_out = cs_lr; c.bias = side ? w->b_right : w->b_left;
-    c.use_rowscale = mask != nullptr; c.rowscale = maskf; c.cm_inner = N; c.cm_pitch = np8; c.out_cols = d;
-    AF2_TRY(launch_gemm(c, s));
-  }
-  GemmCall cg = linear_call(xn, d, w->w_ogate, d, (int)T, d, d);
-  cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = d; cg.bias = w->b_ogate;
-  if (!fused_front) AF2_TRY(launch_gemm(cg, s));
+  AF2_TRY(triangle_front(w, x, mask, T, N, np8, d, xn, maskf, Lc, Rc, cs_lr, gate, s));
   // per-channel contraction, batch = channels
   for (int b = 0; b < B; ++b) {
     GemmCall c;
@@ -961,15 +946,8 @@ int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned 
     AF2_TRY(launch_gemm(c, s));
   }
   // LN over channels * out_gate -> token-major bf16
-  ChanLnParams cp;
-  memset(&cp, 0, sizeof(cp));
-  cp.src = Oc; cp.chan_stride = cs_o; cp.pitch = np4; cp.rows = B * N; cp.n = N; cp.d = d; cp.mode = 0;
-  cp.gamma = w->on_gamma; cp.beta = w->on_beta; cp.gate = gate; cp.eps = 1e-5f; cp.y = tn;
-  AF2_TRY(launch_chan_to_token(cp, s));
-  GemmCall co = linear_call(tn, d, w->w_out, d, (int)T, d, d);
-  co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = w->b_out; co.resid = x; co.ld_resid = d;
-  AF2_TRY(launch_gemm(co, s));
-  return AF2_OK;
+  return contract_tail(chan_ln_params(Oc, cs_o, np4, B * N, N, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
+                       w->w_out, w->b_out, x, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1001,32 +979,12 @@ int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const u
   uint32_t* mwords = ar.take<uint32_t>((long long)((S + 31) / 32) * N);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "outer_mean: workspace too small");
 
-  const bool fused_front = g_proj_ctas > 0 && w->w_cat && w->b_cat && proj_dim_ok(d) && np8 == N;
-  LnParams lp;
-  memset(&lp, 0, sizeof(lp));
-  lp.x = m; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = mn; lp.T = Tm; lp.d = d; lp.eps = 1e-5f;
-  if (!fused_front) AF2_TRY(launch_layernorm(lp, s));
-  if (msa_mask) {
-    if (!fused_front) { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(Tm), 256, 0, s>>>(msa_mask, maskf, Tm); }
-    CUDA_OK(cudaGetLastError());
+  // the normaliser goes first: launched between the two GEMMs, its kernels would keep the contraction from starting under
+  // the projection's tail (programmatic dependent launch)
+  if (msa_mask)
     for (int b = 0; b < B; ++b)
       AF2_TRY(launch_outer_scale(msa_mask + (long long)b * S * N, scale + (long long)b * N * N, mwords, 0, N, S, N, eps, s));
-  }
-  if (np8 != N) CUDA_OK(cudaMemsetAsync(LRc, 0, (size_t)2 * d * cs_lr * 2, s));
-  // [left | right] = (LN(m) W^T + b) * mask  -> channel-major [c][b*S + s][i]
-  if (fused_front) {
-    ProjCall pc;
-    memset(&pc, 0, sizeof(pc));
-    pc.x = m; pc.T = Tm; pc.d = d;
-    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = msa_mask; pc.nseg = 1;
-    pc.seg[0] = ProjOut{(2 * d + 255) / 256, EK_STORE_CH, 2 * d, LRc, cs_lr};
-    AF2_TRY(launch_proj(pc, s));
-  } else {
-    GemmCall c = linear_call(mn, d, w->w_lr, d, (int)Tm, 2 * d, d);
-    c.mode = EPI_STORE_BF16; c.layout = LAYOUT_CHANNEL; c.out = LRc; c.ld_out = cs_lr; c.bias = w->b_lr;
-    c.use_rowscale = msa_mask != nullptr; c.rowscale = maskf; c.cm_inner = N; c.cm_pitch = np8;
-    AF2_TRY(launch_gemm(c, s));
-  }
+  AF2_TRY(outer_front(w, m, msa_mask, Tm, N, np8, d, mn, maskf, LRc, cs_lr, s));
   // O_c[i][j] = sum_s L_c[s][i] R_c[s][j]  (MN-major operands, K = S)
   for (int b = 0; b < B; ++b) {
     GemmCall g;
@@ -1037,15 +995,9 @@ int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const u
     g.mode = EPI_STORE_F32; g.layout = LAYOUT_TOKEN; g.out = Oc + (long long)b * N * np4; g.ld_out = np4; g.out_batch = cs_o;
     AF2_TRY(launch_gemm(g, s));
   }
-  ChanLnParams cp;
-  memset(&cp, 0, sizeof(cp));
-  cp.src = Oc; cp.chan_stride = cs_o; cp.pitch = np4; cp.rows = B * N; cp.n = N; cp.d = d; cp.mode = 1;
-  cp.scale = msa_mask ? scale : nullptr; cp.scale_const = 1.0f / (float)S; cp.y = tn;
-  AF2_TRY(launch_chan_to_token(cp, s));
-  GemmCall co = linear_call(tn, d, w->w_out, d, (int)Tx, d, d);
-  co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = w->b_out; co.resid = x; co.ld_resid = d;
-  AF2_TRY(launch_gemm(co, s));
-  return AF2_OK;
+  return contract_tail(chan_ln_params(Oc, cs_o, np4, B * N, N, d, 1, nullptr, nullptr, nullptr, msa_mask ? scale : nullptr,
+                                      1.0f / (float)S, 0.f, tn),
+                       w->w_out, w->b_out, x, s);
 }
 
 
@@ -1109,42 +1061,7 @@ int af2_triangle_project(const af2_trimul_weights* w, const float* x, const unsi
   __nv_bfloat16* xn = ar.take<__nv_bfloat16>(tokens * d);
   float* maskf = ar.take<float>(tokens);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_project: workspace too small");
-  if (g_proj_ctas > 0 && w->w_cat && w->b_cat && w->bn == 256 && proj_dim_ok(d) && pitch == inner) {
-    ProjCall pc;
-    memset(&pc, 0, sizeof(pc));
-    pc.x = x; pc.T = tokens; pc.d = d;
-    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = mask; pc.nseg = 3;
-    const int tl = (d + 127) / 128;
-    pc.seg[0] = ProjOut{tl, EK_GATED_CH_SIG, d, Lc, chan_stride};
-    pc.seg[1] = ProjOut{tl, EK_GATED_CH_SIG, d, Rc, chan_stride};
-    pc.seg[2] = ProjOut{(d + 255) / 256, EK_STORE_TOK_SIG, d, gate, (long long)d};
-    return launch_proj(pc, s);
-  }
-  LnParams lp;
-  memset(&lp, 0, sizeof(lp));
-  lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
-  AF2_TRY(launch_layernorm(lp, s));
-  if (mask) {
-    { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(tokens), 256, 0, s>>>(mask, maskf, tokens); }
-    CUDA_OK(cudaGetLastError());
-  }
-  if (pitch != inner) {
-    CUDA_OK(cudaMemsetAsync(Lc, 0, (size_t)d * chan_stride * 2, s));
-    CUDA_OK(cudaMemsetAsync(Rc, 0, (size_t)d * chan_stride * 2, s));
-  }
-  const int half = w->bn / 2;
-  const int npk = (d + half - 1) / half * w->bn;
-  for (int side = 0; side < 2; ++side) {
-    GemmCall c = linear_call(xn, d, side ? w->w_right : w->w_left, d, (int)tokens, npk, d);
-    c.bn = w->bn; c.mode = EPI_GATED_BF16; c.act = ACT_SIGMOID; c.layout = LAYOUT_CHANNEL;
-    c.out = side ? Rc : Lc; c.ld_out = chan_stride; c.bias = side ? w->b_right : w->b_left;
-    c.use_rowscale = mask != nullptr; c.rowscale = maskf; c.cm_inner = inner; c.cm_pitch = pitch; c.out_cols = d;
-    AF2_TRY(launch_gemm(c, s));
-  }
-  GemmCall cg = linear_call(xn, d, w->w_ogate, d, (int)tokens, d, d);
-  cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = d; cg.bias = w->b_ogate;
-  AF2_TRY(launch_gemm(cg, s));
-  return AF2_OK;
+  return triangle_front(w, x, mask, tokens, inner, pitch, d, xn, maskf, Lc, Rc, chan_stride, gate, s);
 }
 
 long long af2_triangle_contract_workspace(int rows, int cols, int d) {
@@ -1172,7 +1089,7 @@ int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc,
   const __nv_bfloat16* R = static_cast<const __nv_bfloat16*>(Rg);
   // one launch over all gathered pieces when their size tiles the kernel's boxes (rank-4 tensor maps), else one per piece
   bool fused_pieces = false;
-  if (pieces > 1 && g_gather_fused) {
+  if (pieces > 1) {
     GemmCall c;
     memset(&c, 0, sizeof(c));
     c.batch = d; c.K = K; c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.ld_out = cp4; c.out_batch = cs_o; c.out = Oc;
@@ -1214,15 +1131,8 @@ int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc,
     }
     AF2_TRY(launch_gemm(c, s));
   }
-  ChanLnParams cp;
-  memset(&cp, 0, sizeof(cp));
-  cp.src = Oc; cp.chan_stride = cs_o; cp.pitch = cp4; cp.rows = rows; cp.n = cols; cp.d = d; cp.mode = 0;
-  cp.gamma = w->on_gamma; cp.beta = w->on_beta; cp.gate = static_cast<const __nv_bfloat16*>(gate); cp.eps = 1e-5f; cp.y = tn;
-  AF2_TRY(launch_chan_to_token(cp, s));
-  GemmCall co = linear_call(tn, d, w->w_out, d, (int)T, d, d);
-  co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = w->b_out; co.resid = x; co.ld_resid = d;
-  AF2_TRY(launch_gemm(co, s));
-  return AF2_OK;
+  return contract_tail(chan_ln_params(Oc, cs_o, cp4, rows, cols, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
+                       w->w_out, w->b_out, x, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1245,28 +1155,7 @@ int af2_outer_project(const af2_outer_weights* w, const float* m, const unsigned
   __nv_bfloat16* mn = ar.take<__nv_bfloat16>(tokens * d);
   float* maskf = ar.take<float>(tokens);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "outer_project: workspace too small");
-  if (g_proj_ctas > 0 && w->w_cat && w->b_cat && proj_dim_ok(d) && pitch == inner) {
-    ProjCall pc;
-    memset(&pc, 0, sizeof(pc));
-    pc.x = m; pc.T = tokens; pc.d = d;
-    pc.w_cat = w->w_cat; pc.b_cat = w->b_cat; pc.rowmask = msa_mask; pc.nseg = 1;
-    pc.seg[0] = ProjOut{(2 * d + 255) / 256, EK_STORE_CH, 2 * d, LRc, chan_stride};
-    return launch_proj(pc, s);
-  }
-  LnParams lp;
-  memset(&lp, 0, sizeof(lp));
-  lp.x = m; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = mn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
-  AF2_TRY(launch_layernorm(lp, s));
-  if (msa_mask) {
-    { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(tokens), 256, 0, s>>>(msa_mask, maskf, tokens); }
-    CUDA_OK(cudaGetLastError());
-  }
-  if (pitch != inner) CUDA_OK(cudaMemsetAsync(LRc, 0, (size_t)2 * d * chan_stride * 2, s));
-  GemmCall c = linear_call(mn, d, w->w_lr, d, (int)tokens, 2 * d, d);
-  c.mode = EPI_STORE_BF16; c.layout = LAYOUT_CHANNEL; c.out = LRc; c.ld_out = chan_stride; c.bias = w->b_lr;
-  c.use_rowscale = msa_mask != nullptr; c.rowscale = maskf; c.cm_inner = inner; c.cm_pitch = pitch;
-  AF2_TRY(launch_gemm(c, s));
-  return AF2_OK;
+  return outer_front(w, m, msa_mask, tokens, inner, pitch, d, mn, maskf, LRc, chan_stride, s);
 }
 
 long long af2_outer_contract_workspace(int rows, int N, int d) {
@@ -1296,7 +1185,7 @@ int af2_outer_contract(const af2_outer_weights* w, float* x, const void* Lc, lon
   const __nv_bfloat16* L = static_cast<const __nv_bfloat16*>(Lc);
   const __nv_bfloat16* R = static_cast<const __nv_bfloat16*>(Rg);
   const int pc = N / pieces;
-  const bool fused_pieces = pieces > 1 && g_gather_fused && pc % 64 == 0;
+  const bool fused_pieces = pieces > 1 && pc % 64 == 0;
   if (fused_pieces) {   // one launch: B columns j = p * pc + jj addressed through a rank-4 map over the gathered pieces
     GemmCall g;
     memset(&g, 0, sizeof(g));
@@ -1315,15 +1204,9 @@ int af2_outer_contract(const af2_outer_weights* w, float* x, const void* Lc, lon
     g.mode = EPI_STORE_F32; g.layout = LAYOUT_TOKEN; g.out = Oc + (long long)p * pc; g.ld_out = np4; g.out_batch = cs_o;
     AF2_TRY(launch_gemm(g, s));
   }
-  ChanLnParams cp;
-  memset(&cp, 0, sizeof(cp));
-  cp.src = Oc; cp.chan_stride = cs_o; cp.pitch = np4; cp.rows = rows; cp.n = N; cp.d = d; cp.mode = 1;
-  cp.scale = msa_mask_full ? scale : nullptr; cp.scale_const = 1.0f / (float)S; cp.y = tn;
-  AF2_TRY(launch_chan_to_token(cp, s));
-  GemmCall co = linear_call(tn, d, w->w_out, d, (int)T, d, d);
-  co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = w->b_out; co.resid = x; co.ld_resid = d;
-  AF2_TRY(launch_gemm(co, s));
-  return AF2_OK;
+  return contract_tail(chan_ln_params(Oc, cs_o, np4, rows, N, d, 1, nullptr, nullptr, nullptr, msa_mask_full ? scale : nullptr,
+                                      1.0f / (float)S, 0.f, tn),
+                       w->w_out, w->b_out, x, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1403,17 +1286,6 @@ int af2_gemm_bf16_f32_gathered(const void* A, long long lda, long long a_batch, 
   c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = C; c.ld_out = ldc; c.out_batch = c_batch;
   c.a_pr = a_pr; c.a_piece = a_piece; c.b_pr = b_pr; c.b_piece = b_piece;
   return launch_gemm(c, static_cast<cudaStream_t>(stream));
-}
-
-static ChanLnParams chan_ln_params(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode,
-                                   const float* gamma, const float* beta, const void* gate, const float* scale,
-                                   float scale_const, float eps, void* y) {
-  ChanLnParams p;
-  memset(&p, 0, sizeof(p));
-  p.src = src; p.chan_stride = chan_stride; p.pitch = pitch; p.rows = rows; p.n = n; p.d = d; p.mode = mode;
-  p.gamma = gamma; p.beta = beta; p.gate = static_cast<const __nv_bfloat16*>(gate); p.scale = scale;
-  p.scale_const = scale_const; p.eps = eps; p.y = static_cast<__nv_bfloat16*>(y);
-  return p;
 }
 
 static int chan_ln_check(const ChanLnParams& p) {

@@ -156,39 +156,6 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-// ------------------------------------------------------------------------------------------
-// L2 eviction-priority hints (experiment AF2_X_EVICT_LAST, DESIGN.md): the fp32 pair stream is read and written by almost
-// every kernel of a block; marking its lines evict_last keeps part of it in L2 between kernels while the bf16
-// intermediates stream through with normal priority.  The policy operand is always passed (evict_normal = no-op).
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t l2_policy(bool evict_last) {
-  uint64_t p;
-  if (evict_last) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void tma_load_3d_hint(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, uint64_t pol) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(pol)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_3d_hint(const CUtensorMap* m, const void* src, int c0, int c1, int c2, uint64_t pol) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "l"(pol)
-               : "memory");
-}
-__device__ __forceinline__ float4 ldg_stream_hint(const float4* p, uint64_t pol) {
-  float4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ float2 ldg_f2_hint(const float2* p, uint64_t pol) {
-  float2 v;
-  asm volatile("ld.global.nc.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(v.x), "=f"(v.y) : "l"(p), "l"(pol));
-  return v;
-}
 
 // ------------------------------------------------------------------------------------------
 // Programmatic dependent launch.  Every persistent kernel of the block is launched with

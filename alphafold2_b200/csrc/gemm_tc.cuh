@@ -69,7 +69,6 @@ struct GemmParams {
   // apart.  Rank-4 maps (k | mn, row | k, piece, batch) address them in place -- one launch instead of one per piece.
   //   a_pr / b_pr: rows (K-major) or columns (MN-major) per piece of A / B; 0 = plain rank-3 map.
   int a_pr, b_pr;
-  int x_evict_last;            // 1: residual loads / output stores of the fp32 stream carry an L2 evict_last hint
   NTile tile;
 };
 

@@ -198,7 +198,6 @@ struct PairBiasParams {
   int heads;
   long long bias_hs;
   int n_inner, pitch;
-  int x_evict_last;         // 1: loads of x carry an L2 evict_last hint (AF2_X_EVICT_LAST)
   int transpose;            // 1: token t = (i, j) is stored at [j][i] instead of [i][j] (the attention kernel's K-major bias operand)
 };
 
@@ -286,7 +285,6 @@ __global__ void __launch_bounds__(256, 2) pair_bias_mma_kernel(const PairBiasPar
     blo[ks][1] = pack_bf16x2(w1.x - bf16lo_to_f32(bfrag[ks][1]), w1.y - bf16hi_to_f32(bfrag[ks][1]));
   }
   const int groups = static_cast<int>((p.T + 15) / 16);
-  const uint64_t pol = l2_policy(p.x_evict_last != 0);
   pdl_wait();            // (the w_edge fragments above are weights: safe to load before the predecessor has finished)
   for (int gi = warp_global; gi < groups; gi += nwarps) {
     const long long r0 = static_cast<long long>(gi) * 16 + g, r1 = r0 + 8;
@@ -297,10 +295,10 @@ __global__ void __launch_bounds__(256, 2) pair_bias_mma_kernel(const PairBiasPar
 #pragma unroll
     for (int ks = 0; ks < KSTEPS; ++ks) {
       float2 a[4];
-      a[0] = l0 ? ldg_f2_hint(reinterpret_cast<const float2*>(x0 + ks * 16), pol) : make_float2(0.f, 0.f);
-      a[1] = l1 ? ldg_f2_hint(reinterpret_cast<const float2*>(x1 + ks * 16), pol) : make_float2(0.f, 0.f);
-      a[2] = l0 ? ldg_f2_hint(reinterpret_cast<const float2*>(x0 + ks * 16 + 8), pol) : make_float2(0.f, 0.f);
-      a[3] = l1 ? ldg_f2_hint(reinterpret_cast<const float2*>(x1 + ks * 16 + 8), pol) : make_float2(0.f, 0.f);
+      a[0] = l0 ? __ldg(reinterpret_cast<const float2*>(x0 + ks * 16)) : make_float2(0.f, 0.f);
+      a[1] = l1 ? __ldg(reinterpret_cast<const float2*>(x1 + ks * 16)) : make_float2(0.f, 0.f);
+      a[2] = l0 ? __ldg(reinterpret_cast<const float2*>(x0 + ks * 16 + 8)) : make_float2(0.f, 0.f);
+      a[3] = l1 ? __ldg(reinterpret_cast<const float2*>(x1 + ks * 16 + 8)) : make_float2(0.f, 0.f);
       uint32_t hi[4], lo[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {

@@ -146,25 +146,15 @@ def pack_gated(w_val, b_val, w_gate, b_gate, half: int):
         w[t * 2 * half + half: t * 2 * half + half + (hi - lo)] = w_gate[lo:hi]
         b[t * 2 * half: t * 2 * half + (hi - lo)] = b_val[lo:hi]
         b[t * 2 * half + half: t * 2 * half + half + (hi - lo)] = b_gate[lo:hi]
-    return w, b.contiguous()          # fp32; callers round to bf16 (after folding the LayerNorm affine where needed)
+    return w, b.contiguous()          # fp32; callers round to bf16
 
 
 def _pad_rows(t: torch.Tensor, mult: int = 256) -> torch.Tensor:
-    """Zero-pad dim 0 to a multiple of `mult` (segments of the fused projection kernel start on 256-column tiles)."""
+    """Zero-pad dim 0 to a multiple of `mult`."""
     r = (-t.shape[0]) % mult
     if r == 0:
         return t
     return torch.cat([t, torch.zeros((r,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)], 0)
-
-
-def _cat_segments(ws, bs, gamma, beta):
-    """Operands of the fused LayerNorm -> projection kernel (proj_tc.cuh): every segment zero-padded to 256-row tiles and
-    the LayerNorm affine folded in, W' = W diag(gamma) (bf16), b' = W beta + b (fp32, accumulator-column order); the
-    kernel's producer then only computes (x - mean) * rstd."""
-    w = torch.cat([_pad_rows(x.detach().float()) for x in ws], 0)
-    b = torch.cat([_pad_rows(x.detach().float()) for x in bs], 0)
-    g, be = gamma.detach().float(), beta.detach().float()
-    return _bf16(w * g[None, :]), (b + w @ be).contiguous()
 
 
 def _p(t):
@@ -187,10 +177,8 @@ def pack_feed_forward(norm_w, norm_b, w1, b1, w2, b2) -> Packed:
     a_b, g_b = b1[:hidden].detach().float(), b1[hidden:].detach().float()
     w1f, b1p = pack_gated(a_w, a_b, g_w, g_b, half)
     t = dict(g=_f32(norm_w), b=_f32(norm_b), w1=_bf16(w1f), b1=b1p, w2=_bf16(w2), b2=_f32(b2))
-    if half == 128:                                         # the fused kernel works on 256-column accumulator tiles
-        t["wcat"], t["bcat"] = _cat_segments([w1f], [b1p], norm_w, norm_b)
     s = _lib.FFWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["w1"].data_ptr(), t["b1"].data_ptr(),
-                       t["w2"].data_ptr(), t["b2"].data_ptr(), 2 * half, _p(t.get("wcat")), _p(t.get("bcat")), None)
+                       t["w2"].data_ptr(), t["b2"].data_ptr(), 2 * half)
     return Packed(s, t)
 
 
@@ -203,10 +191,9 @@ def pack_attention(norm_w, norm_b, wq, wkv, wg, bg, wo, bo, w_edge, dim_head: in
     t = dict(g=_f32(norm_w), b=_f32(norm_b), wqkv=_bf16(wqkv), wg=_bf16(wg), bg=_f32(bg), wo=_bf16(wo), bo=_f32(bo))
     if w_edge is not None:
         t["we"] = _f32(w_edge.detach().float() * log2e)
-    t["wcat"], t["bcat"] = _cat_segments([wqkv, wg], [torch.zeros(wqkv.shape[0], device=wqkv.device), bg], norm_w, norm_b)
     s = _lib.AttnWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["wqkv"].data_ptr(), t["wg"].data_ptr(),
                          t["bg"].data_ptr(), t["wo"].data_ptr(), t["bo"].data_ptr(),
-                         t["we"].data_ptr() if w_edge is not None else None, t["wcat"].data_ptr(), t["bcat"].data_ptr(), None)
+                         t["we"].data_ptr() if w_edge is not None else None)
     return Packed(s, t)
 
 
@@ -218,22 +205,17 @@ def pack_triangle_multiply(norm_w, norm_b, wl, bl, wr, br, wlg, blg, wrg, brg, w
     wrp, brp = pack_gated(f(wr), f(br), f(wrg), f(brg), half)
     t = dict(g=_f32(norm_w), b=_f32(norm_b), wl=_bf16(wlp), bl=blp, wr=_bf16(wrp), br=brp, wog=_bf16(wog), bog=_f32(bog),
              ong=_f32(onw), onb=_f32(onb), wo=_bf16(wo), bo=_f32(bo))
-    if half == 128:
-        t["wcat"], t["bcat"] = _cat_segments([wlp, wrp, wog], [blp, brp, bog], norm_w, norm_b)
     s = _lib.TriMulWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["wl"].data_ptr(), t["bl"].data_ptr(),
                            t["wr"].data_ptr(), t["br"].data_ptr(), t["wog"].data_ptr(), t["bog"].data_ptr(),
-                           t["ong"].data_ptr(), t["onb"].data_ptr(), t["wo"].data_ptr(), t["bo"].data_ptr(), 2 * half,
-                           _p(t.get("wcat")), _p(t.get("bcat")), None, None)
+                           t["ong"].data_ptr(), t["onb"].data_ptr(), t["wo"].data_ptr(), t["bo"].data_ptr(), 2 * half)
     return Packed(s, t)
 
 
 def pack_outer_mean(norm_w, norm_b, wl, bl, wr, br, wo, bo) -> Packed:
     t = dict(g=_f32(norm_w), b=_f32(norm_b), wlr=_bf16(torch.cat([wl.detach(), wr.detach()], 0)),
              blr=_f32(torch.cat([bl.detach(), br.detach()], 0)), wo=_bf16(wo), bo=_f32(bo))
-    t["wcat"], t["bcat"] = _cat_segments([torch.cat([wl.detach(), wr.detach()], 0)], [t["blr"]], norm_w, norm_b)
     s = _lib.OuterWeights(t["g"].data_ptr(), t["b"].data_ptr(), t["wlr"].data_ptr(), t["blr"].data_ptr(),
-                          t["wo"].data_ptr(), t["bo"].data_ptr(), t["wcat"].data_ptr(), t["bcat"].data_ptr(),
-                          None, None)
+                          t["wo"].data_ptr(), t["bo"].data_ptr())
     return Packed(s, t)
 
 
@@ -401,34 +383,6 @@ def apply_rotary_pos_emb(x: torch.Tensor, sinu_pos) -> torch.Tensor:
     _lib.check(_lib.load().af2_rotary(x.data_ptr(), sin.data_ptr(), cos.data_ptr(), y.data_ptr(), b, h, n, dh,
                                       sin.shape[-1], sin.shape[0], _stream_ptr()))
     return y
-
-
-# --------------------------------------------------------------------------------------------------
-# L2 residency of the pair stream (AF2_L2_PERSIST, default off until measured -- see DESIGN.md)
-# --------------------------------------------------------------------------------------------------
-L2_PERSIST = float(_os.environ.get("AF2_L2_PERSIST", "0") or 0)     # 0: off; (0, 1]: hit ratio of the window over x
-
-
-class l2_resident:
-    """with l2_resident(x): kernels launched on the current stream keep x's address range persisting in L2."""
-
-    def __init__(self, t: Optional[torch.Tensor]):
-        self.t = t if (L2_PERSIST > 0 and t is not None and t.is_cuda) else None
-
-    def __enter__(self):
-        if self.t is not None:
-            try:
-                _lib.check(_lib.load().af2_l2_persist(self.t.data_ptr(), self.t.numel() * self.t.element_size(), float(L2_PERSIST), _stream_ptr()))
-            except RuntimeError as e:
-                import sys
-                print(f"[alphafold2_b200] L2 persistence not applied: {e}", file=sys.stderr)
-                self.t = None
-        return self
-
-    def __exit__(self, *exc):
-        if self.t is not None:
-            _lib.check(_lib.load().af2_l2_persist(None, 0, 0.0, _stream_ptr()))
-        return False
 
 
 # --------------------------------------------------------------------------------------------------

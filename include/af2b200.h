@@ -32,13 +32,6 @@ const char* af2_last_error(void);
 int af2_abi_version(void);
 /* 0 if the current device is compute capability 9.0 (H100, sm_90a), AF2_ERR_UNSUPPORTED_DEVICE otherwise */
 int af2_check_device(void);
-/* nonzero: LN->projection clusters run on the fused LayerNorm->projection kernel (1 and 2 select the same kernel);
- * 0 (default): LayerNorm kernel + GEMM launches.  Also selectable with the environment variable AF2_PROJ_CTAS, read by
- * af2_check_device */
-void af2_set_proj_mode(int ctas);
-/* kept for ABI compatibility: no kernel of this build records a timeline; both return AF2_ERR_BAD_ARG */
-int af2_debug_proj_trace(long long* out);
-int af2_debug_attn_trace(long long* out);
 
 /* Kernel launches issued by this library since load (bench.py's gpu_launches). */
 unsigned long long af2_launch_count(void);
@@ -57,11 +50,6 @@ typedef struct {
   const void* w1; const float* b1;                    /* FeedForward.net.0         packed [n1p, d]  */
   const void* w2; const float* b2;                    /* FeedForward.net.3         [d, hid] , [d]   */
   int bn;                                             /* column tile used for the w1 packing        */
-  /* fused LayerNorm->projection kernel (proj_tc.cuh): every projection of the module that reads LN(x), concatenated,
-   * each segment zero-padded to a multiple of 256 accumulator columns; b_cat is the matching fp32 bias (zeros where none).
-   * NULL -> the unfused LayerNorm + GEMM launches are used.  FeedForward: w_cat == w1, b_cat == b1 (bn must be 256). */
-  const void* w_cat; const float* b_cat;
-  const void* w_ext;   /* unused (NULL); kept for the struct layout -- the fused kernel reads b_cat */
 } af2_ff_weights;
 int af2_feed_forward(const af2_ff_weights* w, float* x, long long tokens, int d, int hidden,
                      void* workspace, long long workspace_bytes, af2_stream_t stream);
@@ -78,8 +66,6 @@ typedef struct {
   const void* w_gate; const float* b_gate;            /* Attention.gating          [I, d], [I]      */
   const void* w_out; const float* b_out;              /* Attention.to_out          [d, I], [d]      */
   const float* w_edge;                                /* edges_to_attn_bias.0      [H, d] fp32/NULL */
-  const void* w_cat; const float* b_cat;              /* [pad256(3I) rows w_qkv | pad256(I) rows w_gate], bias likewise */
-  const void* w_ext;
 } af2_attn_weights;
 int af2_axial_attention(const af2_attn_weights* w, float* x, const float* edges, const unsigned char* mask,
                         int B, int h, int wdim, int d, int heads, int dim_head, int row_attn,
@@ -103,8 +89,6 @@ typedef struct {
   const float* on_gamma; const float* on_beta;        /* to_out_norm                                */
   const void* w_out; const float* b_out;              /* to_out                    [d, d], [d]      */
   int bn;
-  const void* w_cat; const float* b_cat;              /* [w_left packed | w_right packed | pad256(d) rows w_ogate]  */
-  const void* w_ext; const void* w_ext_out;           /* unused (NULL); kept for the struct layout                   */
 } af2_trimul_weights;
 int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned char* mask, int B, int N, int d,
                           int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);
@@ -117,8 +101,6 @@ typedef struct {
   const float* ln_gamma; const float* ln_beta;        /* .norm                                      */
   const void* w_lr; const float* b_lr;                /* [2d, d]: left_proj | right_proj, [2d]      */
   const void* w_out; const float* b_out;              /* proj_out                  [d, d], [d]      */
-  const void* w_cat; const float* b_cat;              /* pad256(2d) rows of w_lr, bias likewise                      */
-  const void* w_ext; const void* w_ext_out;
 } af2_outer_weights;
 int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const unsigned char* msa_mask,
                    int B, int S, int N, int d, float eps, void* workspace, long long workspace_bytes,
@@ -419,10 +401,6 @@ typedef struct {
 long long af2_template_angles_strict_workspace(int B, int T, int n, int K, int d);
 int af2_template_angles_strict(const af2_template_angle_weights_strict* w, const float* angles, float* m, int B, int T, int n, int K,
                                int d, int m_rows, int row0, void* workspace, long long workspace_bytes, af2_stream_t stream);
-
-/* L2 residency hint for the fp32 pair stream: every kernel launched on `stream` afterwards treats [ptr, ptr + bytes) as
- * persisting in L2 (cudaAccessPolicyWindow; clipped to the device's set-aside / window limits).  ptr == NULL clears it. */
-int af2_l2_persist(const void* ptr, long long bytes, float hit_ratio, af2_stream_t stream);
 
 /* ---- peer-memory exchange for the sharded trunk (alphafold2_b200/parallel.py; no reference counterpart: the reference
  * has no multi-GPU path, SURVEY.md 8(e)) ----

@@ -27,7 +27,7 @@ def test_header_symbols_exported(lib):
 
 
 def test_abi_version(lib):
-    assert lib.af2_abi_version() == 2
+    assert lib.af2_abi_version() == 3
     assert lib.af2_last_error() is not None
 
 

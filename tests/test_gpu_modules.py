@@ -129,6 +129,61 @@ def test_evoformer_block_oracle(d, H, dh, N, S, B):
     check(f"evoformer_block/oracle/d{d}N{N}S{S}/m", mo, rm)
 
 
+# single modules at widths and lengths the shapes above miss: d = 192, 3 heads of 32, token counts that are no multiple of a
+# 64-row tile, N = 70 / 72 / 136 (padded channel-major pitches) with masks
+@pytest.mark.parametrize("d,T0,T1", [(256, 8, 250), (128, 3, 391), (192, 1, 128), (256, 300, 256)])
+def test_feed_forward_oracle(d, T0, T1):
+    import alphafold2_b200 as A
+    ff = A.FeedForward(dim=d)
+    st = _rand_state(ff, 1)
+    ff = ff.cuda().eval()
+    x = torch.randn(1, T0, T1, d, generator=torch.Generator().manual_seed(2))
+    check(f"feed_forward/oracle/d{d}T{T0}x{T1}", ff(x.cuda()), O.feed_forward(to64(st), "", x.double()))
+
+
+@pytest.mark.parametrize("d,H,dh,N,row", [(256, 8, 64, 72, True), (128, 4, 32, 64, False), (256, 3, 32, 40, True)])
+def test_axial_attention_oracle(d, H, dh, N, row):
+    import alphafold2_b200 as A
+    ax = A.AxialAttention(dim=d, heads=H, dim_head=dh, row_attn=row, col_attn=not row, accept_edges=True)
+    st = _rand_state(ax, 3)
+    ax = ax.cuda().eval()
+    x = torch.randn(1, N, N, d, generator=torch.Generator().manual_seed(4))
+    m1 = torch.ones(1, N, dtype=torch.bool)
+    m1[:, -5:] = False
+    mask = m1[:, :, None] & m1[:, None, :]
+    xc = x.cuda()
+    out = ax(xc, edges=xc, mask=mask.cuda())
+    ref = O.axial_attention(to64(st), "", x.double(), H, row, edges=x.double(), mask=mask)
+    check(f"axial_attention/oracle/d{d}H{H}x{dh}N{N}", out, ref)
+
+
+@pytest.mark.parametrize("d,N,mix", [(256, 72, "outgoing"), (128, 136, "ingoing"), (256, 128, "ingoing"), (256, 70, "outgoing")])
+def test_triangle_multiply_oracle(d, N, mix):
+    import alphafold2_b200 as A
+    tm = A.TriangleMultiplicativeModule(dim=d, mix=mix)
+    st = _rand_state(tm, 5)
+    tm = tm.cuda().eval()
+    x = torch.randn(1, N, N, d, generator=torch.Generator().manual_seed(6))
+    m1 = torch.ones(1, N, dtype=torch.bool)
+    m1[:, -7:] = False
+    mask = m1[:, :, None] & m1[:, None, :]
+    out = tm(x.cuda(), mask=mask.cuda())
+    check(f"triangle_multiply/oracle/d{d}N{N}/{mix}", out, O.triangle_multiply(to64(st), "", x.double(), mix, mask))
+
+
+@pytest.mark.parametrize("d,N,S", [(256, 72, 9), (128, 64, 33), (256, 50, 5)])
+def test_outer_mean_oracle(d, N, S):
+    import alphafold2_b200 as A
+    om = A.OuterMean(dim=d)
+    st = _rand_state(om, 7)
+    om = om.cuda().eval()
+    g = torch.Generator().manual_seed(8)
+    m = torch.randn(1, S, N, d, generator=g)
+    mask = torch.rand(1, S, N, generator=g) > 0.2
+    out = om(m.cuda(), mask=mask.cuda())
+    check(f"outer_mean/oracle/d{d}N{N}S{S}", out, O.outer_mean(to64(st), "", m.double(), mask))
+
+
 def test_no_cpu_fallback():
     import alphafold2_b200 as A
     ff = A.FeedForward(dim=64)

@@ -1,5 +1,5 @@
 """Small cases for compute-sanitizer: one C1-shape EvoformerBlock (wgmma GEMMs and attention, per-channel GEMMs, TMA
-channel->token; AF2_PROJ_CTAS=2 adds the fused projection kernel) and one attention with n > 256 (several key blocks)."""
+channel->token) and one attention with n > 256 (several key blocks)."""
 import os
 import sys
 

@@ -21,8 +21,6 @@ WANT = [
 
 
 def kernel_class(name):
-    if "proj_tc_kernel" in name:
-        return "gemm_linear(wgmma)"
     if "gemm_tc_kernel" in name:
         return "gemm_per_channel(wgmma)" if name.rstrip(">").endswith(", 7") else "gemm_linear(wgmma)"
     if "attention_tc_kernel" in name:

@@ -14,6 +14,7 @@
 #include "../../include/af2b200.h"
 #include "attention_tc.cuh"
 #include "chan2tok_tma.cuh"
+#include "ff_fused.cuh"
 #include "gemm_tc.cuh"
 #include "simt_kernels.cuh"
 #include "strict_kernels.cuh"
@@ -387,6 +388,45 @@ GemmCall linear_call(const void* A, long long lda, const void* W, long long ldw,
   c.A = A; c.lda = lda; c.Bm = W; c.ldb = ldw; c.M = M; c.N = N; c.K = K; c.batch = 1;
   c.mn_major = false; c.bn = pick_bn(N);
   return c;
+}
+
+// -------------------------------------------------------------------------------------------------
+// Fused GEGLU feed-forward launch (ff_fused.cuh)
+// -------------------------------------------------------------------------------------------------
+// The fused kernel reads W1 packed with 256-row tiles ([128 value | 128 gate] rows, ops.pack_gated), W2 in HC-column
+// chunks and everything through TMA or 8-byte vector accesses; other shapes take the two-GEMM path.
+bool ff_fused_ok(const af2_ff_weights* w, const float* x, const void* xn, int d, int hidden) {
+  return (d == 128 || d == 256) && hidden % 128 == 0 && w->bn == 256 && w->b1 && w->b2 && aligned16(x) && aligned16(xn) &&
+         aligned16(w->w1) && aligned16(w->w2) && aligned16(w->b1) && aligned16(w->b2);
+}
+
+template <int D, int HC>
+int launch_ff_fused(const af2_ff_weights* w, float* x, const __nv_bfloat16* xn, long long T, int hidden, cudaStream_t s) {
+  using L = FfSmem<D, HC>;
+  static bool configured[MAX_DEVICES] = {false};
+  auto kern = ff_fused_kernel<D, HC>;
+  if (!configured[cur_dev()]) {
+    CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+    configured[cur_dev()] = true;
+  }
+  if (T <= 0) return AF2_OK;
+  CUtensorMap tx, t1, t2;
+  const unsigned long long dx[2] = {(unsigned long long)D, (unsigned long long)T}, sx[1] = {(unsigned long long)D * 2};
+  const unsigned long long d1[2] = {(unsigned long long)D, 2ull * hidden}, s1[1] = {(unsigned long long)D * 2};
+  const unsigned long long d2[2] = {(unsigned long long)hidden, (unsigned long long)D}, s2[1] = {(unsigned long long)hidden * 2};
+  const unsigned b64[2] = {64, 64}, bw1[2] = {64, (unsigned)HC}, bw2[2] = {(unsigned)HC, (unsigned)D};
+  AF2_TRY(make_tmap(&tx, xn, 2, dx, sx, b64, CU_TENSOR_MAP_SWIZZLE_128B));
+  AF2_TRY(make_tmap(&t1, w->w1, 2, d1, s1, bw1, CU_TENSOR_MAP_SWIZZLE_128B));
+  AF2_TRY(make_tmap(&t2, w->w2, 2, d2, s2, bw2, HC == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B));
+  FfParams p;
+  p.x = x; p.b1 = w->b1; p.b2 = w->b2; p.T = (int)T; p.hidden = hidden;
+  const long long tiles = (T + FF_BM - 1) / FF_BM;
+  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
+  const double flops = 2.0 * T * (2.0 * D * hidden + (double)hidden * D);
+  const double bytes = (double)T * D * 2 + 3.0 * D * hidden * 2 + (double)T * D * 8;   // xn, W1 and W2 once, x read + written
+  ProfScope ps(s, KC_GEMM_LINEAR, flops, bytes);
+  CUDA_OK(launch_pdl(kern, dim3(grid), dim3(FF_THREADS), L::TOTAL, s, tx, t1, t2, p));
+  return AF2_OK;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -795,14 +835,20 @@ int af2_feed_forward(const af2_ff_weights* w, float* x, long long tokens, int d,
   if (tokens > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "feed_forward: too many tokens");
   Arena ar(workspace, workspace_bytes);
   __nv_bfloat16* xn = ar.take<__nv_bfloat16>(tokens * d);
+  if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "feed_forward: workspace too small");
+  LnParams lp;
+  memset(&lp, 0, sizeof(lp));
+  lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
+  if (ff_fused_ok(w, x, xn, d, hidden)) {
+    AF2_TRY(launch_layernorm(lp, s));
+    // 64 hidden units per chunk: 32 measured slower (n64 GEMM1 tiles read more shared memory per FLOP)
+    return d == 256 ? launch_ff_fused<256, 64>(w, x, xn, tokens, hidden, s) : launch_ff_fused<128, 64>(w, x, xn, tokens, hidden, s);
+  }
   __nv_bfloat16* hbuf = ar.take<__nv_bfloat16>(tokens * hidden);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "feed_forward: workspace too small");
   // h = a * gelu(g)
   const int half = w->bn / 2;
   const int n1p = (hidden + half - 1) / half * w->bn;   // packed accumulator columns
-  LnParams lp;
-  memset(&lp, 0, sizeof(lp));
-  lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
   AF2_TRY(launch_layernorm(lp, s));
   GemmCall c1 = linear_call(xn, d, w->w1, d, (int)tokens, n1p, d);
   c1.bn = w->bn; c1.mode = EPI_GATED_BF16; c1.act = ACT_GELU; c1.layout = LAYOUT_TOKEN;

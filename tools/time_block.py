@@ -3,7 +3,8 @@
 
 AF2_PROFILE=1 adds a torch.profiler pass (CUDA activities, after the timed loop) that groups kernel time by name and, for
 the linear GEMMs (K-major, BN 256), by epilogue kind: ms per block, us per 128 x 256 output tile on one SM (kernel time x
-SM count / tiles), and TFLOP/s and GB/s from algorithmic FLOPs and bytes.  The card name, power limit and max SM clock are read in the same run.  AF2_PROFILE_OUT=path also
+SM count / tiles), and TFLOP/s and GB/s from algorithmic FLOPs and bytes.  The fused feed-forward kernel has a row of its
+own: ms per block, TFLOP/s, HBM GB/s and the L2->SM rate of its weight reads (W1 and W2 once per 128-row tile).  The card name, power limit and max SM clock are read in the same run.  AF2_PROFILE_OUT=path also
 writes the result as JSON."""
 import json
 import os
@@ -61,12 +62,22 @@ def linear_gemms(N, S, d, I):
     out = []
     for T in (Tm, Tm, Tx, Tx):        # MSA row / column attention, triangle attention start / end
         out += [(1, T, 3 * I, d), (2, T, I, d), (6, T, d, I)]
-    for T in (Tm, Tx):                # MSA and pair FeedForward (GEGLU, mult 4)
-        out += [(4, T, 8 * d, d), (6, T, d, 4 * d)]
     out += [(3, Tm, 2 * d, d), (6, Tx, d, d)]                        # outer mean: left|right, out
     for _ in range(2):                # triangle multiply outgoing / ingoing: left, right, out gate, out
         out += [(5, Tx, 2 * d, d), (5, Tx, 2 * d, d), (2, Tx, d, d), (6, Tx, d, d)]
     return out
+
+
+def ff_launches(N, S, d):
+    """(T, d, hidden) of the fused feed-forward launches of one block (csrc/ff_fused.cuh): MSA and pair transitions."""
+    return [(S * N, d, 4 * d), (N * N, d, 4 * d)]
+
+
+def ff_cost(T, d, hidden):
+    """Algorithmic FLOPs, HBM bytes (xn read, x read and written, the weights once) and L2->SM weight bytes (W1 and W2,
+    3 d hidden bf16, once per 128-row tile) of one fused feed-forward launch."""
+    wbytes = 3 * d * hidden * 2
+    return 2.0 * T * 3 * d * hidden, float(2 * T * d + 8 * T * d + wbytes), float(-(-T // 128) * wbytes)
 
 
 def gemm_cost(ek, M, Nacc, K):
@@ -123,8 +134,18 @@ if os.environ.get("AF2_PROFILE") == "1":
         rows.append(dict(epilogue=EK_NAMES.get(ek, str(ek)), launches=launches, launches_expected=n_exp,
                          ms_per_block=ms_, us_per_tile_128x256_per_sm=ms_ * 1e3 * n_sm / tl,
                          tflops=f / (ms_ * 1e-3) / 1e12, gbs=b_ / (ms_ * 1e-3) / 1e9))
+    ff_ms, ff_n = 0.0, 0
+    for name, (ms_, cnt) in kernels.items():
+        if "ff_fused_kernel" in name:
+            ff_ms += ms_
+            ff_n += cnt // it
+    f, hb, wb = (sum(v) for v in zip(*(ff_cost(*a) for a in ff_launches(N, S, CFG["dim"]))))
+    ff_row = dict(kernel="ff_fused", launches=ff_n, launches_expected=len(ff_launches(N, S, CFG["dim"])), ms_per_block=ff_ms,
+                  tflops=f / (ff_ms * 1e-3) / 1e12 if ff_ms else None, hbm_gbs=hb / (ff_ms * 1e-3) / 1e9 if ff_ms else None,
+                  weight_l2_gbs=wb / (ff_ms * 1e-3) / 1e9 if ff_ms else None)
     res = dict(N=N, S=S, iters=it, card=card(), lib=_lib.LIB_PATH,
-               linear_gemm_ms_per_block=sum(r["ms_per_block"] for r in rows), linear_gemm_by_epilogue=rows,
+               linear_gemm_ms_per_block=sum(r["ms_per_block"] for r in rows) + ff_ms, linear_gemm_by_epilogue=rows,
+               feed_forward=ff_row,
                kernels_ms_per_block=dict(sorted(((k, v[0]) for k, v in kernels.items()), key=lambda kv: -kv[1])[:25]))
     print(json.dumps(res))
     if os.environ.get("AF2_PROFILE_OUT"):

@@ -140,6 +140,22 @@ _SIGNATURES = {
     "af2_template_pointwise_attention_strict_workspace": (ll, [ci, ci, ci, ci, ci, ci]),
     "af2_template_pointwise_bf16": (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, ll, ci, ci, vp]),
     "af2_template_pointwise_f32": (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, ll, ci, ci, vp]),
+    "af2_template_pointwise_bf16_state": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ll, ci, ci, vp]),
+    "af2_template_pointwise_f32_state": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ll, ci, ci, vp]),
+    "af2_template_pointwise_begin_workspace": (ll, [ci, ci, ci]),
+    "af2_template_pointwise_begin": (ci, [C.POINTER(TemplateAttnWeights), vp, ci, ci, ci, ci, ci, vp, vp, vp, ll, vp]),
+    "af2_template_pointwise_group_workspace": (ll, [ci, ci, ci, ci, ci, ci]),
+    "af2_template_pointwise_group": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp,
+                                          vp, ci, ci, vp, ll, vp]),
+    "af2_template_pointwise_end_workspace": (ll, [ci, ci, ci, ci]),
+    "af2_template_pointwise_end": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_template_pointwise_begin_strict_workspace": (ll, [ci, ci, ci]),
+    "af2_template_pointwise_begin_strict": (ci, [C.POINTER(TemplateAttnWeightsStrict), vp, ci, ci, ci, ci, ci, vp, vp, ll, vp]),
+    "af2_template_pointwise_group_strict_workspace": (ll, [ci, ci, ci, ci, ci, ci]),
+    "af2_template_pointwise_group_strict": (ci, [C.POINTER(TemplateAttnWeightsStrict), vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp,
+                                                 vp, vp, vp, ci, ci, vp, ll, vp]),
+    "af2_template_pointwise_end_strict_workspace": (ll, [ci, ci, ci, ci]),
+    "af2_template_pointwise_end_strict": (ci, [C.POINTER(TemplateAttnWeightsStrict), vp, vp, vp, ci, ci, ci, ci, ci, vp, ll, vp]),
     "af2_template_embed": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),
     "af2_template_embed_workspace": (ll, [ll, ci]),
     "af2_template_embed_strict": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),

@@ -205,6 +205,10 @@ class Attention(_Packable):
         the pointwise template attention of alphafold2.py:764-785 (t [b * T, n, n, d], t_mask [b * T, n, n] crossed)."""
         return ops.template_pointwise_attention_(self.packed(), x, t, x_mask, t_mask, self.heads, self.dim_head)
 
+    def context_groups(self, x, x_mask):
+        """add_context_ with the templates given one group at a time (ops.TemplateAttentionGroups): same result, bitwise."""
+        return ops.TemplateAttentionGroups(self.packed(), x, x_mask, self.heads, self.dim_head)
+
     def forward(self, x, mask=None, attn_bias=None, context=None, context_mask=None, tie_dim=None):
         raise NotImplementedError(
             "alphafold2_b200.Attention runs through AxialAttention (self-attention) or Alphafold2's template branch "
@@ -547,12 +551,36 @@ class Alphafold2(nn.Module):
             self.template_pairwise_embedder.update_(t, tm2)
         return t, tm2
 
-    def embed_templates_(self, x, x_mask, templates_feats, templates_mask):
+    def embed_templates_(self, x, x_mask, templates_feats, templates_mask, group=None):
         """alphafold2.py:743-785 in place on the fp32 pair tensor x [b, n, n, d]: template pair stack, then the pointwise
         attention of every pair over its T templates, scaled by `any template valid` and added to x.  Under shard_evoformer
-        every rank computes this whole (it runs before the sharded trunk)."""
-        t, tm2 = self.template_pair_stack(templates_feats, templates_mask)
-        self.template_pointwise_attn.add_context_(x, t, x_mask, tm2)
+        every rank computes this whole (it runs before the sharded trunk).
+
+        The templates run in groups of G: each group's pair stack at batch b * G, then its step of the pointwise attention,
+        whose online softmax carries over to the next group.  The result does not depend on G (bitwise), only the memory does:
+        G = T when the whole branch fits what the device can still allocate (ops.plan_template_groups), fewer otherwise.
+        `group` forces G (tests).  The G used is kept in self.last_template_group."""
+        b, T = templates_feats.shape[:2]
+        n, d = x.shape[1], x.shape[3]
+        attn = self.template_pointwise_attn
+        if group is None:
+            # 15 % headroom: the caching allocator cannot always reuse the blocks it frees (a growing workspace is allocated
+            # before the old one is released); plans right at the limit ran out of memory at N_res 1024 and 2048 on an H100
+            budget = int(ops.device_budget(x.device) * 0.85)
+            group = ops.plan_template_groups(b, T, n, d, attn.heads, attn.dim_head, ops.precision_of(attn), budget,
+                                             templates_feats.shape[-1])
+        G = max(1, min(int(group), T))
+        self.last_template_group = G
+        if G == T:
+            t, tm2 = self.template_pair_stack(templates_feats, templates_mask)
+            attn.add_context_(x, t, x_mask, tm2)
+            return x
+        acc = attn.context_groups(x, x_mask)
+        for t0 in range(0, T, G):
+            t1 = min(t0 + G, T)
+            t, tm2 = self.template_pair_stack(templates_feats[:, t0:t1], templates_mask[:, t0:t1])
+            acc.add(t, tm2, last=t1 == T)
+            del t, tm2                                   # free this group's t before the next one is embedded
         return x
 
     def _check_recyclables(self, b, n, device, recyclables):

@@ -335,7 +335,10 @@ int launch_gemm(const GemmCall& c, cudaStream_t s) {
   if (p.epi_tma) {
     const bool f32 = c.mode == EPI_RESID_F32 || c.mode == EPI_STORE_F32;
     const unsigned long long es = f32 ? 4 : 2;
-    const unsigned long long bstride = (unsigned long long)(c.batch > 1 ? c.out_batch : c.ld_out * c.M) * es;
+    // batch 1: the batch stride is never stepped, but TMA still needs it below 2^40 B; the span of one batch element (for
+    // the channel-major layout ld_out is the channel stride: ld_out * M overflowed from N_res = 1024 on)
+    const unsigned long long bstride =
+        (unsigned long long)(c.batch > 1 ? c.out_batch : (c.layout == LAYOUT_CHANNEL ? c.ld_out * p.out_cols : c.ld_out * c.M)) * es;
     if (c.layout == LAYOUT_CHANNEL) {
       // [batch][col][row block][row in block]: 64-row x 64-column boxes written from a [col][row] stage
       unsigned long long dc[4] = {(unsigned long long)p.cm_inner, (unsigned long long)(c.M / p.cm_inner), (unsigned long long)p.out_cols, (unsigned long long)c.batch};

@@ -15,6 +15,13 @@
 // bound on T: the softmax is online (running max, running sum, rescaled accumulator), in fp32.
 //   E = bf16 : q pre-scaled by dim_head^-0.5 * log2(e), logits in the log2 domain on ex2.approx, gate already sigmoid-ed.
 //   E = float: strict mode -- q pre-scaled by dim_head^-0.5, expf, gate given as logits (sigmoid by expf here).
+//
+// Templates in groups: kv / t_mask may hold only the templates of one group (T = the group's size).  The softmax state then
+// carries from launch to launch in fp32: running max and running sum per pair and head ([P][heads], stored by the head's
+// first lane), the rescaled accumulator per pair and channel ([P][I]) and the "any template valid" flag (pooled, 0 / 1).
+// !first: start from the stored state instead of (-inf, 0, 0, false);  !last: store the state instead of finishing.  The
+// recurrence is the same whatever the grouping (the first template of a launch is not special), so the output is bitwise
+// that of one launch over all templates; first && last is the plain one-launch kernel and touches no state.
 #pragma once
 #include <cfloat>
 #include "common.cuh"
@@ -26,12 +33,31 @@ struct TplParams {
   const void* q; const void* gate; const void* kv;       // q [P][ld_q], gate [P][ld_gate], kv [B T pairs][2I] (k | v)
   const uint8_t* x_mask;                                  // [P] or nullptr (all valid)
   const uint8_t* t_mask;                                  // [B T pairs] or nullptr (all valid)
-  void* out;                                              // [P][I]
+  void* out;                                              // [P][I]; may be q (ld_q == I) or, for E = float, acc: a thread
+                                                          // reads those elements before it writes the same ones
   float* pooled;                                          // [P]
   long long pairs;                                        // pair positions per batch element (n * n)
   long long ld_q, ld_gate;                                // row strides of q / gate (elements)
   int B, T, heads, dh;
+  float* run_max; float* run_sum;                         // [P][heads] softmax state (only read / written when !first / !last)
+  float* acc;                                             // [P][I] fp32 accumulator (same)
+  int first, last;                                        // first / last group of templates
 };
+
+// VEC consecutive fp32 values, 16-byte accesses (the accumulator state)
+template <int N>
+__device__ __forceinline__ void tpl_load_f32(const float* p, float (&v)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; i += 4) {
+    const float4 u = __ldcs(reinterpret_cast<const float4*>(p + i));
+    v[i] = u.x; v[i + 1] = u.y; v[i + 2] = u.z; v[i + 3] = u.w;
+  }
+}
+template <int N>
+__device__ __forceinline__ void tpl_store_f32(float* p, const float (&v)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; i += 4) __stcs(reinterpret_cast<float4*>(p + i), make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
+}
 
 template <typename E> struct TplVec;
 template <> struct TplVec<__nv_bfloat16> {
@@ -63,9 +89,11 @@ template <> struct TplVec<float> {
 
 // grid-stride over warps: all 32 lanes of a warp step together, so the head groups (dh / VEC lanes, a power of two that
 // divides 32, starting at a multiple of its size) always shuffle inside one warp
-template <typename E>
+// CARRY = false: one launch over all templates (first = last = 1 at compile time, no state code at all)
+template <typename E, bool CARRY>
 __global__ void __launch_bounds__(256) template_pointwise_kernel(const TplParams p) {
   using V = TplVec<E>;
+  const bool first = !CARRY || p.first, last = !CARRY || p.last;
   constexpr int VEC = V::N;
   const int I = p.heads * p.dh;
   const int C = I / VEC;                       // work items per pair
@@ -91,6 +119,13 @@ __global__ void __launch_bounds__(256) template_pointwise_kernel(const TplParams
     const bool xm = !p.x_mask || (active && p.x_mask[pr]);
     float mx = -INFINITY, l = 0.f;
     bool any = false;
+    const long long sh = pr * p.heads + c / G;   // this lane's head in the [P][heads] state
+    if (!first && active) {
+      mx = p.run_max[sh];
+      l = p.run_sum[sh];
+      tpl_load_f32(p.acc + pr * I + (long long)c * VEC, acc);
+      if (c == 0) any = p.pooled[pr] != 0.f;
+    }
     const long long row0 = b * p.T * p.pairs + ij;
 #pragma unroll 4
     for (int t = 0; t < p.T; ++t) {
@@ -120,7 +155,11 @@ __global__ void __launch_bounds__(256) template_pointwise_kernel(const TplParams
       for (int e = 0; e < VEC; ++e) acc[e] = fmaf(acc[e], alpha, pt * v[e]);
       mx = mn;
     }
-    if (active) {
+    if (active && !last) {
+      tpl_store_f32(p.acc + pr * I + (long long)c * VEC, acc);
+      if (c % G == 0) { p.run_max[sh] = mx; p.run_sum[sh] = l; }
+      if (c == 0) p.pooled[pr] = any ? 1.0f : 0.0f;
+    } else if (active) {
       const float inv = 1.0f / l;
 #pragma unroll
       for (int e = 0; e < VEC; ++e) acc[e] = acc[e] * inv * V::gate(g[e]);

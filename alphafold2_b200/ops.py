@@ -781,6 +781,135 @@ def template_pointwise_attention_(pk: Packed, x: torch.Tensor, t: torch.Tensor, 
     return x
 
 
+class TemplateAttentionGroups:
+    """template_pointwise_attention_ over the templates one group at a time (af2_template_pointwise_begin / _group / _end):
+        g = TemplateAttentionGroups(pk, x, x_mask, heads, dim_head)
+        g.add(t, t_mask, last=False) ...; g.add(t, t_mask, last=True)     # t [B * G, n, n, d], t_mask [B * G, n, n] per group
+    adds to x exactly what one template_pointwise_attention_ over the concatenated groups adds (bitwise).  Between the calls
+    it holds q and gate of x and the fp32 online-softmax state; a group's t may be freed as soon as its add() returns."""
+
+    def __init__(self, pk: Packed, x: torch.Tensor, x_mask: Optional[torch.Tensor], heads: int, dim_head: int):
+        _require(x, torch.float32, "x")
+        if x.dim() != 4 or x.shape[1] != x.shape[2]:
+            raise ValueError(f"x must be [B, n, n, d], got {tuple(x.shape)}")
+        B, n, _, d = x.shape
+        self.pk, self.x, self.heads, self.dim_head = pk, x, heads, dim_head
+        self.xm = _mask_u8(x_mask, (B, n, n), "x_mask")
+        self.first, self.done = True, False
+        P, I, dev = B * n * n, heads * dim_head, x.device
+        lib = _lib.load()
+        self.strict = pk.kind == "strict"
+        self.run_max = torch.empty(P, heads, dtype=torch.float32, device=dev)
+        self.run_sum = torch.empty(P, heads, dtype=torch.float32, device=dev)
+        self.acc = torch.empty(P, I, dtype=torch.float32, device=dev)
+        self.pooled = torch.empty(P, dtype=torch.float32, device=dev)
+        if self.strict:
+            self.qg = torch.empty(P, 2 * I, dtype=torch.float32, device=dev)
+            self.out = self.acc                     # the last group writes the gated output over the accumulator
+            ws = workspace(lib.af2_template_pointwise_begin_strict_workspace(B, n, d), dev)
+            _lib.check(lib.af2_template_pointwise_begin_strict(C.byref(pk.struct), x.data_ptr(), B, n, d, heads, dim_head,
+                                                               self.qg.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
+        else:
+            self.q = torch.empty(P, I, dtype=torch.bfloat16, device=dev)
+            self.gate = torch.empty(P, I, dtype=torch.bfloat16, device=dev)
+            self.out = self.q                       # ... over q
+            ws = workspace(lib.af2_template_pointwise_begin_workspace(B, n, d), dev)
+            _lib.check(lib.af2_template_pointwise_begin(C.byref(pk.struct), x.data_ptr(), B, n, d, heads, dim_head, self.q.data_ptr(),
+                                                        self.gate.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
+
+    def add(self, t: torch.Tensor, t_mask: Optional[torch.Tensor], last: bool) -> None:
+        """One group of templates; on the last one (last=True) x gets the attention output."""
+        if self.done:
+            raise RuntimeError("TemplateAttentionGroups: the last group has already been added")
+        _require(t, torch.float32, "t")
+        B, n, _, d = self.x.shape
+        if t.dim() != 4 or t.shape[0] % B or t.shape[0] == 0 or tuple(t.shape[1:]) != (n, n, d):
+            raise ValueError(f"t must be [B * G, {n}, {n}, {d}], got {tuple(t.shape)}")
+        G = t.shape[0] // B
+        tm = _mask_u8(t_mask, (B * G, n, n), "t_mask")
+        lib = _lib.load()
+        h, dh = self.heads, self.dim_head
+        if self.strict:
+            ws = workspace(lib.af2_template_pointwise_group_strict_workspace(B, G, n, d, h, dh), t.device)
+            fn, qg = lib.af2_template_pointwise_group_strict, (self.qg.data_ptr(),)
+        else:
+            ws = workspace(lib.af2_template_pointwise_group_workspace(B, G, n, d, h, dh), t.device)
+            fn, qg = lib.af2_template_pointwise_group, (self.q.data_ptr(), self.gate.data_ptr())
+        _lib.check(fn(C.byref(self.pk.struct), t.data_ptr(), _ptr(self.xm), _ptr(tm), B, G, n, d, h, dh, *qg, self.run_max.data_ptr(),
+                      self.run_sum.data_ptr(), self.acc.data_ptr(), self.pooled.data_ptr(), self.out.data_ptr(), int(self.first),
+                      int(last), ws.data_ptr(), ws.numel(), _stream_ptr()))
+        self.first = False
+        if last:
+            self.done = True
+            if self.strict:
+                ws = workspace(lib.af2_template_pointwise_end_strict_workspace(B, n, h, dh), t.device)
+                fn = lib.af2_template_pointwise_end_strict
+            else:
+                ws = workspace(lib.af2_template_pointwise_end_workspace(B, n, h, dh), t.device)
+                fn = lib.af2_template_pointwise_end
+            _lib.check(fn(C.byref(self.pk.struct), self.x.data_ptr(), self.out.data_ptr(), self.pooled.data_ptr(), B, n, d, h, dh,
+                          ws.data_ptr(), ws.numel(), _stream_ptr()))
+
+
+def _ws_alloc(nbytes: int) -> int:
+    return int(nbytes * 1.05) + 4096                # what workspace() allocates for a request of nbytes
+
+
+def template_branch_bytes(b: int, T: int, G: int, n: int, d: int, heads: int, dim_head: int, precision: str,
+                          templates_dim: int = 32) -> int:
+    """Device bytes the template branch (Alphafold2.embed_templates_) allocates beyond x and its own inputs when it runs the T
+    templates in groups of G: the grow-only workspace sized for the largest call (to_template_embed, the pair-stack modules at
+    batch b * G, the pointwise attention), plus what lives beside it: t and the crossed mask of one group and, with more than
+    one group, that group's copy of templates_feats, q and gate of x and the fp32 softmax state.  Computed from the library's
+    workspace queries: no GPU needed."""
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+    lib = _lib.load()
+    strict = precision == "strict"
+    G = max(1, min(G, T))
+    bg, P, I = b * G, b * n * n, heads * dim_head
+    rows = bg * n * n
+    sfx = "_strict" if strict else ""
+    ax = lib.af2_axial_attention_strict_workspace if strict else lib.af2_axial_attention_workspace
+    ws = [getattr(lib, f"af2_template_embed{sfx}_workspace")(rows, templates_dim),
+          getattr(lib, f"af2_triangle_multiply{sfx}_workspace")(bg, n, d),
+          ax(bg, n, n, d, heads, dim_head, 1), ax(bg, n, n, d, heads, dim_head, 0)]
+    persist = rows * d * 4 + rows                                          # t, crossed mask
+    if G == T:
+        ws.append(getattr(lib, f"af2_template_pointwise_attention{sfx}_workspace")(b, T, n, d, heads, dim_head))
+    else:
+        ws += [getattr(lib, f"af2_template_pointwise_begin{sfx}_workspace")(b, n, d),
+               getattr(lib, f"af2_template_pointwise_group{sfx}_workspace")(b, G, n, d, heads, dim_head),
+               getattr(lib, f"af2_template_pointwise_end{sfx}_workspace")(b, n, heads, dim_head)]
+        persist += rows * templates_dim * 4                                # the group's contiguous templates_feats
+        persist += P * 2 * I * (4 if strict else 2)                        # q | gate
+        persist += P * (2 * heads + I + 1) * 4                             # run_max, run_sum, acc, pooled
+    return _ws_alloc(max(ws)) + persist
+
+
+def plan_template_groups(b: int, T: int, n: int, d: int, heads: int, dim_head: int, precision: str, budget: int,
+                         templates_dim: int = 32) -> int:
+    """How many templates the template branch runs at a time: T whenever template_branch_bytes fits `budget` (bytes), else the
+    largest G that fits (the last group may be smaller), and 1 when nothing fits (the allocation then fails as it would)."""
+    if T <= 1 or template_branch_bytes(b, T, T, n, d, heads, dim_head, precision, templates_dim) <= budget:
+        return max(T, 1)
+    for G in range(T - 1, 1, -1):
+        if template_branch_bytes(b, T, G, n, d, heads, dim_head, precision, templates_dim) <= budget:
+            return G
+    return 1
+
+
+def device_budget(device) -> int:
+    """Bytes the template branch can still allocate on `device`: what the driver reports free, plus what PyTorch's caching
+    allocator holds unused, plus the current grow-only workspace (which the branch reuses)."""
+    device = torch.device(device)
+    free, _ = torch.cuda.mem_get_info(device)
+    cached = torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+    store = _WORKSPACE if _WS_PRIVATE is None else _WS_PRIVATE[0]
+    ws = store.get(device)
+    return int(free + cached + (ws.numel() if ws is not None else 0))
+
+
 def template_angle_features(pk: Packed, angles: torch.Tensor, m: torch.Tensor, row0: int) -> torch.Tensor:
     """template_angle_mlp (alphafold2.py:789-790): angles [B, T, n, K] fp32 -> rows row0 .. row0 + T - 1 of m [B, R, n, d] fp32
     (the reference concatenates them after the S MSA rows: row0 = S).  Returns m."""

@@ -377,6 +377,53 @@ int af2_template_pointwise_bf16(const void* q, const void* gate, const void* kv,
 int af2_template_pointwise_f32(const float* q, const float* gate_logits, const float* kv, const unsigned char* x_mask,
                                const unsigned char* t_mask, float* out, float* pooled, int B, int T, long long pairs, int heads,
                                int dim_head, af2_stream_t stream);
+/* The same kernel over one group of templates, carrying the online-softmax state from launch to launch: kv / t_mask hold the
+ * group's T templates only.  State, all fp32: run_max and run_sum [P][heads], acc [P][I] (16-byte aligned), and pooled [P],
+ * which holds "any template valid" (0 / 1) between groups.  first = 1: start from no state (nothing is read);  last = 1: write out
+ * and pooled as above (nothing else);  last = 0: write the state instead (out is not touched and may be NULL).  first = last = 1
+ * is af2_template_pointwise_bf16 / _f32 and the state pointers may be NULL.  Running every group in order gives out and pooled
+ * bitwise equal to one launch over all templates.  out may be q (_bf16) or acc (_f32): each element is read before it is
+ * written, by the same thread. */
+int af2_template_pointwise_bf16_state(const void* q, const void* gate, const void* kv, const unsigned char* x_mask,
+                                      const unsigned char* t_mask, void* out, float* pooled, float* run_max, float* run_sum, float* acc,
+                                      int first, int last, int B, int T, long long pairs, int heads, int dim_head, af2_stream_t stream);
+int af2_template_pointwise_f32_state(const float* q, const float* gate_logits, const float* kv, const unsigned char* x_mask,
+                                     const unsigned char* t_mask, float* out, float* pooled, float* run_max, float* run_sum, float* acc,
+                                     int first, int last, int B, int T, long long pairs, int heads, int dim_head, af2_stream_t stream);
+/* af2_template_pointwise_attention in groups of templates, so that only one group's t and k|v are in memory at a time
+ * (af2_template_pointwise_attention{,_strict} is exactly begin, one group of all T with first = last = 1, end):
+ *   begin: q, gate from x into caller-owned buffers: bf16 q [P][I] and gate [P][I] (sigmoid-ed);  strict: qg fp32 [P][2I]
+ *     = [q * dim_head^-0.5 | gating logits].  P = B n^2.
+ *   group: for G templates, t fp32 [B G][n][n][d] and their crossed mask t_mask [B G][n][n] (template g of pair (b, i, j) is
+ *     row (b G + g) n^2 + i n + j), in order over the groups with first = 1 on the first and last = 1 on the last: the k|v
+ *     projection and the state-carrying kernel above.  run_max, run_sum, acc, pooled: the caller-owned state (fp32; acc
+ *     16-byte aligned; run_max / run_sum / acc may be NULL when first = last = 1).  On the last group the gated attention output
+ *     goes to out: bf16 [P][I], which may be q;  strict fp32 [P][I], which may be acc.
+ *   end: x += pooled * (to_out(out) + b_out).
+ * The state lives in caller memory because each call draws its workspace afresh. */
+long long af2_template_pointwise_begin_workspace(int B, int n, int d);
+int af2_template_pointwise_begin(const af2_template_attn_weights* w, const float* x, int B, int n, int d, int heads, int dim_head,
+                                 void* q, void* gate, void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_group_workspace(int B, int G, int n, int d, int heads, int dim_head);
+int af2_template_pointwise_group(const af2_template_attn_weights* w, const float* t, const unsigned char* x_mask,
+                                 const unsigned char* t_mask, int B, int G, int n, int d, int heads, int dim_head, const void* q,
+                                 const void* gate, float* run_max, float* run_sum, float* acc, float* pooled, void* out, int first,
+                                 int last, void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_end_workspace(int B, int n, int heads, int dim_head);
+int af2_template_pointwise_end(const af2_template_attn_weights* w, float* x, const void* out, const float* pooled, int B, int n, int d,
+                               int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_begin_strict_workspace(int B, int n, int d);
+int af2_template_pointwise_begin_strict(const af2_template_attn_weights_strict* w, const float* x, int B, int n, int d, int heads,
+                                        int dim_head, float* qg, void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_group_strict_workspace(int B, int G, int n, int d, int heads, int dim_head);
+int af2_template_pointwise_group_strict(const af2_template_attn_weights_strict* w, const float* t, const unsigned char* x_mask,
+                                        const unsigned char* t_mask, int B, int G, int n, int d, int heads, int dim_head, const float* qg,
+                                        float* run_max, float* run_sum, float* acc, float* pooled, float* out, int first, int last,
+                                        void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_end_strict_workspace(int B, int n, int heads, int dim_head);
+int af2_template_pointwise_end_strict(const af2_template_attn_weights_strict* w, float* x, const float* out, const float* pooled, int B,
+                                      int n, int d, int heads, int dim_head, void* workspace, long long workspace_bytes,
+                                      af2_stream_t stream);
 /* to_template_embed (alphafold2.py:751): t fp32 [rows][d] = feats fp32 [rows][K] W^T + bias.  w bf16 [d][align8(K)] (zero pad
  * columns); _strict: w split [d][3][align8(K)]. */
 long long af2_template_embed_workspace(long long rows, int K);

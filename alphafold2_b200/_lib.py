@@ -92,6 +92,7 @@ _SIGNATURES = {
     "af2_triangle_project_workspace": (ll, [ll, ci]),
     "af2_triangle_contract": (ci, [C.POINTER(TriMulWeights), vp, vp, ll, vp, ll, ll, ci, vp, ci, ci, ci, ci, ci, vp, ll, vp]),
     "af2_triangle_contract_workspace": (ll, [ci, ci, ci]),
+    "af2_triangle_contract_pitched": (ci, [C.POINTER(TriMulWeights), vp, vp, ll, ll, vp, ll, ll, vp, ci, ci, ci, ci, ci, vp, ll, vp]),
     "af2_outer_project": (ci, [C.POINTER(OuterWeights), vp, vp, ll, ci, ci, vp, ll, vp, ll, vp]),
     "af2_outer_project_workspace": (ll, [ll, ci]),
     "af2_outer_contract": (ci, [C.POINTER(OuterWeights), vp, vp, ll, vp, ll, ll, ci, vp, ci, ci, ci, ci, ci, cf, vp, ll, vp]),

@@ -350,6 +350,33 @@ class OuterMean(_Packable):
 # ------------------------------------------------------------------------------------------------------
 # Evoformer blocks (alphafold2.py:353-467)
 # ------------------------------------------------------------------------------------------------------
+def _pair_band(pair, x, S, band):
+    """Pair rows per band for the pair track of `pair` (a PairwiseAttentionBlock) on x [B, N, N, d] with S MSA rows beside it:
+    N (the whole-tensor calls) when they fit 85 % of what the device can still allocate (the template planner's headroom:
+    the caching allocator cannot always reuse the blocks it frees), else ops.plan_pair_band's band.  `band` forces it (tests:
+    a multiple of 8, which keeps every operand window 16-byte aligned for TMA; the planner's bands are multiples of
+    ops.PAIR_BAND_ALIGN).  Strict mode is a parity mode and always runs whole.  Records pair.last_pair_band."""
+    N = x.shape[1]
+    ta = pair.triangle_attention_ingoing
+    if not x.is_cuda or ops.precision_of(ta) == "strict":
+        band = N
+    elif band is None:
+        shape = (x.shape[0], N, S, x.shape[3], ta.attn.heads, ta.attn.dim_head)
+        if ops.workspace_holds(x.device, ops.pair_block_bytes(*shape, N)):
+            band = N                      # the workspace already holds the whole-tensor calls: no device query per block
+        else:
+            band = ops.plan_pair_band(*shape, int(ops.device_budget(x.device) * 0.85))
+    elif int(band) < N and (int(band) <= 0 or int(band) % 8):
+        raise ValueError(f"pair band {band} must be a positive multiple of 8")
+    band = min(int(band), N)
+    if band < N and ta.global_query_attn:
+        raise NotImplementedError(
+            f"N_res {N} needs the pair track in bands of {band} rows, but tied-query column attention (global_query_attn, "
+            "the extra-MSA stack) averages its queries over all columns and cannot run in column bands")
+    pair.last_pair_band = band
+    return band
+
+
 class PairwiseAttentionBlock(nn.Module):
     def __init__(self, dim, seq_len, heads, dim_head, dropout=0., global_column_attn=False):
         super().__init__()
@@ -359,8 +386,23 @@ class PairwiseAttentionBlock(nn.Module):
         self.triangle_multiply_outgoing = TriangleMultiplicativeModule(dim=dim, mix='outgoing')
         self.triangle_multiply_ingoing = TriangleMultiplicativeModule(dim=dim, mix='ingoing')
 
-    def update_(self, x, mask=None, msa_repr=None, msa_mask=None):
-        """In-place residual chain of alphafold2.py:378-385 on an fp32 pair tensor."""
+    def update_(self, x, mask=None, msa_repr=None, msa_mask=None, band=None):
+        """In-place residual chain of alphafold2.py:378-385 on an fp32 pair tensor.
+
+        Runs in bands of pair rows (banded.pair_block_, bitwise the same result) when the whole-tensor calls would not fit
+        what the device can still allocate; `band` forces the rows per band (tests).  The band used is kept in
+        self.last_pair_band (N: today's whole-tensor calls)."""
+        band = _pair_band(self, x, msa_repr.shape[1] if exists(msa_repr) else 0, band)
+        if band < x.shape[1]:
+            from . import banded
+            from .parallel import CudaStageOps
+            st = CudaStageOps()
+            mask = mask.bool().contiguous() if exists(mask) else None
+            msa_mask = msa_mask.bool().contiguous() if exists(msa_mask) else None
+            for b in range(x.shape[0]):
+                pick = lambda t: None if t is None else t[b]  # noqa: E731
+                banded.pair_block_(self, x[b], pick(mask), pick(msa_repr), pick(msa_mask), band, st)
+            return x
         if exists(msa_repr):
             self.outer_mean.add_to_(x, msa_repr, msa_mask)
         self.triangle_multiply_outgoing.add_to_(x, mask)
@@ -404,13 +446,23 @@ class EvoformerBlock(nn.Module):
             FeedForward(dim=dim, dropout=ff_dropout),
         ])
 
-    def update_(self, x, m, mask, msa_mask):
-        """alphafold2.py:432-446 on private fp32 tensors, in place."""
+    def update_(self, x, m, mask, msa_mask, band=None):
+        """alphafold2.py:432-446 on private fp32 tensors, in place.  The pair track (pair block and transition) runs in bands
+        of pair rows when the whole-tensor calls do not fit (PairwiseAttentionBlock.update_); `band` forces it (tests).
+        The plan is made before any device work of the block."""
         attn, ff, msa_attn, msa_ff = self.layer
+        band = _pair_band(attn, x, m.shape[1], band)
+        self.last_pair_band = band
         msa_attn.update_(m, msa_mask, x)
         msa_ff.add_to_(m)
-        attn.update_(x, mask, m, msa_mask)
-        ff.add_to_(x)
+        attn.update_(x, mask, m, msa_mask, band=band)
+        if band < x.shape[1]:
+            from . import banded
+            from .parallel import CudaStageOps
+            for b in range(x.shape[0]):
+                banded.feed_forward_(ff, x[b], band, CudaStageOps())
+        else:
+            ff.add_to_(x)
         return x, m
 
     def forward(self, inputs):
@@ -436,18 +488,22 @@ class Evoformer(nn.Module):
             mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
             for layer in self.layers:
                 layer.update_(xo, mo, mk, mmk)
+                self.last_pair_band = layer.last_pair_band
         return xo.to(x.dtype), mo.to(m.dtype)
 
-    def run_(self, x, m, mask=None, msa_mask=None):
+    def run_(self, x, m, mask=None, msa_mask=None, band=None):
         """Same as forward, for callers that own fp32 contiguous x / m and allow them to be updated in place (no private
-        copies).  A sharded trunk (parallel.shard_evoformer replaces `forward`) goes through its schedule instead."""
+        copies).  A sharded trunk (parallel.shard_evoformer replaces `forward`) goes through its schedule instead.
+        `band` forces the pair rows per band of every block (tests; see PairwiseAttentionBlock.update_); the band the last
+        block used is kept in self.last_pair_band."""
         if "forward" in self.__dict__ or x.dtype != torch.float32 or m.dtype != torch.float32 or not (x.is_contiguous() and m.is_contiguous()):
             return self(x, m, mask=mask, msa_mask=msa_mask)
         with torch.no_grad():
             mk = mask.bool().contiguous() if exists(mask) else None
             mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
             for layer in self.layers:
-                layer.update_(x, m, mk, mmk)
+                layer.update_(x, m, mk, mmk, band=band)
+                self.last_pair_band = layer.last_pair_band
         return x, m
 
 

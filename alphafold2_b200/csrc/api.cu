@@ -718,8 +718,14 @@ int triangle_front(const af2_trimul_weights* w, const float* x, const unsigned c
     CUDA_OK(cudaGetLastError());
   }
   if (pitch != inner) {   // pad columns of the channel-major operands are read by TMA as K / MN padding: keep them zero
-    CUDA_OK(cudaMemsetAsync(Lc, 0, (size_t)d * chan_stride * 2, s));
-    CUDA_OK(cudaMemsetAsync(Rc, 0, (size_t)d * chan_stride * 2, s));
+    const long long span = tokens / inner * pitch;   // this call's rows of one channel
+    if (chan_stride == span) {
+      CUDA_OK(cudaMemsetAsync(Lc, 0, (size_t)d * chan_stride * 2, s));
+      CUDA_OK(cudaMemsetAsync(Rc, 0, (size_t)d * chan_stride * 2, s));
+    } else {                // a band of rows inside larger operands: only its own rows, other bands' rows stay as they are
+      CUDA_OK(cudaMemset2DAsync(Lc, (size_t)chan_stride * 2, 0, (size_t)span * 2, (size_t)d, s));
+      CUDA_OK(cudaMemset2DAsync(Rc, (size_t)chan_stride * 2, 0, (size_t)span * 2, (size_t)d, s));
+    }
   }
   const int half = w->bn / 2;
   const int npk = (d + half - 1) / half * w->bn;
@@ -1180,6 +1186,43 @@ int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc,
     }
     AF2_TRY(launch_gemm(c, s));
   }
+  return contract_tail(chan_ln_params(Oc, cs_o, cp4, rows, cols, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
+                       w->w_out, w->b_out, x, s);
+}
+
+// af2_triangle_contract of one L / R pair with explicit pitches: the operands may be windows into larger channel-major
+// tensors (the banded single-GPU schedule contracts rows [i0, i0 + rows) of the ingoing product against the column window
+// R[c][k][i0 .. i0 + rows) of the whole R).  Same GEMM tile (pick_bn(cols)) and tail as the whole-tensor call.
+//   outgoing: L [c][rows][ld_l] (k < K), R [c][cols][ld_r] (k < K)
+//   ingoing : L [c][K][ld_l] (j < cols), R [c][K][ld_r] (i < rows)
+int af2_triangle_contract_pitched(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, long long ld_l,
+                                  const void* Rc, long long cs_r, long long ld_r, const void* gate, int rows, int cols, int K,
+                                  int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream) {
+  NvtxRange nvtx_("af2_triangle_contract_pitched");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!w || !x || !Lc || !Rc || !gate) return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: null argument");
+  if (rows <= 0 || cols <= 0 || K <= 0 || d % 32) return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: rows %d cols %d K %d d %d", rows, cols, K, d);
+  if (ld_l % 8 || ld_r % 8 || cs_l % 8 || cs_r % 8)
+    return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: pitches and channel strides must be multiples of 8 elements");
+  const long long mn_l = ingoing ? cols : K, mn_r = ingoing ? rows : K;   // elements used along each operand's pitch
+  if (ld_l < mn_l || ld_r < mn_r) return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: pitch shorter than the operand row");
+  const long long T = (long long)rows * cols;
+  const int cp4 = (int)align_up(cols, 4);
+  const long long cs_o = (long long)rows * cp4;
+  Arena ar(workspace, workspace_bytes);
+  float* Oc = ar.take<float>(d * cs_o);
+  __nv_bfloat16* tn = ar.take<__nv_bfloat16>(T * d);
+  if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_contract_pitched: workspace too small");
+  GemmCall c;
+  memset(&c, 0, sizeof(c));
+  c.batch = d; c.K = K; c.M = rows; c.N = cols; c.bn = pick_bn(cols);
+  c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = Oc; c.ld_out = cp4; c.out_batch = cs_o;
+  if (!ingoing) {   // O_c = L_c R_c^T, both K-major
+    c.A = Lc; c.lda = ld_l; c.a_batch = cs_l; c.Bm = Rc; c.ldb = ld_r; c.b_batch = cs_r; c.mn_major = false;
+  } else {          // O_c[i][j] = sum_k R_c[k][i] L_c[k][j], both MN-major
+    c.A = Rc; c.lda = ld_r; c.a_batch = cs_r; c.Bm = Lc; c.ldb = ld_l; c.b_batch = cs_l; c.mn_major = true;
+  }
+  AF2_TRY(launch_gemm(c, s));
   return contract_tail(chan_ln_params(Oc, cs_o, cp4, rows, cols, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
                        w->w_out, w->b_out, x, s);
 }

@@ -5,6 +5,7 @@ PyTorch is used for device memory and streams only; every FLOP of the hot path r
 from __future__ import annotations
 
 import ctypes as C
+import functools
 from typing import Dict, Optional
 
 import torch
@@ -899,9 +900,69 @@ def plan_template_groups(b: int, T: int, n: int, d: int, heads: int, dim_head: i
     return 1
 
 
+PAIR_BAND_ALIGN = 256      # band boundaries: every band call then picks the whole-tensor call's GEMM tile and chan_to_token kernel
+
+
+def _align8(n: int) -> int:
+    return (n + 7) // 8 * 8
+
+
+@functools.lru_cache(maxsize=256)
+def pair_block_bytes(B: int, N: int, S: int, d: int, heads: int, dim_head: int, R: int) -> int:
+    """Device bytes one Evoformer block (bf16 path) allocates beyond x [B, N, N, d] and m [B, S, N, d] when its pair track runs
+    in bands of R pair rows (EvoformerBlock.update_; S = 0: a pair block without the MSA track, as in the template stack).
+    R >= N is today's whole-tensor schedule: the grow-only workspace sized for its largest call.  R < N: the workspace sized
+    for the MSA track and one band's calls, plus the largest set of operands one pair stage keeps for the whole tensor
+    (triangle multiply: L, R and gate of all rows; column attention: the pair bias and one column band's copy of x and of
+    the mask; outer mean: the projected m and one band's left operand).  Computed from the library's workspace queries."""
+    lib = _lib.load()
+    ax = lib.af2_axial_attention_workspace
+    ff = lambda tokens: lib.af2_feed_forward_workspace(tokens, d, 4 * d)  # noqa: E731
+    ws = [ax(B, S, N, d, heads, dim_head, 1), ax(B, S, N, d, heads, dim_head, 0), ff(B * S * N)] if S > 0 else []
+    if R >= N:
+        if S > 0:
+            ws.append(lib.af2_outer_mean_workspace(B, S, N, d))
+        ws += [lib.af2_triangle_multiply_workspace(B, N, d), ax(B, N, N, d, heads, dim_head, 1), ax(B, N, N, d, heads, dim_head, 0),
+               ff(B * N * N)]
+        return _ws_alloc(max(ws))
+    np8 = _align8(N)
+    ws += [lib.af2_triangle_project_workspace(R * N, d), lib.af2_triangle_contract_workspace(R, N, d),
+           ax(1, R, N, d, heads, dim_head, 1), ax(1, N, R, d, heads, dim_head, 0), ff(R * N)]
+    keep = [2 * d * N * np8 * 2 + N * N * d * 2,                               # triangle multiply: L, R, gate
+            heads * N * np8 * 2 + N * R * (d * 4 + 1)]                         # column attention: bias, band of x and mask
+    if S > 0:
+        ws += [lib.af2_outer_project_workspace(S * N, d), lib.af2_outer_contract_workspace(R, N, d)]
+        keep.append(2 * d * S * np8 * 2 + d * S * _align8(R) * 2)             # outer mean: projected m, band's left operand
+    return _ws_alloc(max(ws)) + max(keep)
+
+
+def plan_pair_band(B: int, N: int, S: int, d: int, heads: int, dim_head: int, budget: int) -> int:
+    """Pair rows per band of one Evoformer block: N (today's whole-tensor calls) whenever pair_block_bytes(..., N) fits `budget`
+    (bytes), else the largest multiple of PAIR_BAND_ALIGN below N that fits.  Raises MemoryError when not even one band of
+    PAIR_BAND_ALIGN rows fits."""
+    if pair_block_bytes(B, N, S, d, heads, dim_head, N) <= budget:
+        return N
+    R = (N - 1) // PAIR_BAND_ALIGN * PAIR_BAND_ALIGN
+    while R >= PAIR_BAND_ALIGN:
+        if pair_block_bytes(B, N, S, d, heads, dim_head, R) <= budget:
+            return R
+        R -= PAIR_BAND_ALIGN
+    least = pair_block_bytes(B, N, S, d, heads, dim_head, min(PAIR_BAND_ALIGN, N))
+    raise MemoryError(f"one Evoformer block at N_res {N} (batch {B}, {S} MSA rows, dim {d}) needs {least / 2**30:.2f} GiB beyond "
+                      f"x and m even in bands of {PAIR_BAND_ALIGN} pair rows; {budget / 2**30:.2f} GiB can be allocated")
+
+
+def workspace_holds(device, nbytes: int) -> bool:
+    """Whether the current grow-only workspace of `device` is already at least `nbytes` (a call needing no more allocates
+    nothing)."""
+    store = _WORKSPACE if _WS_PRIVATE is None else _WS_PRIVATE[0]
+    ws = store.get(torch.device(device))
+    return ws is not None and ws.numel() >= nbytes
+
+
 def device_budget(device) -> int:
-    """Bytes the template branch can still allocate on `device`: what the driver reports free, plus what PyTorch's caching
-    allocator holds unused, plus the current grow-only workspace (which the branch reuses)."""
+    """Bytes the template branch or a pair block can still allocate on `device`: what the driver reports free, plus what
+    PyTorch's caching allocator holds unused, plus the current grow-only workspace (which every op reuses)."""
     device = torch.device(device)
     free, _ = torch.cuda.mem_get_info(device)
     cached = torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)

@@ -373,22 +373,36 @@ class CudaStageOps:
                                           None if mk is None else mk.data_ptr(), row0, rows, N, S, d, float(om.eps),
                                           ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
 
-    def tri_project(self, tm, x_loc: torch.Tensor, mask_loc: Optional[torch.Tensor]):
-        """x [rows, cols, d] -> (L, R) bf16 [d, rows, align8(cols)] channel-major, gate bf16 [rows*cols, d]."""
+    def tri_operands(self, N: int, d: int, like: torch.Tensor):
+        """Whole-tensor triangle-multiply operands for the banded schedule: L, R bf16 [d, N, align8(N)] (pad columns zero),
+        gate bf16 [N*N, d]; tri_project(out=...) fills them band by band."""
+        L = torch.zeros(d, N, _align8(N), dtype=torch.bfloat16, device=like.device)
+        return L, torch.zeros_like(L), torch.empty(N * N, d, dtype=torch.bfloat16, device=like.device)
+
+    def tri_project(self, tm, x_loc: torch.Tensor, mask_loc: Optional[torch.Tensor], out=None):
+        """x [rows, cols, d] -> (L, R) bf16 [d, rows, align8(cols)] channel-major, gate bf16 [rows*cols, d].
+        out = (L, R, gate): write into these instead, e.g. the row window [:, i0:i1] of tri_operands' L and R (their channel
+        stride is kept) and rows [i0*cols, i1*cols) of its gate."""
         pk = tm.packed()
         rows, cols, d = x_loc.shape
-        L = torch.empty(d, rows, _align8(cols), dtype=torch.bfloat16, device=x_loc.device)
-        R = torch.empty_like(L)
-        gate = torch.empty(rows * cols, d, dtype=torch.bfloat16, device=x_loc.device)
+        if out is None:
+            L = torch.empty(d, rows, _align8(cols), dtype=torch.bfloat16, device=x_loc.device)
+            R = torch.empty_like(L)
+            gate = torch.empty(rows * cols, d, dtype=torch.bfloat16, device=x_loc.device)
+        else:
+            L, R, gate = out
+            if L.stride() != R.stride() or tuple(L.shape) != (d, rows, _align8(cols)) or L.stride(1) != _align8(cols):
+                raise ValueError("tri_project: out L / R must be [d, rows, align8(cols)] windows with one channel stride")
         lib = _lib.load()
         ws = _ops.workspace(lib.af2_triangle_project_workspace(rows * cols, d), x_loc.device)
         mk = None if mask_loc is None else mask_loc.contiguous()
         _lib.check(lib.af2_triangle_project(C.byref(pk.struct), x_loc.data_ptr(), None if mk is None else mk.data_ptr(),
-                                            rows * cols, cols, d, L.data_ptr(), R.data_ptr(), rows * _align8(cols),
+                                            rows * cols, cols, d, L.data_ptr(), R.data_ptr(), L.stride(0),
                                             gate.data_ptr(), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
         return L, R, gate
 
     def tri_contract_(self, tm, x_loc: torch.Tensor, L: torch.Tensor, Rg: torch.Tensor, gate: torch.Tensor, ingoing: bool, pieces: int):
+        """L may be a row window of a larger channel-major operand (its channel stride is passed on)."""
         pk = tm.packed()
         rows, cols, d = x_loc.shape
         K = L.shape[1] if ingoing else cols
@@ -397,9 +411,22 @@ class CudaStageOps:
         lib = _lib.load()
         ws = _ops.workspace(lib.af2_triangle_contract_workspace(rows, cols, d), x_loc.device)
         per_piece = Rg.numel() // pieces
-        _lib.check(lib.af2_triangle_contract(C.byref(pk.struct), x_loc.data_ptr(), L.data_ptr(), L.shape[1] * L.shape[2],
-                                             Rg.data_ptr(), Rg.shape[1] * Rg.shape[2], per_piece, pieces, gate.data_ptr(),
+        _lib.check(lib.af2_triangle_contract(C.byref(pk.struct), x_loc.data_ptr(), L.data_ptr(), L.stride(0),
+                                             Rg.data_ptr(), Rg.stride(0), per_piece, pieces, gate.data_ptr(),
                                              rows, cols, K, d, int(ingoing), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
+
+    def tri_contract_window_(self, tm, x_rows: torch.Tensor, L: torch.Tensor, R_win: torch.Tensor, gate: torch.Tensor):
+        """Ingoing contraction of pair rows [i0, i1): x_rows [rows, N, d] += to_out(LN_c(O) * gate) with
+        O[i][j] = sum_k R[k][i0 + i] L[k][j]; L bf16 [d, N, align8(N)], R_win = R[:, :, i0:i1] (a column window, read in
+        place through af2_triangle_contract_pitched), gate [rows*N, d]."""
+        pk = tm.packed()
+        rows, cols, d = x_rows.shape
+        K = L.shape[1]
+        lib = _lib.load()
+        ws = _ops.workspace(lib.af2_triangle_contract_workspace(rows, cols, d), x_rows.device)
+        _lib.check(lib.af2_triangle_contract_pitched(C.byref(pk.struct), x_rows.data_ptr(), L.data_ptr(), L.stride(0), L.stride(1),
+                                                     R_win.data_ptr(), R_win.stride(0), R_win.stride(1), gate.data_ptr(), rows, cols,
+                                                     K, d, 1, ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -131,6 +131,13 @@ int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc,
                           long long cs_r, long long piece_stride, int pieces, const void* gate, int rows, int cols,
                           int K, int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);
 long long af2_triangle_contract_workspace(int rows, int cols, int d);
+/* af2_triangle_contract of one L / R pair with explicit pitches ld_l / ld_r (elements, multiples of 8) and channel strides
+ * cs_l / cs_r: the operands may be windows into larger channel-major tensors.  Workspace: af2_triangle_contract_workspace.
+ *   outgoing: L [c][rows][ld_l] (k < K), R [c][cols][ld_r] (k < K)
+ *   ingoing : L [c][K][ld_l] (j < cols), R [c][K][ld_r] (i < rows; e.g. the column window R[c][k][i0 .. i0 + rows)) */
+int af2_triangle_contract_pitched(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, long long ld_l,
+                                  const void* Rc, long long cs_r, long long ld_r, const void* gate, int rows, int cols, int K,
+                                  int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);
 /* LN + left|right projections of m [S, inner, d] (masked) -> channel-major LRc [2d][chan_stride] */
 int af2_outer_project(const af2_outer_weights* w, const float* m, const unsigned char* msa_mask, long long tokens,
                       int inner, int d, void* LRc, long long chan_stride, void* workspace, long long workspace_bytes,

@@ -118,6 +118,7 @@ _SIGNATURES = {
     "af2_embed_pair_init_workspace": (ll, [ci, ci, ci]),
     "af2_embed_pair_init": (ci, [vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, vp, ll, vp]),
     "af2_distogram_head": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]),
+    "af2_angle_heads": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
     "af2_recycle_embed": (ci, [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, ll, ci, ci, ci, cf, vp]),
     "af2_split_bf16": (ci, [vp, vp, ll, ci, vp]),
     "af2_gemm_split_f32": (ci, [vp, vp, vp, ll, ci, ci, ci, ci, vp]),

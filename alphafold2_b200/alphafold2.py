@@ -236,6 +236,30 @@ class _TemplateAngleMLP(_Packable, nn.Sequential):
         return ops.template_angle_features(self.packed(), angles, m, row0)
 
 
+class _AngleHeads(_Packable):
+    """Packed weights of the three angle heads for af2_angle_heads.  to_prob_theta / to_prob_phi / to_prob_omega stay the model's
+    own nn.Linear modules (the reference's state_dict keys); this cache is kept outside the module tree and keys on their
+    parameters."""
+
+    def __init__(self, theta: nn.Linear, phi: nn.Linear, omega: nn.Linear):
+        super().__init__()
+        self.__dict__["heads"] = (theta, phi, omega)
+
+    def parameters(self, recurse: bool = True):
+        for h in self.heads:
+            yield from h.parameters(recurse)
+
+    def buckets(self):
+        return tuple(h.out_features for h in self.heads)
+
+    def _pack(self):
+        t, p, o = self.heads
+        return ops.pack_angle_heads(t.weight, t.bias, p.weight, p.bias, o.weight, o.bias)
+
+    def run(self, x, symmetrize_omega: bool):
+        return ops.angle_heads(self.packed(), x, symmetrize_omega)
+
+
 class AxialAttention(_Packable):
     def __init__(self, dim, heads, row_attn=True, col_attn=True, accept_edges=False, global_query_attn=False, **kwargs):
         super().__init__()
@@ -574,6 +598,14 @@ class Alphafold2(nn.Module):
         self.recycling_distance_buckets = recycling_distance_buckets
         self._warned_training = False
 
+    def angle_heads(self) -> _AngleHeads:
+        """The packed-weight cache of to_prob_theta / to_prob_phi / to_prob_omega (predict_angles=True only)."""
+        ah = self.__dict__.get("_angle_heads")
+        if ah is None or ah.heads != (self.to_prob_theta, self.to_prob_phi, self.to_prob_omega):
+            ah = _AngleHeads(self.to_prob_theta, self.to_prob_phi, self.to_prob_omega)
+            self.__dict__["_angle_heads"] = ah
+        return ah
+
     def _check_templates(self, seq, mask, templates_feats, templates_mask, templates_angles):
         """The template inputs the reference cannot handle crash it inside einops / torch.cat; here they raise ValueError up
         front, before any device work."""
@@ -753,7 +785,9 @@ class Alphafold2(nn.Module):
             x, m = self.net.run_(x, m, mask=x_mask, msa_mask=msa_mask)     # alphafold2.py:802-807
 
             ret = ReturnValues()
-            if self.predict_angles:
+            fused_angles = self.predict_angles and x.is_cuda and x.dtype == torch.float32 and \
+                ops.angle_heads_ok(x.shape[-1], self.angle_heads().buckets())
+            if self.predict_angles and not fused_angles:
                 ret.theta_logits = self.to_prob_theta(x)
                 ret.phi_logits = self.to_prob_phi(x)
             ln, lin = self.to_distogram_logits[0], self.to_distogram_logits[1]
@@ -764,7 +798,10 @@ class Alphafold2(nn.Module):
             else:
                 trunk_embeds = (x + x.transpose(1, 2)) * 0.5
                 ret.distance = self.to_distogram_logits(trunk_embeds)
-            if self.predict_angles:
+            if fused_angles:
+                # alphafold2.py:813-836 in one kernel that reads x once: omega's (x + x^T) / 2 is formed on chip
+                ret.theta_logits, ret.phi_logits, ret.omega_logits = self.angle_heads().run(x.contiguous(), self.symmetrize_omega)
+            elif self.predict_angles:
                 if self.symmetrize_omega and trunk_embeds is None:
                     trunk_embeds = (x + x.transpose(1, 2)) * 0.5
                 ret.omega_logits = self.to_prob_omega(trunk_embeds if self.symmetrize_omega else x)

@@ -20,6 +20,7 @@
 #include "strict_kernels.cuh"
 #include "glue_kernels.cuh"
 #include "template_attn.cuh"
+#include "heads.cuh"
 
 using namespace af2;
 
@@ -1423,3 +1424,4 @@ int af2_outer_scale(const unsigned char* mask, float* scale, void* words, int ro
 #include "strict_api.inl"
 #include "peer_api.inl"
 #include "template_api.inl"
+#include "heads_api.inl"

@@ -448,6 +448,49 @@ def distogram_head(x, ln_w, ln_b, w, b) -> torch.Tensor:
     return out
 
 
+ANGLE_COLS = 64          # output columns of af2_angle_heads' tile (csrc/heads.cuh: AH_COLS)
+
+
+def angle_heads_ok(d: int, buckets) -> bool:
+    """Whether af2_angle_heads takes dim d and buckets (n_theta, n_phi, n_omega) in both omega modes (include/af2b200.h)."""
+    nt, np_, no = (int(v) for v in buckets)
+    row0 = min((nt + np_) // 8 * 8, 32)      # the symmetrised pass's 32-row weight window (csrc/heads_api.inl)
+    return (d % 32 == 0 and 0 < d <= 320 and min(nt, np_, no) >= 1 and nt + np_ + no <= ANGLE_COLS
+            and nt + np_ - row0 + no <= 32)
+
+
+def pack_angle_heads(w_theta, b_theta, w_phi, b_phi, w_omega, b_omega) -> Packed:
+    """The three heads as one 64-row weight [W_t; W_p; W_o; 0] in split-bf16 planes, bf16 [d / 32][3][64][32], and its bias [64]."""
+    ws = [w.detach().float() for w in (w_theta, w_phi, w_omega)]
+    d = ws[0].shape[1]
+    rows = sum(w.shape[0] for w in ws)
+    w = torch.zeros(ANGLE_COLS, d, dtype=torch.float32, device=ws[0].device)
+    w[:rows] = torch.cat(ws, 0)
+    bias = torch.zeros(ANGLE_COLS, dtype=torch.float32, device=w.device)
+    bias[:rows] = torch.cat([b.detach().float() for b in (b_theta, b_phi, b_omega)])
+    planes = split_weight(w).reshape(ANGLE_COLS, SPLIT_PLANES, d // 32, 32).permute(2, 1, 0, 3).contiguous()
+    pk = Packed(None, dict(planes=planes, bias=bias), "split")
+    pk.buckets = tuple(int(t.shape[0]) for t in ws)
+    return pk
+
+
+def angle_heads(pk: Packed, x: torch.Tensor, symmetrize_omega: bool):
+    """alphafold2.py:813-836: (theta, phi, omega) logits [b, n, n, buckets] fp32 from the trunk output x [b, n, n, d] in one kernel
+    that reads x once; omega from (x + x^T) / 2 when symmetrize_omega, formed in shared memory (no temporary of x's size)."""
+    _require(x, torch.float32, "x")
+    B, n, n2, d = x.shape
+    if n != n2:
+        raise ValueError(f"x must be [b, n, n, d], got {tuple(x.shape)}")
+    nt, np_, no = pk.buckets
+    theta = torch.empty(B, n, n, nt, dtype=torch.float32, device=x.device)
+    phi = torch.empty(B, n, n, np_, dtype=torch.float32, device=x.device)
+    omega = torch.empty(B, n, n, no, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.load().af2_angle_heads(x.data_ptr(), pk.tensors["planes"].data_ptr(), pk.tensors["bias"].data_ptr(),
+                                           theta.data_ptr(), phi.data_ptr(), omega.data_ptr(), B, n, d, nt, np_, no,
+                                           int(bool(symmetrize_omega)), _stream_ptr()))
+    return theta, phi, omega
+
+
 _RECYCLE_BOUNDARIES: Dict[tuple, torch.Tensor] = {}
 
 

@@ -327,6 +327,17 @@ int af2_embed_pair_init(const long long* seq, const long long* msa, const float*
                         long long workspace_bytes, af2_stream_t stream);
 int af2_distogram_head(const float* x, const float* gamma, const float* beta, const float* w, const float* bias, float* out, int B,
                        int n, int d, int buckets, af2_stream_t stream);
+/* af2_angle_heads: alphafold2.py:813-836 (predict_angles) -- one pass over x [B][n][n][d] fp32:
+ *   theta[b][i][j] = W_t x[b][i][j] + b_t    [B][n][n][n_theta]      phi = W_p x + b_p    [B][n][n][n_phi]
+ *   omega[b][i][j] = W_o s + b_o             [B][n][n][n_omega],     s = (x[b][i][j] + x[b][j][i]) * 0.5 if symmetrize, else x[b][i][j]
+ *   (symmetrized, omega is bitwise symmetric in i, j).  fp32 results from split-bf16 tensor-core passes: the same kernel serves
+ *   both precision modes.
+ *   w_planes: bf16 [d / 32][3][64][32], the three split planes (p0 = bf16(w), p1 = bf16(w - p0), p2 = bf16(w - p0 - p1)) of the
+ *     64-row weight [W_t; W_p; W_o; zero rows], 32 channels per block; bias [64] fp32 [b_t; b_p; b_o; zeros].
+ *   d % 32 == 0 and d <= 320 (dim 320 symmetrized, 384 otherwise: shared memory); n_theta + n_phi + n_omega <= 64; symmetrized,
+ *   omega's columns fit the 32-column window from min(8 floor((n_theta + n_phi) / 8), 32).  x and w_planes 16-byte aligned.  No workspace.  Otherwise AF2_ERR_BAD_ARG. */
+int af2_angle_heads(const float* x, const void* w_planes, const float* bias, float* theta, float* phi, float* omega, int B, int n,
+                    int d, int n_theta, int n_phi, int n_omega, int symmetrize, af2_stream_t stream);
 /* af2_recycle_embed: alphafold2.py:730-739 -- the recycling embedder, in place, one launch:
  *   x[b][i][j] = (x[b][i][j] + LN_pair(prev_pair[b][i][j])) + table[k(b, i, j)]        x, prev_pair [B][n][n][d]
  *   m[b][0][j] = m[b][0][j] + LN_msa(single_row[b][j])                                 single_row [B][n][d]; no other row of m changes

@@ -48,3 +48,14 @@ if case in ("all", "strict") and os.environ.get("AF2_SAN_STRICT", "1") != "0" an
         print("strict block ok")
     except NotImplementedError as e:
         print("strict mode not built:", e)
+if case in ("all", "angles"):
+    # angle heads: ragged n (a partial last tile), two batch elements, both omega modes
+    model = A.Alphafold2(dim=64, depth=1, heads=2, dim_head=32, predict_angles=True)
+    randomize_zero_init_(model)
+    model = model.cuda().eval()
+    x = torch.randn(2, 19, 19, 64, device="cuda")
+    for sym in (False, True):
+        out = model.angle_heads().run(x, sym)
+        torch.cuda.synchronize()
+        assert all(torch.isfinite(o).all() for o in out)
+    print("angle heads ok")

@@ -158,6 +158,13 @@ _SIGNATURES = {
                                                  vp, vp, vp, ci, ci, vp, ll, vp]),
     "af2_template_pointwise_end_strict_workspace": (ll, [ci, ci, ci, ci]),
     "af2_template_pointwise_end_strict": (ci, [C.POINTER(TemplateAttnWeightsStrict), vp, vp, vp, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_template_pointwise_rows_begin_workspace": (ll, [ll, ci]),
+    "af2_template_pointwise_rows_begin": (ci, [C.POINTER(TemplateAttnWeights), vp, ll, ci, ci, ci, vp, vp, vp, ll, vp]),
+    "af2_template_pointwise_rows_group_workspace": (ll, [ci, ll, ci, ci, ci]),
+    "af2_template_pointwise_rows_group": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, ci, ll, ll, ci, ci, ci, vp, vp, vp, vp, vp,
+                                               vp, vp, ci, ci, vp, ll, vp]),
+    "af2_template_pointwise_rows_end_workspace": (ll, [ll, ci, ci]),
+    "af2_template_pointwise_rows_end": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, ll, ci, ci, ci, vp, ll, vp]),
     "af2_template_embed": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),
     "af2_template_embed_workspace": (ll, [ll, ci]),
     "af2_template_embed_strict": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),

@@ -628,18 +628,42 @@ class Alphafold2(nn.Module):
             if tuple(templates_mask.shape) != tuple(templates_angles.shape[:3]):
                 raise ValueError(f"templates_mask must be {tuple(templates_angles.shape[:3])}, got {tuple(templates_mask.shape)}")
 
-    def template_pair_stack(self, templates_feats, templates_mask):
+    def template_pair_stack(self, templates_feats, templates_mask, band=None):
         """alphafold2.py:751-760: t = to_template_embed(feats) -> [b * T, n, n, d] fp32, then templates_embed_layers passes of
-        the SAME template_pairwise_embedder (shared weights, no OuterMean) under the crossed mask.  Returns (t, crossed mask)."""
+        the SAME template_pairwise_embedder (shared weights, no OuterMean) under the crossed mask.  Returns (t, crossed mask).
+        `band` forces the pair rows per band of the pair blocks (PairwiseAttentionBlock.update_)."""
         b, T, n = templates_feats.shape[:3]
         tm = templates_mask.bool()
         tm2 = (tm[:, :, :, None] & tm[:, :, None, :]).reshape(b * T, n, n).contiguous()
         t = self.to_template_embed.embed(templates_feats.detach().float().contiguous()).reshape(b * T, n, n, -1)
         for _ in range(self.templates_embed_layers):
-            self.template_pairwise_embedder.update_(t, tm2)
+            self.template_pairwise_embedder.update_(t, tm2, band=band)
         return t, tm2
 
-    def embed_templates_(self, x, x_mask, templates_feats, templates_mask, group=None):
+    def _template_plan(self, x, templates_feats, group, band):
+        """(G, band) of embed_templates_; band = n is the whole-tensor path.  Strict mode (a parity mode) is never banded."""
+        b, T = templates_feats.shape[:2]
+        n, d = x.shape[1], x.shape[3]
+        attn = self.template_pointwise_attn
+        strict = ops.precision_of(attn) == "strict"
+        if band is not None and not strict and int(band) < n and (int(band) <= 0 or int(band) % 8):
+            raise ValueError(f"template band {band} must be a positive multiple of 8")
+        forced = band is not None and not strict
+        band = min(int(band), n) if forced else n
+        if group is None and forced and band < n:
+            group = 1                                    # forced bands: one template at a time, as the planner bands
+        elif group is None:
+            # 15 % headroom: the caching allocator cannot always reuse the blocks it frees (a growing workspace is allocated
+            # before the old one is released); plans right at the limit ran out of memory at N_res 1024 and 2048 on an H100
+            budget = int(ops.device_budget(x.device) * 0.85)
+            plan = (b, T, n, d, attn.heads, attn.dim_head, ops.precision_of(attn), budget, templates_feats.shape[-1])
+            if forced:
+                group = ops.plan_template_groups(*plan)
+            else:
+                group, band = ops.plan_template_branch(*plan)
+        return max(1, min(int(group), T)), band
+
+    def embed_templates_(self, x, x_mask, templates_feats, templates_mask, group=None, band=None):
         """alphafold2.py:743-785 in place on the fp32 pair tensor x [b, n, n, d]: template pair stack, then the pointwise
         attention of every pair over its T templates, scaled by `any template valid` and added to x.  Under shard_evoformer
         every rank computes this whole (it runs before the sharded trunk).
@@ -647,18 +671,29 @@ class Alphafold2(nn.Module):
         The templates run in groups of G: each group's pair stack at batch b * G, then its step of the pointwise attention,
         whose online softmax carries over to the next group.  The result does not depend on G (bitwise), only the memory does:
         G = T when the whole branch fits what the device can still allocate (ops.plan_template_groups), fewer otherwise.
-        `group` forces G (tests).  The G used is kept in self.last_template_group."""
-        b, T = templates_feats.shape[:2]
-        n, d = x.shape[1], x.shape[3]
+        `group` forces G (tests).  The G used is kept in self.last_template_group.
+
+        When not even one template fits (bf16 mode), the pointwise attention runs in bands of pair rows as well
+        (ops.plan_template_branch, ops.TemplateAttentionRows): per group the pair stack, in the same bands, then per batch
+        element and band q and gate of the band's rows of x, the group's k|v of those rows and the state-carrying kernel,
+        and after the last group to_out into the band's rows of x.  Only the softmax state is kept for every pair; the result
+        is bitwise the same.  `band` forces the rows per band (tests: a positive multiple of 8).  The band used is kept in
+        self.last_template_band (n: the whole-tensor calls)."""
+        T = templates_feats.shape[1]
+        n = x.shape[1]
         attn = self.template_pointwise_attn
-        if group is None:
-            # 15 % headroom: the caching allocator cannot always reuse the blocks it frees (a growing workspace is allocated
-            # before the old one is released); plans right at the limit ran out of memory at N_res 1024 and 2048 on an H100
-            budget = int(ops.device_budget(x.device) * 0.85)
-            group = ops.plan_template_groups(b, T, n, d, attn.heads, attn.dim_head, ops.precision_of(attn), budget,
-                                             templates_feats.shape[-1])
-        G = max(1, min(int(group), T))
+        G, band = self._template_plan(x, templates_feats, group, band)
         self.last_template_group = G
+        self.last_template_band = band
+        if band < n:
+            ops.release_workspace(x.device)          # the plan counted it as free: the softmax state may need its memory
+            acc = ops.TemplateAttentionRows(attn.packed(), x, x_mask, attn.heads, attn.dim_head, band)
+            for t0 in range(0, T, G):
+                t1 = min(t0 + G, T)
+                t, tm2 = self.template_pair_stack(templates_feats[:, t0:t1], templates_mask[:, t0:t1], band=band)
+                acc.add(t, tm2, last=t1 == T)
+                del t, tm2
+            return x
         if G == T:
             t, tm2 = self.template_pair_stack(templates_feats, templates_mask)
             attn.add_context_(x, t, x_mask, tm2)

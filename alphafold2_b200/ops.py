@@ -895,17 +895,86 @@ class TemplateAttentionGroups:
                           ws.data_ptr(), ws.numel(), _stream_ptr()))
 
 
+class TemplateAttentionRows:
+    """TemplateAttentionGroups one band of pair rows at a time (af2_template_pointwise_rows_begin / _group / _end, bf16 only):
+        r = TemplateAttentionRows(pk, x, x_mask, heads, dim_head, band)
+        r.add(t, t_mask, last=False) ...; r.add(t, t_mask, last=True)      # t [B * G, n, n, d], t_mask [B * G, n, n] per group
+    Each add() runs, per batch element and band of `band` pair rows, q and gate of the band's rows of x, the k|v projection of
+    the band's rows of the group's templates and the state-carrying kernel; the last one also adds to_out to the band's rows of
+    x.  Between the calls only the fp32 softmax state is kept for every pair; q, gate and k|v exist for one band at a time.
+    x changes only in the last add(), band by band, after the band's own q and gate are made, so the result is bitwise that of
+    TemplateAttentionGroups."""
+
+    def __init__(self, pk: Packed, x: torch.Tensor, x_mask: Optional[torch.Tensor], heads: int, dim_head: int, band: int):
+        _require(x, torch.float32, "x")
+        if pk.kind == "strict":
+            raise NotImplementedError("the pointwise template attention runs in bands of pair rows in bf16 mode only")
+        if x.dim() != 4 or x.shape[1] != x.shape[2]:
+            raise ValueError(f"x must be [B, n, n, d], got {tuple(x.shape)}")
+        B, n, _, d = x.shape
+        if int(band) <= 0 or (int(band) < n and int(band) % 8):
+            raise ValueError(f"template band {band} must be a positive multiple of 8")
+        self.pk, self.x, self.heads, self.dim_head, self.band = pk, x, heads, dim_head, min(int(band), n)
+        self.xm = _mask_u8(x_mask, (B, n, n), "x_mask")
+        self.first, self.done = True, False
+        P, I, dev = B * n * n, heads * dim_head, x.device
+        self.run_max = torch.empty(P, heads, dtype=torch.float32, device=dev)
+        self.run_sum = torch.empty(P, heads, dtype=torch.float32, device=dev)
+        self.acc = torch.empty(P, I, dtype=torch.float32, device=dev)
+        self.pooled = torch.empty(P, dtype=torch.float32, device=dev)
+        W = self.band * n
+        self.q = torch.empty(W, I, dtype=torch.bfloat16, device=dev)      # the last group writes the gated output over q
+        self.gate = torch.empty(W, I, dtype=torch.bfloat16, device=dev)
+
+    def add(self, t: torch.Tensor, t_mask: Optional[torch.Tensor], last: bool) -> None:
+        """One group of templates over every band; on the last one (last=True) x gets the attention output."""
+        if self.done:
+            raise RuntimeError("TemplateAttentionRows: the last group has already been added")
+        _require(t, torch.float32, "t")
+        x = self.x
+        B, n, _, d = x.shape
+        if t.dim() != 4 or t.shape[0] % B or t.shape[0] == 0 or tuple(t.shape[1:]) != (n, n, d):
+            raise ValueError(f"t must be [B * G, {n}, {n}, {d}], got {tuple(t.shape)}")
+        G = t.shape[0] // B
+        tm = _mask_u8(t_mask, (B * G, n, n), "t_mask")
+        lib = _lib.load()
+        h, dh, R, nn = self.heads, self.dim_head, self.band, n * n
+        W = R * n
+        ws = workspace(max(lib.af2_template_pointwise_rows_begin_workspace(W, d),
+                           lib.af2_template_pointwise_rows_group_workspace(G, W, d, h, dh),
+                           lib.af2_template_pointwise_rows_end_workspace(W, h, dh)), x.device)
+        I, q, gate, s, w = h * dh, self.q.data_ptr(), self.gate.data_ptr(), _stream_ptr(), C.byref(self.pk.struct)
+        for b in range(B):
+            for i0 in range(0, n, R):
+                P = (min(i0 + R, n) - i0) * n
+                o, ot = b * nn + i0 * n, b * G * nn + i0 * n             # window offsets in x and in template 0 of t
+                _lib.check(lib.af2_template_pointwise_rows_begin(w, _addr(x, o * d), P, d, h, dh, q, gate, ws.data_ptr(), ws.numel(), s))
+                _lib.check(lib.af2_template_pointwise_rows_group(
+                    w, _addr(t, ot * d), None if self.xm is None else _addr(self.xm, o), None if tm is None else _addr(tm, ot), G, P, nn,
+                    d, h, dh, q, gate, _addr(self.run_max, o * h), _addr(self.run_sum, o * h), _addr(self.acc, o * I),
+                    _addr(self.pooled, o), q, int(self.first), int(last), ws.data_ptr(), ws.numel(), s))
+                if last:
+                    _lib.check(lib.af2_template_pointwise_rows_end(w, _addr(x, o * d), q, _addr(self.pooled, o), P, d, h, dh,
+                                                                   ws.data_ptr(), ws.numel(), s))
+        self.first = False
+        self.done = last
+
+
 def _ws_alloc(nbytes: int) -> int:
     return int(nbytes * 1.05) + 4096                # what workspace() allocates for a request of nbytes
 
 
 def template_branch_bytes(b: int, T: int, G: int, n: int, d: int, heads: int, dim_head: int, precision: str,
-                          templates_dim: int = 32) -> int:
+                          templates_dim: int = 32, band: Optional[int] = None) -> int:
     """Device bytes the template branch (Alphafold2.embed_templates_) allocates beyond x and its own inputs when it runs the T
     templates in groups of G: the grow-only workspace sized for the largest call (to_template_embed, the pair-stack modules at
     batch b * G, the pointwise attention), plus what lives beside it: t and the crossed mask of one group and, with more than
     one group, that group's copy of templates_feats, q and gate of x and the fp32 softmax state.  Computed from the library's
-    workspace queries: no GPU needed."""
+    workspace queries: no GPU needed.
+
+    band < n (bf16 only): the branch in bands of `band` pair rows (TemplateAttentionRows, the pair stack in the same bands):
+    the fp32 softmax state of every pair, one group's t, crossed mask and templates_feats copy, one band's q and gate, plus
+    the larger of the banded pair block (pair_block_bytes with S = 0) and one band's begin / group / end workspace."""
     if precision not in PRECISIONS:
         raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
     lib = _lib.load()
@@ -913,6 +982,18 @@ def template_branch_bytes(b: int, T: int, G: int, n: int, d: int, heads: int, di
     G = max(1, min(G, T))
     bg, P, I = b * G, b * n * n, heads * dim_head
     rows = bg * n * n
+    if band is not None and band < n:
+        if strict:
+            raise ValueError("strict mode runs the template branch whole: no band")
+        W = band * n
+        ws = [lib.af2_template_embed_workspace(rows, templates_dim), lib.af2_template_pointwise_rows_begin_workspace(W, d),
+              lib.af2_template_pointwise_rows_group_workspace(G, W, d, heads, dim_head),
+              lib.af2_template_pointwise_rows_end_workspace(W, heads, dim_head)]
+        persist = rows * d * 4 + rows + rows * templates_dim * 4               # t, crossed mask, templates_feats copy
+        persist += P * (2 * heads + I + 1) * 4 + W * 2 * I * 2                 # whole-tensor state, one band's q | gate
+        # the workspace is grow-only: a band's window workspace larger than the pair block's stays beside the block's operands
+        pair_ws, keep = _pair_block_parts(bg, n, 0, d, heads, dim_head, band)
+        return _ws_alloc(max(pair_ws, *ws)) + keep + persist
     sfx = "_strict" if strict else ""
     ax = lib.af2_axial_attention_strict_workspace if strict else lib.af2_axial_attention_workspace
     ws = [getattr(lib, f"af2_template_embed{sfx}_workspace")(rows, templates_dim),
@@ -943,6 +1024,27 @@ def plan_template_groups(b: int, T: int, n: int, d: int, heads: int, dim_head: i
     return 1
 
 
+def plan_template_branch(b: int, T: int, n: int, d: int, heads: int, dim_head: int, precision: str, budget: int,
+                         templates_dim: int = 32):
+    """(G, band) of the template branch: plan_template_groups' G and band = n (the whole-tensor calls) whenever some G fits
+    `budget` (bytes), and always in strict mode (whole-tensor only); else G = 1 and the largest multiple of PAIR_BAND_ALIGN
+    pair rows below n that fits (template_branch_bytes with band).  Raises MemoryError when not even one band of
+    PAIR_BAND_ALIGN rows fits, before any device work."""
+    G = plan_template_groups(b, T, n, d, heads, dim_head, precision, budget, templates_dim)
+    if precision == "strict" or template_branch_bytes(b, T, G, n, d, heads, dim_head, precision, templates_dim) <= budget:
+        return G, n
+    R = (n - 1) // PAIR_BAND_ALIGN * PAIR_BAND_ALIGN
+    while R >= PAIR_BAND_ALIGN:
+        if template_branch_bytes(b, T, 1, n, d, heads, dim_head, precision, templates_dim, band=R) <= budget:
+            return 1, R
+        R -= PAIR_BAND_ALIGN
+    least = template_branch_bytes(b, T, 1, n, d, heads, dim_head, precision, templates_dim,
+                                  band=PAIR_BAND_ALIGN if n > PAIR_BAND_ALIGN else None)
+    raise MemoryError(f"the template branch at N_res {n} (batch {b}, {T} templates, dim {d}) needs {least / 2**30:.2f} GiB beyond x "
+                      f"and its inputs even one template at a time in bands of {PAIR_BAND_ALIGN} pair rows; "
+                      f"{budget / 2**30:.2f} GiB can be allocated")
+
+
 PAIR_BAND_ALIGN = 256      # band boundaries: every band call then picks the whole-tensor call's GEMM tile and chan_to_token kernel
 
 
@@ -958,6 +1060,13 @@ def pair_block_bytes(B: int, N: int, S: int, d: int, heads: int, dim_head: int, 
     for the MSA track and one band's calls, plus the largest set of operands one pair stage keeps for the whole tensor
     (triangle multiply: L, R and gate of all rows; column attention: the pair bias and one column band's copy of x and of
     the mask; outer mean: the projected m and one band's left operand).  Computed from the library's workspace queries."""
+    ws, keep = _pair_block_parts(B, N, S, d, heads, dim_head, R)
+    return _ws_alloc(ws) + keep
+
+
+@functools.lru_cache(maxsize=256)
+def _pair_block_parts(B: int, N: int, S: int, d: int, heads: int, dim_head: int, R: int):
+    """pair_block_bytes in its two parts: (largest workspace request, bytes of the operands kept beside the workspace)."""
     lib = _lib.load()
     ax = lib.af2_axial_attention_workspace
     ff = lambda tokens: lib.af2_feed_forward_workspace(tokens, d, 4 * d)  # noqa: E731
@@ -967,7 +1076,7 @@ def pair_block_bytes(B: int, N: int, S: int, d: int, heads: int, dim_head: int, 
             ws.append(lib.af2_outer_mean_workspace(B, S, N, d))
         ws += [lib.af2_triangle_multiply_workspace(B, N, d), ax(B, N, N, d, heads, dim_head, 1), ax(B, N, N, d, heads, dim_head, 0),
                ff(B * N * N)]
-        return _ws_alloc(max(ws))
+        return max(ws), 0
     np8 = _align8(N)
     ws += [lib.af2_triangle_project_workspace(R * N, d), lib.af2_triangle_contract_workspace(R, N, d),
            ax(1, R, N, d, heads, dim_head, 1), ax(1, N, R, d, heads, dim_head, 0), ff(R * N)]
@@ -976,7 +1085,7 @@ def pair_block_bytes(B: int, N: int, S: int, d: int, heads: int, dim_head: int, 
     if S > 0:
         ws += [lib.af2_outer_project_workspace(S * N, d), lib.af2_outer_contract_workspace(R, N, d)]
         keep.append(2 * d * S * np8 * 2 + d * S * _align8(R) * 2)             # outer mean: projected m, band's left operand
-    return _ws_alloc(max(ws)) + max(keep)
+    return max(ws), max(keep)
 
 
 def plan_pair_band(B: int, N: int, S: int, d: int, heads: int, dim_head: int, budget: int) -> int:
@@ -1001,6 +1110,16 @@ def workspace_holds(device, nbytes: int) -> bool:
     store = _WORKSPACE if _WS_PRIVATE is None else _WS_PRIVATE[0]
     ws = store.get(torch.device(device))
     return ws is not None and ws.numel() >= nbytes
+
+
+def release_workspace(device) -> None:
+    """Drop the grow-only workspace of `device` and return its memory to the driver, so that tensors which outlive single ops
+    can use it; the next op allocates a workspace of the size it needs.  device_budget counts the workspace as available,
+    which holds only once it is released (a workspace left at the trunk's whole-tensor size by an earlier forward would
+    otherwise stay beside them).  A no-op inside a locked private_workspace scope."""
+    store, locked = (_WORKSPACE, False) if _WS_PRIVATE is None else _WS_PRIVATE
+    if not locked and store.pop(torch.device(device), None) is not None:
+        torch.cuda.empty_cache()
 
 
 def device_budget(device) -> int:

@@ -442,6 +442,26 @@ long long af2_template_pointwise_end_strict_workspace(int B, int n, int heads, i
 int af2_template_pointwise_end_strict(const af2_template_attn_weights_strict* w, float* x, const float* out, const float* pooled, int B,
                                       int n, int d, int heads, int dim_head, void* workspace, long long workspace_bytes,
                                       af2_stream_t stream);
+/* begin / group / end (bf16) on a window of P consecutive pairs of one batch element, e.g. a band of pair rows [i0, i1) of
+ * batch element b: P = (i1 - i0) n, window offset o = b n^2 + i0 n.  Every pointer points at the window: x + o d, q, gate and
+ * out [P][I] (window-sized, caller-owned), x_mask + o, and the window's slice of the whole-tensor state: run_max + o heads,
+ * run_sum + o heads, acc + o I, pooled + o.  group: t points at template 0's first window row, t_mask at its crossed-mask
+ * entry; template g's rows start g t_stride pairs later (t_stride >= P; for t [B G][n][n][d] from the grouped entry points,
+ * t + (b G n^2 + i0 n) d and t_stride = n^2).  Workspaces are sized for the window only.  Running, for every group in order,
+ * every window's begin and group (first / last as above), and end after the last group, gives x bitwise equal to the
+ * whole-tensor calls.  x, t, q, gate, out and acc 16-byte aligned; d a multiple of 8. */
+long long af2_template_pointwise_rows_begin_workspace(long long P, int d);
+int af2_template_pointwise_rows_begin(const af2_template_attn_weights* w, const float* x, long long P, int d, int heads, int dim_head,
+                                      void* q, void* gate, void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_rows_group_workspace(int G, long long P, int d, int heads, int dim_head);
+int af2_template_pointwise_rows_group(const af2_template_attn_weights* w, const float* t, const unsigned char* x_mask,
+                                      const unsigned char* t_mask, int G, long long P, long long t_stride, int d, int heads,
+                                      int dim_head, const void* q, const void* gate, float* run_max, float* run_sum, float* acc,
+                                      float* pooled, void* out, int first, int last, void* workspace, long long workspace_bytes,
+                                      af2_stream_t stream);
+long long af2_template_pointwise_rows_end_workspace(long long P, int heads, int dim_head);
+int af2_template_pointwise_rows_end(const af2_template_attn_weights* w, float* x, const void* out, const float* pooled, long long P,
+                                    int d, int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
 /* to_template_embed (alphafold2.py:751): t fp32 [rows][d] = feats fp32 [rows][K] W^T + bias.  w bf16 [d][align8(K)] (zero pad
  * columns); _strict: w split [d][3][align8(K)]. */
 long long af2_template_embed_workspace(long long rows, int K);

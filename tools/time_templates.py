@@ -1,11 +1,15 @@
 """Device time of Alphafold2.forward with templates at the C2 shape, split into its template parts (CUDA events):
    python tools/time_templates.py [--templates 4] [--steps 10] [--n-res 256] [--msa-rows 128] [--depth 12] [--group G]
+                                  [--band R] [--precision bf16|strict] [--save-distance PATH]
    -> one JSON line
 
 Model and inputs as bench.py's C2 step (dim 256, depth 12, heads 8, dim_head 64, N_res 256, MSA 128 x 256, batch 1, all-ones
 masks) plus T templates: templates_feats, templates_angles and an all-ones templates_mask.  --n-res / --msa-rows / --depth
-change the shape; --group forces the number of templates the branch runs at a time (default: what
-ops.plan_template_groups picks from the free memory; template_group reports it).  Reported in ms per call:
+change the shape; --group forces the number of templates the branch runs at a time and --band the pair rows per band of
+its pointwise attention (default: what ops.plan_template_branch picks from the free memory; template_group and
+template_band report them, template_band = N_res when the branch runs whole, and planned_template_bytes is
+ops.template_branch_bytes for that choice).  --save-distance writes the distogram of one forward (torch.save).  Reported in
+ms per call:
   forward_ms / forward_without_templates_ms   Alphafold2.forward with and without the template inputs
   peak_alloc_*_bytes                          torch.cuda.max_memory_allocated over one such forward (from a fresh workspace)
   pair_stack_ms                               to_template_embed + templates_embed_layers pair blocks over b * T pair tensors
@@ -41,6 +45,9 @@ def main():
     ap.add_argument("--msa-rows", type=int, default=N_SEQ)
     ap.add_argument("--depth", type=int, default=CFG["depth"])
     ap.add_argument("--group", type=int, default=None, help="templates per group (default: planned from free memory)")
+    ap.add_argument("--band", type=int, default=None, help="pair rows per band of the template branch (default: planned)")
+    ap.add_argument("--precision", choices=ops.PRECISIONS, default="bf16")
+    ap.add_argument("--save-distance", default=None, help="torch.save the distogram of one forward to this path")
     args = ap.parse_args()
     T, n, S = args.templates, args.n_res, args.msa_rows
     cfg = dict(CFG, depth=args.depth)
@@ -49,9 +56,9 @@ def main():
     torch.manual_seed(0)
     model = A.Alphafold2(**cfg)
     randomize_zero_init_(model)
-    model = model.to(dev).eval()
-    if args.group is not None:
-        model.embed_templates_ = functools.partial(type(model).embed_templates_, model, group=args.group)
+    model = A.set_precision(model.to(dev).eval(), args.precision)
+    if args.group is not None or args.band is not None:
+        model.embed_templates_ = functools.partial(type(model).embed_templates_, model, group=args.group, band=args.band)
     seq = torch.randint(0, 21, (1, n), device=dev)
     msa = torch.randint(0, 21, (1, S, n), device=dev)
     mask = torch.ones(1, n, dtype=torch.bool, device=dev)
@@ -91,14 +98,27 @@ def main():
     fwd = lambda: model(seq, msa, mask=mask, msa_mask=msa_mask, templates_feats=feats, templates_mask=tm,  # noqa: E731
                         templates_angles=angles)
     fwd_plain = lambda: model(seq, msa, mask=mask, msa_mask=msa_mask)  # noqa: E731
-    res["peak_alloc_with_templates_bytes"] = peak(fwd)
+    try:
+        res["peak_alloc_with_templates_bytes"] = peak(fwd)
+    except MemoryError as ex:                      # the planner refuses before any device work of the branch
+        res["memory_error"] = str(ex)
+        print(json.dumps(dict(res, **_card(dev))))
+        return
     res["template_group"] = model.last_template_group
+    res["template_band"] = model.last_template_band
+    res["planned_template_bytes"] = ops.template_branch_bytes(
+        1, T, model.last_template_group, n, cfg["dim"], cfg["heads"], cfg["dim_head"], args.precision,
+        model.to_template_embed.in_features, band=model.last_template_band)
     res["peak_alloc_without_templates_bytes"] = peak(fwd_plain)
     res["forward_ms"] = timed(fwd)
     res["forward_without_templates_ms"] = timed(fwd_plain)
-    res["distance_checksum"] = float(fwd().distance.double().sum().item())
-    if model.last_template_group < T:
-        res["parts"] = "skipped: the forward ran the templates in groups"
+    with torch.no_grad():
+        dist = fwd().distance
+    res["distance_checksum"] = float(dist.double().sum().item())
+    if args.save_distance:
+        torch.save(dist.cpu(), args.save_distance)
+    if model.last_template_group < T or model.last_template_band < n:
+        res["parts"] = "skipped: the forward ran the templates in groups or bands"
         print(json.dumps(dict(res, **_card(dev))))
         return
     with torch.no_grad():

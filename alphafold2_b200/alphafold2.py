@@ -401,6 +401,27 @@ def _pair_band(pair, x, S, band):
     return band
 
 
+def _block_bands(pair, x, S, band, msa_band):
+    """(pair rows, MSA rows) per band of one Evoformer block whose pair block is `pair`, on x [B, N, N, d] and S MSA rows.
+    Unforced: (N, S) when the workspace already holds the whole block, else ops.plan_block_bands, which keeps _pair_band's
+    plan with the MSA track whole whenever that fits.  `band` forces the pair rows (as in _pair_band) and `msa_band` the MSA
+    rows (any positive integer: row bands start at multiples of d * 4 bytes and column bands are compact copies).  Strict
+    mode always runs whole."""
+    N = x.shape[1]
+    ta = pair.triangle_attention_ingoing
+    if not x.is_cuda or ops.precision_of(ta) == "strict":
+        return _pair_band(pair, x, S, band), S
+    if msa_band is not None:
+        if int(msa_band) <= 0:
+            raise ValueError(f"MSA band {msa_band} must be a positive number of MSA rows")
+        msa_band = min(int(msa_band), S)
+    if band is None and msa_band is None:
+        shape = (x.shape[0], N, S, x.shape[3], ta.attn.heads, ta.attn.dim_head)
+        if not ops.workspace_holds(x.device, ops.pair_block_bytes(*shape, N)):
+            band, msa_band = ops.plan_block_bands(*shape, int(ops.device_budget(x.device) * 0.85))
+    return _pair_band(pair, x, S, band), S if msa_band is None else msa_band
+
+
 class PairwiseAttentionBlock(nn.Module):
     def __init__(self, dim, seq_len, heads, dim_head, dropout=0., global_column_attn=False):
         super().__init__()
@@ -410,24 +431,33 @@ class PairwiseAttentionBlock(nn.Module):
         self.triangle_multiply_outgoing = TriangleMultiplicativeModule(dim=dim, mix='outgoing')
         self.triangle_multiply_ingoing = TriangleMultiplicativeModule(dim=dim, mix='ingoing')
 
-    def update_(self, x, mask=None, msa_repr=None, msa_mask=None, band=None):
+    def update_(self, x, mask=None, msa_repr=None, msa_mask=None, band=None, msa_band=None):
         """In-place residual chain of alphafold2.py:378-385 on an fp32 pair tensor.
 
         Runs in bands of pair rows (banded.pair_block_, bitwise the same result) when the whole-tensor calls would not fit
         what the device can still allocate; `band` forces the rows per band (tests).  The band used is kept in
-        self.last_pair_band (N: today's whole-tensor calls)."""
-        band = _pair_band(self, x, msa_repr.shape[1] if exists(msa_repr) else 0, band)
-        if band < x.shape[1]:
+        self.last_pair_band (N: today's whole-tensor calls).  msa_band < S projects m for the outer mean in chunks of that many
+        MSA rows (EvoformerBlock.update_ passes it when the MSA track runs in bands); with the pair rows whole the outer mean
+        is then that projection and one contraction over all rows, and every other call stays whole."""
+        S = msa_repr.shape[1] if exists(msa_repr) else 0
+        band = _pair_band(self, x, S, band)
+        msa_rows = int(msa_band) if msa_band is not None and int(msa_band) < S else None
+        if not x.is_cuda or ops.precision_of(self.outer_mean) == "strict":
+            msa_rows = None                       # strict mode (a parity mode) runs whole
+        if band < x.shape[1] or msa_rows is not None:
             from . import banded
             from .parallel import CudaStageOps
             st = CudaStageOps()
             mask = mask.bool().contiguous() if exists(mask) else None
             msa_mask = msa_mask.bool().contiguous() if exists(msa_mask) else None
+            pick = lambda t, b: None if t is None else t[b]  # noqa: E731
+            if band < x.shape[1]:
+                for b in range(x.shape[0]):
+                    banded.pair_block_(self, x[b], pick(mask, b), pick(msa_repr, b), pick(msa_mask, b), band, st, msa_rows)
+                return x
             for b in range(x.shape[0]):
-                pick = lambda t: None if t is None else t[b]  # noqa: E731
-                banded.pair_block_(self, x[b], pick(mask), pick(msa_repr), pick(msa_mask), band, st)
-            return x
-        if exists(msa_repr):
+                banded.outer_mean_(self.outer_mean, x[b], msa_repr[b], pick(msa_mask, b), msa_rows, st)
+        elif exists(msa_repr):
             self.outer_mean.add_to_(x, msa_repr, msa_mask)
         self.triangle_multiply_outgoing.add_to_(x, mask)
         self.triangle_multiply_ingoing.add_to_(x, mask)
@@ -470,16 +500,27 @@ class EvoformerBlock(nn.Module):
             FeedForward(dim=dim, dropout=ff_dropout),
         ])
 
-    def update_(self, x, m, mask, msa_mask, band=None):
+    def update_(self, x, m, mask, msa_mask, band=None, msa_band=None):
         """alphafold2.py:432-446 on private fp32 tensors, in place.  The pair track (pair block and transition) runs in bands
         of pair rows when the whole-tensor calls do not fit (PairwiseAttentionBlock.update_); `band` forces it (tests).
-        The plan is made before any device work of the block."""
+        When even the smallest pair bands do not fit beside the whole MSA track (deep MSAs), the MSA track runs in bands of
+        MSA rows as well (banded.msa_track_, bitwise the same result); `msa_band` forces the MSA rows per band (tests: any
+        positive integer).  The plan (ops.plan_block_bands) is made before any device work of the block; the bands used are
+        kept in self.last_pair_band and self.last_msa_band (N and S: the whole-tensor calls)."""
         attn, ff, msa_attn, msa_ff = self.layer
-        band = _pair_band(attn, x, m.shape[1], band)
+        band, msa_band = _block_bands(attn, x, m.shape[1], band, msa_band)
         self.last_pair_band = band
-        msa_attn.update_(m, msa_mask, x)
-        msa_ff.add_to_(m)
-        attn.update_(x, mask, m, msa_mask, band=band)
+        self.last_msa_band = msa_band
+        if msa_band < m.shape[1]:
+            from . import banded
+            from .parallel import CudaStageOps
+            mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
+            for b in range(x.shape[0]):
+                banded.msa_track_(msa_attn, msa_ff, m[b], None if mmk is None else mmk[b], x[b], msa_band, CudaStageOps())
+        else:
+            msa_attn.update_(m, msa_mask, x)
+            msa_ff.add_to_(m)
+        attn.update_(x, mask, m, msa_mask, band=band, msa_band=msa_band)
         if band < x.shape[1]:
             from . import banded
             from .parallel import CudaStageOps
@@ -513,21 +554,23 @@ class Evoformer(nn.Module):
             for layer in self.layers:
                 layer.update_(xo, mo, mk, mmk)
                 self.last_pair_band = layer.last_pair_band
+                self.last_msa_band = layer.last_msa_band
         return xo.to(x.dtype), mo.to(m.dtype)
 
-    def run_(self, x, m, mask=None, msa_mask=None, band=None):
+    def run_(self, x, m, mask=None, msa_mask=None, band=None, msa_band=None):
         """Same as forward, for callers that own fp32 contiguous x / m and allow them to be updated in place (no private
         copies).  A sharded trunk (parallel.shard_evoformer replaces `forward`) goes through its schedule instead.
-        `band` forces the pair rows per band of every block (tests; see PairwiseAttentionBlock.update_); the band the last
-        block used is kept in self.last_pair_band."""
+        `band` forces the pair rows and `msa_band` the MSA rows per band of every block (tests; see EvoformerBlock.update_);
+        the bands the last block used are kept in self.last_pair_band and self.last_msa_band."""
         if "forward" in self.__dict__ or x.dtype != torch.float32 or m.dtype != torch.float32 or not (x.is_contiguous() and m.is_contiguous()):
             return self(x, m, mask=mask, msa_mask=msa_mask)
         with torch.no_grad():
             mk = mask.bool().contiguous() if exists(mask) else None
             mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
             for layer in self.layers:
-                layer.update_(x, m, mk, mmk, band=band)
+                layer.update_(x, m, mk, mmk, band=band, msa_band=msa_band)
                 self.last_pair_band = layer.last_pair_band
+                self.last_msa_band = layer.last_msa_band
         return x, m
 
 

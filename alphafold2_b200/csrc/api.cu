@@ -754,7 +754,14 @@ int outer_front(const af2_outer_weights* w, const float* m, const unsigned char*
     { ProfScope ps(s, KC_MISC, 0.0, 0.0); mask_to_float_kernel<<<ew_grid(tokens), 256, 0, s>>>(msa_mask, maskf, tokens); }
     CUDA_OK(cudaGetLastError());
   }
-  if (pitch != inner) CUDA_OK(cudaMemsetAsync(LRc, 0, (size_t)2 * d * chan_stride * 2, s));
+  if (pitch != inner) {   // pad columns are read by TMA as MN padding of the contraction: keep them zero
+    const long long span = tokens / inner * pitch;   // this call's MSA rows of one channel
+    if (chan_stride == span) {
+      CUDA_OK(cudaMemsetAsync(LRc, 0, (size_t)2 * d * chan_stride * 2, s));
+    } else {                // a chunk of MSA rows inside a larger operand: only its own rows, other chunks' rows stay as they are
+      CUDA_OK(cudaMemset2DAsync(LRc, (size_t)chan_stride * 2, 0, (size_t)span * 2, (size_t)2 * d, s));
+    }
+  }
   GemmCall c = linear_call(mn, d, w->w_lr, d, (int)tokens, 2 * d, d);
   c.mode = EPI_STORE_BF16; c.layout = LAYOUT_CHANNEL; c.out = LRc; c.ld_out = chan_stride; c.bias = w->b_lr;
   c.use_rowscale = msa_mask != nullptr; c.rowscale = maskf; c.cm_inner = inner; c.cm_pitch = pitch;
@@ -1243,7 +1250,10 @@ int af2_outer_project(const af2_outer_weights* w, const float* m, const unsigned
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!w || !m || !LRc) return fail(AF2_ERR_BAD_ARG, "outer_project: null argument");
   if (d % 32) return fail(AF2_ERR_BAD_ARG, "outer_project: dim %d must be a multiple of 32", d);
+  if (inner <= 0 || tokens % inner || tokens > 0x7fffffffLL)
+    return fail(AF2_ERR_BAD_ARG, "outer_project: %lld tokens must be a multiple of inner %d and at most 2^31 - 1", tokens, inner);
   const int pitch = (int)align_up(inner, 8);
+  if (chan_stride < tokens / inner * pitch) return fail(AF2_ERR_BAD_ARG, "outer_project: channel stride shorter than the rows written");
   Arena ar(workspace, workspace_bytes);
   __nv_bfloat16* mn = ar.take<__nv_bfloat16>(tokens * d);
   float* maskf = ar.take<float>(tokens);

@@ -434,7 +434,7 @@ __global__ void outer_scale_rows_kernel(const uint8_t* __restrict__ mask, float*
     const int j = idx % N;
     const int i = row0 + static_cast<int>(idx / N);
     int cnt = 0;
-    for (int s = 0; s < S; ++s) cnt += (mask[s * N + i] != 0) & (mask[s * N + j] != 0);
+    for (int s = 0; s < S; ++s) cnt += (mask[static_cast<long long>(s) * N + i] != 0) & (mask[static_cast<long long>(s) * N + j] != 0);
     scale[idx] = 1.0f / (static_cast<float>(S) * (static_cast<float>(cnt) + eps));
   }
 }

@@ -1104,6 +1104,69 @@ def plan_pair_band(B: int, N: int, S: int, d: int, heads: int, dim_head: int, bu
                       f"x and m even in bands of {PAIR_BAND_ALIGN} pair rows; {budget / 2**30:.2f} GiB can be allocated")
 
 
+MSA_BAND_ALIGN = 64       # the planner's MSA bands: multiples of 64 rows (any band gives the same bits; this bounds the search)
+
+
+@functools.lru_cache(maxsize=4096)
+def msa_block_bytes(B: int, N: int, S: int, d: int, heads: int, dim_head: int, R: int, RS: int) -> int:
+    """Device bytes one Evoformer block (bf16 path) allocates beyond x and m with the pair track in bands of R pair rows and the
+    MSA track in bands of RS MSA rows (banded.msa_track_, one batch element at a time).  RS >= S is pair_block_bytes(..., R).
+    RS < S: the workspace sized for the largest of one MSA row band's attention and transition, one column band's attention
+    (banded.msa_column_band columns), one projection chunk, the outer contraction (R rows, or N when the pair rows are whole) and
+    the pair track's calls at R (whole at batch B when R >= N); beside it the largest set of operands kept at one time: the
+    row attention's pair bias, one column band's copy of m and of its mask, the whole projected m (LR) and one band's left
+    operand, or the pair track's operands at R."""
+    if RS >= S:
+        return pair_block_bytes(B, N, S, d, heads, dim_head, R)
+    from .banded import msa_column_band
+    lib = _lib.load()
+    ax = lib.af2_axial_attention_workspace
+    np8 = _align8(N)
+    Cb = msa_column_band(S, N, RS)
+    pair_ws, pair_keep = _pair_block_parts(B, N, 0, d, heads, dim_head, R)
+    ws = [pair_ws, ax(1, RS, N, d, heads, dim_head, 1), ax(1, S, Cb, d, heads, dim_head, 0),
+          lib.af2_feed_forward_workspace(RS * N, d, 4 * d), lib.af2_outer_project_workspace(RS * N, d),
+          lib.af2_outer_contract_workspace(min(R, N), N, d)]
+    keep = [pair_keep,
+            heads * N * np8 * 2,                                                  # row attention: the pair bias of x
+            _pt_round(S * Cb * d * 4) + _pt_round(S * Cb),                        # column attention: band of m and mask
+            _pt_round(2 * d * S * np8 * 2) + (_pt_round(d * S * _align8(R) * 2) if R < N else 0)]   # outer mean: LR, left window
+    return _pt_round(_ws_alloc(max(ws))) + max(keep)
+
+
+def _pt_round(nbytes: int) -> int:
+    """What PyTorch's caching allocator takes for a large request: a multiple of 2 MiB (at these sizes the rounding is no
+    longer lost in the planner's other margins)."""
+    return (nbytes + (1 << 21) - 1) >> 21 << 21
+
+
+def plan_block_bands(B: int, N: int, S: int, d: int, heads: int, dim_head: int, budget: int):
+    """(R, RS): pair rows and MSA rows per band of one Evoformer block.  (plan_pair_band(...), S) whenever that fits `budget`
+    (bytes), so every shape that runs with the MSA track whole keeps its plan.  Otherwise the largest R (N, or a multiple of
+    PAIR_BAND_ALIGN) for which some RS fits, then the largest RS (a multiple of MSA_BAND_ALIGN below S) that fits with it: pair
+    bands copy and cost time, MSA row bands do not.  Raises MemoryError, before any device work, when not even
+    R = PAIR_BAND_ALIGN with RS = MSA_BAND_ALIGN fits."""
+    try:
+        return plan_pair_band(B, N, S, d, heads, dim_head, budget), S
+    except MemoryError:
+        pass
+    least = min(PAIR_BAND_ALIGN, N)
+    if S > MSA_BAND_ALIGN:
+        fits = lambda R, RS: msa_block_bytes(B, N, S, d, heads, dim_head, R, RS) <= budget  # noqa: E731
+        for R in [N] + list(range((N - 1) // PAIR_BAND_ALIGN * PAIR_BAND_ALIGN, PAIR_BAND_ALIGN - 1, -PAIR_BAND_ALIGN)):
+            if fits(R, MSA_BAND_ALIGN):
+                RS = (S - 1) // MSA_BAND_ALIGN * MSA_BAND_ALIGN
+                while not fits(R, RS):
+                    RS -= MSA_BAND_ALIGN
+                return R, RS
+        need = msa_block_bytes(B, N, S, d, heads, dim_head, least, MSA_BAND_ALIGN)
+    else:
+        need = pair_block_bytes(B, N, S, d, heads, dim_head, least)
+    raise MemoryError(f"one Evoformer block at N_res {N} (batch {B}, {S} MSA rows, dim {d}) needs {need / 2**30:.2f} GiB beyond "
+                      f"x and m even in bands of {least} pair rows and {min(MSA_BAND_ALIGN, S)} MSA rows; "
+                      f"{budget / 2**30:.2f} GiB can be allocated")
+
+
 def workspace_holds(device, nbytes: int) -> bool:
     """Whether the current grow-only workspace of `device` is already at least `nbytes` (a call needing no more allocates
     nothing)."""

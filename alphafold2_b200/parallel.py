@@ -331,16 +331,25 @@ class CudaStageOps:
     def feed_forward_(self, ff, x: torch.Tensor):
         _ops.feed_forward_(ff.packed(), x)
 
-    def outer_project(self, om, m_cols: torch.Tensor, mask_cols: Optional[torch.Tensor]) -> torch.Tensor:
-        """m [S, nl, d] -> bf16 [2d, S, align8(nl)] channel-major left | right."""
+    def outer_operand(self, S: int, N: int, d: int, like: torch.Tensor) -> torch.Tensor:
+        """Whole outer-mean operand for the banded schedule: bf16 [2d, S, align8(N)]; outer_project(out=...) fills it in chunks
+        of MSA rows (each chunk zeroes its own pad columns)."""
+        return torch.empty(2 * d, S, _align8(N), dtype=torch.bfloat16, device=like.device)
+
+    def outer_project(self, om, m_cols: torch.Tensor, mask_cols: Optional[torch.Tensor], out=None) -> torch.Tensor:
+        """m [S, nl, d] -> bf16 [2d, S, align8(nl)] channel-major left | right.
+        out: write into this instead, e.g. the MSA-row window [:, s0:s1] of outer_operand's tensor (its channel stride is kept)."""
         pk = om.packed()
         S, nl, d = m_cols.shape
-        out = torch.empty(2 * d, S, _align8(nl), dtype=torch.bfloat16, device=m_cols.device)
+        if out is None:
+            out = torch.empty(2 * d, S, _align8(nl), dtype=torch.bfloat16, device=m_cols.device)
+        elif tuple(out.shape) != (2 * d, S, _align8(nl)) or out.stride(1) != _align8(nl) or out.stride(2) != 1:
+            raise ValueError("outer_project: out must be a [2d, rows, align8(cols)] window with one channel stride")
         lib = _lib.load()
         ws = _ops.workspace(lib.af2_outer_project_workspace(S * nl, d), m_cols.device)
         mk = None if mask_cols is None else mask_cols.contiguous()
         _lib.check(lib.af2_outer_project(C.byref(pk.struct), m_cols.data_ptr(), None if mk is None else mk.data_ptr(), S * nl,
-                                         nl, d, out.data_ptr(), S * _align8(nl), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
+                                         nl, d, out.data_ptr(), out.stride(0), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
         return out
 
     @staticmethod

@@ -1,16 +1,21 @@
-"""Time Alphafold2.forward at a long N_res on one GPU, whole or with the pair track in bands of pair rows.
+"""Time Alphafold2.forward at a long N_res or a deep MSA on one GPU, whole or with the pair track in bands of pair rows and
+the MSA track in bands of MSA rows.
 
     python tools/time_long.py --n-res 4096 --msa-rows 32 --depth 1
     python tools/time_long.py --n-res 2048 --band 2048 512 --repeat 5     # whole and 512-row bands, alternated
+    python tools/time_long.py --n-res 2048 --msa-rows 8448                # the planner's MSA bands
+    python tools/time_long.py --n-res 1024 --msa-rows 4096 --msa-band 4096 512 --repeat 3
 
---band lists the rows per band to run (0: the planner's choice, N_res or more: the whole-tensor calls); the runs of the
-list alternate for --repeat rounds, after one warm-up forward each.  One JSON line per forward:
+--band lists the pair rows per band to run (0: the planner's choice, N_res or more: the whole-tensor calls) and --msa-band
+the MSA rows per band (0: the planner's choice, msa-rows or more: the whole MSA track); every pair of the two lists runs,
+alternating for --repeat rounds after one warm-up forward each.  One JSON line per forward:
   ms            forward time (CUDA events around the call, after a device synchronise)
-  band          rows per band the trunk used (Evoformer.last_pair_band)
+  band          pair rows per band the trunk used (Evoformer.last_pair_band), msa_band the MSA rows (last_msa_band)
   peak_gb       peak memory allocated by the forward beyond what was allocated before it (fresh grow-only workspace)
-  block_gb      ops.pair_block_bytes for that band, and xm_gb the x and m it comes on top of
+  block_gb      ops.msa_block_bytes for those bands, and xm_gb the x and m it comes on top of
   copy_ms       time of the column-band copies of one block (x[:, j0:j1] -> compact buffer -> back, every band), timed
                 alone on the same x; copy_share = depth * copy_ms / ms
+  msa_copy_ms   the same for the MSA column bands (m[:, j0:j1] and its mask), msa_copy_share = depth * msa_copy_ms / ms
 The first line names the card and its power limit (nvidia-smi).
 """
 import argparse
@@ -35,10 +40,10 @@ def _card():
         return "unknown"
 
 
-def _copy_ms(N, d, band, mask):
+def _copy_ms(N, d, band, mask, rows=None):
     """The column attention's band copies of one block, alone: per column band x[:, j0:j1] (and its mask) to a compact
-    buffer and back."""
-    x = torch.empty(N, N, d, device="cuda")
+    buffer and back.  rows: the same for m [rows, N, d] (MSA column bands)."""
+    x = torch.empty(rows or N, N, d, device="cuda")
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     for it in range(2):                                   # the first pass warms the allocator
         ev[0].record()
@@ -60,6 +65,7 @@ def main():
     ap.add_argument("--msa-rows", type=int, default=32)
     ap.add_argument("--depth", type=int, default=1)
     ap.add_argument("--band", type=int, nargs="+", default=[0])
+    ap.add_argument("--msa-band", type=int, nargs="+", default=[0])
     ap.add_argument("--repeat", type=int, default=3)
     ap.add_argument("--dim", type=int, default=256)
     ap.add_argument("--heads", type=int, default=8)
@@ -69,7 +75,7 @@ def main():
         raise SystemExit("time_long.py measures on the GPU; no CUDA device found")
 
     import alphafold2_b200 as A
-    from alphafold2_b200 import ops
+    from alphafold2_b200 import banded, ops
     from oracle import evoformer_oracle as O
 
     N, S, d = a.n_res, a.msa_rows, a.dim
@@ -86,8 +92,9 @@ def main():
     run_ = type(model.net).run_
     xm = (N * N + S * N) * d * 4
 
-    def forward(band):
-        model.net.run_ = functools.partial(run_, model.net, band=band) if band else functools.partial(run_, model.net)
+    def forward(band, msa_band):
+        kw = {k: v for k, v in (("band", band), ("msa_band", msa_band)) if v}
+        model.net.run_ = functools.partial(run_, model.net, **kw)
         ops._WORKSPACE.clear()
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
@@ -101,21 +108,27 @@ def main():
         torch.cuda.synchronize()
         ok = bool(torch.isfinite(ret.distance).all())
         del ret
-        return ev[0].elapsed_time(ev[1]), torch.cuda.max_memory_allocated() - base, model.net.last_pair_band, ok
+        return (ev[0].elapsed_time(ev[1]), torch.cuda.max_memory_allocated() - base, model.net.last_pair_band,
+                model.net.last_msa_band, ok)
 
-    copies = {}
-    for band in a.band:
-        forward(band)                                     # warm-up: module loads, weight packing, allocator
+    runs = [(band, msa_band) for band in a.band for msa_band in a.msa_band]
+    copies, msa_copies = {}, {}
+    for band, msa_band in runs:
+        forward(band, msa_band)                           # warm-up: module loads, weight packing, allocator
     for r in range(a.repeat):
-        for band in a.band:
-            ms, peak, used, ok = forward(band)
+        for band, msa_band in runs:
+            ms, peak, used, used_msa, ok = forward(band, msa_band)
             if used < N and used not in copies:
                 copies[used] = _copy_ms(N, d, used, mask[0, :, None] & mask[0, None, :])
-            cp = copies.get(used, 0.0)
-            print(json.dumps({"round": r, "band_arg": band, "band": used, "ms": round(ms, 1), "peak_gb": round(peak / 1e9, 2),
-                              "block_gb": round(ops.pair_block_bytes(1, N, S, d, a.heads, a.dim_head, used) / 1e9, 2),
-                              "xm_gb": round(xm / 1e9, 2), "copy_ms": round(cp, 1),
-                              "copy_share": round(a.depth * cp / ms, 4), "finite": ok}), flush=True)
+            if used_msa < S and used_msa not in msa_copies:
+                msa_copies[used_msa] = _copy_ms(N, d, banded.msa_column_band(S, N, used_msa), msa_mask[0], rows=S)
+            cp, mcp = copies.get(used, 0.0), msa_copies.get(used_msa, 0.0)
+            print(json.dumps({"round": r, "band_arg": band, "msa_band_arg": msa_band, "band": used, "msa_band": used_msa,
+                              "ms": round(ms, 1), "peak_gb": round(peak / 1e9, 2),
+                              "block_gb": round(ops.msa_block_bytes(1, N, S, d, a.heads, a.dim_head, used, used_msa) / 1e9, 2),
+                              "xm_gb": round(xm / 1e9, 2), "copy_ms": round(cp, 1), "copy_share": round(a.depth * cp / ms, 4),
+                              "msa_copy_ms": round(mcp, 1), "msa_copy_share": round(a.depth * mcp / ms, 4), "finite": ok}),
+                  flush=True)
 
 
 if __name__ == "__main__":

@@ -18,7 +18,9 @@ import functools
 import pytest
 import torch
 
+import embed_bounds as E
 from conftest import load_golden
+from gpu_util import check_bound
 from oracle import evoformer_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -213,19 +215,17 @@ def test_deep_msa_whole_m_kernels_against_torch():
     msa = torch.randint(0, 21, (1, S, N), generator=g).cuda()
     x, m = ops.embed_pair_init(seq, msa, emb, w_pair, b_pair, pos, R, m_rows=S + T)
     rows = torch.tensor([0, 1, S // 2] + list(range(S - 8, S)), device="cuda")
-    want = emb[msa[0, rows]] + emb[seq[0]][None]
-    err = (m[0, rows] - want).abs().max().item()
-    assert err < 1e-5, f"MSA init: max |err| {err:.3e} on MSA rows {rows.tolist()}"
+    _, want = E.token_embed(emb, seq, msa[:, rows])             # (emb[msa] + emb[seq]) in fp32, the kernel's order
+    assert torch.equal(m[0, rows], want[0]), f"MSA init not bitwise on MSA rows {rows.tolist()}"
     want = m[0, rows].clone()
-    # template angle rows S .. S + T - 1
+    # template angle rows S .. S + T - 1, against the module's fp64 output (the end-to-end bound of test_gpu_embed_heads.py)
     K = 55
     w1, b1 = (torch.randn(d, K, generator=g) * K ** -0.5).cuda(), torch.randn(d, generator=g).cuda()
     w2, b2 = (torch.randn(d, d, generator=g) * d ** -0.5).cuda(), torch.randn(d, generator=g).cuda()
     angles = torch.randn(1, T, N, K, generator=g).cuda()
     ops.template_angle_features(ops.pack_template_angles(w1, b1, w2, b2), angles, m, S)
-    ref = torch.nn.functional.gelu(angles.double() @ w1.double().T + b1.double()) @ w2.double().T + b2.double()
-    err = (m[0, S:].double() - ref[0]).abs().max().item()
-    assert err < 5e-2 * ref.abs().max().item(), f"template angle rows: max |err| {err:.3e}"
+    ref, bound = E.angles_module_ref(angles.view(-1, K), w1, b1, w2, b2, strict=False)
+    check_bound(f"bf16/template_angles/deep_msa/N{N}S{S}/module", m[0, S:].reshape(T * N, d), ref, bound)
     assert torch.equal(m[0, rows], want), "the angle rows wrote into the MSA rows"
     # recycling: row 0 of m += LN(single row) (m's batch stride is (S + T) * N * d elements); x += LN(0) + table[bucket] = 0
     row0 = m[0, 0].clone()

@@ -1,8 +1,7 @@
-"""-m gpu: the SURVEY.md 8(f) rows built in round 2.
-  n1  pre- / post-trunk glue as fused kernels (alphafold2.py:676-726, 821-823): embedding gather + pair init + rel-pos,
-      symmetrise + LayerNorm + distogram Linear -- against the plain-torch evaluation of the same lines in fp64;
-  n2  extra-MSA stack: tied-query ("global") ingoing triangle attention (alphafold2.py:142-151, 250, 367) and
-      Alphafold2.forward(extra_msa=...) (alphafold2.py:789-798 incl. quirk Q11) -- against fixtures from the unmodified reference."""
+"""-m gpu: the extra-MSA stack (SURVEY.md 8(f) row n2): tied-query ("global") ingoing triangle attention
+(alphafold2.py:142-151, 250, 367) and Alphafold2.forward(extra_msa=...) (alphafold2.py:789-798 incl. quirk Q11) -- against
+fixtures from the unmodified reference.  The pre- / post-trunk glue kernels of row n1 (pair init, distogram head) are tested
+element-wise in test_gpu_embed_heads.py."""
 import pytest
 import torch
 
@@ -11,46 +10,6 @@ from gpu_util import check, check_strict
 from oracle import evoformer_oracle as O
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.mark.parametrize("d,n,S,B,with_embeds", [(256, 256, 128, 1, False), (128, 70, 5, 2, True), (32, 24, 3, 2, False)])
-def test_glue_embed_pair_init(d, n, S, B, with_embeds):
-    from alphafold2_b200 import ops
-    g = torch.Generator().manual_seed(d + n)
-    V, R = 22, 32
-    emb = torch.randn(V, d, generator=g)
-    wp, bp = torch.randn(2 * d, d, generator=g) * d ** -0.5, torch.randn(2 * d, generator=g) * 0.1
-    pos = torch.randn(2 * R + 1, d, generator=g)
-    seq = torch.randint(0, 21, (B, n), generator=g)
-    msa = torch.randint(0, 21, (B, S, n), generator=g)
-    se = torch.randn(B, n, d, generator=g) if with_embeds else None
-    me = torch.randn(B, S, n, d, generator=g) if with_embeds else None
-    si = (torch.arange(n) * 3 + (torch.arange(n) > n // 2) * 50) if with_embeds else None
-    cu = lambda t: None if t is None else t.cuda()  # noqa: E731
-    x, m = ops.embed_pair_init(seq.cuda(), msa.cuda(), emb.cuda(), wp.cuda(), bp.cuda(), pos.cuda(), R, cu(se), cu(me), cu(si))
-    # alphafold2.py:676-726 in fp64
-    e = emb.double()[seq] + (se.double() if with_embeds else 0)
-    mr = emb.double()[msa] + (me.double() if with_embeds else 0) + e[:, None]
-    lr = e @ wp.double().T + bp.double()
-    idx = si if si is not None else torch.arange(n)
-    rel = (idx[:, None] - idx[None, :]).clamp(-R, R) + R
-    xr = lr[:, :, None, :d] + lr[:, None, :, d:] + pos.double()[rel][None]
-    assert (x.double().cpu() - xr).abs().max().item() < 2e-5
-    assert (m.double().cpu() - mr).abs().max().item() < 1e-5
-
-
-@pytest.mark.parametrize("d,n,B", [(256, 256, 1), (128, 70, 2), (384, 33, 1)])
-def test_glue_distogram_head(d, n, B):
-    from alphafold2_b200 import ops
-    g = torch.Generator().manual_seed(d + n)
-    x = torch.randn(B, n, n, d, generator=g) * 3
-    lw, lb = 1 + 0.1 * torch.randn(d, generator=g), 0.1 * torch.randn(d, generator=g)
-    w, b = torch.randn(37, d, generator=g) * d ** -0.5, torch.randn(37, generator=g) * 0.1
-    out = ops.distogram_head(x.cuda(), lw.cuda(), lb.cuda(), w.cuda(), b.cuda())
-    te = (x.double() + x.double().transpose(1, 2)) * 0.5
-    ref = torch.nn.functional.layer_norm(te, (d,), lw.double(), lb.double(), 1e-5) @ w.double().T + b.double()
-    assert tuple(out.shape) == (B, n, n, 37)
-    assert (out.double().cpu() - ref).abs().max().item() < 2e-5
 
 
 @pytest.mark.parametrize("precision", ["bf16", "strict"])

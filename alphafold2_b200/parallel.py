@@ -132,18 +132,40 @@ class PeerExchange:
         self.base = None
         self.opened = []
 
+    @staticmethod
+    def layout(N: int, S: int, d: int, P: int) -> dict:
+        """Where the buffers of one rank's arena lie: off[(track, layout)] is a buffer's byte offset, shapes[(track, layout)]
+        its fp32 shape, total the arena's size in bytes.  The control block comes first; every buffer starts on 256 B."""
+        ctrl = int(_lib.load().af2_peer_ctrl_bytes())
+        al = lambda n: (n + 255) // 256 * 256  # noqa: E731
+        pair_b, msa_b = al(N // P * N * d * 4), al(S // P * N * d * 4)
+        PAIR, MSA = PeerExchange.PAIR, PeerExchange.MSA
+        return dict(off={(PAIR, "row"): ctrl, (PAIR, "col"): ctrl + pair_b,
+                         (MSA, "row"): ctrl + 2 * pair_b, (MSA, "col"): ctrl + 2 * pair_b + msa_b},
+                    shapes={(PAIR, "row"): (N // P, N, d), (PAIR, "col"): (N, N // P, d),
+                            (MSA, "row"): (S // P, N, d), (MSA, "col"): (S, N // P, d)},
+                    total=ctrl + 2 * pair_b + 2 * msa_b)
+
+    @classmethod
+    def attach(cls, P: int, rank: int, base: int, table: torch.Tensor, device: torch.device, layout: dict, group=None):
+        """Rank `rank` of an exchange over arenas that already exist: base is this rank's arena (laid out by `layout`), table
+        the device int64 [P] of every rank's arena base as this process addresses it (its own included)."""
+        self = cls()
+        self.group, self.P, self.rank, self.device = group, P, rank, device
+        self.base, self.table = base, table
+        self.off, self.shapes = layout["off"], layout["shapes"]
+        self.arena = torch.as_tensor(_RawCuda(base, layout["total"]), device=device)
+        self.exchanges = 0
+        return self
+
     @classmethod
     def create(cls, group, device: torch.device, N: int, S: int, d: int):
         P, r = dist.get_world_size(group), dist.get_rank(group)
         lib = _lib.load()
-        self = cls()
+        self = cls()                   # holds the local arena and the peer mappings until every rank has them
         self.group, self.P, self.rank, self.device = group, P, r, device
-        ctrl = int(lib.af2_peer_ctrl_bytes())
-        al = lambda n: (n + 255) // 256 * 256  # noqa: E731
-        pair_b, msa_b = al(N // P * N * d * 4), al(S // P * N * d * 4)
-        self.off = {(cls.PAIR, "row"): ctrl, (cls.PAIR, "col"): ctrl + pair_b,
-                    (cls.MSA, "row"): ctrl + 2 * pair_b, (cls.MSA, "col"): ctrl + 2 * pair_b + msa_b}
-        total = ctrl + 2 * pair_b + 2 * msa_b
+        lay = cls.layout(N, S, d, P)
+        total = lay["total"]
         ok = P <= 32 and device.type == "cuda"
         handle = torch.zeros(72, dtype=torch.uint8)
         # 1. local arena + IPC handle (no collective inside: every rank reaches the all_gather below whatever happens here)
@@ -198,11 +220,9 @@ class PeerExchange:
             dist.barrier(group=group)              # nobody frees an arena a peer still has mapped
             self._release_local()
             return None
-        self.table = torch.tensor(bases, dtype=torch.int64, device=device)            # device array of the P arena bases
-        self.shapes = {(cls.PAIR, "row"): (N // P, N, d), (cls.PAIR, "col"): (N, N // P, d),
-                       (cls.MSA, "row"): (S // P, N, d), (cls.MSA, "col"): (S, N // P, d)}
-        self.exchanges = 0
-        return self
+        ex = cls.attach(P, r, self.base, torch.tensor(bases, dtype=torch.int64, device=device), device, lay, group)
+        ex.opened = self.opened                                                        # unmapped by close()
+        return ex
 
     def buffer(self, track: int, layout: str) -> torch.Tensor:
         shape = self.shapes[(track, layout)]

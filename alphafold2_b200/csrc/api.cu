@@ -593,6 +593,11 @@ int launch_chan_to_token(const ChanLnParams& p, cudaStream_t s, int variant = C2
 // -------------------------------------------------------------------------------------------------
 // attention launch (one folded batch group)
 // -------------------------------------------------------------------------------------------------
+// head widths of the bf16 tensor-core attention kernel (strict mode takes any multiple of 4)
+static bool attention_dim_head_ok(int dh) { return dh == 16 || dh == 32 || dh == 64 || dh == 128; }
+#define DIM_HEAD_UNSUPPORTED \
+  "dim_head %d unsupported (16, 32, 64 or 128 in bf16 mode; strict mode takes any multiple of 4)"
+
 template <int DH>
 int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tg,
                           const AttnParams& p, cudaStream_t s) {
@@ -621,19 +626,23 @@ int launch_attention_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CU
 int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nbatch, long long tok_sb, long long tok_si,
                      const __nv_bfloat16* bias, int npad, const uint8_t* mask, const __nv_bfloat16* gate,
                      __nv_bfloat16* out, cudaStream_t s) {
-  if (dh != 32 && dh != 64) return fail(AF2_ERR_BAD_ARG, "attention: dim_head %d unsupported (32 or 64)", dh);
+  if (!attention_dim_head_ok(dh)) return fail(AF2_ERR_BAD_ARG, "attention: " DIM_HEAD_UNSUPPORTED, dh);
   const long long I = (long long)heads * dh;
   const long long ld = 3 * I;
   CUtensorMap tq, tk, tv, tg;
   unsigned long long dims[4] = {(unsigned long long)dh, (unsigned long long)n, (unsigned long long)heads, (unsigned long long)nbatch};
   unsigned long long str[3] = {(unsigned long long)(tok_si * ld * 2), (unsigned long long)(dh * 2), (unsigned long long)(tok_sb * ld * 2)};
   unsigned long long gstr[3] = {(unsigned long long)(tok_si * I * 2), (unsigned long long)(dh * 2), (unsigned long long)(tok_sb * I * 2)};
-  unsigned box[4] = {(unsigned)dh, 128, 1, 1};
-  const CUtensorMapSwizzle swz = (dh == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  // a 128B-swizzled box row holds at most 64 channels: DH 128 tiles are loaded as two 64-channel boxes
+  unsigned box[4] = {(unsigned)(dh < 64 ? dh : 64), 128, 1, 1};
+  const CUtensorMapSwizzle swz = dh >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                 : dh == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
   // A box row is ONE head's slice of a token (dh * 2 bytes); the CTAs resident together read all heads of the same tokens
   // (head-innermost item order).  256B promotion measured no faster than promotion to the row size under that order (one
-  // H100, C2 shapes, tools/time_attention.py), so the L2 fill stays at the row size.
-  const CUtensorMapL2promotion promo = (dh == 64) ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_64B;
+  // H100, C2 shapes, tools/time_attention.py), so the L2 fill stays at the row size: 64 B (the least promotion) at DH 16
+  // and 32, 128 B at 64, 256 B at 128.
+  const CUtensorMapL2promotion promo = dh == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
+                                       : dh == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_64B;
   const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   AF2_TRY(make_tmap(&tq, qkv, 4, dims, str, box, swz, bf, promo));
   AF2_TRY(make_tmap(&tk, qkv + I, 4, dims, str, box, swz, bf, promo));
@@ -644,8 +653,13 @@ int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nba
   memset(&p, 0, sizeof(p));
   p.n = n; p.heads = heads; p.nbatch = nbatch; p.has_bias = bias != nullptr; p.bias = bias; p.npad = npad;
   p.mask = mask; p.mask_sb = tok_sb; p.mask_si = tok_si;
-  p.out = out; p.tok_sb = tok_sb; p.tok_si = tok_si; p.ld_out = I;
-  return dh == 64 ? launch_attention_inst<64>(tq, tk, tv, tg, p, s) : launch_attention_inst<32>(tq, tk, tv, tg, p, s);
+  p.out = out; p.tok_sb = tok_sb; p.tok_si = tok_si; p.ld_out = I; p.gate = gate;
+  switch (dh) {
+    case 16: return launch_attention_inst<16>(tq, tk, tv, tg, p, s);
+    case 32: return launch_attention_inst<32>(tq, tk, tv, tg, p, s);
+    case 64: return launch_attention_inst<64>(tq, tk, tv, tg, p, s);
+    default: return launch_attention_inst<128>(tq, tk, tv, tg, p, s);
+  }
 }
 
 // OuterMean normaliser of pair rows [row0, row0 + rows) of one batch element (quirk Q3): bit-packed kernel when the packed
@@ -892,7 +906,7 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   NvtxRange nvtx_(row_attn ? "af2_axial_attention(row)" : "af2_axial_attention(col)");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!w || !x) return fail(AF2_ERR_BAD_ARG, "axial_attention: null argument");
-  if (dim_head != 32 && dim_head != 64) return fail(AF2_ERR_BAD_ARG, "axial_attention: dim_head %d unsupported (32 or 64)", dim_head);
+  if (!attention_dim_head_ok(dim_head)) return fail(AF2_ERR_BAD_ARG, "axial_attention: " DIM_HEAD_UNSUPPORTED, dim_head);
   if (d % 8) return fail(AF2_ERR_BAD_ARG, "axial_attention: dim %d must be a multiple of 8", d);
   const long long T = (long long)B * h * wdim, I = (long long)heads * dim_head;
   if (T > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "axial_attention: too many tokens");

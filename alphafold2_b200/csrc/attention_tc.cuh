@@ -19,6 +19,11 @@
 //     epilogue               O / l * sigmoid-gate (gate tile from shared memory) -> bf16 [token, h*DH + e]
 // Slots and stages are handed over with phase-tracked mbarriers only: an item slot (Q | gate | key codes) is refilled once
 // all 256 consumer threads have arrived on its `slot_empty` barrier after their epilogue.
+// Head widths (DH = dim_head): 16, 32, 64 and 128.  A row of Q / K / V / gate is DH * 2 bytes; DH 16 / 32 / 64 use one
+// swizzle atom of that width (32B / 64B / 128B swizzle).  DH 128 rows are 256 B, wider than a 128B-swizzled TMA box, so
+// every DH 128 tile is two 64-channel halves (two TMA boxes) stored one after the other: QK^T steps through both halves,
+// and V is an MN-major B operand whose N = 128 spans both (LBO = the half stride).  To keep two 128-key K / V stages in
+// flight within 227 KB at n = 16,384, DH 128 item slots hold Q only and the epilogue reads the gate from global memory.
 // Logits are produced directly in the log2 domain: the host folds dim_head^-0.5 * log2(e) into to_q and
 // log2(e) into edges_to_attn_bias, so the softmax is exp2(v - max) with no per-element scaling.
 //
@@ -43,6 +48,7 @@ struct AttnParams {
   __nv_bfloat16* out;         // [token, heads*DH]; token(b', i) = b'*tok_sb + i*tok_si
   long long tok_sb, tok_si;
   long long ld_out;
+  const __nv_bfloat16* gate;  // [token, heads*DH], pitch ld_out: read directly by the DH 128 epilogue (the others TMA it)
 };
 
 constexpr int ATTN_THREADS = 384;
@@ -52,12 +58,19 @@ constexpr int ATTN_CONSUMERS = 256;                 // threads of warpgroups 1 a
 
 template <int DH>
 struct AttnSmem {
+  static_assert(DH == 16 || DH == 32 || DH == 64 || DH == 128, "attention: DH must be 16, 32, 64 or 128");
+  static constexpr bool GATE_SMEM = DH != 128;        // DH 128: the gate is read from global memory in the epilogue
+  static constexpr int STAGES = DH == 128 ? 2 : ATTN_STAGES;
+  static constexpr int ATOM_B = DH == 128 ? 128 : DH * 2;   // bytes per row of one swizzle atom (= one TMA box row)
+  static constexpr int NATOM = DH * 2 / ATOM_B;              // 64-channel halves per row: 2 at DH 128, else 1
   static constexpr int Q_BYTES = 128 * DH * 2;        // one Q or gate tile
-  static constexpr int SLOT_BYTES = 2 * Q_BYTES;      // item slot: Q | gate
+  static constexpr int Q_ATOM = 128 * ATOM_B;         // one half of a Q / gate tile
+  static constexpr int SLOT_BYTES = (GATE_SMEM ? 2 : 1) * Q_BYTES;   // item slot: Q | gate (DH 128: Q)
   static constexpr int KV_BYTES = ATTN_KB * DH * 2;
+  static constexpr int KV_ATOM = ATTN_KB * ATOM_B;    // one half of a K or V tile
   static constexpr int STAGE_BYTES = 2 * KV_BYTES;    // K | V
   static constexpr int STAGE_OFF = 2 * SLOT_BYTES;
-  static constexpr int BAR_OFF = STAGE_OFF + ATTN_STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFF = STAGE_OFF + STAGES * STAGE_BYTES;
   static constexpr int KM_OFF = BAR_OFF + 128;        // key codes of the two item slots, kpad(n) each: 0 padding, 1 masked, 2 valid
   static constexpr int kpad(int n) { return (n + ATTN_KB - 1) / ATTN_KB * ATTN_KB; }
   static constexpr int bytes(int n) { return KM_OFF + 2 * kpad(n); }
@@ -72,23 +85,24 @@ __device__ __forceinline__ AttnItem attn_item(int item, int heads, int nqb) {
 }
 
 // tmQ/tmK/tmV/tmG: 4-D maps over the projection buffer (Q, K, V) and the gate, dims (e [DH], i [n], h [heads],
-// b' [nbatch]), box (DH, 128, 1, 1), swizzle = DH*2 bytes.
+// b' [nbatch]), box (min(DH, 64), 128, 1, 1), swizzle = the box row's bytes.  tmG is not read at DH 128.
 template <int DH>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmG,
                     const __grid_constant__ AttnParams p) {
   using L = AttnSmem<DH>;
-  constexpr uint32_t SWZ = (DH == 64) ? SWZ_128 : SWZ_64;
-  constexpr uint32_t ROWB = DH * 2;                 // bytes per Q/K/V/gate row
+  constexpr uint32_t SWZ = (DH >= 64) ? SWZ_128 : (DH == 32 ? SWZ_64 : SWZ_32);
+  constexpr uint32_t ROWB = L::ATOM_B;              // bytes per row of a Q/K/V/gate swizzle atom
   constexpr uint32_t SBO = 8 * ROWB;                // 8-row swizzle atom
+  constexpr int KSTEP_PER_ATOM = ROWB / 32;         // k16 steps of QK^T inside one atom row
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint64_t* slot_full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);   // [2] Q and gate tiles landed
   uint64_t* code_full = slot_full + 2;                                   // [2] key codes written
   uint64_t* slot_empty = code_full + 2;                                  // [2] the consumers are done with the slot
-  uint64_t* full_bar = slot_empty + 2;                                   // [ATTN_STAGES] K / V landed
-  uint64_t* empty_bar = full_bar + ATTN_STAGES;                          // [ATTN_STAGES] K / V consumed
+  uint64_t* full_bar = slot_empty + 2;                                   // [L::STAGES] K / V landed
+  uint64_t* empty_bar = full_bar + L::STAGES;                            // [L::STAGES] K / V consumed
 
   const int n = p.n;
   const int nqb = (n + 127) / 128;
@@ -107,7 +121,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       mbar_init(&code_full[s], 32);              // every lane of the key-code warp
       mbar_init(&slot_empty[s], ATTN_CONSUMERS);
     }
-    for (int s = 0; s < ATTN_STAGES; ++s) {
+    for (int s = 0; s < L::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);   // one arrive per softmax warpgroup
     }
@@ -124,7 +138,8 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     // ================================ producer warpgroup ================================
     regs_dealloc<40>();
     if (warp == 0 && lane == 0) {
-      // TMA: Q | gate into the item slot, then K / V into the ring; runs ahead by up to one item slot and ATTN_STAGES stages
+      // TMA: Q | gate into the item slot, then K / V into the ring; runs ahead by up to one item slot and L::STAGES stages.
+      // A tile is NATOM boxes of 64 channels (DH 128) or one box of DH channels, stored one after the other.
       int kbg = 0;   // key blocks issued by this CTA so far: ring stage and phase
       for (int item = blockIdx.x, it = 0; item < items; item += gridDim.x, ++it) {
         const AttnItem w = attn_item(item, p.heads, nqb);
@@ -132,15 +147,19 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         mbar_wait(&slot_empty[slot], ((it >> 1) & 1) ^ 1);
         uint8_t* q = smem + slot * L::SLOT_BYTES;
         mbar_arrive_expect_tx(&slot_full[slot], L::SLOT_BYTES);
-        tma_load_4d(q, &tmQ, &slot_full[slot], 0, w.qb * 128, w.h, w.b);
-        tma_load_4d(q + L::Q_BYTES, &tmG, &slot_full[slot], 0, w.qb * 128, w.h, w.b);
+#pragma unroll
+        for (int a = 0; a < L::NATOM; ++a) tma_load_4d(q + a * L::Q_ATOM, &tmQ, &slot_full[slot], a * 64, w.qb * 128, w.h, w.b);
+        if constexpr (L::GATE_SMEM) tma_load_4d(q + L::Q_BYTES, &tmG, &slot_full[slot], 0, w.qb * 128, w.h, w.b);
         for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-          const int s = kbg % ATTN_STAGES;
-          mbar_wait(&empty_bar[s], ((kbg / ATTN_STAGES) & 1) ^ 1);
+          const int s = kbg % L::STAGES;
+          mbar_wait(&empty_bar[s], ((kbg / L::STAGES) & 1) ^ 1);
           uint8_t* st = smem + L::STAGE_OFF + s * L::STAGE_BYTES;
           mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          tma_load_4d(st, &tmK, &full_bar[s], 0, kb * ATTN_KB, w.h, w.b);
-          tma_load_4d(st + L::KV_BYTES, &tmV, &full_bar[s], 0, kb * ATTN_KB, w.h, w.b);
+#pragma unroll
+          for (int a = 0; a < L::NATOM; ++a) tma_load_4d(st + a * L::KV_ATOM, &tmK, &full_bar[s], a * 64, kb * ATTN_KB, w.h, w.b);
+#pragma unroll
+          for (int a = 0; a < L::NATOM; ++a)
+            tma_load_4d(st + L::KV_BYTES + a * L::KV_ATOM, &tmV, &full_bar[s], a * 64, kb * ATTN_KB, w.h, w.b);
         }
       }
     } else if (warp == 1) {
@@ -188,14 +207,18 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     mbar_wait(&slot_full[slot], use);
 
     for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-      const int st = kbg % ATTN_STAGES;
-      mbar_wait(&full_bar[st], (kbg / ATTN_STAGES) & 1);
+      const int st = kbg % L::STAGES;
+      mbar_wait(&full_bar[st], (kbg / L::STAGES) & 1);
       const uint32_t sk = smem_u32(smem + L::STAGE_OFF + st * L::STAGE_BYTES);
       const uint32_t sv = sk + L::KV_BYTES;
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < DH / 16; ++k)
-        wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc(sq + k * 32, 16, SBO, SWZ), wgmma_desc(sk + k * 32, 16, SBO, SWZ), k != 0 ? 1u : 0u);
+      for (int k = 0; k < DH / 16; ++k) {
+        // k16 step k: 32-byte column (k % KSTEP_PER_ATOM) of 64-channel half k / KSTEP_PER_ATOM (always half 0 below DH 128)
+        const uint32_t qo = (k / KSTEP_PER_ATOM) * L::Q_ATOM + (k % KSTEP_PER_ATOM) * 32;
+        const uint32_t ko = (k / KSTEP_PER_ATOM) * L::KV_ATOM + (k % KSTEP_PER_ATOM) * 32;
+        wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc(sq + qo, 16, SBO, SWZ), wgmma_desc(sk + ko, 16, SBO, SWZ), k != 0 ? 1u : 0u);
+      }
       wgmma_commit();
       wgmma_wait<0>();
       reg_fence(s);
@@ -262,10 +285,13 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < ATTN_KB / 16; ++kk) {
-        // V tile [key][DH] is the MN-major B operand: 16 keys per step, 8-key groups SBO apart
-        const uint64_t vdesc = wgmma_desc(sv + kk * 16 * ROWB, 8192, SBO, SWZ);
-        if constexpr (DH == 64) wgmma_m64n64k16_rs<1>(o, pa[kk], vdesc, 1u);
-        else wgmma_m64n32k16_rs<1>(o, pa[kk], vdesc, 1u);
+        // V tile [key][DH] is the MN-major B operand: 16 keys per step, 8-key groups SBO apart; at DH 128 N spans the two
+        // 64-channel halves, LBO apart (the LBO is not read when N fits one swizzle atom)
+        const uint64_t vdesc = wgmma_desc(sv + kk * 16 * ROWB, DH == 128 ? L::KV_ATOM : 8192, SBO, SWZ);
+        if constexpr (DH == 128) wgmma_m64n128k16_rs<1>(o, pa[kk], vdesc, 1u);
+        else if constexpr (DH == 64) wgmma_m64n64k16_rs<1>(o, pa[kk], vdesc, 1u);
+        else if constexpr (DH == 32) wgmma_m64n32k16_rs<1>(o, pa[kk], vdesc, 1u);
+        else wgmma_m64n16k16_rs<1>(o, pa[kk], vdesc, 1u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -287,9 +313,16 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 #pragma unroll
       for (int i = 0; i < DH / 8; ++i) {
         const int e = 8 * i + 2 * (lane & 3);
-        // the TMA swizzle moves 16-byte chunk c of row r to chunk c ^ (r % 8) (128 B rows) or c ^ (r / 2 % 4) (64 B rows)
-        const uint32_t off = r * ROWB + e * 2;
-        const uint32_t gw = *reinterpret_cast<const uint32_t*>(gtile + (off ^ (((off >> 7) & (DH == 64 ? 7u : 3u)) << 4)));
+        uint32_t gw;
+        if constexpr (L::GATE_SMEM) {
+          // the TMA swizzle moves 16-byte chunk c of row r to chunk c ^ (r % 8) (128 B rows), c ^ (r / 2 % 4) (64 B rows)
+          // or c ^ (r / 4 % 2) (32 B rows)
+          constexpr uint32_t CMASK = DH == 64 ? 7u : (DH == 32 ? 3u : 1u);
+          const uint32_t off = r * ROWB + e * 2;
+          gw = *reinterpret_cast<const uint32_t*>(gtile + (off ^ (((off >> 7) & CMASK) << 4)));
+        } else {
+          gw = __ldg(reinterpret_cast<const unsigned int*>(p.gate + tok * p.ld_out + w.h * DH + e));
+        }
         *reinterpret_cast<uint32_t*>(out + e) =
             pack_bf16x2(o[4 * i + 2 * hf] * inv * bf16lo_to_f32(gw), o[4 * i + 2 * hf + 1] * inv * bf16hi_to_f32(gw));
       }

@@ -186,7 +186,8 @@ int af2_gemm_bf16_epilogue(const void* A, long long lda, long long a_batch, cons
  * tok = b * tok_sb + i * tok_si of each of the nbatch folded rows / columns.  qkv bf16 [tokens, 3 * heads * dim_head]
  * (q | k | v), gate bf16 [tokens, heads * dim_head] (sigmoid already applied), bias bf16 [heads][n][align8(n)] or NULL,
  * mask bool indexed like the tokens or NULL: logits where !(mask[i] & mask[j]) are replaced by -FLT_MAX (a fully masked
- * query averages all n values).  dim_head 32 or 64. */
+ * query averages all n values).  dim_head 16, 32, 64 or 128 (the bf16 axial-attention entries take the same set; their
+ * strict-mode forms take any multiple of 4). */
 int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, const unsigned char* mask, void* out, int n,
                        int nbatch, int heads, int dim_head, long long tok_sb, long long tok_si, af2_stream_t stream);
 /* af2_gemm_bf16_f32 with the tile width `bn` (64 / 128 / 256) as given and gathered operands, as the sharded contractions

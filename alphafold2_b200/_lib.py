@@ -70,6 +70,10 @@ class TemplateAngleWeights(C.Structure):
 TemplateAngleWeightsStrict = TemplateAngleWeights      # same layout, split-bf16 weights
 
 
+class PeerChunk(C.Structure):
+    _fields_ = [("src_off", ll), ("dst_off", ll), ("dst_row_stride", ll), ("row_bytes", ll), ("rows", ci), ("reserved", ci)]
+
+
 _SIGNATURES = {
     "af2_last_error": (C.c_char_p, []),
     "af2_abi_version": (ci, []),
@@ -183,6 +187,7 @@ _SIGNATURES = {
     "af2_peer_close": (ci, [vp]),
     "af2_peer_error": (ci, [vp]),
     "af2_peer_exchange": (ci, [vp, ll, ll, vp, ll, ll, ci, ll, ci, ci, ci, vp]),
+    "af2_peer_exchange_chunks": (ci, [vp, ll, C.POINTER(PeerChunk), vp, ci, ci, ci, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -2,7 +2,10 @@
 
 The reference has no multi-device path (SURVEY.md §2.2); this is the GPU-native addition named by the north
 star: one sequence's forward is split over the MSA-row and pair-row axes (FastFold-DAP style).  At block entry
-rank r owns pair rows x[r*N/P:(r+1)*N/P, :, :] and MSA rows m[r*S/P:(r+1)*S/P, :, :]; weights are replicated.
+rank r owns pair rows x[r*N/P:(r+1)*N/P, :, :] and MSA rows m[r*S/P:(r+1)*S/P, :, :]; weights are replicated.  When P
+does not divide N or S the shards are balanced instead (shard_offsets: the first N % P ranks hold one row more; MSA
+shards may be empty), the all-to-alls take split sizes, gathered pieces are padded to the largest shard, and the
+contractions read the gathered pieces merged into one compact operand.
 Every sub-op is embarrassingly parallel along ONE axis, so the schedule switches the sharded axis with
 all-to-alls and all-gathers the one operand a contraction needs in full (SURVEY.md §8e):
 
@@ -33,30 +36,102 @@ def _align8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
+def shard_offsets(n: int, P: int) -> list:
+    """Balanced shards of n rows over P ranks: rank r owns rows [off[r], off[r+1]) with off[r] = r*(n//P) + min(r, n%P),
+    so the first n % P ranks hold one row more.  A shard is empty when n < P."""
+    q, rem = divmod(n, P)
+    return [r * q + min(r, rem) for r in range(P + 1)]
+
+
+def shard_counts(n: int, P: int) -> list:
+    off = shard_offsets(n, P)
+    return [b - a for a, b in zip(off, off[1:])]
+
+
+def _pad_dim(t: torch.Tensor, dim: int, size: int) -> torch.Tensor:
+    """t zero-padded along `dim` to `size` (the largest shard's extent, so that every rank contributes one shape)."""
+    if t.shape[dim] == size:
+        return t.contiguous()
+    shape = list(t.shape)
+    shape[dim] = size
+    out = t.new_zeros(shape)
+    out.narrow(dim, 0, t.shape[dim]).copy_(t)
+    return out
+
+
 # ------------------------------------------------------------------------------------------------------------
-# collectives (concatenate along dim 0 so that both NCCL and gloo accept them)
+# collectives (concatenate along dim 0 so that both NCCL and gloo accept them).  counts / rows / cols: every rank's shard
+# size along the split axes when the shards are uneven (shard_counts); None when every rank holds the same size.
 # ------------------------------------------------------------------------------------------------------------
-def all_gather_cat0(t: torch.Tensor, group) -> torch.Tensor:
+def all_gather_cat0(t: torch.Tensor, group, counts=None) -> torch.Tensor:
+    """Every rank's t concatenated along dim 0 in rank order.  With counts, rank p holds counts[p] rows: each piece is padded
+    to the largest and the receiver drops the padding."""
+    if counts is not None:
+        mx = max(counts)
+        g = all_gather_cat0(_pad_dim(t, 0, mx), group)
+        return torch.cat([g[p * mx:p * mx + c] for p, c in enumerate(counts)])
     P = dist.get_world_size(group)
     out = torch.empty((P * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
     dist.all_gather_into_tensor(out, t.contiguous(), group=group)
     return out
 
 
-def rows_to_cols(t_row: torch.Tensor, group) -> torch.Tensor:
-    """[R, C, d] (my R rows, all C columns) -> [P*R, C/P, d] (all rows, my columns)."""
+def _rows_to_cols_splits(t_row: torch.Tensor, rows, cols, r: int):
+    """all_to_all_single operands of rows_to_cols over uneven shards: (send, recv, input splits, output splits)."""
+    R, _, d = t_row.shape
+    c0 = [0]
+    for c in cols:
+        c0.append(c0[-1] + c)
+    send = torch.cat([t_row[:, c0[p]:c0[p + 1]].reshape(-1) for p in range(len(cols))])     # chunk p: my rows x columns of rank p
+    recv = t_row.new_empty(sum(rows) * cols[r] * d)                                           # chunk p: rows of rank p x my columns
+    return send, recv, [R * c * d for c in cols], [rp * cols[r] * d for rp in rows]
+
+
+def rows_to_cols(t_row: torch.Tensor, group, rows=None, cols=None) -> torch.Tensor:
+    """[R, C, d] (my R rows, all C columns) -> [P*R, C/P, d] (all rows, my columns).
+    With rows / cols (every rank's row and column counts): [R_r, C, d] -> [sum(rows), cols[r], d]."""
     P = dist.get_world_size(group)
     R, Cc, d = t_row.shape
+    if rows is not None:
+        r = dist.get_rank(group)
+        send, recv, isz, osz = _rows_to_cols_splits(t_row, rows, cols, r)
+        dist.all_to_all_single(recv, send, output_split_sizes=osz, input_split_sizes=isz, group=group)
+        return recv.view(sum(rows), cols[r], d)
     send = t_row.view(R, P, Cc // P, d).permute(1, 0, 2, 3).contiguous()      # chunk p: my rows x columns of rank p
     recv = torch.empty_like(send)
     dist.all_to_all_single(recv, send, group=group)                           # chunk p: rows of rank p x my columns
     return recv.view(P * R, Cc // P, d)
 
 
-def cols_to_rows(t_col: torch.Tensor, group) -> torch.Tensor:
-    """[P*R, Cl, d] (all rows, my Cl columns) -> [R, P*Cl, d] (my rows, all columns)."""
+def _cols_to_rows_splits(t_col: torch.Tensor, rows, cols, r: int):
+    """all_to_all_single operands of cols_to_rows over uneven shards: (send, recv, input splits, output splits)."""
+    _, Cl, d = t_col.shape
+    send = t_col.contiguous().view(-1)                                        # chunk p: rows of rank p x my columns
+    recv = t_col.new_empty(rows[r] * sum(cols) * d)                           # chunk p: my rows x columns of rank p
+    return send, recv, [rp * Cl * d for rp in rows], [rows[r] * c * d for c in cols]
+
+
+def _place_row_chunks(out: torch.Tensor, recv: torch.Tensor, cols):
+    """out [R, sum(cols), d] <- the received chunks (chunk p = my rows x the cols[p] columns of rank p)."""
+    R, _, d = out.shape
+    o = c0 = 0
+    for c in cols:
+        out[:, c0:c0 + c].copy_(recv[o:o + R * c * d].view(R, c, d))
+        o, c0 = o + R * c * d, c0 + c
+
+
+def cols_to_rows(t_col: torch.Tensor, group, rows=None, cols=None) -> torch.Tensor:
+    """[P*R, Cl, d] (all rows, my Cl columns) -> [R, P*Cl, d] (my rows, all columns).
+    With rows / cols (every rank's row and column counts): [sum(rows), cols[r], d] -> [rows[r], sum(cols), d]."""
     P = dist.get_world_size(group)
     RR, Cl, d = t_col.shape
+    if rows is not None:
+        r = dist.get_rank(group)
+        send, recv, isz, osz = _cols_to_rows_splits(t_col, rows, cols, r)
+        dist.all_to_all_single(recv, send, output_split_sizes=osz, input_split_sizes=isz, group=group)
+        out = t_col.new_empty(rows[r], sum(cols), d)
+        _place_row_chunks(out, recv, cols)
+        return out
     R = RR // P
     send = t_col.contiguous().view(P, R, Cl, d)                               # chunk p: rows of rank p x my columns
     recv = torch.empty_like(send)
@@ -68,9 +143,10 @@ class _Deferred:
     """cols_to_rows on a side stream: the MSA tensor goes back to row shards while the pair track of the same block runs
     (nothing reads it before the next block's row attention).  With NCCL the collective itself runs on the process
     group's stream either way and the side stream removes the main stream's wait for it; with the peer-memory exchange
-    (ex) the exchange kernel itself runs on the side stream, on barrier channel 1.  `get()` joins."""
+    (ex) the exchange kernel itself runs on the side stream, on barrier channel 1.  `get()` joins.
+    rows / cols: as for cols_to_rows (uneven shards)."""
 
-    def __init__(self, t_col: torch.Tensor, group, side, ex=None):
+    def __init__(self, t_col: torch.Tensor, group, side, ex=None, rows=None, cols=None):
         cur = torch.cuda.current_stream()
         if ex is not None:
             ready = cur.record_event()
@@ -82,8 +158,20 @@ class _Deferred:
             return
         P = dist.get_world_size(group)
         RR, Cl, d = t_col.shape
-        R = RR // P
         self.keep = t_col                                                     # source stays alive until the side stream is done
+        if rows is not None:
+            r = dist.get_rank(group)
+            send, recv, isz, osz = _cols_to_rows_splits(t_col, rows, cols, r)   # allocated on the main stream: its pool, its ordering
+            self.out = torch.empty(rows[r], sum(cols), d, dtype=t_col.dtype, device=t_col.device)
+            self.bufs = (send, recv)
+            ready = cur.record_event()
+            with torch.cuda.stream(side):
+                side.wait_event(ready)
+                dist.all_to_all_single(recv, send, output_split_sizes=osz, input_split_sizes=isz, group=group)
+                _place_row_chunks(self.out, recv, cols)
+                self.done = side.record_event()
+            return
+        R = RR // P
         send = t_col.contiguous().view(P, R, Cl, d)
         recv = torch.empty_like(send)                                         # allocated on the main stream: its pool, its ordering
         self.out = torch.empty(R, P * Cl, d, dtype=t_col.dtype, device=t_col.device)
@@ -133,27 +221,32 @@ class PeerExchange:
         self.opened = []
 
     @staticmethod
-    def layout(N: int, S: int, d: int, P: int) -> dict:
+    def layout(N: int, S: int, d: int, P: int, rank: int = 0) -> dict:
         """Where the buffers of one rank's arena lie: off[(track, layout)] is a buffer's byte offset, shapes[(track, layout)]
-        its fp32 shape, total the arena's size in bytes.  The control block comes first; every buffer starts on 256 B."""
+        its fp32 shape on rank `rank`, total the arena's size in bytes, offsets[track] the shard_offsets of the track's rows
+        (the columns of both tracks are the pair rows' shards).  The control block comes first; every buffer starts on 256 B
+        and is sized for the largest shard (ceil(N/P), ceil(S/P)), so it starts at the same offset in every rank's arena."""
         ctrl = int(_lib.load().af2_peer_ctrl_bytes())
         al = lambda n: (n + 255) // 256 * 256  # noqa: E731
-        pair_b, msa_b = al(N // P * N * d * 4), al(S // P * N * d * 4)
+        Rn, Rs = -(-N // P), -(-S // P)
+        pair_row, pair_col, msa_row, msa_col = al(Rn * N * d * 4), al(N * Rn * d * 4), al(Rs * N * d * 4), al(S * Rn * d * 4)
+        on, os_ = shard_offsets(N, P), shard_offsets(S, P)
+        nr, ns = on[rank + 1] - on[rank], os_[rank + 1] - os_[rank]
         PAIR, MSA = PeerExchange.PAIR, PeerExchange.MSA
-        return dict(off={(PAIR, "row"): ctrl, (PAIR, "col"): ctrl + pair_b,
-                         (MSA, "row"): ctrl + 2 * pair_b, (MSA, "col"): ctrl + 2 * pair_b + msa_b},
-                    shapes={(PAIR, "row"): (N // P, N, d), (PAIR, "col"): (N, N // P, d),
-                            (MSA, "row"): (S // P, N, d), (MSA, "col"): (S, N // P, d)},
-                    total=ctrl + 2 * pair_b + 2 * msa_b)
+        return dict(off={(PAIR, "row"): ctrl, (PAIR, "col"): ctrl + pair_row,
+                         (MSA, "row"): ctrl + pair_row + pair_col, (MSA, "col"): ctrl + pair_row + pair_col + msa_row},
+                    shapes={(PAIR, "row"): (nr, N, d), (PAIR, "col"): (N, nr, d),
+                            (MSA, "row"): (ns, N, d), (MSA, "col"): (S, nr, d)},
+                    total=ctrl + pair_row + pair_col + msa_row + msa_col, offsets={PAIR: on, MSA: os_})
 
     @classmethod
     def attach(cls, P: int, rank: int, base: int, table: torch.Tensor, device: torch.device, layout: dict, group=None):
-        """Rank `rank` of an exchange over arenas that already exist: base is this rank's arena (laid out by `layout`), table
-        the device int64 [P] of every rank's arena base as this process addresses it (its own included)."""
+        """Rank `rank` of an exchange over arenas that already exist: base is this rank's arena (laid out by `layout` for
+        this rank), table the device int64 [P] of every rank's arena base as this process addresses it (its own included)."""
         self = cls()
         self.group, self.P, self.rank, self.device = group, P, rank, device
         self.base, self.table = base, table
-        self.off, self.shapes = layout["off"], layout["shapes"]
+        self.off, self.shapes, self.offsets = layout["off"], layout["shapes"], layout["offsets"]
         self.arena = torch.as_tensor(_RawCuda(base, layout["total"]), device=device)
         self.exchanges = 0
         return self
@@ -164,7 +257,7 @@ class PeerExchange:
         lib = _lib.load()
         self = cls()                   # holds the local arena and the peer mappings until every rank has them
         self.group, self.P, self.rank, self.device = group, P, r, device
-        lay = cls.layout(N, S, d, P)
+        lay = cls.layout(N, S, d, P, r)
         total = lay["total"]
         ok = P <= 32 and device.type == "cuda"
         handle = torch.zeros(72, dtype=torch.uint8)
@@ -252,22 +345,71 @@ class PeerExchange:
         return dict(src_peer_stride=R * chunk, src_row_stride=chunk, dst_off=rank * chunk, dst_row_stride=P * chunk,
                     rows=R, row_bytes=chunk)
 
+    @staticmethod
+    def plan_rows_to_cols_ragged(row_off, col_off, d: int, rank: int, itemsize: int = 4):
+        """af2_peer_exchange_chunks arguments (bytes) for uneven shards (row_off / col_off: shard_offsets of the row and column
+        axes): [R_rank, C, d] row shards -> [R_total, C_p, d] column shards.  chunks[p] = my rows x the columns of rank p; it
+        lands in rank p's column buffer at row row_off[rank], whose rows are C_p columns wide.  For even shards the chunks are
+        plan_rows_to_cols with src_off = p * src_peer_stride.  Pure arithmetic, like plan_rows_to_cols."""
+        C, R = col_off[-1], row_off[rank + 1] - row_off[rank]
+        chunks = []
+        for p in range(len(col_off) - 1):
+            w = (col_off[p + 1] - col_off[p]) * d * itemsize
+            chunks.append(dict(src_off=col_off[p] * d * itemsize, dst_off=row_off[rank] * w, dst_row_stride=w, rows=R, row_bytes=w))
+        return dict(src_row_stride=C * d * itemsize, chunks=chunks)
+
+    @staticmethod
+    def plan_cols_to_rows_ragged(row_off, col_off, d: int, rank: int, itemsize: int = 4):
+        """The way back for uneven shards: [R_total, C_rank, d] -> [R_p, C, d].  chunks[p] = the rows of rank p x my columns
+        (contiguous at the source; none when rank p has no rows); it lands in rank p's row buffer at columns col_off[rank]..
+        of every row."""
+        C = col_off[-1]
+        w = (col_off[rank + 1] - col_off[rank]) * d * itemsize
+        chunks = [dict(src_off=row_off[p] * w, dst_off=col_off[rank] * d * itemsize, dst_row_stride=C * d * itemsize,
+                       rows=row_off[p + 1] - row_off[p], row_bytes=w) for p in range(len(col_off) - 1)]
+        return dict(src_row_stride=w, chunks=chunks)
+
     def _run(self, src: torch.Tensor, plan: dict, dst_buffer_off: int, channel: int):
         self._exchange(src, plan["src_peer_stride"], plan["src_row_stride"], dst_buffer_off + plan["dst_off"], plan["dst_row_stride"],
                        plan["rows"], plan["row_bytes"], channel)
 
+    def _run_chunks(self, src_ptr: int, plan: dict, dst_buffer_off: int, channel: int):
+        table = (_lib.PeerChunk * self.P)(*[_lib.PeerChunk(c["src_off"], dst_buffer_off + c["dst_off"], c["dst_row_stride"],
+                                                           c["row_bytes"], c["rows"], 0) for c in plan["chunks"]])
+        _lib.check(_lib.load().af2_peer_exchange_chunks(src_ptr, plan["src_row_stride"], table, self.table.data_ptr(), channel,
+                                                         self.rank, self.P, _ops._stream_ptr()))
+        self.exchanges += 1
+
+    def _even(self, track: int) -> bool:
+        """Every rank holds the same rows of the track and the same columns: the single-shape exchange applies."""
+        return all(o % self.P == 0 for o in (self.offsets[track][-1], self.offsets[self.PAIR][-1]))
+
+    def _check_src(self, t: torch.Tensor, track: int, layout: str):
+        assert tuple(t.shape) == self.shapes[(track, layout)]
+        assert t.numel() == 0 or t.data_ptr() == self.base + self.off[(track, layout)]
+
     def rows_to_cols(self, t_row: torch.Tensor, track: int, channel: int = 0) -> torch.Tensor:
-        """[R, C, d] (my rows, all columns; the track's row buffer) -> the track's column buffer [P*R, C/P, d]."""
+        """[R, C, d] (my rows, all columns; the track's row buffer) -> the track's column buffer [P*R, C/P, d]
+        ([R_total, C_rank, d] for uneven shards)."""
         R, Cc, d = t_row.shape
-        assert t_row.data_ptr() == self.base + self.off[(track, "row")] and tuple(t_row.shape) == self.shapes[(track, "row")]
-        self._run(t_row, self.plan_rows_to_cols(R, Cc, d, self.P, self.rank), self.off[(track, "col")], channel)
+        self._check_src(t_row, track, "row")
+        if self._even(track):
+            self._run(t_row, self.plan_rows_to_cols(R, Cc, d, self.P, self.rank), self.off[(track, "col")], channel)
+        else:
+            plan = self.plan_rows_to_cols_ragged(self.offsets[track], self.offsets[self.PAIR], d, self.rank)
+            self._run_chunks(self.base + self.off[(track, "row")], plan, self.off[(track, "col")], channel)
         return self.buffer(track, "col")
 
     def cols_to_rows(self, t_col: torch.Tensor, track: int, channel: int = 0) -> torch.Tensor:
-        """[P*R, Cl, d] (all rows, my columns; the track's column buffer) -> the track's row buffer [R, P*Cl, d]."""
+        """[P*R, Cl, d] (all rows, my columns; the track's column buffer) -> the track's row buffer [R, P*Cl, d]
+        ([R_rank, C, d] for uneven shards)."""
         RR, Cl, d = t_col.shape
-        assert t_col.data_ptr() == self.base + self.off[(track, "col")] and tuple(t_col.shape) == self.shapes[(track, "col")]
-        self._run(t_col, self.plan_cols_to_rows(RR, Cl, d, self.P, self.rank), self.off[(track, "row")], channel)
+        self._check_src(t_col, track, "col")
+        if self._even(track):
+            self._run(t_col, self.plan_cols_to_rows(RR, Cl, d, self.P, self.rank), self.off[(track, "row")], channel)
+        else:
+            plan = self.plan_cols_to_rows_ragged(self.offsets[track], self.offsets[self.PAIR], d, self.rank)
+            self._run_chunks(self.base + self.off[(track, "col")], plan, self.off[(track, "row")], channel)
         return self.buffer(track, "row")
 
     def error(self) -> bool:
@@ -373,13 +515,23 @@ class CudaStageOps:
         return out
 
     @staticmethod
-    def _merge_mn_pieces(Rg: torch.Tensor, pieces: int, d: int, n_total: int):
+    def _merge_mn_pieces(Rg: torch.Tensor, pieces, d: int, n_total: int):
         """Gathered MN-major operand [pieces*d, K, align8(n_total/pieces)] with fewer than 64 columns per piece: the kernel's
         64-column TMA boxes cannot span pieces, so instead of `pieces` tiny launches the pieces are re-packed once into ONE
         operand [d, K, align8(n_total)] (a pass over the gathered tensor, ~10 us at C2) and contracted in a single launch.
         Each piece's alignment padding is dropped on the way: column p*(n_total/pieces)+c of the result is column c of piece p.
-        Pieces of >= 64 columns are addressed in place."""
+        Pieces of >= 64 columns are addressed in place.
+        pieces may instead be the column count of every piece (uneven shards, [P*d, K, w] with piece p's columns in its
+        first pieces[p]): those are always merged, column sum(pieces[:p])+c of the result being column c of piece p."""
         K, w = Rg.shape[1], Rg.shape[2]
+        if not isinstance(pieces, int):
+            assert sum(pieces) == n_total
+            out = torch.zeros(d, K, _align8(n_total), dtype=Rg.dtype, device=Rg.device)
+            src, c0 = Rg.view(len(pieces), d, K, w), 0
+            for p, wp in enumerate(pieces):
+                out[:, :, c0:c0 + wp].copy_(src[p, :, :, :wp])
+                c0 += wp
+            return out, 1
         if pieces == 1 or w >= 64:
             return Rg, pieces
         wt = n_total // pieces
@@ -387,8 +539,16 @@ class CudaStageOps:
         out[:, :, :n_total].view(d, K, pieces, wt).copy_(Rg.view(pieces, d, K, w)[..., :wt].permute(1, 2, 0, 3))
         return out, 1
 
-    def outer_contract_(self, om, x_rows: torch.Tensor, L: torch.Tensor, Rg: torch.Tensor, msa_mask_full, row0: int, pieces: int):
-        """x_rows [rows, N, d] += OuterMean; L [d, S, align8(rows)], Rg [pieces*d, S, align8(N/pieces)]."""
+    @staticmethod
+    def _merge_k_pieces(Rg: torch.Tensor, rows, d: int):
+        """Gathered K-major operand of uneven shards [P*d, Rmax, K'] (piece p's rows in its first rows[p]) -> the compact
+        [d, sum(rows), K'] of the unsharded call, rows in rank order."""
+        src = Rg.view(len(rows), d, Rg.shape[1], Rg.shape[2])
+        return torch.cat([src[p, :, :rp] for p, rp in enumerate(rows)], 1), 1
+
+    def outer_contract_(self, om, x_rows: torch.Tensor, L: torch.Tensor, Rg: torch.Tensor, msa_mask_full, row0: int, pieces):
+        """x_rows [rows, N, d] += OuterMean; L [d, S, align8(rows)], Rg [pieces*d, S, align8(N/pieces)].
+        pieces: the number of equal pieces, or every piece's column count (uneven shards; see _merge_mn_pieces)."""
         pk = om.packed()
         rows, N, d = x_rows.shape
         S = L.shape[1]
@@ -430,19 +590,42 @@ class CudaStageOps:
                                             gate.data_ptr(), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
         return L, R, gate
 
-    def tri_contract_(self, tm, x_loc: torch.Tensor, L: torch.Tensor, Rg: torch.Tensor, gate: torch.Tensor, ingoing: bool, pieces: int):
-        """L may be a row window of a larger channel-major operand (its channel stride is passed on)."""
+    def tri_contract_(self, tm, x_loc: torch.Tensor, L: torch.Tensor, Rg: torch.Tensor, gate: torch.Tensor, ingoing: bool, pieces):
+        """L may be a row window of a larger channel-major operand (its channel stride is passed on).  pieces: the number of
+        equal gathered pieces, or every piece's size along the gathered axis (uneven shards: merged into one operand)."""
         pk = tm.packed()
         rows, cols, d = x_loc.shape
         K = L.shape[1] if ingoing else cols
+        if ingoing and not isinstance(pieces, int) and (cols % 4 == 0) != (rows % 4 == 0):
+            return self._tri_contract_ingoing_padded_(tm, x_loc, L, Rg, gate, pieces)
         if ingoing:
             Rg, pieces = self._merge_mn_pieces(Rg, pieces, d, rows)
+        elif not isinstance(pieces, int):
+            Rg, pieces = self._merge_k_pieces(Rg, pieces, d)
         lib = _lib.load()
         ws = _ops.workspace(lib.af2_triangle_contract_workspace(rows, cols, d), x_loc.device)
         per_piece = Rg.numel() // pieces
         _lib.check(lib.af2_triangle_contract(C.byref(pk.struct), x_loc.data_ptr(), L.data_ptr(), L.stride(0),
                                              Rg.data_ptr(), Rg.stride(0), per_piece, pieces, gate.data_ptr(),
                                              rows, cols, K, d, int(ingoing), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
+
+    def _tri_contract_ingoing_padded_(self, tm, x_col: torch.Tensor, L: torch.Tensor, Rg: torch.Tensor, gate: torch.Tensor, pieces):
+        """Ingoing contraction of an uneven column shard x_col [N, cols, d] whose width would make the contraction's
+        channel -> token LayerNorm run another kernel than the unsharded call (N columns) runs: that kernel is picked by
+        whether the output rows are dense, i.e. cols % 4 == 0 (api.cu c2t_select), and two kernels round differently.
+        The shard is contracted padded with zero columns to a width that is dense exactly when N is (align4(cols) if
+        N % 4 == 0, else cols + 1); the padding columns' outputs are dropped.  Every kept element is computed as in the
+        unsharded call (the GEMM and the LayerNorm are per output element / per token)."""
+        N, cols, d = x_col.shape
+        cp = (cols + 3) // 4 * 4 if N % 4 == 0 else cols + 1
+        x_pad = torch.zeros(N, cp, d, dtype=x_col.dtype, device=x_col.device)
+        x_pad[:, :cols].copy_(x_col)
+        L_pad = torch.zeros(d, L.shape[1], _align8(cp), dtype=L.dtype, device=L.device)
+        L_pad[:, :, :cols].copy_(L[:, :, :cols])
+        g_pad = torch.zeros(N, cp, d, dtype=gate.dtype, device=gate.device)
+        g_pad[:, :cols].copy_(gate.view(N, cols, d))
+        self.tri_contract_(tm, x_pad, L_pad, Rg, g_pad.view(N * cp, d), True, pieces)
+        x_col.copy_(x_pad[:, :cols])
 
     def tri_contract_window_(self, tm, x_rows: torch.Tensor, L: torch.Tensor, R_win: torch.Tensor, gate: torch.Tensor):
         """Ingoing contraction of pair rows [i0, i1): x_rows [rows, N, d] += to_out(LN_c(O) * gate) with
@@ -467,6 +650,10 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
 
     x [1, N, N, d], m [1, S, N, d], mask [1, N, N] bool, msa_mask [1, S, N] bool are the full (replicated) inputs;
     returns the full (x, m) on every rank when gather_output, else this rank's row shards.
+
+    Any N >= P and S >= 1: rank r owns pair rows (and columns) [on[r], on[r+1]) and MSA rows [os[r], os[r+1]) with
+    on = shard_offsets(N, P), os = shard_offsets(S, P); the first N % P (S % P) ranks hold one row more, and MSA shards
+    are empty when S < P.  Shapes that P divides take the equal-shard path unchanged.
     """
     if stage_ops is None and _ops.precision_of(evo) == "strict":
         raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
@@ -476,35 +663,52 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
     if x.shape[0] != 1:
         raise ValueError("the sharded trunk handles one sequence per call (batch 1)")
     N, S = x.shape[1], m.shape[1]
-    if N % P or S % P:
-        raise ValueError(f"N_res={N} and N_seq={S} must be divisible by the number of ranks {P}")
-    Rn, Rs = N // P, S // P
+    if N < P:
+        raise ValueError(f"N_res={N} is smaller than the number of ranks {P}: every rank needs at least one pair row")
+    on, os_ = shard_offsets(N, P), shard_offsets(S, P)
+    n0, n1, s0, s1 = on[r], on[r + 1], os_[r], os_[r + 1]
+    # shard sizes of every rank for the collectives, None where P divides the axis (equal shards: the plain collectives)
+    pair_counts = shard_counts(N, P) if N % P else None
+    msa_counts = shard_counts(S, P) if S % P else None
+    msa_ragged = pair_counts is not None or msa_counts is not None          # the MSA columns are the pair shards
+    msa_splits = (shard_counts(S, P), shard_counts(N, P)) if msa_ragged else (None, None)
+    Rn_max = -(-N // P)
     with torch.no_grad():
         ex = peer_exchange_for(group, x.device, N, S, x.shape[-1]) if stage_ops is None else None
         if ex is not None:                                            # the shards live in the peer-mapped arena
             x_row, m_row = ex.buffer(PeerExchange.PAIR, "row"), ex.buffer(PeerExchange.MSA, "row")
-            x_row.copy_(x[0, r * Rn:(r + 1) * Rn])
-            m_row.copy_(m[0, r * Rs:(r + 1) * Rs])
+            x_row.copy_(x[0, n0:n1])
+            m_row.copy_(m[0, s0:s1])
             pair_to_cols = lambda t: ex.rows_to_cols(t, PeerExchange.PAIR)  # noqa: E731
             pair_to_rows = lambda t: ex.cols_to_rows(t, PeerExchange.PAIR)  # noqa: E731
             msa_to_cols = lambda t: ex.rows_to_cols(t, PeerExchange.MSA)  # noqa: E731
             msa_to_rows = lambda t: ex.cols_to_rows(t, PeerExchange.MSA)  # noqa: E731
         else:
-            x_row = x[0, r * Rn:(r + 1) * Rn].detach().to(torch.float32).contiguous().clone()      # [N/P, N, d]
-            m_row = m[0, r * Rs:(r + 1) * Rs].detach().to(torch.float32).contiguous().clone()      # [S/P, N, d]
-            pair_to_cols = msa_to_cols = lambda t: rows_to_cols(t, group)  # noqa: E731
-            pair_to_rows = msa_to_rows = lambda t: cols_to_rows(t, group)  # noqa: E731
+            x_row = x[0, n0:n1].detach().to(torch.float32).contiguous().clone()      # [N/P, N, d]
+            m_row = m[0, s0:s1].detach().to(torch.float32).contiguous().clone()      # [S/P, N, d]
+            pair_to_cols = lambda t: rows_to_cols(t, group, pair_counts, pair_counts)  # noqa: E731
+            pair_to_rows = lambda t: cols_to_rows(t, group, pair_counts, pair_counts)  # noqa: E731
+            msa_to_cols = lambda t: rows_to_cols(t, group, *msa_splits)  # noqa: E731
+            msa_to_rows = lambda t: cols_to_rows(t, group, *msa_splits)  # noqa: E731
         mask_full = None if mask is None else mask[0].bool()
         mm_full = None if msa_mask is None else msa_mask[0].bool().contiguous()
-        mask_rows = None if mask_full is None else mask_full[r * Rn:(r + 1) * Rn].contiguous()
-        mask_cols = None if mask_full is None else mask_full[:, r * Rn:(r + 1) * Rn].contiguous()
-        mm_rows = None if mm_full is None else mm_full[r * Rs:(r + 1) * Rs].contiguous()
-        mm_cols = None if mm_full is None else mm_full[:, r * Rn:(r + 1) * Rn].contiguous()
+        mask_rows = None if mask_full is None else mask_full[n0:n1].contiguous()
+        mask_cols = None if mask_full is None else mask_full[:, n0:n1].contiguous()
+        mm_rows = None if mm_full is None else mm_full[s0:s1].contiguous()
+        mm_cols = None if mm_full is None else mm_full[:, n0:n1].contiguous()
 
         def gathered_bias(ax, xr):
             b = ops.pair_bias(ax, xr)                                 # [H, Rn, npad]
-            g = all_gather_cat0(b.transpose(0, 1).contiguous(), group)   # [N, H, npad] rows in global order
+            g = all_gather_cat0(b.transpose(0, 1).contiguous(), group, pair_counts)   # [N, H, npad] rows in global order
             return g.transpose(0, 1).contiguous()                    # [H, N, npad]
+
+        def gathered_operand(t, dim):
+            """A contraction's gathered operand and its `pieces`: P equal pieces, or with uneven shards each rank's piece
+            padded along `dim` (dim 1: rows, K-major; dim 2: columns, MN-major, aligned to 8 like the kernels' pitch) and
+            the pair shard sizes, which tell the stage op what to keep of each piece."""
+            if pair_counts is None:
+                return all_gather_cat0(t, group), P
+            return all_gather_cat0(_pad_dim(t, dim, Rn_max if dim == 1 else _align8(Rn_max)), group), tuple(pair_counts)
 
         overlap = OVERLAP_MSA_RETURN and x_row.is_cuda and P > 1
         side = torch.cuda.Stream() if overlap else None
@@ -516,27 +720,30 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
             bias_m = gathered_bias(msa_attn.row_attn, x_row)
             if pending is not None:
                 m_row, pending = pending.get(), None
-            ops.axial_attention_(msa_attn.row_attn, m_row, bias_m, mm_rows, True)
+            if m_row.shape[0]:                                                          # an empty MSA shard has nothing to attend
+                ops.axial_attention_(msa_attn.row_attn, m_row, bias_m, mm_rows, True)
             m_col = msa_to_cols(m_row)                                                  # [S, N/P, d]
             ops.axial_attention_(msa_attn.col_attn, m_col, None, mm_cols, False)
             ops.feed_forward_(msa_ff, m_col)
             # --- outer mean into the pair rows (alphafold2.py:379) ---
             LR = ops.outer_project(pair.outer_mean, m_col, mm_cols)                      # [2d, S, pitch(N/P)]
-            Rg = all_gather_cat0(LR[d:], group)                                          # [P*d, S, pitch]
-            ops.outer_contract_(pair.outer_mean, x_row, LR[:d], Rg, mm_full, r * Rn, P)
+            Rg, pieces = gathered_operand(LR[d:], 2)                                     # [P*d, S, pitch]
+            ops.outer_contract_(pair.outer_mean, x_row, LR[:d], Rg, mm_full, n0, pieces)
             if overlap:
-                pending = _Deferred(m_col, group, side, ex)                             # joins at the next block's row attention
+                pending = _Deferred(m_col, group, side, ex, *msa_splits)                # joins at the next block's row attention
             else:
                 m_row = msa_to_rows(m_col)
             # --- triangle multiply outgoing on pair rows (alphafold2.py:381) ---
             tm = pair.triangle_multiply_outgoing
             L, R, G = ops.tri_project(tm, x_row, mask_rows)
-            ops.tri_contract_(tm, x_row, L, all_gather_cat0(R, group), G, False, P)
+            Rg, pieces = gathered_operand(R, 1)
+            ops.tri_contract_(tm, x_row, L, Rg, G, False, pieces)
             # --- triangle multiply ingoing on pair columns (alphafold2.py:382) ---
             x_col = pair_to_cols(x_row)                                                  # [N, N/P, d]
             tm = pair.triangle_multiply_ingoing
             L, R, G = ops.tri_project(tm, x_col, mask_cols)
-            ops.tri_contract_(tm, x_col, L, all_gather_cat0(R, group), G, True, P)
+            Rg, pieces = gathered_operand(R, 2)
+            ops.tri_contract_(tm, x_col, L, Rg, G, True, pieces)
             # --- triangle attention outgoing = row attention on pair rows (alphafold2.py:383) ---
             x_row = pair_to_rows(x_col)
             ta = pair.triangle_attention_outgoing
@@ -554,8 +761,8 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
             m_row, pending = pending.get(), None
         if not gather_output:
             return (x_row.clone(), m_row.clone()) if ex is not None else (x_row, m_row)   # arena buffers are reused by the next call
-        xo = all_gather_cat0(x_row, group)[None]
-        mo = all_gather_cat0(m_row, group)[None]
+        xo = all_gather_cat0(x_row, group, pair_counts)[None]
+        mo = all_gather_cat0(m_row, group, msa_counts)[None]
     return xo.to(x.dtype), mo.to(m.dtype)
 
 

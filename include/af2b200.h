@@ -509,6 +509,16 @@ int af2_peer_error(const void* my_base);
 int af2_peer_exchange(const void* src, long long src_peer_stride, long long src_row_stride, void* const* peer_base,
                       long long dst_off, long long dst_row_stride, int rows, long long row_bytes, int channel, int rank, int P,
                       af2_stream_t stream);
+/* The same exchange for uneven shards: chunks is a HOST array of P entries, chunks[p] the chunk bound for rank p
+ * (`rows` rows of `row_bytes`, read at src + src_off + row*src_row_stride, stored into rank p's arena at
+ * dst_off + row*dst_row_stride).  rows may be 0 (0 .. 65535); a rank with nothing to send still joins the barrier.
+ * Offsets, strides and row bytes are multiples of 16, row_bytes >= 16 where rows > 0.  At most 32 ranks. */
+typedef struct {
+  long long src_off, dst_off, dst_row_stride, row_bytes;
+  int rows, reserved;
+} af2_peer_chunk;
+int af2_peer_exchange_chunks(const void* src, long long src_row_stride, const af2_peer_chunk* chunks, void* const* peer_base,
+                             int channel, int rank, int P, af2_stream_t stream);
 
 #ifdef __cplusplus
 }

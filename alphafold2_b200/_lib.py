@@ -92,6 +92,8 @@ _SIGNATURES = {
     "af2_outer_mean_workspace": (ll, [ci, ci, ci, ci]),
     "af2_pair_bias": (ci, [vp, vp, vp, ci, ci, ci, ci, vp]),
     "af2_axial_attention_prebias": (ci, [C.POINTER(AttnWeights), vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_axial_attention_tied_begin": (ci, [C.POINTER(AttnWeights), vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, ll, vp]),
+    "af2_axial_attention_tied_end": (ci, [C.POINTER(AttnWeights), vp, vp, vp, ci, ci, ci, ci, ci, vp, ci, ci, vp, ll, vp]),
     "af2_triangle_project": (ci, [C.POINTER(TriMulWeights), vp, vp, ll, ci, ci, vp, vp, ll, vp, vp, ll, vp]),
     "af2_triangle_project_workspace": (ll, [ll, ci]),
     "af2_triangle_contract": (ci, [C.POINTER(TriMulWeights), vp, vp, ll, vp, ll, ll, ci, vp, ci, ci, ci, ci, ci, vp, ll, vp]),

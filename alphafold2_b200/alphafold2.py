@@ -709,7 +709,7 @@ class Alphafold2(nn.Module):
     def embed_templates_(self, x, x_mask, templates_feats, templates_mask, group=None, band=None):
         """alphafold2.py:743-785 in place on the fp32 pair tensor x [b, n, n, d]: template pair stack, then the pointwise
         attention of every pair over its T templates, scaled by `any template valid` and added to x.  Under shard_evoformer
-        every rank computes this whole (it runs before the sharded trunk).
+        every rank computes this whole (it runs before the sharded trunk); parallel.shard_alphafold2 shards it instead.
 
         The templates run in groups of G: each group's pair stack at batch b * G, then its step of the pointwise attention,
         whose online softmax carries over to the next group.  The result does not depend on G (bitwise), only the memory does:

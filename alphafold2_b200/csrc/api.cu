@@ -900,29 +900,45 @@ long long af2_axial_attention_workspace(int B, int h, int wdim, int d, int heads
          align_up((long long)B * heads * n * npad * 2, 256) + 1024;
 }
 
-static int axial_attention_impl(const af2_attn_weights* w, float* x, const float* edges, const void* pre_bias,
-                                const unsigned char* mask, int B, int h, int wdim, int d, int heads, int dim_head,
-                                int row_attn, void* workspace, long long workspace_bytes, af2_stream_t stream, int tied = 0) {
-  NvtxRange nvtx_(row_attn ? "af2_axial_attention(row)" : "af2_axial_attention(col)");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+// One axial attention call: its shape and its workspace carve-up (af2_axial_attention_workspace).  The whole-call entry points
+// run axial_project and axial_attend on one plan; the tied-query pair af2_axial_attention_tied_begin / _end runs them in two
+// calls on the same workspace, with the cross-shard query mean between them.
+struct AxialPlan {
+  long long T, I;
+  int n, nb, npad;
+  bool has_bias;
+  __nv_bfloat16 *xn, *qkv, *gate, *og, *bias;
+};
+
+static int axial_plan(AxialPlan& p, const af2_attn_weights* w, const float* x, const float* edges, const void* pre_bias, int B,
+                      int h, int wdim, int d, int heads, int dim_head, int row_attn, void* workspace, long long workspace_bytes) {
   if (!w || !x) return fail(AF2_ERR_BAD_ARG, "axial_attention: null argument");
   if (!attention_dim_head_ok(dim_head)) return fail(AF2_ERR_BAD_ARG, "axial_attention: " DIM_HEAD_UNSUPPORTED, dim_head);
   if (d % 8) return fail(AF2_ERR_BAD_ARG, "axial_attention: dim %d must be a multiple of 8", d);
-  const long long T = (long long)B * h * wdim, I = (long long)heads * dim_head;
-  if (T > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "axial_attention: too many tokens");
-  const int n = row_attn ? wdim : h;
-  const int nb = row_attn ? h : wdim;
-  const int npad = (int)align_up(n, 8);
-  const bool has_bias = pre_bias != nullptr || (edges != nullptr && w->w_edge != nullptr);
+  p.T = (long long)B * h * wdim; p.I = (long long)heads * dim_head;
+  if (p.T > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "axial_attention: too many tokens");
+  p.n = row_attn ? wdim : h;
+  p.nb = row_attn ? h : wdim;
+  p.npad = (int)align_up(p.n, 8);
+  p.has_bias = pre_bias != nullptr || (edges != nullptr && w->w_edge != nullptr);
   Arena ar(workspace, workspace_bytes);
-  __nv_bfloat16* xn = ar.take<__nv_bfloat16>(T * d);
-  __nv_bfloat16* qkv = ar.take<__nv_bfloat16>(T * 3 * I);
-  __nv_bfloat16* gate = ar.take<__nv_bfloat16>(T * I);
-  __nv_bfloat16* og = ar.take<__nv_bfloat16>(T * I);
-  __nv_bfloat16* bias = ar.take<__nv_bfloat16>((long long)B * heads * n * npad);
+  p.xn = ar.take<__nv_bfloat16>(p.T * d);
+  p.qkv = ar.take<__nv_bfloat16>(p.T * 3 * p.I);
+  p.gate = ar.take<__nv_bfloat16>(p.T * p.I);
+  p.og = ar.take<__nv_bfloat16>(p.T * p.I);
+  p.bias = ar.take<__nv_bfloat16>((long long)B * heads * p.n * p.npad);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "axial_attention: workspace too small");
-  if (pre_bias) bias = const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(pre_bias));   // [B][H][n][npad], zero padded
+  if (pre_bias) p.bias = const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(pre_bias));   // [B][H][n][npad], zero padded
+  return AF2_OK;
+}
 
+// 1. LayerNorm (+ pair bias from the raw edges) and 2. the q|k|v and gate projections into the plan's workspace
+static int axial_project(const AxialPlan& p, const af2_attn_weights* w, float* x, const float* edges, const void* pre_bias,
+                         int B, int d, int heads, cudaStream_t s) {
+  const long long T = p.T, I = p.I;
+  const int n = p.n, npad = p.npad;
+  const bool has_bias = p.has_bias;
+  __nv_bfloat16 *xn = p.xn, *qkv = p.qkv, *gate = p.gate, *bias = p.bias;
   // 1. LayerNorm (+ pair bias from the RAW edges; fused when the edges are x itself)
   LnParams lp;
   memset(&lp, 0, sizeof(lp));
@@ -957,21 +973,45 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   AF2_TRY(launch_gemm(cq, s));
   GemmCall cg = linear_call(xn, d, w->w_gate, d, (int)T, (int)I, d);
   cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = I; cg.bias = w->b_gate;
-  AF2_TRY(launch_gemm(cg, s));
-  // 3. attention per batch element
+  return launch_gemm(cg, s);
+}
+
+// 3. attention per batch element (queries tied first when `tied`) and 4. to_out + bias + residual into x
+static int axial_attend(const AxialPlan& p, const af2_attn_weights* w, float* x, const unsigned char* mask, int B, int h,
+                        int wdim, int d, int heads, int dim_head, int row_attn, int tied, cudaStream_t s) {
+  const long long T = p.T, I = p.I;
+  const int n = p.n, nb = p.nb, npad = p.npad;
   const long long tok_sb = row_attn ? wdim : 1, tok_si = row_attn ? 1 : wdim;
   for (int b = 0; b < B; ++b) {
     const long long t0 = (long long)b * h * wdim;
     // MSAColumnGlobalAttention-style tied queries (alphafold2.py:142-151): q <- mean over the folded batch
-    if (tied) AF2_TRY(tie_queries<__nv_bfloat16>(qkv + t0 * 3 * I, 3 * I, (int)I, n, nb, tok_sb, tok_si, s));
-    AF2_TRY(launch_attention(qkv + t0 * 3 * I, heads, dim_head, n, nb, tok_sb, tok_si,
-                             has_bias ? bias + (long long)b * heads * n * npad : nullptr, npad,
-                             mask ? mask + t0 : nullptr, gate + t0 * I, og + t0 * I, s));
+    if (tied) AF2_TRY(tie_queries<__nv_bfloat16>(p.qkv + t0 * 3 * I, 3 * I, (int)I, n, nb, tok_sb, tok_si, s));
+    AF2_TRY(launch_attention(p.qkv + t0 * 3 * I, heads, dim_head, n, nb, tok_sb, tok_si,
+                             p.has_bias ? p.bias + (long long)b * heads * n * npad : nullptr, npad,
+                             mask ? mask + t0 : nullptr, p.gate + t0 * I, p.og + t0 * I, s));
   }
   // 4. to_out + bias + residual
-  GemmCall co = linear_call(og, I, w->w_out, I, (int)T, d, (int)I);
+  GemmCall co = linear_call(p.og, I, w->w_out, I, (int)T, d, (int)I);
   co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = w->b_out; co.resid = x; co.ld_resid = d;
   AF2_TRY(launch_gemm(co, s));
+  return AF2_OK;
+}
+
+static int axial_attention_impl(const af2_attn_weights* w, float* x, const float* edges, const void* pre_bias,
+                                const unsigned char* mask, int B, int h, int wdim, int d, int heads, int dim_head,
+                                int row_attn, void* workspace, long long workspace_bytes, af2_stream_t stream, int tied = 0) {
+  NvtxRange nvtx_(row_attn ? "af2_axial_attention(row)" : "af2_axial_attention(col)");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AxialPlan p;
+  AF2_TRY(axial_plan(p, w, x, edges, pre_bias, B, h, wdim, d, heads, dim_head, row_attn, workspace, workspace_bytes));
+  AF2_TRY(axial_project(p, w, x, edges, pre_bias, B, d, heads, s));
+  return axial_attend(p, w, x, mask, B, h, wdim, d, heads, dim_head, row_attn, tied, s);
+}
+
+// the sharded tied-query column attention: the checks shared by af2_axial_attention_tied_begin and _end
+static int tied_args_ok(const af2_attn_weights* w, const float* x, const void* sums, const void* workspace, int h, int wdim) {
+  if (!w || !x || !sums || !workspace) return fail(AF2_ERR_BAD_ARG, "axial_attention_tied: null argument");
+  if (h < 1 || wdim < 1) return fail(AF2_ERR_BAD_ARG, "axial_attention_tied: empty shard h=%d wdim=%d", h, wdim);
   return AF2_OK;
 }
 
@@ -1098,6 +1138,42 @@ int af2_axial_attention_prebias(const af2_attn_weights* w, float* x, const void*
                                 long long workspace_bytes, af2_stream_t stream) {
   return axial_attention_impl(w, x, nullptr, bias_bf16, mask, B, h, wdim, d, heads, dim_head, row_attn, workspace,
                               workspace_bytes, stream);
+}
+
+// tied-query column attention of a column shard x [h][wdim][d] (batch 1), in two calls around the caller's collective
+int af2_axial_attention_tied_begin(const af2_attn_weights* w, float* x, const void* bias_bf16, const unsigned char* mask, int h,
+                                   int wdim, int d, int heads, int dim_head, float* qsum_out, void* workspace,
+                                   long long workspace_bytes, af2_stream_t stream) {
+  NvtxRange nvtx_("af2_axial_attention_tied_begin");
+  (void)mask;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AF2_TRY(tied_args_ok(w, x, qsum_out, workspace, h, wdim));
+  AxialPlan p;
+  AF2_TRY(axial_plan(p, w, x, nullptr, bias_bf16, 1, h, wdim, d, heads, dim_head, 0, workspace, workspace_bytes));
+  AF2_TRY(axial_project(p, w, x, nullptr, bias_bf16, 1, d, heads, s));
+  ProfScope ps(s, KC_MISC, 0.0, 0.0);
+  tie_queries_sum_kernel<<<ew_grid((long long)h * p.I), 256, 0, s>>>(p.qkv, 3 * p.I, (int)p.I, h, wdim, 1, wdim, qsum_out);
+  CUDA_OK(cudaGetLastError());
+  return AF2_OK;
+}
+
+int af2_axial_attention_tied_end(const af2_attn_weights* w, float* x, const void* bias_bf16, const unsigned char* mask, int h,
+                                 int wdim, int d, int heads, int dim_head, const float* parts, int nparts, int ncols_total,
+                                 void* workspace, long long workspace_bytes, af2_stream_t stream) {
+  NvtxRange nvtx_("af2_axial_attention_tied_end");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AF2_TRY(tied_args_ok(w, x, parts, workspace, h, wdim));
+  if (nparts < 1) return fail(AF2_ERR_BAD_ARG, "axial_attention_tied_end: nparts %d < 1", nparts);
+  if (ncols_total < wdim) return fail(AF2_ERR_BAD_ARG, "axial_attention_tied_end: ncols_total %d < wdim %d", ncols_total, wdim);
+  AxialPlan p;
+  AF2_TRY(axial_plan(p, w, x, nullptr, bias_bf16, 1, h, wdim, d, heads, dim_head, 0, workspace, workspace_bytes));
+  {
+    ProfScope ps(s, KC_MISC, 0.0, 0.0);
+    tie_queries_parts_kernel<<<ew_grid((long long)h * p.I), 256, 0, s>>>(p.qkv, 3 * p.I, (int)p.I, h, wdim, 1, wdim, parts, nparts,
+                                                                          ncols_total);
+    CUDA_OK(cudaGetLastError());
+  }
+  return axial_attend(p, w, x, mask, 1, h, wdim, d, heads, dim_head, 0, 0, s);
 }
 
 // bias rows of a shard of the pair tensor: out[h][r][j] (pitch npad, caller zero-fills the pad) = <x[r, j, :], w_edge[h, :]>

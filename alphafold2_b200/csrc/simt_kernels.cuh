@@ -500,6 +500,41 @@ __global__ void __launch_bounds__(256) tie_queries_kernel(T* __restrict__ buf, l
   }
 }
 
+// Tied queries over a shard of the folded batch (the sharded schedule, whose ranks hold column shards), in two steps around a
+// collective.  sum: sum[i][c] <- fp32 sum of the bf16 queries over this shard's nbatch folded columns, from 0 in column order
+// (tie_queries_kernel's accumulation).  parts: the nparts sums of all shards [nparts][n][cols] are added from 0 in part order,
+// divided by ncols_total and stored as bf16 over every local column.  One part holding every column gives tie_queries_kernel's
+// bits.
+__global__ void __launch_bounds__(256) tie_queries_sum_kernel(const __nv_bfloat16* __restrict__ buf, long long ld, int cols, int n,
+                                                              int nbatch, long long tok_sb, long long tok_si, float* __restrict__ sum) {
+  const long long total = static_cast<long long>(n) * cols;
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(idx % cols);
+    const long long i = idx / cols;
+    const __nv_bfloat16* base = buf + i * tok_si * ld + c;
+    float acc = 0.f;
+    for (int b = 0; b < nbatch; ++b) acc += tie_ld<__nv_bfloat16>(base + b * tok_sb * ld);
+    sum[idx] = acc;
+  }
+}
+
+__global__ void __launch_bounds__(256) tie_queries_parts_kernel(__nv_bfloat16* __restrict__ buf, long long ld, int cols, int n,
+                                                                int nbatch, long long tok_sb, long long tok_si,
+                                                                const float* __restrict__ parts, int nparts, int ncols_total) {
+  const long long total = static_cast<long long>(n) * cols;
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(idx % cols);
+    const long long i = idx / cols;
+    float acc = 0.f;
+    for (int p = 0; p < nparts; ++p) acc += parts[p * total + idx];
+    const float mean = acc / static_cast<float>(ncols_total);
+    __nv_bfloat16* base = buf + i * tok_si * ld + c;
+    for (int b = 0; b < nbatch; ++b) tie_st<__nv_bfloat16>(base + b * tok_sb * ld, mean);
+  }
+}
+
 // bool mask -> float 0/1 row scale
 __global__ void mask_to_float_kernel(const uint8_t* __restrict__ mask, float* __restrict__ out, long long n) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;

@@ -490,6 +490,25 @@ class CudaStageOps:
                                                    None if m8 is None else m8.data_ptr(), 1, h, w, d, ax.attn.heads,
                                                    ax.attn.dim_head, int(row_attn), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
 
+    def tied_column_attention_(self, ax, x: torch.Tensor, bias: Optional[torch.Tensor], mask: Optional[torch.Tensor], reduce,
+                               ncols_total: int):
+        """Tied-query column attention (global_query_attn) of a column shard x [h, w, d] fp32 in place, whose queries average
+        over ncols_total columns held by several ranks.  reduce: this shard's fp32 query sums [h, I] -> every shard's, in
+        column-shard order [nparts * h, I] (the schedule: an all-gather).  bias as for axial_attention_."""
+        pk = ax.packed()
+        h, w, d = x.shape
+        H, dh = ax.attn.heads, ax.attn.dim_head
+        lib = _lib.load()
+        ws = _ops.workspace(lib.af2_axial_attention_workspace(1, h, w, d, H, dh, 0), x.device)
+        m8 = None if mask is None else mask.contiguous()
+        args = (C.byref(pk.struct), x.data_ptr(), None if bias is None else bias.data_ptr(), None if m8 is None else m8.data_ptr(),
+                h, w, d, H, dh)
+        qsum = torch.empty(h, H * dh, dtype=torch.float32, device=x.device)
+        _lib.check(lib.af2_axial_attention_tied_begin(*args, qsum.data_ptr(), ws.data_ptr(), ws.numel(), _ops._stream_ptr()))
+        parts = reduce(qsum).contiguous()              # the workspace keeps LN(x), q|k|v and the gate until the end call
+        _lib.check(lib.af2_axial_attention_tied_end(*args, parts.data_ptr(), parts.shape[0] // h, ncols_total, ws.data_ptr(),
+                                                    ws.numel(), _ops._stream_ptr()))
+
     def feed_forward_(self, ff, x: torch.Tensor):
         _ops.feed_forward_(ff.packed(), x)
 
@@ -644,6 +663,80 @@ class CudaStageOps:
 # ------------------------------------------------------------------------------------------------------------
 # the schedule
 # ------------------------------------------------------------------------------------------------------------
+class _PairShards:
+    """A pair tensor [N, N, d] sharded over the ranks of `group` for the pair track: rank r owns pair rows (and columns)
+    [n0, n1) = shard_offsets(N, P)[r:r + 2].  Holds the masks' row and column shards, the exchanges between the two layouts
+    (to_cols: [Rn, N, d] -> [N, Rn, d], to_rows: back) and the gathers of the pair track."""
+
+    def __init__(self, group, N: int, mask_full: Optional[torch.Tensor], to_cols, to_rows):
+        self.group, self.N, self.P = group, N, dist.get_world_size(group)
+        on = shard_offsets(N, self.P)
+        r = dist.get_rank(group)
+        self.n0, self.n1 = on[r], on[r + 1]
+        self.counts = shard_counts(N, self.P) if N % self.P else None     # None: equal shards, the plain collectives
+        self.Rn_max = -(-N // self.P)
+        self.mask_rows = None if mask_full is None else mask_full[self.n0:self.n1].contiguous()
+        self.mask_cols = None if mask_full is None else mask_full[:, self.n0:self.n1].contiguous()
+        self.to_cols, self.to_rows = to_cols, to_rows
+
+    def bias(self, ops, ax, x_row):
+        b = ops.pair_bias(ax, x_row)                                  # [H, Rn, npad]
+        g = all_gather_cat0(b.transpose(0, 1).contiguous(), self.group, self.counts)   # [N, H, npad] rows in global order
+        return g.transpose(0, 1).contiguous()                        # [H, N, npad]
+
+    def operand(self, t, dim):
+        """A contraction's gathered operand and its `pieces`: P equal pieces, or with uneven shards each rank's piece padded
+        along `dim` (dim 1: rows, K-major; dim 2: columns, MN-major, aligned to 8 like the kernels' pitch) and the pair shard
+        sizes, which tell the stage op what to keep of each piece."""
+        if self.counts is None:
+            return all_gather_cat0(t, self.group), self.P
+        return all_gather_cat0(_pad_dim(t, dim, self.Rn_max if dim == 1 else _align8(self.Rn_max)), self.group), tuple(self.counts)
+
+    def query_sums(self, qsum):
+        """The tied queries' partial sums [N, I] of every rank, in rank (= column-shard) order: [P * N, I].  Every rank's
+        partial has the same shape, so even uneven shards need no padding."""
+        return all_gather_cat0(qsum, self.group)
+
+
+def sharded_pair_track(ops, pair, x_row: torch.Tensor, sh: _PairShards, outer=None, ff=None) -> torch.Tensor:
+    """The pair track of one block (alphafold2.py:379-385, 444) on this rank's pair rows x_row [Rn, N, d]; returns the new row
+    shard (with the peer-memory exchange, the arena's row buffer).  pair: a PairwiseAttentionBlock.
+    outer: (L, Rg, msa_mask_full, pieces), the outer mean's operands (the trunk): contracted into x_row first.  ff: the pair
+    transition, run on the column shard before the way back (the trunk).  The template pair stack passes neither.
+    A pair block with tied-query ingoing attention (global_query_attn, the extra-MSA stack) gathers the queries' partial sums
+    over the column shards (one all-gather more)."""
+    if outer is not None:
+        L, Rg, mm_full, pieces = outer
+        ops.outer_contract_(pair.outer_mean, x_row, L, Rg, mm_full, sh.n0, pieces)
+    # --- triangle multiply outgoing on pair rows (alphafold2.py:381) ---
+    tm = pair.triangle_multiply_outgoing
+    L, R, G = ops.tri_project(tm, x_row, sh.mask_rows)
+    Rg, pieces = sh.operand(R, 1)
+    ops.tri_contract_(tm, x_row, L, Rg, G, False, pieces)
+    # --- triangle multiply ingoing on pair columns (alphafold2.py:382) ---
+    x_col = sh.to_cols(x_row)                                                    # [N, N/P, d]
+    tm = pair.triangle_multiply_ingoing
+    L, R, G = ops.tri_project(tm, x_col, sh.mask_cols)
+    Rg, pieces = sh.operand(R, 2)
+    ops.tri_contract_(tm, x_col, L, Rg, G, True, pieces)
+    # --- triangle attention outgoing = row attention on pair rows (alphafold2.py:383) ---
+    x_row = sh.to_rows(x_col)
+    ta = pair.triangle_attention_outgoing
+    ops.axial_attention_(ta, x_row, sh.bias(ops, ta, x_row), sh.mask_rows, True)
+    # --- triangle attention ingoing = column attention on pair columns (alphafold2.py:384) ---
+    ta = pair.triangle_attention_ingoing
+    bias = sh.bias(ops, ta, x_row)
+    x_col = sh.to_cols(x_row)
+    if ta.global_query_attn:
+        ops.tied_column_attention_(ta, x_col, bias, sh.mask_cols, sh.query_sums, sh.N)
+    else:
+        ops.axial_attention_(ta, x_col, bias, sh.mask_cols, False)
+    # --- pair transition (pointwise), back to rows (alphafold2.py:444) ---
+    if ff is not None:
+        ops.feed_forward_(ff, x_col)
+    return sh.to_rows(x_col)
+
+
 def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optional[torch.Tensor] = None,
                               msa_mask: Optional[torch.Tensor] = None, group=None, stage_ops=None, gather_output: bool = True):
     """Evoformer.forward (alphafold2.py:458-467) for ONE sequence sharded over the ranks of `group`.
@@ -653,7 +746,8 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
 
     Any N >= P and S >= 1: rank r owns pair rows (and columns) [on[r], on[r+1]) and MSA rows [os[r], os[r+1]) with
     on = shard_offsets(N, P), os = shard_offsets(S, P); the first N % P (S % P) ranks hold one row more, and MSA shards
-    are empty when S < P.  Shapes that P divides take the equal-shard path unchanged.
+    are empty when S < P.  Shapes that P divides take the equal-shard path unchanged.  Tied-query ingoing attention
+    (global_query_attn: the extra-MSA stack) averages its queries over all N columns through one more all-gather per block.
     """
     if stage_ops is None and _ops.precision_of(evo) == "strict":
         raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
@@ -672,7 +766,6 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
     msa_counts = shard_counts(S, P) if S % P else None
     msa_ragged = pair_counts is not None or msa_counts is not None          # the MSA columns are the pair shards
     msa_splits = (shard_counts(S, P), shard_counts(N, P)) if msa_ragged else (None, None)
-    Rn_max = -(-N // P)
     with torch.no_grad():
         ex = peer_exchange_for(group, x.device, N, S, x.shape[-1]) if stage_ops is None else None
         if ex is not None:                                            # the shards live in the peer-mapped arena
@@ -692,23 +785,9 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
             msa_to_rows = lambda t: cols_to_rows(t, group, *msa_splits)  # noqa: E731
         mask_full = None if mask is None else mask[0].bool()
         mm_full = None if msa_mask is None else msa_mask[0].bool().contiguous()
-        mask_rows = None if mask_full is None else mask_full[n0:n1].contiguous()
-        mask_cols = None if mask_full is None else mask_full[:, n0:n1].contiguous()
+        sh = _PairShards(group, N, mask_full, pair_to_cols, pair_to_rows)
         mm_rows = None if mm_full is None else mm_full[s0:s1].contiguous()
         mm_cols = None if mm_full is None else mm_full[:, n0:n1].contiguous()
-
-        def gathered_bias(ax, xr):
-            b = ops.pair_bias(ax, xr)                                 # [H, Rn, npad]
-            g = all_gather_cat0(b.transpose(0, 1).contiguous(), group, pair_counts)   # [N, H, npad] rows in global order
-            return g.transpose(0, 1).contiguous()                    # [H, N, npad]
-
-        def gathered_operand(t, dim):
-            """A contraction's gathered operand and its `pieces`: P equal pieces, or with uneven shards each rank's piece
-            padded along `dim` (dim 1: rows, K-major; dim 2: columns, MN-major, aligned to 8 like the kernels' pitch) and
-            the pair shard sizes, which tell the stage op what to keep of each piece."""
-            if pair_counts is None:
-                return all_gather_cat0(t, group), P
-            return all_gather_cat0(_pad_dim(t, dim, Rn_max if dim == 1 else _align8(Rn_max)), group), tuple(pair_counts)
 
         overlap = OVERLAP_MSA_RETURN and x_row.is_cuda and P > 1
         side = torch.cuda.Stream() if overlap else None
@@ -717,7 +796,7 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
             pair, ff, msa_attn, msa_ff = block.layer
             d = x_row.shape[-1]
             # --- MSA track (alphafold2.py:438-439) ---
-            bias_m = gathered_bias(msa_attn.row_attn, x_row)
+            bias_m = sh.bias(ops, msa_attn.row_attn, x_row)
             if pending is not None:
                 m_row, pending = pending.get(), None
             if m_row.shape[0]:                                                          # an empty MSA shard has nothing to attend
@@ -725,37 +804,15 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
             m_col = msa_to_cols(m_row)                                                  # [S, N/P, d]
             ops.axial_attention_(msa_attn.col_attn, m_col, None, mm_cols, False)
             ops.feed_forward_(msa_ff, m_col)
-            # --- outer mean into the pair rows (alphafold2.py:379) ---
+            # --- outer mean operands (alphafold2.py:379), contracted into the pair rows by the pair track ---
             LR = ops.outer_project(pair.outer_mean, m_col, mm_cols)                      # [2d, S, pitch(N/P)]
-            Rg, pieces = gathered_operand(LR[d:], 2)                                     # [P*d, S, pitch]
-            ops.outer_contract_(pair.outer_mean, x_row, LR[:d], Rg, mm_full, n0, pieces)
+            Rg, pieces = sh.operand(LR[d:], 2)                                           # [P*d, S, pitch]
+            # the MSA tensor goes back to row shards beside the pair track; nothing in it reads m
             if overlap:
                 pending = _Deferred(m_col, group, side, ex, *msa_splits)                # joins at the next block's row attention
             else:
                 m_row = msa_to_rows(m_col)
-            # --- triangle multiply outgoing on pair rows (alphafold2.py:381) ---
-            tm = pair.triangle_multiply_outgoing
-            L, R, G = ops.tri_project(tm, x_row, mask_rows)
-            Rg, pieces = gathered_operand(R, 1)
-            ops.tri_contract_(tm, x_row, L, Rg, G, False, pieces)
-            # --- triangle multiply ingoing on pair columns (alphafold2.py:382) ---
-            x_col = pair_to_cols(x_row)                                                  # [N, N/P, d]
-            tm = pair.triangle_multiply_ingoing
-            L, R, G = ops.tri_project(tm, x_col, mask_cols)
-            Rg, pieces = gathered_operand(R, 2)
-            ops.tri_contract_(tm, x_col, L, Rg, G, True, pieces)
-            # --- triangle attention outgoing = row attention on pair rows (alphafold2.py:383) ---
-            x_row = pair_to_rows(x_col)
-            ta = pair.triangle_attention_outgoing
-            ops.axial_attention_(ta, x_row, gathered_bias(ta, x_row), mask_rows, True)
-            # --- triangle attention ingoing = column attention on pair columns (alphafold2.py:384) ---
-            ta = pair.triangle_attention_ingoing
-            bias = gathered_bias(ta, x_row)
-            x_col = pair_to_cols(x_row)
-            ops.axial_attention_(ta, x_col, bias, mask_cols, False)
-            # --- pair transition (pointwise), back to rows (alphafold2.py:444) ---
-            ops.feed_forward_(ff, x_col)
-            x_row = pair_to_rows(x_col)
+            x_row = sharded_pair_track(ops, pair, x_row, sh, outer=(LR[:d], Rg, mm_full, pieces), ff=ff)
 
         if pending is not None:
             m_row, pending = pending.get(), None
@@ -937,4 +994,105 @@ def shard_evoformer(model, group=None, use_graph: Optional[bool] = None):
     evo.forward = fwd
     evo._af2_sharded = True
     evo._af2_graph = graphed
+    return model
+
+
+def _pair_arena(group, device: torch.device, N: int, d: int):
+    """A peer-memory arena this process already holds for pair tensors [N, N, d] over `group` (any MSA depth), or None."""
+    for (g, dev, n, _, dd), ex in _PEER_ARENAS.items():
+        if ex is not None and (g, dev, n, dd) == (id(group), device.index, N, d):
+            return ex
+    return None
+
+
+def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tensor], templates_feats: torch.Tensor,
+                             templates_mask: torch.Tensor, group=None) -> torch.Tensor:
+    """Alphafold2.embed_templates_ (alphafold2.py:743-785) with the pair work sharded over the ranks of `group`, in place on
+    the full fp32 x [1, n, n, d] that every rank holds.  Rank r owns pair rows [n0, n1) = shard_offsets(n, P)[r:r + 2].
+
+    The templates run one at a time, so a rank's memory does not grow with T.  For template k: to_template_embed of this
+    rank's rows of templates_feats[0, k] (GEMM rows are independent: bitwise the rows of the whole call), the crossed mask's
+    row and column shards, templates_embed_layers passes of sharded_pair_track (no outer mean, no transition), then one step
+    of the state-carrying pointwise attention over this rank's pairs (af2_template_pointwise_rows_*, q and gate from
+    x[0, n0:n1]).  After the last template to_out adds into those rows and an all-gather of the rows gives every rank the full
+    x.  The row <-> column exchanges use the peer-memory arena the sharded trunk already holds for (n, d), when there is
+    one (from the second forward on), and NCCL all-to-alls otherwise: both move the same bytes.  Runs eagerly."""
+    attn = model.template_pointwise_attn
+    if _ops.precision_of(attn) == "strict":
+        raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
+    if x.shape[0] != 1:
+        raise ValueError("the sharded template branch handles one sequence per call (batch 1)")
+    if x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError("the sharded template branch updates a contiguous fp32 x in place")
+    P = dist.get_world_size(group)
+    T, n, d = templates_feats.shape[1], x.shape[1], x.shape[3]
+    if n < P:
+        raise ValueError(f"N_res={n} is smaller than the number of ranks {P}: every rank needs at least one pair row")
+    ops = CudaStageOps()
+    lib = _lib.load()
+    pair = model.template_pairwise_embedder
+    H, dh = attn.heads, attn.dim_head
+    I = H * dh
+    with torch.no_grad():
+        on = shard_offsets(n, P)
+        r = dist.get_rank(group)
+        n0, n1 = on[r], on[r + 1]
+        counts = shard_counts(n, P) if n % P else None
+        ex = _pair_arena(group, x.device, n, d)
+        if ex is not None:
+            to_cols = lambda t: ex.rows_to_cols(t, PeerExchange.PAIR)  # noqa: E731
+            to_rows = lambda t: ex.cols_to_rows(t, PeerExchange.PAIR)  # noqa: E731
+        else:
+            to_cols = lambda t: rows_to_cols(t, group, counts, counts)  # noqa: E731
+            to_rows = lambda t: cols_to_rows(t, group, counts, counts)  # noqa: E731
+        Pn = (n1 - n0) * n                                                  # this rank's pairs
+        x_rows = x[0, n0:n1]                                                # a contiguous window of x
+        xm = None if x_mask is None else x_mask[0, n0:n1].bool().contiguous()
+        tm = templates_mask[0].bool()
+        embed = model.to_template_embed.packed()
+        w = C.byref(attn.packed().struct)
+        s = _ops._stream_ptr()
+        run_max = torch.empty(Pn, H, dtype=torch.float32, device=x.device)
+        run_sum = torch.empty_like(run_max)
+        acc = torch.empty(Pn, I, dtype=torch.float32, device=x.device)
+        pooled = torch.empty(Pn, dtype=torch.float32, device=x.device)
+        q = torch.empty(Pn, I, dtype=torch.bfloat16, device=x.device)      # the last template writes the gated output over q
+        gate = torch.empty_like(q)
+        ws = _ops.workspace(lib.af2_template_pointwise_rows_begin_workspace(Pn, d), x.device)
+        _lib.check(lib.af2_template_pointwise_rows_begin(w, x_rows.data_ptr(), Pn, d, H, dh, q.data_ptr(), gate.data_ptr(),
+                                                         ws.data_ptr(), ws.numel(), s))
+        for k in range(T):
+            t_row = _ops.template_embed(embed, templates_feats[0, k, n0:n1].detach().float().contiguous())   # [Rn, n, d]
+            sh = _PairShards(group, n, tm[k][:, None] & tm[k][None, :], to_cols, to_rows)                     # crossed mask
+            if ex is not None:
+                t_row = ex.buffer(PeerExchange.PAIR, "row").copy_(t_row)
+            for _ in range(model.templates_embed_layers):
+                t_row = sharded_pair_track(ops, pair, t_row, sh)
+            t_row = t_row.contiguous()
+            ws = _ops.workspace(lib.af2_template_pointwise_rows_group_workspace(1, Pn, d, H, dh), x.device)
+            _lib.check(lib.af2_template_pointwise_rows_group(
+                w, t_row.data_ptr(), None if xm is None else xm.data_ptr(), sh.mask_rows.data_ptr(), 1, Pn, Pn, d, H, dh,
+                q.data_ptr(), gate.data_ptr(), run_max.data_ptr(), run_sum.data_ptr(), acc.data_ptr(), pooled.data_ptr(),
+                q.data_ptr(), int(k == 0), int(k == T - 1), ws.data_ptr(), ws.numel(), s))
+            del t_row
+        ws = _ops.workspace(lib.af2_template_pointwise_rows_end_workspace(Pn, H, dh), x.device)
+        _lib.check(lib.af2_template_pointwise_rows_end(w, x_rows.data_ptr(), q.data_ptr(), pooled.data_ptr(), Pn, d, H, dh,
+                                                       ws.data_ptr(), ws.numel(), s))
+        x[0].copy_(all_gather_cat0(x_rows, group, counts))
+    return x
+
+
+def shard_alphafold2(model, group=None, use_graph: Optional[bool] = None):
+    """Shard all of an Alphafold2's pair-tensor work over the ranks of `group`: the trunk (model.net) and the extra-MSA stack
+    (model.extra_msa_evoformer, whose tied-query attention the schedule averages over all column shards) through
+    shard_evoformer, each replayed as a CUDA graph when use_graph (see shard_evoformer), and the template branch
+    (embed_templates_) through sharded_embed_templates_, eagerly.  Every rank must call forward with identical inputs (batch 1)
+    and gets the full outputs back.  Returns `model`."""
+    shard_evoformer(model.net, group, use_graph)
+    shard_evoformer(model.extra_msa_evoformer, group, use_graph)
+
+    def embed_templates_(x, x_mask, templates_feats, templates_mask):
+        return sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group)
+
+    model.embed_templates_ = embed_templates_
     return model

@@ -119,6 +119,23 @@ int af2_pair_bias(const float* x_rows, const float* w_edge, void* bias_out, int 
 int af2_axial_attention_prebias(const af2_attn_weights* w, float* x, const void* bias_bf16, const unsigned char* mask,
                                 int B, int h, int wdim, int d, int heads, int dim_head, int row_attn, void* workspace,
                                 long long workspace_bytes, af2_stream_t stream);
+/* Tied-query ("global") column attention of a column shard x [h][wdim][d] (batch 1, bf16 mode) whose tied queries average
+ * over ncols_total columns held by several ranks, in two calls on one workspace (af2_axial_attention_workspace(1, h, wdim, d,
+ * heads, dim_head, 0)) that the caller leaves untouched between them:
+ *   _begin: LayerNorm and the q|k|v and gate projections into the workspace, then qsum_out fp32 [h][heads * dim_head] = the sum
+ *     of the bf16 queries over this call's wdim columns, added from 0 in column order;
+ *   (the caller gathers every shard's qsum_out in column-shard order: parts [nparts][h][heads * dim_head])
+ *   _end: q <- bf16((sum of the parts from 0 in part order) / ncols_total) in every local column, then the attention and
+ *     to_out + residual into x.
+ * Both take the same operands (bias_bf16 [H][h][align8(h)] or NULL, mask [h][wdim] or NULL); only _end reads them.  With
+ * nparts = 1 and ncols_total = wdim the pair is bitwise af2_axial_attention_ex(flags = 1) with this bias.  AF2_ERR_BAD_ARG on
+ * a null w, x, qsum_out / parts or workspace, h or wdim < 1, nparts < 1 or ncols_total < wdim. */
+int af2_axial_attention_tied_begin(const af2_attn_weights* w, float* x, const void* bias_bf16, const unsigned char* mask, int h,
+                                   int wdim, int d, int heads, int dim_head, float* qsum_out, void* workspace,
+                                   long long workspace_bytes, af2_stream_t stream);
+int af2_axial_attention_tied_end(const af2_attn_weights* w, float* x, const void* bias_bf16, const unsigned char* mask, int h,
+                                 int wdim, int d, int heads, int dim_head, const float* parts, int nparts, int ncols_total,
+                                 void* workspace, long long workspace_bytes, af2_stream_t stream);
 /* LN + left/right (masked, gated) -> channel-major Lc, Rc [d][chan_stride]; sigmoid(out_gate) -> gate [tokens, d] */
 int af2_triangle_project(const af2_trimul_weights* w, const float* x, const unsigned char* mask, long long tokens,
                          int inner, int d, void* Lc, void* Rc, long long chan_stride, void* gate, void* workspace,

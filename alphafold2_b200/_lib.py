@@ -126,6 +126,10 @@ _SIGNATURES = {
     "af2_distogram_head": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]),
     "af2_angle_heads": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
     "af2_recycle_embed": (ci, [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, ll, ci, ci, ci, cf, vp]),
+    "af2_embed_pair_init_rows": (ci, [vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_distogram_head_rows": (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]),
+    "af2_angle_heads_rows": (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
+    "af2_recycle_embed_rows": (ci, [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, ll, ci, ci, ci, cf, ci, ci, vp]),
     "af2_split_bf16": (ci, [vp, vp, ll, ci, vp]),
     "af2_gemm_split_f32": (ci, [vp, vp, vp, ll, ci, ci, ci, ci, vp]),
     "af2_gemm_split_epilogue": (ci, [vp, ll, ll, ll, vp, ll, ll, ll, ci, ci, ci, ci, ci, C.POINTER(GemmEpilogue), vp]),

@@ -770,23 +770,27 @@ class Alphafold2(nn.Module):
                 raise ValueError(f"recyclables.{name} is on {t.device}, seq on {device}")
         return ts
 
-    def embed_recyclables_(self, x, m, recyclables):
+    def embed_recyclables_(self, x, m, recyclables, row0=None):
         """alphafold2.py:730-739 in place on the fp32 pair tensor x [b, n, n, d] and row 0 of m [b, rows, n, d], one kernel:
         x += LN(pairwise_repr), then += recycling_distance_embed[bucket(|coords_i - coords_j|)]; m[:, 0] += LN(single_msa_repr_row).
-        Masks do not gate it (as in the reference).  Under shard_evoformer every rank computes it whole (it runs before the trunk)."""
-        ts = self._check_recyclables(x.shape[0], x.shape[1], x.device, recyclables)
+        Masks do not gate it (as in the reference).  Under shard_evoformer every rank computes it whole (it runs before the trunk).
+        row0: x holds only pair rows [row0, row0 + rows) ([b, rows, n, d]; parallel.shard_alphafold2(pair_rows=True)), and only
+        those rows of pairwise_repr are read."""
+        n = x.shape[1] if row0 is None else x.shape[2]
+        ts = self._check_recyclables(x.shape[0], n, x.device, recyclables)
+        if row0 is not None:
+            ts = (ts[0], ts[1], ts[2][:, row0:row0 + x.shape[1]])
         coords, single, pair = (t.detach().to(torch.float32).contiguous() for t in ts)
-        ops.recycle_embed_(x, m, coords, single, pair, self.recycling_msa_norm.weight, self.recycling_msa_norm.bias,
-                           self.recycling_pairwise_norm.weight, self.recycling_pairwise_norm.bias,
-                           self.recycling_distance_embed.weight, eps=self.recycling_pairwise_norm.eps)
+        args = (coords, single, pair, self.recycling_msa_norm.weight, self.recycling_msa_norm.bias, self.recycling_pairwise_norm.weight,
+                self.recycling_pairwise_norm.bias, self.recycling_distance_embed.weight)
+        if row0 is None:
+            ops.recycle_embed_(x, m, *args, eps=self.recycling_pairwise_norm.eps)
+        else:
+            ops.recycle_embed_rows_(x, m, *args, row0, eps=self.recycling_pairwise_norm.eps)
         return x, m
 
-    def forward(
-        self, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None, seq_index=None,
-        seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None, templates_angles=None,
-        embedds=None, recyclables=None, return_trunk=False, return_confidence=False, return_recyclables=False,
-        return_aux_logits=False
-    ):
+    def _check_inputs(self, seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, recyclables):
+        """The checks forward makes before any device work."""
         assert not (self.disable_token_embed and not exists(seq_embed)), 'sequence embedding must be supplied if one has disabled token embedding'
         assert not (self.disable_token_embed and not exists(msa_embed)), 'msa embedding must be supplied if one has disabled token embedding'
         _forward_only(seq_embed, msa_embed, embedds, templates_feats, templates_angles)
@@ -796,6 +800,32 @@ class Alphafold2(nn.Module):
         if self.training and not self._warned_training:
             warnings.warn("alphafold2_b200 is forward-only: running inference semantics (no MLM noising, no autograd)")
             self._warned_training = True
+
+    def embed_template_angles_(self, m, msa_mask, templates_angles, templates_mask):
+        """alphafold2.py:787-792: template_angle_mlp into the T rows of m after its S MSA rows; returns msa_mask with the
+        templates' rows appended."""
+        S = m.shape[1] - templates_angles.shape[1]
+        self.template_angle_mlp.write_(templates_angles.detach().float().contiguous(), m, S)
+        return torch.cat((msa_mask.bool(), templates_mask.bool()), dim=1)
+
+    def extra_msa_inputs(self, msa, extra_msa_mask):
+        """alphafold2.py:789-798, reproduced WITH its quirks (SURVEY.md Q11, do not "fix"): the extra-MSA stack embeds `msa`, not
+        `extra_msa` (:790); only its pair output is kept; the default mask torch.ones_like(extra_m) has the embedding's rank and
+        makes the reference fail in its first mask fold -- same here (ValueError).  Returns (extra_m, extra mask)."""
+        extra_m = self.token_emb(msa).float().contiguous()
+        em = extra_msa_mask if exists(extra_msa_mask) else torch.ones_like(extra_m).bool()
+        if em.dim() != 3:
+            raise ValueError("extra_msa_mask must be given with shape [b, n_msa, n] (the reference's default, "
+                             "alphafold2.py:791, has the wrong rank and fails in einops too)")
+        return extra_m, em
+
+    def forward(
+        self, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None, seq_index=None,
+        seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None, templates_angles=None,
+        embedds=None, recyclables=None, return_trunk=False, return_confidence=False, return_recyclables=False,
+        return_aux_logits=False
+    ):
+        self._check_inputs(seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, recyclables)
 
         with torch.no_grad():
             if not exists(msa):                                        # alphafold2.py:656-658
@@ -845,19 +875,10 @@ class Alphafold2(nn.Module):
             if exists(templates_feats):                                # alphafold2.py:743-785
                 self.embed_templates_(x, x_mask, templates_feats, templates_mask)
             if exists(templates_angles):                               # alphafold2.py:787-792
-                S = m.shape[1] - templates_angles.shape[1]
-                self.template_angle_mlp.write_(templates_angles.detach().float().contiguous(), m, S)
-                msa_mask = torch.cat((msa_mask.bool(), templates_mask.bool()), dim=1)
+                msa_mask = self.embed_template_angles_(m, msa_mask, templates_angles, templates_mask)
 
-            if exists(extra_msa):
-                # alphafold2.py:789-798, reproduced WITH its quirks (SURVEY.md Q11, do not "fix"): the stack embeds `msa`, not
-                # `extra_msa` (:790); only its pair output is kept; the default mask torch.ones_like(extra_m) has the
-                # embedding's rank and makes the reference fail in its first mask fold -- same here (ValueError).
-                extra_m = self.token_emb(msa).float().contiguous()
-                em = extra_msa_mask if exists(extra_msa_mask) else torch.ones_like(extra_m).bool()
-                if em.dim() != 3:
-                    raise ValueError("extra_msa_mask must be given with shape [b, n_msa, n] (the reference's default, "
-                                     "alphafold2.py:791, has the wrong rank and fails in einops too)")
+            if exists(extra_msa):                                      # alphafold2.py:789-798
+                extra_m, em = self.extra_msa_inputs(msa, extra_msa_mask)
                 x, _ = self.extra_msa_evoformer.run_(x.contiguous(), extra_m, mask=x_mask, msa_mask=em)
 
             x, m = self.net.run_(x, m, mask=x_mask, msa_mask=msa_mask)     # alphafold2.py:802-807

@@ -62,19 +62,20 @@ __global__ void __launch_bounds__(256) glue_msa_init_kernel(const long long* __r
   }
 }
 
-// x[b][i][j][:] = (left[b][i] + right[b][j]) + pos_emb[clamp(idx[i] - idx[j], -R, R) + R]
+// x[b][i - row0][j][:] = (left[b][i] + right[b][j]) + pos_emb[clamp(idx[i] - idx[j], -R, R) + R]   for i in [row0, row0 + rows)
+// (x [B][rows][n][d]; the whole tensor is row0 = 0, rows = n)
 __global__ void __launch_bounds__(256) glue_pair_init_kernel(const float* __restrict__ lr, const float* __restrict__ pos,
                                                              const long long* __restrict__ seq_index, float* __restrict__ x,
-                                                             int B, int n, int d, int R) {
+                                                             int B, int n, int d, int R, int row0, int rows) {
   const int d4 = d >> 2;
-  const long long total = static_cast<long long>(B) * n * n * d4;
+  const long long total = static_cast<long long>(B) * rows * n * d4;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int c4 = static_cast<int>(idx % d4);
     const long long t = idx / d4;
     const int j = static_cast<int>(t % n);
-    const int i = static_cast<int>((t / n) % n);
-    const long long b = t / (static_cast<long long>(n) * n);
+    const int i = row0 + static_cast<int>((t / n) % rows);
+    const long long b = t / (static_cast<long long>(rows) * n);
     const float4 l = reinterpret_cast<const float4*>(lr + (b * n + i) * 2 * d)[c4];
     const float4 r = reinterpret_cast<const float4*>(lr + (b * n + j) * 2 * d + d)[c4];
     long long rel = seq_index ? (seq_index[i] - seq_index[j]) : static_cast<long long>(i - j);
@@ -86,14 +87,17 @@ __global__ void __launch_bounds__(256) glue_pair_init_kernel(const float* __rest
   }
 }
 
-// distogram head: out[b][i][j][0:nb] = Linear_{d -> nb}( LayerNorm( (x[b][i][j] + x[b][j][i]) * 0.5 ) )
+// distogram head: out[b][i][j][0:nb] = Linear_{d -> nb}( LayerNorm( (x[b][i][j] + xt[b][j][i]) * 0.5 ) )
+// x [B][rows][n][D], xt [B][n][ldt][D]: the whole tensor is xt = x, rows = ldt = n; a row shard i in [row0, row0 + rows) reads
+// x = its rows and xt = its column shard [n][rows][D] (xt[j][i - row0] = x_whole[j][i]), ldt = rows.
 // one warp per token, d = 32 * VPL channels; lane owns the float4 chunks lane, lane + 32, ... of the row (coalesced global
 // loads, conflict-free shared-memory reads of W); W staged in smem
 template <int VPL>
-__global__ void __launch_bounds__(256) glue_distogram_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
+__global__ void __launch_bounds__(256) glue_distogram_kernel(const float* __restrict__ x, const float* __restrict__ xt, long long ldt,
+                                                             const float* __restrict__ gamma,
                                                              const float* __restrict__ beta, const float* __restrict__ W,
                                                              const float* __restrict__ bias, float* __restrict__ out,
-                                                             int B, int n, int nb, float eps) {
+                                                             int B, int rows, int n, int nb, float eps) {
   constexpr int D = 32 * VPL;
   extern __shared__ float ws[];                 // [nb][D] + [nb] bias
   for (int i = threadIdx.x; i < nb * D; i += blockDim.x) ws[i] = W[i];
@@ -102,16 +106,16 @@ __global__ void __launch_bounds__(256) glue_distogram_kernel(const float* __rest
   const int lane = threadIdx.x & 31;
   const long long warp_global = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nwarps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
-  const long long T = static_cast<long long>(B) * n * n;
+  const long long T = static_cast<long long>(B) * rows * n;
   float g[VPL], be[VPL];
 #pragma unroll
   for (int k = 0; k < VPL; ++k) { g[k] = gamma[(lane + 32 * (k >> 2)) * 4 + (k & 3)]; be[k] = beta[(lane + 32 * (k >> 2)) * 4 + (k & 3)]; }
   for (long long t = warp_global; t < T; t += nwarps) {
     const int j = static_cast<int>(t % n);
-    const int i = static_cast<int>((t / n) % n);
-    const long long b = t / (static_cast<long long>(n) * n);
+    const int i = static_cast<int>((t / n) % rows);
+    const long long b = t / (static_cast<long long>(rows) * n);
     const float* xa = x + t * D + lane * 4;
-    const float* xb = x + ((b * n + j) * n + i) * D + lane * 4;
+    const float* xb = xt + ((b * n + j) * ldt + i) * D + lane * 4;
     float v[VPL];
     float s = 0.f;
 #pragma unroll
@@ -149,7 +153,8 @@ __global__ void __launch_bounds__(256) glue_distogram_kernel(const float* __rest
 }
 
 // recycling embedder (alphafold2.py:730-739), in place, one warp per token of one grid:
-//   pair tokens t < B n^2, t = (b, i, j):  x[t] = (x[t] + LN_pair(p[t])) + table[bucket(|coords[b][i] - coords[b][j]|)]
+//   pair tokens t < B rows n, t = (b, i - row0, j), i in [row0, row0 + rows) (x and p [B][rows][n][d]; the whole tensor is
+//   row0 = 0, rows = n):                   x[t] = (x[t] + LN_pair(p[t])) + table[bucket(|coords[b][i] - coords[b][j]|)]
 //   MSA-row tokens (b, j) after them:      m[b][0][j] = m[b][0][j] + LN_msa(s[b][j])   (m's batch stride m_bstride elements)
 // LayerNorm is fp32 and two-pass (mean, then the centred biased variance), 1 / sqrtf (IEEE).  The distance is the direct one:
 // coordinate differences in fp32, squares summed by fmaf over the c coordinates in order, IEEE sqrtf.  bucket = lower bound of
@@ -197,19 +202,20 @@ __global__ void __launch_bounds__(256) glue_recycle_kernel(const float* __restri
                                                            const float* __restrict__ msa_b, const float* __restrict__ pair_g,
                                                            const float* __restrict__ pair_b, const float* __restrict__ table,
                                                            const float* __restrict__ bnd, int nb, float* __restrict__ x,
-                                                           float* __restrict__ m, long long m_bstride, int B, int n, int d, float eps) {
+                                                           float* __restrict__ m, long long m_bstride, int B, int n, int d, float eps,
+                                                           int row0, int rows) {
   const int lane = threadIdx.x & 31;
   const int d4 = d >> 2;
   const long long warp_global = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nwarps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
-  const long long T1 = static_cast<long long>(B) * n * n;
+  const long long T1 = static_cast<long long>(B) * rows * n;
   const long long T = T1 + static_cast<long long>(B) * n;
   float y[4 * NCH];
   for (long long t = warp_global; t < T; t += nwarps) {
     if (t < T1) {
       const int j = static_cast<int>(t % n);
-      const int i = static_cast<int>((t / n) % n);
-      const long long b = t / (static_cast<long long>(n) * n);
+      const int i = row0 + static_cast<int>((t / n) % rows);
+      const long long b = t / (static_cast<long long>(rows) * n);
       float4 xv[NCH];
 #pragma unroll
       for (int k = 0; k < NCH; ++k)

@@ -14,6 +14,12 @@
 //   SYM: s of tile (I, J) is formed in fp32 from both tiles, and the 32 weight rows from omega_row0 (which hold omega's rows,
 //   inside the 64-row block) run on it (m64n32).
 //   omega is then stored at (i, j) and (j, i) from the same value, so it is bitwise symmetric.
+// Row variant (ROWS, one batch element): the output rows are a shard [row0, row0 + rows) of the pair rows.  Work item: (row
+// tile I of the shard, column tile J), every J; tile (I, J) comes from the shard's rows x_rows [rows][n][d] and, with SYM, the
+// transposed tile from the shard's columns x_cols [n][rows][d] (x_cols[j][i - row0] = x[j][i]) through the second tensor map,
+// loaded exactly like the whole kernel's tile (J, I).  Only tile (I, J) is stored (omega at (i, j) alone): every value is
+// formed from the same operands in the same order as the whole kernel's value at (row0 + i, j), so the shard is bitwise its
+// rows.  Row tiles start at the shard's first row, whatever row0 is.
 // Each chunk accumulates into a fresh fp32 register accumulator that is then added (IEEE, round to nearest) to the item's
 // running sum, so the tensor cores' accumulation only ever sums 32 channels; bias last.  The next chunk is split into the
 // second plane buffer while the tensor cores run the current one.
@@ -37,10 +43,11 @@ struct AngleHeadsParams {
   float* phi;             // [B][n][n][np]
   float* omega;           // [B][n][n][no]
   int B, n, d;
+  int rows;               // output rows per batch element: n, or the shard's rows (ROWS)
   int nt, np, no;
   int omega_row0;         // SYM: first weight row of the 32-row window that holds omega's rows (a multiple of 8, <= 32)
   int tiles;              // ceil(n / 8)
-  long long items;        // B * tiles * (tiles + 1) / 2
+  long long items;        // B * tiles * (tiles + 1) / 2;  ROWS: ceil(rows / 8) * tiles
   int stages;             // TMA ring depth
 };
 
@@ -98,9 +105,26 @@ __device__ __forceinline__ void ah_accumulate(float (&tot)[R], const float (&acc
   for (int i = 0; i < R; ++i) tot[i] += acc[i];
 }
 
-template <bool SYM>
+// item -> (b, I, J) of either variant; diag: a diagonal tile of the whole kernel (one tile, stored once)
+template <bool ROWS>
+__device__ __forceinline__ void ah_decode(long long it, int tiles, int& b, int& I, int& J, bool& diag) {
+  if constexpr (ROWS) {
+    b = 0;
+    I = static_cast<int>(it / tiles);
+    J = static_cast<int>(it - static_cast<long long>(I) * tiles);
+    diag = false;
+  } else {
+    ah_item(it, tiles, b, I, J);
+    diag = I == J;
+  }
+}
+
+// tmX: x [B][n][n][d] (ROWS: x_rows [1][rows][n][d]); tmC: the tensor the transposed tile comes from, x itself (ROWS:
+// x_cols [1][n][rows][d])
+template <bool SYM, bool ROWS>
 __global__ void __launch_bounds__(AH_THREADS, 1)
-angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ AngleHeadsParams p) {
+angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmC,
+                   const __grid_constant__ AngleHeadsParams p) {
   using L = AngleHeadsSmem<SYM>;
   constexpr int NT = L::TILES;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -116,6 +140,7 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
   const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmX);
+    prefetch_tmap(&tmC);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 1);
@@ -131,16 +156,17 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
       uint32_t phase = 0;
       for (long long it = blockIdx.x; it < p.items; it += gridDim.x) {
         int b, I, J;
-        ah_item(it, p.tiles, b, I, J);
-        const bool diag = I == J;
+        bool diag;
+        ah_decode<ROWS>(it, p.tiles, b, I, J, diag);
+        const bool two = ROWS ? SYM : !diag;                  // the transposed tile is loaded
         for (int kc = 0; kc < nk; ++kc) {
           mbar_wait(&empty_bar[slot], phase ^ 1);
           uint8_t* dst = ring + slot * 2 * AH_BOX;
-          mbar_arrive_expect_tx(&full_bar[slot], diag ? AH_BOX : 2 * AH_BOX);
+          mbar_arrive_expect_tx(&full_bar[slot], two ? 2 * AH_BOX : AH_BOX);
           // box [1][8 i][8 j][32 c] at (c, j, i, b): rows of the box are tokens t = 8 (i - i0) + (j - j0); out-of-range i / j
           // are zero-filled and never stored
           tma_load_4d(dst, &tmX, &full_bar[slot], kc * AH_KC, J * AH_TILE, I * AH_TILE, b);
-          if (!diag) tma_load_4d(dst + AH_BOX, &tmX, &full_bar[slot], kc * AH_KC, I * AH_TILE, J * AH_TILE, b);
+          if (two) tma_load_4d(dst + AH_BOX, &tmC, &full_bar[slot], kc * AH_KC, I * AH_TILE, J * AH_TILE, b);
           if (++slot == p.stages) { slot = 0; phase ^= 1; }
         }
       }
@@ -174,8 +200,9 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
 
   for (long long it = blockIdx.x; it < p.items; it += gridDim.x) {
     int b, I, J;
-    ah_item(it, p.tiles, b, I, J);
-    const bool diag = I == J;
+    bool diag;
+    ah_decode<ROWS>(it, p.tiles, b, I, J, diag);
+    const bool two = ROWS ? SYM : !diag;
 #pragma unroll
     for (int i = 0; i < 32; ++i) totA[i] = totC[i] = 0.f;
 #pragma unroll
@@ -184,14 +211,14 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
     for (int kc = 0; kc < nk; ++kc) {
       mbar_wait(&full_bar[slot], phase);
       const uint8_t* xa = ring + slot * 2 * AH_BOX;
-      const uint8_t* xc = diag ? xa : xa + AH_BOX;
+      const uint8_t* xc = two ? xa + AH_BOX : xa;
       uint8_t* pl = planes + (kc & 1) * (NT * 3 * AH_PLANE);
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const int t = t0 + 16 * u;
         const float4 a = *reinterpret_cast<const float4*>(xa + t * 128 + q * 16);
         ah_split_store(pl, t, q, a);
-        ah_split_store(pl + 3 * AH_PLANE, t, q, *reinterpret_cast<const float4*>(xc + t * 128 + q * 16));
+        if constexpr (!ROWS) ah_split_store(pl + 3 * AH_PLANE, t, q, *reinterpret_cast<const float4*>(xc + t * 128 + q * 16));
         if constexpr (SYM) {
           // s at token t = (ii, jj) of tile (I, J) pairs with token (jj, ii) of tile (J, I)
           const int tt = (t & 7) * 8 + (t >> 3);
@@ -204,10 +231,12 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
       if (kc > 0) {                     // the previous chunk's passes ran while this chunk was split
         wgmma_wait<0>();
         reg_fence(accA);
-        reg_fence(accC);
         reg_fence(accS);
         ah_accumulate(totA, accA);
-        ah_accumulate(totC, accC);
+        if constexpr (!ROWS) {
+          reg_fence(accC);
+          ah_accumulate(totC, accC);
+        }
         if constexpr (SYM) ah_accumulate(totS, accS);
       }
       // every warp has split this chunk and waited for the previous chunk's passes: the next chunk may rewrite their plane
@@ -227,7 +256,7 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
           const uint32_t scale_d = (ps | ks) != 0 ? 1u : 0u;
           const uint64_t bdesc = desc(wb + PB[ps] * AH_PLANE + ks * 32);
           wgmma_m64n64k16_ss<0, 0>(accA, desc(pa_u + PA[ps] * AH_PLANE + ks * 32), bdesc, scale_d);
-          wgmma_m64n64k16_ss<0, 0>(accC, desc(pa_u + (3 + PA[ps]) * AH_PLANE + ks * 32), bdesc, scale_d);
+          if constexpr (!ROWS) wgmma_m64n64k16_ss<0, 0>(accC, desc(pa_u + (3 + PA[ps]) * AH_PLANE + ks * 32), bdesc, scale_d);
           if constexpr (SYM)
             wgmma_m64n32k16_ss<0, 0>(accS, desc(pa_u + (6 + PA[ps]) * AH_PLANE + ks * 32),
                                      desc(wb + PB[ps] * AH_PLANE + p.omega_row0 * 64 + ks * 32), scale_d);
@@ -237,17 +266,19 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
     }
     wgmma_wait<0>();
     reg_fence(accA);
-    reg_fence(accC);
     reg_fence(accS);
     ah_accumulate(totA, accA);
-    ah_accumulate(totC, accC);
+    if constexpr (!ROWS) {
+      reg_fence(accC);
+      ah_accumulate(totC, accC);
+    }
     if constexpr (SYM) ah_accumulate(totS, accS);
     named_bar_sync(1, 128);             // every warp has seen the item's last passes retire before any splits the next item
 
     // ---- epilogue: + bias, rows r_lo and r_lo + 8 of each tile; columns 8 j + q2 + {0, 1} ----
-    const long long bn = static_cast<long long>(b) * p.n;
+    const long long bn = static_cast<long long>(b) * p.rows;
     auto store_tile = [&](const float (&tot)[32], int h, int i, int j) {
-      if (i >= p.n || j >= p.n) return;
+      if (i >= p.rows || j >= p.n) return;
       const long long tok = (bn + i) * p.n + j;
 #pragma unroll
       for (int jx = 0; jx < 8; ++jx) {
@@ -266,11 +297,11 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
       const int m = r_lo + 8 * h;
       const int ii = m >> 3, jj = m & 7;
       store_tile(totA, h, I * AH_TILE + ii, J * AH_TILE + jj);
-      if (!diag) store_tile(totC, h, J * AH_TILE + ii, I * AH_TILE + jj);
+      if (!ROWS && !diag) store_tile(totC, h, J * AH_TILE + ii, I * AH_TILE + jj);
       if constexpr (SYM) {
         // omega of s at (i, j) and (j, i); within a diagonal tile each unordered pair once
         const int i = I * AH_TILE + ii, j = J * AH_TILE + jj;
-        if (i < p.n && j < p.n && (!diag || ii <= jj)) {
+        if (i < p.rows && j < p.n && (!diag || ii <= jj)) {
           const long long t1 = (bn + i) * p.n + j, t2 = (bn + j) * p.n + i;
 #pragma unroll
           for (int jx = 0; jx < 4; ++jx) {
@@ -280,7 +311,7 @@ angle_heads_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
               if (col >= o0 && col < o0 + p.no) {
                 const float v = totS[4 * jx + 2 * h + e] + __ldg(p.bias + col);
                 p.omega[t1 * p.no + (col - o0)] = v;
-                p.omega[t2 * p.no + (col - o0)] = v;
+                if constexpr (!ROWS) p.omega[t2 * p.no + (col - o0)] = v;
               }
             }
           }

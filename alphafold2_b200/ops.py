@@ -398,6 +398,18 @@ def embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: 
                     m_rows: Optional[int] = None):
     """alphafold2.py:676-726 in three fused kernels: returns (x [b,n,n,d], m [b,m_rows,n,d]) fp32.  m_rows > s leaves rows s..
     m_rows - 1 of m unwritten (the template angle features go there)."""
+    return _embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist, seq_embed, msa_embed, seq_index, m_rows, None)
+
+
+def embed_pair_init_rows(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: int, row0: int, rows: int, seq_embed=None,
+                         msa_embed=None, seq_index=None, m_rows: Optional[int] = None):
+    """embed_pair_init writing only pair rows [row0, row0 + rows): returns (x_rows [b,rows,n,d], m [b,m_rows,n,d] whole), bitwise
+    those rows of embed_pair_init's x and its m (af2_embed_pair_init_rows)."""
+    return _embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist, seq_embed, msa_embed, seq_index, m_rows,
+                            (int(row0), int(rows)))
+
+
+def _embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist, seq_embed, msa_embed, seq_index, m_rows, window):
     if not seq.is_cuda:
         raise RuntimeError("seq must be a CUDA tensor (alphafold2_b200 has no CPU fallback)")
     emb = _w32(token_emb)
@@ -407,7 +419,7 @@ def embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: 
     d = emb.shape[1]
     seq = seq.to(torch.int64).contiguous()
     msa = msa.to(torch.int64).contiguous()
-    x = torch.empty(B, n, n, d, dtype=torch.float32, device=seq.device)
+    x = torch.empty(B, n if window is None else max(window[1], 0), n, d, dtype=torch.float32, device=seq.device)
     R = S if m_rows is None else int(m_rows)
     if R < S:
         raise ValueError(f"m_rows {R} < {S} MSA rows")
@@ -418,17 +430,23 @@ def embed_pair_init(seq, msa, token_emb, w_pair, b_pair, pos_emb, max_rel_dist: 
     lib = _lib.load()
     ws = workspace(lib.af2_embed_pair_init_workspace(B, n, d), seq.device)
     wp, bp, pe = _w32(w_pair), _w32(b_pair), _w32(pos_emb)
+
+    def call(sq, ms, s_e, m_e, xo, mo, nb):
+        head = (sq.data_ptr(), ms.data_ptr(), emb.data_ptr(), emb.shape[0], _ptr(s_e), _ptr(m_e), wp.data_ptr(), bp.data_ptr(),
+                pe.data_ptr(), int(max_rel_dist), _ptr(si), xo.data_ptr(), mo.data_ptr(), nb, S, n, d)
+        tail = (ws.data_ptr(), ws.numel(), _stream_ptr())
+        if window is None:
+            _lib.check(lib.af2_embed_pair_init(*head, *tail))
+        else:
+            _lib.check(lib.af2_embed_pair_init_rows(*head, *window, *tail))
+
     if R != S and B > 1:
         # the kernels write S contiguous rows per batch element: one call per element into its slice of m
         for b in range(B):
             pick = lambda t: None if t is None else t[b]  # noqa: E731
-            _lib.check(lib.af2_embed_pair_init(seq[b].data_ptr(), msa[b].data_ptr(), emb.data_ptr(), emb.shape[0], _ptr(pick(se)),
-                                               _ptr(pick(me)), wp.data_ptr(), bp.data_ptr(), pe.data_ptr(), int(max_rel_dist), _ptr(si),
-                                               x[b].data_ptr(), m[b].data_ptr(), 1, S, n, d, ws.data_ptr(), ws.numel(), _stream_ptr()))
+            call(seq[b], msa[b], pick(se), pick(me), x[b], m[b], 1)
         return x, m
-    _lib.check(lib.af2_embed_pair_init(seq.data_ptr(), msa.data_ptr(), emb.data_ptr(), emb.shape[0], _ptr(se), _ptr(me), wp.data_ptr(),
-                                       bp.data_ptr(), pe.data_ptr(), int(max_rel_dist), _ptr(si), x.data_ptr(), m.data_ptr(), B, S, n, d,
-                                       ws.data_ptr(), ws.numel(), _stream_ptr()))
+    call(seq, msa, se, me, x, m, B)
     return x, m
 
 
@@ -445,6 +463,31 @@ def distogram_head(x, ln_w, ln_b, w, b) -> torch.Tensor:
     g, be, ww, bb = _w32(ln_w), _w32(ln_b), _w32(w), _w32(b)
     _lib.check(_lib.load().af2_distogram_head(x.data_ptr(), g.data_ptr(), be.data_ptr(), ww.data_ptr(), bb.data_ptr(), out.data_ptr(),
                                               B, n, d, buckets, _stream_ptr()))
+    return out
+
+
+def _rows_cols(x_rows: torch.Tensor, x_cols: Optional[torch.Tensor]):
+    """(rows, n, d) of a row shard x_rows [rows, n, d] and its column shard x_cols [n, rows, d] (None: not needed)."""
+    _require(x_rows, torch.float32, "x_rows")
+    if x_rows.dim() != 3:
+        raise ValueError(f"x_rows must be [rows, n, d], got {tuple(x_rows.shape)}")
+    rows, n, d = x_rows.shape
+    if x_cols is not None:
+        _require(x_cols, torch.float32, "x_cols")
+        if tuple(x_cols.shape) != (n, rows, d):
+            raise ValueError(f"x_cols must be [{n}, {rows}, {d}], got {tuple(x_cols.shape)}")
+    return rows, n, d
+
+
+def distogram_head_rows(x_rows, x_cols, ln_w, ln_b, w, b) -> torch.Tensor:
+    """distogram_head on pair rows [row0, row0 + rows): x_rows [rows, n, d] and the same rows as columns, x_cols [n, rows, d]
+    (x_cols[j][i - row0] = x[j][i]) -> [1, rows, n, buckets] fp32, bitwise those rows of distogram_head(x)."""
+    rows, n, d = _rows_cols(x_rows, x_cols)
+    buckets = w.shape[0]
+    out = torch.empty(1, rows, n, buckets, dtype=torch.float32, device=x_rows.device)
+    g, be, ww, bb = _w32(ln_w), _w32(ln_b), _w32(w), _w32(b)
+    _lib.check(_lib.load().af2_distogram_head_rows(x_rows.data_ptr(), x_cols.data_ptr(), g.data_ptr(), be.data_ptr(), ww.data_ptr(),
+                                                   bb.data_ptr(), out.data_ptr(), rows, n, d, buckets, _stream_ptr()))
     return out
 
 
@@ -491,6 +534,22 @@ def angle_heads(pk: Packed, x: torch.Tensor, symmetrize_omega: bool):
     return theta, phi, omega
 
 
+def angle_heads_rows(pk: Packed, x_rows: torch.Tensor, x_cols: Optional[torch.Tensor], symmetrize_omega: bool):
+    """angle_heads on pair rows [row0, row0 + rows): (theta, phi, omega) [1, rows, n, buckets] fp32 from x_rows [rows, n, d], and
+    with symmetrize_omega from the same rows as columns x_cols [n, rows, d] (x_cols[j][i - row0] = x[j][i]; unused otherwise).
+    Bitwise those rows of angle_heads(x)."""
+    rows, n, d = _rows_cols(x_rows, x_cols if symmetrize_omega else None)
+    nt, np_, no = pk.buckets
+    theta = torch.empty(1, rows, n, nt, dtype=torch.float32, device=x_rows.device)
+    phi = torch.empty(1, rows, n, np_, dtype=torch.float32, device=x_rows.device)
+    omega = torch.empty(1, rows, n, no, dtype=torch.float32, device=x_rows.device)
+    _lib.check(_lib.load().af2_angle_heads_rows(x_rows.data_ptr(), _ptr(x_cols) if symmetrize_omega else None,
+                                                pk.tensors["planes"].data_ptr(), pk.tensors["bias"].data_ptr(), theta.data_ptr(),
+                                                phi.data_ptr(), omega.data_ptr(), rows, n, d, nt, np_, no,
+                                                int(bool(symmetrize_omega)), _stream_ptr()))
+    return theta, phi, omega
+
+
 _RECYCLE_BOUNDARIES: Dict[tuple, torch.Tensor] = {}
 
 
@@ -511,9 +570,24 @@ def recycle_embed_(x, m, coords, single_row, prev_pair, msa_gamma, msa_beta, pai
     """alphafold2.py:730-739 in one kernel, in place: x [b,n,n,d] += LN_pair(prev_pair), then += table[bucket(dist)]; row 0 of
     m [b,rows,n,d] += LN_msa(single_row).  coords [b,n,c], single_row [b,n,d], prev_pair [b,n,n,d]; every tensor fp32 on x's
     device.  `boundaries` defaults to recycling_boundaries(table rows)."""
+    return _recycle_embed(x, m, coords, single_row, prev_pair, msa_gamma, msa_beta, pair_gamma, pair_beta, table, eps, boundaries,
+                          None)
+
+
+def recycle_embed_rows_(x_rows, m, coords, single_row, prev_pair_rows, msa_gamma, msa_beta, pair_gamma, pair_beta, table, row0: int,
+                        eps: float = 1e-5, boundaries: Optional[torch.Tensor] = None):
+    """recycle_embed_ on pair rows [row0, row0 + rows): x_rows and prev_pair_rows [b,rows,n,d] (those rows of x and of the previous
+    pair tensor), coords whole; row 0 of m is updated whole.  Bitwise those rows of recycle_embed_ and the same m."""
+    return _recycle_embed(x_rows, m, coords, single_row, prev_pair_rows, msa_gamma, msa_beta, pair_gamma, pair_beta, table, eps,
+                          boundaries, int(row0))
+
+
+def _recycle_embed(x, m, coords, single_row, prev_pair, msa_gamma, msa_beta, pair_gamma, pair_beta, table, eps, boundaries, row0):
     _require(x, torch.float32, "x")
     _require(m, torch.float32, "m")
-    B, n, _, d = x.shape
+    B, rows, n, d = x.shape
+    if row0 is None and rows != n:
+        raise ValueError(f"x must be [b, n, n, d], got {tuple(x.shape)}")
     if m.dim() != 4 or m.shape[0] != B or m.shape[2] != n or m.shape[3] != d or m.shape[1] < 1:
         raise ValueError(f"m must be [{B}, rows, {n}, {d}], got {tuple(m.shape)}")
     nb = table.shape[0]
@@ -528,15 +602,18 @@ def recycle_embed_(x, m, coords, single_row, prev_pair, msa_gamma, msa_beta, pai
     if ts["boundaries"].numel() < nb:
         raise ValueError(f"boundaries must hold {nb} values, got {ts['boundaries'].numel()}")
     c = ts["coords"].shape[-1]
-    want = {"coords": (B, n, c), "single_row": (B, n, d), "prev_pair": (B, n, n, d), "msa_gamma": (d,), "msa_beta": (d,),
+    want = {"coords": (B, n, c), "single_row": (B, n, d), "prev_pair": (B, rows, n, d), "msa_gamma": (d,), "msa_beta": (d,),
             "pair_gamma": (d,), "pair_beta": (d,), "table": (nb, d)}
     for k, shape in want.items():
         if tuple(ts[k].shape) != shape:
             raise ValueError(f"{k} must be {shape}, got {tuple(ts[k].shape)}")
-    _lib.check(_lib.load().af2_recycle_embed(
-        ts["coords"].data_ptr(), c, ts["single_row"].data_ptr(), ts["prev_pair"].data_ptr(), ts["msa_gamma"].data_ptr(),
-        ts["msa_beta"].data_ptr(), ts["pair_gamma"].data_ptr(), ts["pair_beta"].data_ptr(), ts["table"].data_ptr(),
-        ts["boundaries"].data_ptr(), nb, x.data_ptr(), m.data_ptr(), m.stride(0), B, n, d, float(eps), _stream_ptr()))
+    args = (ts["coords"].data_ptr(), c, ts["single_row"].data_ptr(), ts["prev_pair"].data_ptr(), ts["msa_gamma"].data_ptr(),
+            ts["msa_beta"].data_ptr(), ts["pair_gamma"].data_ptr(), ts["pair_beta"].data_ptr(), ts["table"].data_ptr(),
+            ts["boundaries"].data_ptr(), nb, x.data_ptr(), m.data_ptr(), m.stride(0), B, n, d, float(eps))
+    if row0 is None:
+        _lib.check(_lib.load().af2_recycle_embed(*args, _stream_ptr()))
+    else:
+        _lib.check(_lib.load().af2_recycle_embed_rows(*args, row0, rows, _stream_ptr()))
     return x, m
 
 

@@ -738,11 +738,14 @@ def sharded_pair_track(ops, pair, x_row: torch.Tensor, sh: _PairShards, outer=No
 
 
 def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optional[torch.Tensor] = None,
-                              msa_mask: Optional[torch.Tensor] = None, group=None, stage_ops=None, gather_output: bool = True):
+                              msa_mask: Optional[torch.Tensor] = None, group=None, stage_ops=None, gather_output: bool = True,
+                              rows_in: bool = False):
     """Evoformer.forward (alphafold2.py:458-467) for ONE sequence sharded over the ranks of `group`.
 
     x [1, N, N, d], m [1, S, N, d], mask [1, N, N] bool, msa_mask [1, S, N] bool are the full (replicated) inputs;
     returns the full (x, m) on every rank when gather_output, else this rank's row shards.
+    rows_in: x is this rank's pair rows [1, n1 - n0, N, d] instead (no rank holds the whole pair tensor), and the outputs are
+    the row shards whatever gather_output says.
 
     Any N >= P and S >= 1: rank r owns pair rows (and columns) [on[r], on[r+1]) and MSA rows [os[r], os[r+1]) with
     on = shard_offsets(N, P), os = shard_offsets(S, P); the first N % P (S % P) ranks hold one row more, and MSA shards
@@ -756,11 +759,14 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
     r = dist.get_rank(group)
     if x.shape[0] != 1:
         raise ValueError("the sharded trunk handles one sequence per call (batch 1)")
-    N, S = x.shape[1], m.shape[1]
+    N, S = x.shape[2 if rows_in else 1], m.shape[1]
     if N < P:
         raise ValueError(f"N_res={N} is smaller than the number of ranks {P}: every rank needs at least one pair row")
     on, os_ = shard_offsets(N, P), shard_offsets(S, P)
     n0, n1, s0, s1 = on[r], on[r + 1], os_[r], os_[r + 1]
+    if rows_in and x.shape[1] != n1 - n0:
+        raise ValueError(f"rank {r} owns pair rows [{n0}, {n1}) of {N}; x holds {x.shape[1]} rows")
+    x_src = x[0] if rows_in else x[0, n0:n1]
     # shard sizes of every rank for the collectives, None where P divides the axis (equal shards: the plain collectives)
     pair_counts = shard_counts(N, P) if N % P else None
     msa_counts = shard_counts(S, P) if S % P else None
@@ -770,14 +776,14 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
         ex = peer_exchange_for(group, x.device, N, S, x.shape[-1]) if stage_ops is None else None
         if ex is not None:                                            # the shards live in the peer-mapped arena
             x_row, m_row = ex.buffer(PeerExchange.PAIR, "row"), ex.buffer(PeerExchange.MSA, "row")
-            x_row.copy_(x[0, n0:n1])
+            x_row.copy_(x_src)
             m_row.copy_(m[0, s0:s1])
             pair_to_cols = lambda t: ex.rows_to_cols(t, PeerExchange.PAIR)  # noqa: E731
             pair_to_rows = lambda t: ex.cols_to_rows(t, PeerExchange.PAIR)  # noqa: E731
             msa_to_cols = lambda t: ex.rows_to_cols(t, PeerExchange.MSA)  # noqa: E731
             msa_to_rows = lambda t: ex.cols_to_rows(t, PeerExchange.MSA)  # noqa: E731
         else:
-            x_row = x[0, n0:n1].detach().to(torch.float32).contiguous().clone()      # [N/P, N, d]
+            x_row = x_src.detach().to(torch.float32).contiguous().clone()            # [N/P, N, d]
             m_row = m[0, s0:s1].detach().to(torch.float32).contiguous().clone()      # [S/P, N, d]
             pair_to_cols = lambda t: rows_to_cols(t, group, pair_counts, pair_counts)  # noqa: E731
             pair_to_rows = lambda t: cols_to_rows(t, group, pair_counts, pair_counts)  # noqa: E731
@@ -816,7 +822,7 @@ def sharded_evoformer_forward(evo, x: torch.Tensor, m: torch.Tensor, mask: Optio
 
         if pending is not None:
             m_row, pending = pending.get(), None
-        if not gather_output:
+        if rows_in or not gather_output:
             return (x_row.clone(), m_row.clone()) if ex is not None else (x_row, m_row)   # arena buffers are reused by the next call
         xo = all_gather_cat0(x_row, group, pair_counts)[None]
         mo = all_gather_cat0(m_row, group, msa_counts)[None]
@@ -922,8 +928,8 @@ class _GraphedTrunk:
         import gc
         gc.collect()
 
-    def _eager(self, x, m, mask, msa_mask):
-        return sharded_evoformer_forward(self.evo, x, m, mask, msa_mask, self.group)
+    def _eager(self, x, m, mask, msa_mask, rows_in=False):
+        return sharded_evoformer_forward(self.evo, x, m, mask, msa_mask, self.group, rows_in=rows_in)
 
     def _weights_key(self):
         if self._params is None:
@@ -931,29 +937,29 @@ class _GraphedTrunk:
         return (sum(p._version for p in self._params), sum(p.data_ptr() for p in self._params) & 0xffffffffffff,
                 _ops.pack_epoch(), _ops.precision_of(self.evo))
 
-    def __call__(self, x, m, mask=None, msa_mask=None):
+    def __call__(self, x, m, mask=None, msa_mask=None, rows_in=False):
         if not GRAPH_ENABLED or self.failed is not None or not x.is_cuda:
-            return self._eager(x, m, mask, msa_mask)
+            return self._eager(x, m, mask, msa_mask, rows_in)
         key = (tuple(x.shape), tuple(m.shape), x.dtype, m.dtype, None if mask is None else tuple(mask.shape),
-               None if msa_mask is None else tuple(msa_mask.shape), x.device, self._weights_key())
+               None if msa_mask is None else tuple(msa_mask.shape), x.device, self._weights_key(), rows_in)
         if key != self.key:
             try:
                 self.release()
-                self._capture(key, x, m, mask, msa_mask)
+                self._capture(key, x, m, mask, msa_mask, rows_in)
             except Exception as e:  # noqa: BLE001 - any capture failure falls back to the eager schedule
                 self.failed = repr(e)
                 self.release()
                 import sys
                 print(f"[alphafold2_b200.parallel] CUDA-graph capture failed, running eagerly: {self.failed}", file=sys.stderr)
                 torch.cuda.synchronize()
-                return self._eager(x, m, mask, msa_mask)
+                return self._eager(x, m, mask, msa_mask, rows_in)
         for held, new in zip(self.inputs, (x, m, mask, msa_mask)):
             if held is not None and held.data_ptr() != new.data_ptr():
                 held.copy_(new)
         self.graph.replay()
         return self.outputs[0].clone(), self.outputs[1].clone()
 
-    def _capture(self, key, x, m, mask, msa_mask):
+    def _capture(self, key, x, m, mask, msa_mask, rows_in=False):
         from .alphafold2 import _Packable
         cur = torch.cuda.current_stream()
         side = torch.cuda.Stream()
@@ -961,14 +967,14 @@ class _GraphedTrunk:
         self.ws = {}
         with torch.cuda.stream(side), _ops.private_workspace(self.ws, False):
             for _ in range(2):                      # packs weights, sizes the private workspace, initialises NCCL
-                self._eager(x, m, mask, msa_mask)
+                self._eager(x, m, mask, msa_mask, rows_in)
         cur.wait_stream(side)
         torch.cuda.synchronize()
         self.packed = [mod.packed() for mod in self.evo.modules() if isinstance(mod, _Packable)]
         n0 = _lib.load().af2_launch_count()
         g = torch.cuda.CUDAGraph()
         with _ops.private_workspace(self.ws, True), torch.cuda.graph(g):
-            out = self._eager(x, m, mask, msa_mask)
+            out = self._eager(x, m, mask, msa_mask, rows_in)
         self.launches_per_replay = int(_lib.load().af2_launch_count() - n0)   # kernels of this library inside one replay
         self.graph, self.inputs, self.outputs, self.key = g, (x, m, mask, msa_mask), out, key
 
@@ -986,10 +992,10 @@ def shard_evoformer(model, group=None, use_graph: Optional[bool] = None):
     if graphed is not None:
         _hook_teardown()
 
-    def fwd(x, m, mask=None, msa_mask=None, _evo=evo):
+    def fwd(x, m, mask=None, msa_mask=None, _evo=evo, rows_in=False):
         if graphed is not None:
-            return graphed(x, m, mask, msa_mask)
-        return sharded_evoformer_forward(_evo, x, m, mask, msa_mask, group)
+            return graphed(x, m, mask, msa_mask, rows_in)
+        return sharded_evoformer_forward(_evo, x, m, mask, msa_mask, group, rows_in=rows_in)
 
     evo.forward = fwd
     evo._af2_sharded = True
@@ -1006,7 +1012,7 @@ def _pair_arena(group, device: torch.device, N: int, d: int):
 
 
 def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tensor], templates_feats: torch.Tensor,
-                             templates_mask: torch.Tensor, group=None) -> torch.Tensor:
+                             templates_mask: torch.Tensor, group=None, rows_in: bool = False) -> torch.Tensor:
     """Alphafold2.embed_templates_ (alphafold2.py:743-785) with the pair work sharded over the ranks of `group`, in place on
     the full fp32 x [1, n, n, d] that every rank holds.  Rank r owns pair rows [n0, n1) = shard_offsets(n, P)[r:r + 2].
 
@@ -1016,7 +1022,9 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
     of the state-carrying pointwise attention over this rank's pairs (af2_template_pointwise_rows_*, q and gate from
     x[0, n0:n1]).  After the last template to_out adds into those rows and an all-gather of the rows gives every rank the full
     x.  The row <-> column exchanges use the peer-memory arena the sharded trunk already holds for (n, d), when there is
-    one (from the second forward on), and NCCL all-to-alls otherwise: both move the same bytes.  Runs eagerly."""
+    one (from the second forward on), and NCCL all-to-alls otherwise: both move the same bytes.  Runs eagerly.
+    rows_in: x is this rank's pair rows [1, n1 - n0, n, d] (shard_alphafold2(pair_rows=True)); they are updated in place and
+    nothing is gathered."""
     attn = model.template_pointwise_attn
     if _ops.precision_of(attn) == "strict":
         raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
@@ -1025,7 +1033,7 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
     if x.dtype != torch.float32 or not x.is_contiguous():
         raise ValueError("the sharded template branch updates a contiguous fp32 x in place")
     P = dist.get_world_size(group)
-    T, n, d = templates_feats.shape[1], x.shape[1], x.shape[3]
+    T, n, d = templates_feats.shape[1], x.shape[2 if rows_in else 1], x.shape[3]
     if n < P:
         raise ValueError(f"N_res={n} is smaller than the number of ranks {P}: every rank needs at least one pair row")
     ops = CudaStageOps()
@@ -1046,7 +1054,7 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
             to_cols = lambda t: rows_to_cols(t, group, counts, counts)  # noqa: E731
             to_rows = lambda t: cols_to_rows(t, group, counts, counts)  # noqa: E731
         Pn = (n1 - n0) * n                                                  # this rank's pairs
-        x_rows = x[0, n0:n1]                                                # a contiguous window of x
+        x_rows = x[0] if rows_in else x[0, n0:n1]                           # a contiguous window of x
         xm = None if x_mask is None else x_mask[0, n0:n1].bool().contiguous()
         tm = templates_mask[0].bool()
         embed = model.to_template_embed.packed()
@@ -1078,16 +1086,20 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
         ws = _ops.workspace(lib.af2_template_pointwise_rows_end_workspace(Pn, H, dh), x.device)
         _lib.check(lib.af2_template_pointwise_rows_end(w, x_rows.data_ptr(), q.data_ptr(), pooled.data_ptr(), Pn, d, H, dh,
                                                        ws.data_ptr(), ws.numel(), s))
-        x[0].copy_(all_gather_cat0(x_rows, group, counts))
+        if not rows_in:
+            x[0].copy_(all_gather_cat0(x_rows, group, counts))
     return x
 
 
-def shard_alphafold2(model, group=None, use_graph: Optional[bool] = None):
+def shard_alphafold2(model, group=None, use_graph: Optional[bool] = None, pair_rows: bool = False):
     """Shard all of an Alphafold2's pair-tensor work over the ranks of `group`: the trunk (model.net) and the extra-MSA stack
     (model.extra_msa_evoformer, whose tied-query attention the schedule averages over all column shards) through
     shard_evoformer, each replayed as a CUDA graph when use_graph (see shard_evoformer), and the template branch
     (embed_templates_) through sharded_embed_templates_, eagerly.  Every rank must call forward with identical inputs (batch 1)
-    and gets the full outputs back.  Returns `model`."""
+    and gets the full outputs back.  Returns `model`.
+
+    pair_rows: model(...) runs sharded_alphafold2_rows instead, which keeps the pair tensor in row shards from the embedding
+    to the heads and returns this rank's rows of the outputs (ret.pair_rows = (n0, n1); gather_pair_rows joins them)."""
     shard_evoformer(model.net, group, use_graph)
     shard_evoformer(model.extra_msa_evoformer, group, use_graph)
 
@@ -1095,4 +1107,129 @@ def shard_alphafold2(model, group=None, use_graph: Optional[bool] = None):
         return sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group)
 
     model.embed_templates_ = embed_templates_
+    if pair_rows:
+        def forward(*args, **kwargs):
+            return sharded_alphafold2_rows(model, group, *args, **kwargs)
+
+        model.forward = forward
+    else:
+        model.__dict__.pop("forward", None)              # back to Alphafold2.forward, whatever an earlier call installed
     return model
+
+
+def gather_pair_rows(t: torch.Tensor, group=None) -> torch.Tensor:
+    """Every rank's pair rows t [1, n1 - n0, N, ...] (an output of shard_alphafold2(pair_rows=True): ret.distance,
+    theta_logits, phi_logits, omega_logits) joined into the whole [1, N, N, ...] on every rank (one all-gather)."""
+    N, P = t.shape[2], dist.get_world_size(group)
+    return all_gather_cat0(t[0].contiguous(), group, shard_counts(N, P) if N % P else None)[None]
+
+
+def _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclables, return_trunk):
+    """What sharded_alphafold2_rows cannot run, raised before any device work or collective."""
+    from .alphafold2 import DISTOGRAM_BUCKETS
+    if any(_ops.precision_of(mod) == "strict" for mod in (model.net, model.extra_msa_evoformer, model.template_pointwise_attn)):
+        raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
+    if model.predict_coords and not return_trunk:
+        raise NotImplementedError("predict_coords=True needs the third-party structure module (see Alphafold2.forward)")
+    if seq.dim() != 2 or seq.shape[0] != 1:
+        raise ValueError(f"pair_rows mode handles one sequence per call (batch 1), got seq {tuple(seq.shape)}")
+    P, N = dist.get_world_size(group), seq.shape[1]
+    if N < P:
+        raise ValueError(f"N_res={N} is smaller than the number of ranks {P}: every rank needs at least one pair row")
+    if model.disable_token_embed:
+        raise ValueError("pair_rows mode embeds tokens with the fused pair-init kernel: disable_token_embed is not supported")
+    d = model.dim
+    if not _ops.distogram_head_ok(d, DISTOGRAM_BUCKETS):
+        raise ValueError(f"pair_rows mode: dim {d} is not taken by the distogram head kernel (a multiple of 128, <= 512)")
+    if model.predict_angles and not _ops.angle_heads_ok(d, model.angle_heads().buckets()):
+        raise ValueError(f"pair_rows mode: dim {d} and buckets {model.angle_heads().buckets()} are not taken by the angle heads kernel")
+    if extra_msa is not None and (extra_msa_mask is None or extra_msa_mask.dim() != 3):
+        raise ValueError("extra_msa_mask must be given with shape [b, n_msa, n] (the reference's default, alphafold2.py:791, has "
+                         "the wrong rank and fails in einops too)")
+    pair = getattr(recyclables, "pairwise_repr", None)
+    if not seq.is_cuda or (msa is not None and not msa.is_cuda) or (torch.is_tensor(pair) and not pair.is_cuda):
+        raise ValueError("pair_rows mode runs on CUDA tensors (seq, msa and recyclables on the GPU)")
+
+
+def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None,
+                            seq_index=None, seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None,
+                            templates_angles=None, embedds=None, recyclables=None, return_trunk=False, return_confidence=False,
+                            return_recyclables=False, return_aux_logits=False):
+    """Alphafold2.forward of a model under shard_alphafold2(pair_rows=True): every pair-tensor stage runs on this rank's pair rows
+    [n0, n1) = shard_offsets(N, P)[r:r + 2] and no rank holds the whole pair tensor.  Pair init rows -> recycling rows ->
+    template branch on the rows -> template angles into m -> extra-MSA stack rows -> trunk rows -> one rows -> columns exchange
+    of x -> distogram and angle heads on the rows.  Returns this rank's rows: ret.distance [1, n1 - n0, N, 37], theta / phi /
+    omega_logits the same rows, ret.pair_rows = (n0, n1).  Each is bitwise those rows of the default shard_alphafold2 forward.
+    The inputs stay replicated (every rank passes the same tensors and reads its rows of them); so does the MSA tensor m."""
+    from .alphafold2 import ReturnValues
+    _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclables, return_trunk)
+    model._check_inputs(seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, recyclables)
+    P, r, N = dist.get_world_size(group), dist.get_rank(group), seq.shape[1]
+    on = shard_offsets(N, P)
+    n0, n1 = on[r], on[r + 1]
+    with torch.no_grad():
+        if msa is None:                                                # alphafold2.py:656-658
+            msa = seq[:, None, :]
+            msa_mask = mask[:, None, :] if mask is not None else None
+        if msa_mask is None:
+            msa_mask = torch.ones_like(msa).bool()
+        m_rows = msa.shape[1] + (templates_angles.shape[1] if templates_angles is not None else 0)
+        x, m = _ops.embed_pair_init_rows(seq, msa, model.token_emb.weight, model.to_pairwise_repr.weight, model.to_pairwise_repr.bias,
+                                         model.pos_emb.weight, model.max_rel_dist, n0, n1 - n0, seq_embed, msa_embed, seq_index,
+                                         m_rows=m_rows)
+        x_mask = (mask[:, :, None] & mask[:, None, :]) if mask is not None else None
+        if recyclables is not None:
+            model.embed_recyclables_(x, m, recyclables, row0=n0)
+        if templates_feats is not None:
+            sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group, rows_in=True)
+        if templates_angles is not None:
+            msa_mask = model.embed_template_angles_(m, msa_mask, templates_angles, templates_mask)
+        if extra_msa is not None:
+            extra_m, em = model.extra_msa_inputs(msa, extra_msa_mask)
+            x, _ = model.extra_msa_evoformer(x, extra_m, mask=x_mask, msa_mask=em, rows_in=True)
+            x = x[None]
+        x_row, _ = model.net(x, m, mask=x_mask, msa_mask=msa_mask, rows_in=True)      # [n1 - n0, N, d]
+        del x, m
+        counts = shard_counts(N, P) if N % P else None
+        x_col = rows_to_cols(x_row, group, counts, counts)                       # [N, n1 - n0, d]: the same rows as columns
+        ret = ReturnValues()
+        ln, lin = model.to_distogram_logits[0], model.to_distogram_logits[1]
+        ret.distance = _ops.distogram_head_rows(x_row, x_col, ln.weight, ln.bias, lin.weight, lin.bias)
+        if model.predict_angles:
+            ret.theta_logits, ret.phi_logits, ret.omega_logits = _ops.angle_heads_rows(model.angle_heads().packed(), x_row, x_col,
+                                                                                       model.symmetrize_omega)
+        ret.pair_rows = (n0, n1)
+    return ret
+
+
+def pair_rows_bytes(N: int, S: int, d: int, heads: int, dim_head: int, P: int) -> int:
+    """Device bytes one rank allocates in a shard_alphafold2(pair_rows=True) forward at its peak (the trunk's blocks), for the rank
+    with the most pair rows, Rn = ceil(N / P), and an MSA of S rows (template angle rows included).  Not counted: the caller's
+    replicated inputs (recyclables.pairwise_repr is a whole fp32 pair tensor, templates_feats T of them at templates_dim) and
+    the weights.  Counted, from the library's workspace queries and the schedule's shapes:
+      * the pair rows: the forward's x_rows, the trunk's working shard and its output, the peer arena's row and column buffers
+        (4 fp32 [Rn, N, d] and one [N, Rn, d]), the replicated m and its arena buffers, the pair mask;
+      * the operands a pair stage keeps: the gathered triangle operand (bf16 [d, N, align8(N)]) and the copy it is merged into
+        (CudaStageOps merges the gathered pieces into one operand for uneven shards, and for even shards narrower than 64
+        columns), the local L, R and gate, the gathered pair bias (twice: gathered and transposed); the outer mean's projected
+        m and its gathered right operand, with its merged copy likewise;
+      * the grow-only workspace sized for the largest stage call of a shard.
+    The merged copies are counted at every P > 1, whether or not N % P makes the shards uneven: the estimate is then an upper
+    bound that never decreases with N (an N that P divides needs at most what the next uneven N needs), so the longest N_res
+    that fits a budget is a bound for every shorter length."""
+    lib = _lib.load()
+    Rn, Rs = -(-N // P), -(-S // P)
+    N8 = _align8(N)
+    ax = lib.af2_axial_attention_workspace
+    ff = lambda tokens: lib.af2_feed_forward_workspace(tokens, d, 4 * d)  # noqa: E731
+    ws = max(ax(1, Rn, N, d, heads, dim_head, 1), ax(1, N, Rn, d, heads, dim_head, 0), ax(1, max(Rs, 1), N, d, heads, dim_head, 1),
+             ax(1, S, Rn, d, heads, dim_head, 0), ff(Rn * N), ff(S * Rn), lib.af2_triangle_project_workspace(Rn * N, d),
+             lib.af2_triangle_contract_workspace(Rn, N, d), lib.af2_triangle_contract_workspace(N, Rn, d),
+             lib.af2_outer_project_workspace(S * Rn, d), lib.af2_outer_contract_workspace(Rn, N, d))
+    shard = Rn * N * d * 4
+    resident = 6 * shard + S * N * d * 4 + 2 * (Rs * N * d * 4 + S * Rn * d * 4) + N * N
+    merged = 2 if P > 1 else 1                                # gathered operand + the copy its pieces are merged into
+    tri = merged * P * d * Rn * N8 * 2 + 2 * d * Rn * N8 * 2 + Rn * N * d * 2
+    bias = 2 * heads * N * N8 * 2
+    outer = 2 * d * S * _align8(Rn) * 2 + merged * P * d * S * _align8(Rn) * 2
+    return int(resident + max(tri, outer) + bias + _ops._ws_alloc(ws))

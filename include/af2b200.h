@@ -345,6 +345,22 @@ int af2_embed_pair_init(const long long* seq, const long long* msa, const float*
                         long long workspace_bytes, af2_stream_t stream);
 int af2_distogram_head(const float* x, const float* gamma, const float* beta, const float* w, const float* bias, float* out, int B,
                        int n, int d, int buckets, af2_stream_t stream);
+/* Row shards of the glue and the heads (parallel.shard_alphafold2(pair_rows=True)): each gives, bitwise, the pair rows
+ * [row0, row0 + rows) of its whole-tensor sibling, with the sibling's argument rules plus 0 <= row0, 0 <= rows, row0 + rows <= n;
+ * otherwise AF2_ERR_BAD_ARG and nothing is written.
+ * af2_embed_pair_init_rows: x_rows [B][rows][n][d]; m [B][S][n][d] whole, as af2_embed_pair_init.
+ * af2_distogram_head_rows / af2_angle_heads_rows (one batch element): x_rows [rows][n][d] and the same rows as columns,
+ *   x_cols [n][rows][d] with x_cols[j][i - row0] = x[j][i] (the rows -> columns exchange of the shard) -> [rows][n][buckets].
+ *   af2_angle_heads_rows reads x_cols only when symmetrize (it may be NULL otherwise). */
+int af2_embed_pair_init_rows(const long long* seq, const long long* msa, const float* token_emb, int vocab, const float* seq_embed,
+                             const float* msa_embed, const float* w_pair, const float* b_pair, const float* pos_emb, int max_rel_dist,
+                             const long long* seq_index, float* x_rows, float* m, int B, int S, int n, int d, int row0, int rows,
+                             void* workspace, long long workspace_bytes, af2_stream_t stream);
+int af2_distogram_head_rows(const float* x_rows, const float* x_cols, const float* gamma, const float* beta, const float* w,
+                            const float* bias, float* out, int rows, int n, int d, int buckets, af2_stream_t stream);
+int af2_angle_heads_rows(const float* x_rows, const float* x_cols, const void* w_planes, const float* bias, float* theta, float* phi,
+                         float* omega, int rows, int n, int d, int n_theta, int n_phi, int n_omega, int symmetrize,
+                         af2_stream_t stream);
 /* af2_angle_heads: alphafold2.py:813-836 (predict_angles) -- one pass over x [B][n][n][d] fp32:
  *   theta[b][i][j] = W_t x[b][i][j] + b_t    [B][n][n][n_theta]      phi = W_p x + b_p    [B][n][n][n_phi]
  *   omega[b][i][j] = W_o s + b_o             [B][n][n][n_omega],     s = (x[b][i][j] + x[b][j][i]) * 0.5 if symmetrize, else x[b][i][j]
@@ -370,6 +386,12 @@ int af2_recycle_embed(const float* coords, int c, const float* single_row, const
                       const float* msa_beta, const float* pair_gamma, const float* pair_beta, const float* table,
                       const float* boundaries, int nb, float* x, float* m, long long m_bstride, int B, int n, int d, float eps,
                       af2_stream_t stream);
+/* af2_recycle_embed_rows: the same on pair rows [row0, row0 + rows): x_rows, prev_pair_rows [B][rows][n][d] (coords whole);
+ *   row 0 of m is updated whole, as af2_recycle_embed does. */
+int af2_recycle_embed_rows(const float* coords, int c, const float* single_row, const float* prev_pair_rows, const float* msa_gamma,
+                           const float* msa_beta, const float* pair_gamma, const float* pair_beta, const float* table,
+                           const float* boundaries, int nb, float* x_rows, float* m, long long m_bstride, int B, int n, int d,
+                           float eps, int row0, int rows, af2_stream_t stream);
 
 /* ---------------- template embedder: alphafold2.py:743-785 (SURVEY.md 8f n3) ---------------------------------------------
  * The template pair stack is af2_triangle_multiply / af2_axial_attention with batch B * T.  The rest:

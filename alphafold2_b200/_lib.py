@@ -196,6 +196,10 @@ _SIGNATURES = {
     "af2_structure_tail": (ci, [vp, vp, vp, vp, cf, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ll, ci, vp]),
     "af2_structure_layer_workspace": (ll, [ci, ci, ci, ci]),
     "af2_structure_layer": (ci, [C.POINTER(StructureWeights), vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, cf, vp, ll, vp]),
+    "af2_ipa_attention_rows": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]),
+    "af2_structure_layer_rows_workspace": (ll, [ci, ci, ci, ci]),
+    "af2_structure_layer_rows_begin": (ci, [C.POINTER(StructureWeights), vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, ll, vp]),
+    "af2_structure_layer_rows_end": (ci, [C.POINTER(StructureWeights), vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, cf, vp, ll, vp]),
     # peer-memory exchange of the sharded trunk
     "af2_peer_ctrl_bytes": (ci, []),
     "af2_peer_can_access": (ci, [ci, ci]),

@@ -864,20 +864,26 @@ class Alphafold2(nn.Module):
             del t, tm2                                   # free this group's t before the next one is embedded
         return x
 
-    def _check_recyclables(self, b, n, device, recyclables):
+    def _check_recyclables(self, b, n, device, recyclables, pair_rows=None):
         """Duck-typed like the reference (alphafold2.py:730-739 reads three attributes): its Recyclables and ours are both
-        accepted.  Returns (coords, single_msa_repr_row, pairwise_repr); raises before any device work."""
+        accepted.  Returns (coords, single_msa_repr_row, pairwise_repr); raises before any device work.  pair_rows: pairwise_repr
+        may also be only a rank's pair rows [b, pair_rows, n, d] (parallel.shard_alphafold2(pair_rows=True))."""
         fields = ("coords", "single_msa_repr_row", "pairwise_repr")
         ts = tuple(getattr(recyclables, f, None) for f in fields)
         if not all(torch.is_tensor(t) for t in ts):
             raise NotImplementedError(f"recyclables must carry tensors {', '.join(fields)} (alphafold2.py:24-28); "
                                       f"got {type(recyclables).__name__}")
         coords, single, pair = ts
+        pair_lead = (b, n, n, self.dim)
+        if pair_rows is not None and pair.dim() == 4 and tuple(pair.shape) == (b, pair_rows, n, self.dim):
+            pair_lead = tuple(pair.shape)
         expect = {"coords": (coords, 3, (b, n)), "single_msa_repr_row": (single, 3, (b, n, self.dim)),
-                  "pairwise_repr": (pair, 4, (b, n, n, self.dim))}
+                  "pairwise_repr": (pair, 4, pair_lead)}
         for name, (t, rank, lead) in expect.items():
             if t.dim() != rank or tuple(t.shape[:len(lead)]) != lead or (name == "coords" and t.shape[-1] < 1):
                 want = f"[{b}, {n}, c]" if name == "coords" else str(list(lead))
+                if name == "pairwise_repr" and pair_rows is not None:
+                    want += f" or this rank's rows {[b, pair_rows, n, self.dim]}"
                 raise ValueError(f"recyclables.{name} must be {want}, got {tuple(t.shape)}")
             if not torch.is_floating_point(t):
                 raise ValueError(f"recyclables.{name} must be a floating tensor, got {t.dtype}")
@@ -890,10 +896,10 @@ class Alphafold2(nn.Module):
         x += LN(pairwise_repr), then += recycling_distance_embed[bucket(|coords_i - coords_j|)]; m[:, 0] += LN(single_msa_repr_row).
         Masks do not gate it (as in the reference).  Under shard_evoformer every rank computes it whole (it runs before the trunk).
         row0: x holds only pair rows [row0, row0 + rows) ([b, rows, n, d]; parallel.shard_alphafold2(pair_rows=True)), and only
-        those rows of pairwise_repr are read."""
+        those rows of pairwise_repr are read; pairwise_repr may then be the whole [b, n, n, d] or those rows [b, rows, n, d]."""
         n = x.shape[1] if row0 is None else x.shape[2]
-        ts = self._check_recyclables(x.shape[0], n, x.device, recyclables)
-        if row0 is not None:
+        ts = self._check_recyclables(x.shape[0], n, x.device, recyclables, pair_rows=None if row0 is None else x.shape[1])
+        if row0 is not None and ts[2].shape[1] != x.shape[1]:
             ts = (ts[0], ts[1], ts[2][:, row0:row0 + x.shape[1]])
         coords, single, pair = (t.detach().to(torch.float32).contiguous() for t in ts)
         args = (coords, single, pair, self.recycling_msa_norm.weight, self.recycling_msa_norm.bias, self.recycling_pairwise_norm.weight,
@@ -1057,13 +1063,7 @@ class Alphafold2(nn.Module):
                                       self.msa_to_single_repr_dim.bias)        # :847
         x = x.contiguous()
         pair = ops.pair_projection_(self.pair_projection().packed(), x, out=x if x_private else torch.empty_like(x))   # :848
-        # :863-868: q = (1, 0, 0, 0), t = 0 per residue; R = quat_to_matrix(q) = I
-        quat = torch.zeros(b, n, 4, dtype=torch.float32, device=x.device)
-        quat[..., 0] = 1.
-        trans = torch.zeros(b, n, 3, dtype=torch.float32, device=x.device)
-        rot = torch.eye(3, dtype=torch.float32, device=x.device).repeat(b, n, 1, 1)
-        coords = torch.empty(b, n, 3, dtype=torch.float32, device=x.device)
-        confidence = torch.empty(b, n, 1, dtype=torch.float32, device=x.device)
+        quat, trans, rot, coords, confidence = structure_frames(b, n, x.device)
         mk = mask.bool() if exists(mask) else None
         depth = self.structure_module_depth
         pk = self.structure_weights().packed()
@@ -1073,11 +1073,30 @@ class Alphafold2(nn.Module):
         if depth == 0:                                                         # :889-891 with q = (1, 0, 0, 0), t = 0
             ops.structure_linear(single, self.to_points.weight, self.to_points.bias, out=coords)
             ops.structure_linear(single, self.lddt_linear.weight, self.lddt_linear.bias, out=confidence)
-        # :893 coords.type(original_dtype) is a no-op: coords stay fp32
-        if return_recyclables:                                                 # :895-897
-            ret.recyclables = Recyclables(coords, single_msa_repr_row, pair)
-        if return_aux_logits:                                                  # :899-900
-            return coords, ret
-        if return_confidence:                                                  # :902-903
-            return coords, confidence
-        return coords                                                          # :905 (return_recyclables alone: just coords)
+        return structure_result(ret, coords, confidence, single_msa_repr_row, pair, return_confidence, return_recyclables,
+                                return_aux_logits)
+
+
+def structure_frames(b: int, n: int, device):
+    """alphafold2.py:863-868: q = (1, 0, 0, 0), t = 0 per residue and R = quat_to_matrix(q) = I, with the coords [b, n, 3] and
+    confidence [b, n, 1] buffers of the last layer: (quat, trans, rot, coords, confidence), fp32."""
+    quat = torch.zeros(b, n, 4, dtype=torch.float32, device=device)
+    quat[..., 0] = 1.
+    trans = torch.zeros(b, n, 3, dtype=torch.float32, device=device)
+    rot = torch.eye(3, dtype=torch.float32, device=device).repeat(b, n, 1, 1)
+    coords = torch.empty(b, n, 3, dtype=torch.float32, device=device)
+    confidence = torch.empty(b, n, 1, dtype=torch.float32, device=device)
+    return quat, trans, rot, coords, confidence
+
+
+def structure_result(ret, coords, confidence, single_msa_repr_row, pairwise_repr, return_confidence, return_recyclables,
+                     return_aux_logits):
+    """What Alphafold2.forward returns after the structure module (alphafold2.py:893-905), in the reference's precedence."""
+    # :893 coords.type(original_dtype) is a no-op: coords stay fp32
+    if return_recyclables:                                                     # :895-897
+        ret.recyclables = Recyclables(coords, single_msa_repr_row, pairwise_repr)
+    if return_aux_logits:                                                      # :899-900
+        return coords, ret
+    if return_confidence:                                                      # :902-903
+        return coords, confidence
+    return coords                                                              # :905 (return_recyclables alone: just coords)

@@ -108,7 +108,7 @@ __global__ void ipa_frames_kernel(float* __restrict__ proj, const float* __restr
 }
 
 // ------------------------------------------------------------------------------------------------ invariant point attention
-// One CTA per query row (b, i), every head.  The keys stream in tiles of TJ pair rows pair[b, i, j0 : j0 + TJ, :], which are
+// One CTA per query row (b, row0 + i), every head.  The keys stream in tiles of TJ pair rows pair[b, i, j0 : j0 + TJ, :], which are
 // contiguous, with the keys' projection rows proj[b, j0 : j0 + TJ, :] beside them: two bulk copies per tile on one mbarrier,
 // double buffered.  Per tile, from the one copy of the tile in shared memory:
 //   pair bias   (pair_ij . W_h + b_h) / sqrt 3              warp per key row, all heads at once
@@ -139,15 +139,16 @@ struct IpaSmem {
 
 struct IpaParams {
   const float* proj;        // [B n, 84 H], points global
-  const float* pair;        // [B, n, n, d]
+  const float* pair;        // [B, rows, n, d]
   const float* w_bias;      // [H, d]  to_pairwise_attn_bias.0
   const float* b_bias;      // [H]
   const float* point_weights;  // [H] (before the softplus)
   const unsigned char* mask;   // [B, n] or null
   const float* rot;         // [B n, 9]
   const float* trans;       // [B n, 3]
-  float* out;               // [B n, H (32 + d)]
+  float* out;               // [B rows, H (32 + d)]
   int n, d, H, TJ;
+  int row0, rows;           // the query rows [row0, row0 + rows) of each batch; pair and out hold only these rows
 };
 
 __global__ void __launch_bounds__(IPA_THREADS) ipa_attention_kernel(const IpaParams p) {
@@ -157,9 +158,10 @@ __global__ void __launch_bounds__(IPA_THREADS) ipa_attention_kernel(const IpaPar
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int H = p.H, d = p.d, n = p.n, TJ = p.TJ;
   const int i = blockIdx.x, b = blockIdx.y;
-  const long long row = (long long)b * n + i;
+  const long long row = (long long)b * n + p.row0 + i;  // the query residue: its projection, mask and frame
+  const long long lrow = (long long)b * p.rows + i;     // its pair row and output row
   const int PW = IPA_PROJ * H;
-  const float* pair_row = p.pair + row * n * d;
+  const float* pair_row = p.pair + lrow * n * d;
   const int ntiles = (n + TJ - 1) / TJ;
 
   if (tid == 0) {
@@ -296,7 +298,7 @@ __global__ void __launch_bounds__(IPA_THREADS) ipa_attention_kernel(const IpaPar
 
   // epilogue
   const int OW = H * (2 * IPA_SD + d);
-  float* orow = p.out + row * OW;
+  float* orow = p.out + lrow * OW;
   for (int e = tid; e < H * d; e += IPA_THREADS) {
     const int h = e / d;
     orow[H * 2 * IPA_SD + e] = sm[L.acc + e] / sm[L.stat + H + h];

@@ -1432,6 +1432,33 @@ def ipa_attention(proj: torch.Tensor, pair: torch.Tensor, w_bias, b_bias, point_
     return out
 
 
+def ipa_attention_rows(proj: torch.Tensor, pair_rows: torch.Tensor, w_bias, b_bias, point_weights, mask: Optional[torch.Tensor],
+                       rot: torch.Tensor, trans: torch.Tensor, heads: int, row0: int) -> torch.Tensor:
+    """ipa_attention of the query rows [row0, row0 + R) at batch 1 (af2_ipa_attention_rows): pair_rows [1, R, n, d] holds those
+    pair rows; proj [1, n, 84 heads] (points global), mask [1, n], rot [1, n, 3, 3] and trans [1, n, 3] cover every residue ->
+    the to_out input [1, R, heads (32 + d)] fp32, bitwise those rows of ipa_attention."""
+    _require(pair_rows, torch.float32, "pair_rows")
+    if pair_rows.dim() != 4 or pair_rows.shape[0] != 1:
+        raise ValueError(f"pair_rows must be [1, R, n, d], got {tuple(pair_rows.shape)}")
+    _, R, n, d = pair_rows.shape
+    _check_ipa_shape(1, n, heads, d)
+    if row0 < 0 or row0 + R > n:
+        raise ValueError(f"query rows [{row0}, {row0 + R}) are not inside [0, {n})")
+    _require(proj, torch.float32, "proj")
+    if tuple(proj.shape) != (1, n, IPA_PROJ * heads):
+        raise ValueError(f"proj must be [1, {n}, {IPA_PROJ * heads}], got {tuple(proj.shape)}")
+    _frame_args(rot, trans, n)
+    wb, bb, pw = _w32(w_bias), _w32(b_bias), _w32(point_weights)
+    if tuple(wb.shape) != (heads, d) or tuple(bb.shape) != (heads,) or tuple(pw.shape) != (heads,):
+        raise ValueError(f"w_bias must be [{heads}, {d}], b_bias and point_weights [{heads}]")
+    mk = _mask_u8(mask, (1, n), "mask")
+    out = torch.empty(1, R, heads * (32 + d), dtype=torch.float32, device=pair_rows.device)
+    _lib.check(_lib.load().af2_ipa_attention_rows(proj.data_ptr(), pair_rows.data_ptr(), wb.data_ptr(), bb.data_ptr(), pw.data_ptr(),
+                                                  _ptr(mk), rot.data_ptr(), trans.data_ptr(), out.data_ptr(), n, row0, R, heads, d,
+                                                  _stream_ptr()))
+    return out
+
+
 def structure_tail_(single: torch.Tensor, o: torch.Tensor, gamma, beta, eps: float = 1e-5, w_qu=None, b_qu=None, quat=None,
                     trans=None, rot=None, w_points=None, b_points=None, w_lddt=None, b_lddt=None, coords=None, confidence=None):
     """af2_structure_tail on single [..., d] in place: LayerNorm(single + o); with w_qu the frame update of quat / trans / rot;
@@ -1456,16 +1483,10 @@ def structure_tail_(single: torch.Tensor, o: torch.Tensor, gamma, beta, eps: flo
     return single
 
 
-def structure_layer_(pk: Packed, single: torch.Tensor, pair: torch.Tensor, mask: Optional[torch.Tensor], quat: torch.Tensor,
-                     trans: torch.Tensor, rot: torch.Tensor, coords: Optional[torch.Tensor] = None,
-                     confidence: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """One layer of alphafold2.py:863-885 (af2_structure_layer) on single [B, n, d] in place, with the frames quat [B, n, 4],
-    trans [B, n, 3] and rot [B, n, 3, 3] updated; on the last layer coords [B, n, 3] and confidence [B, n, 1] are written."""
+def _structure_layer_args(pk: Packed, single: torch.Tensor, quat, trans, rot, coords, confidence):
+    """The per-residue operands of a structure layer, checked: (B, n, d) of single [B, n, d]."""
     _require(single, torch.float32, "single")
-    _require(pair, torch.float32, "pair")
     B, n, d = single.shape
-    if tuple(pair.shape) != (B, n, n, d):
-        raise ValueError(f"pair must be [{B}, {n}, {n}, {d}], got {tuple(pair.shape)}")
     _check_ipa_shape(B, n, pk.heads, d)
     for t, name, size in ((quat, "quat", 4), (trans, "trans", 3), (rot, "rot", 9), (coords, "coords", 3), (confidence, "confidence", 1)):
         if t is not None:
@@ -1474,14 +1495,72 @@ def structure_layer_(pk: Packed, single: torch.Tensor, pair: torch.Tensor, mask:
                 raise ValueError(f"{name} must hold {size} values per residue")
     if (coords is None) != (confidence is None):
         raise ValueError("coords and confidence are written together")
+    if pk.eps[0] != pk.eps[1]:
+        raise ValueError("attn_norm and ff_norm must share one eps")
+    return B, n, d
+
+
+def structure_layer_(pk: Packed, single: torch.Tensor, pair: torch.Tensor, mask: Optional[torch.Tensor], quat: torch.Tensor,
+                     trans: torch.Tensor, rot: torch.Tensor, coords: Optional[torch.Tensor] = None,
+                     confidence: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One layer of alphafold2.py:863-885 (af2_structure_layer) on single [B, n, d] in place, with the frames quat [B, n, 4],
+    trans [B, n, 3] and rot [B, n, 3, 3] updated; on the last layer coords [B, n, 3] and confidence [B, n, 1] are written."""
+    _require(pair, torch.float32, "pair")
+    B, n, d = _structure_layer_args(pk, single, quat, trans, rot, coords, confidence)
+    if tuple(pair.shape) != (B, n, n, d):
+        raise ValueError(f"pair must be [{B}, {n}, {n}, {d}], got {tuple(pair.shape)}")
     mk = _mask_u8(mask, (B, n), "mask")
     lib = _lib.load()
     ws = workspace(lib.af2_structure_layer_workspace(B, n, d, pk.heads), single.device)
-    if pk.eps[0] != pk.eps[1]:
-        raise ValueError("attn_norm and ff_norm must share one eps")
     _lib.check(lib.af2_structure_layer(C.byref(pk.struct), single.data_ptr(), pair.data_ptr(), _ptr(mk), quat.data_ptr(), trans.data_ptr(),
                                        rot.data_ptr(), _ptr(coords), _ptr(confidence), B, n, d, pk.heads, pk.eps[0], ws.data_ptr(),
                                        ws.numel(), _stream_ptr()))
+    return single
+
+
+def structure_layer_rows_begin_(pk: Packed, single: torch.Tensor, pair_rows: torch.Tensor, mask: Optional[torch.Tensor],
+                                quat: torch.Tensor, trans: torch.Tensor, rot: torch.Tensor, row0: int,
+                                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The first half of structure_layer_ at batch 1 for the pair rows [row0, row0 + R) that pair_rows [1, R, n, d] holds
+    (af2_structure_layer_rows_begin): the projections and frames of all n residues of single [1, n, d], the attention of the R
+    query rows and their to_out, written into out [1, R, d] (default: a new tensor), which is returned.  single and the frames
+    are read, not written.  The rows of every shard, gathered in row order, are what structure_layer_rows_end_ takes."""
+    _require(pair_rows, torch.float32, "pair_rows")
+    B, n, d = _structure_layer_args(pk, single, quat, trans, rot, None, None)
+    if pair_rows.dim() != 4 or pair_rows.shape[0] != B or tuple(pair_rows.shape[2:]) != (n, d) or B != 1:
+        raise ValueError(f"pair_rows must be [1, R, {n}, {d}] with single [1, {n}, {d}], got {tuple(pair_rows.shape)} and "
+                         f"{tuple(single.shape)}")
+    R = pair_rows.shape[1]
+    if row0 < 0 or row0 + R > n:
+        raise ValueError(f"query rows [{row0}, {row0 + R}) are not inside [0, {n})")
+    out = torch.empty(1, R, d, dtype=torch.float32, device=single.device) if out is None else out
+    _require(out, torch.float32, "out")
+    if tuple(out.shape) != (1, R, d):
+        raise ValueError(f"out must be [1, {R}, {d}], got {tuple(out.shape)}")
+    mk = _mask_u8(mask, (1, n), "mask")
+    lib = _lib.load()
+    ws = workspace(lib.af2_structure_layer_rows_workspace(n, R, d, pk.heads), single.device)
+    _lib.check(lib.af2_structure_layer_rows_begin(C.byref(pk.struct), single.data_ptr(), pair_rows.data_ptr(), _ptr(mk), quat.data_ptr(),
+                                                  trans.data_ptr(), rot.data_ptr(), out.data_ptr(), n, row0, R, d, pk.heads,
+                                                  ws.data_ptr(), ws.numel(), _stream_ptr()))
+    return out
+
+
+def structure_layer_rows_end_(pk: Packed, single: torch.Tensor, o: torch.Tensor, quat: torch.Tensor, trans: torch.Tensor,
+                              rot: torch.Tensor, coords: Optional[torch.Tensor] = None,
+                              confidence: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The second half of structure_layer_ at batch 1 (af2_structure_layer_rows_end): single [1, n, d] <- attn_norm(single + o)
+    with o [1, n, d] the gathered structure_layer_rows_begin_ rows, then the feed-forward, ff_norm and the frame update, in place;
+    on the last layer coords [1, n, 3] and confidence [1, n, 1] are written.  Returns single."""
+    _require(o, torch.float32, "o")
+    B, n, d = _structure_layer_args(pk, single, quat, trans, rot, coords, confidence)
+    if B != 1 or o.shape != single.shape:
+        raise ValueError(f"single and o must both be [1, n, d], got {tuple(single.shape)} and {tuple(o.shape)}")
+    lib = _lib.load()
+    ws = workspace(lib.af2_structure_layer_rows_workspace(n, n, d, pk.heads), single.device)
+    _lib.check(lib.af2_structure_layer_rows_end(C.byref(pk.struct), single.data_ptr(), o.data_ptr(), quat.data_ptr(), trans.data_ptr(),
+                                                rot.data_ptr(), _ptr(coords), _ptr(confidence), n, d, pk.heads, pk.eps[0],
+                                                ws.data_ptr(), ws.numel(), _stream_ptr()))
     return single
 
 
@@ -1507,7 +1586,21 @@ def pair_projection_(pk: Packed, x: torch.Tensor, out: Optional[torch.Tensor] = 
     _require(out, torch.float32, "out")
     if out.shape != x.shape:
         raise ValueError("out must have x's shape")
-    rows = B * n
+    return _pair_projection(pk, x, out, band)
+
+
+def pair_projection_rows_(pk: Packed, x: torch.Tensor, band: Optional[int] = None) -> torch.Tensor:
+    """pair_projection_ in place over pair rows x [B, R, n, d] (a rank's rows under shard_alphafold2(pair_rows=True)), through
+    the same scratch band: bitwise those rows of pair_projection_ of the whole tensor.  Returns x."""
+    _require(x, torch.float32, "x")
+    if x.dim() != 4 or pk.k_in != x.shape[-1] or pk.tensors["w"].shape[0] != x.shape[-1]:
+        raise ValueError(f"x must be [B, R, n, {pk.k_in}] and the projection square, got {tuple(x.shape)}")
+    return _pair_projection(pk, x, x, band)
+
+
+def _pair_projection(pk: Packed, x: torch.Tensor, out: torch.Tensor, band: Optional[int]) -> torch.Tensor:
+    B, R, n, d = x.shape
+    rows = B * R
     strict = pk.kind == "strict"
     if band is None:
         band = plan_pair_projection_band(rows, n, d, pk.kind, int(device_budget(x.device) * 0.85))

@@ -1129,13 +1129,25 @@ def _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclable
     from .alphafold2 import DISTOGRAM_BUCKETS
     if any(_ops.precision_of(mod) == "strict" for mod in (model.net, model.extra_msa_evoformer, model.template_pointwise_attn)):
         raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
-    if model.predict_coords and not return_trunk:
-        raise NotImplementedError("predict_coords=True needs the third-party structure module (see Alphafold2.forward)")
+    coords = model.predict_coords and not return_trunk
+    if coords and getattr(model, "ipa_block", None) is None:
+        raise NotImplementedError("predict_coords=True needs the structure module (IPABlock, alphafold2.py:19-20, 841-905): call "
+                                  "alphafold2_b200.attach_structure_module(model) first")
     if seq.dim() != 2 or seq.shape[0] != 1:
         raise ValueError(f"pair_rows mode handles one sequence per call (batch 1), got seq {tuple(seq.shape)}")
     P, N = dist.get_world_size(group), seq.shape[1]
     if N < P:
         raise ValueError(f"N_res={N} is smaller than the number of ranks {P}: every rank needs at least one pair row")
+    if coords:
+        _ops._check_ipa_shape(1, N, model.ipa_block.attn.heads, model.dim)
+    pair = getattr(recyclables, "pairwise_repr", None)
+    if torch.is_tensor(pair):
+        on = shard_offsets(N, P)
+        r = dist.get_rank(group)
+        whole, rows = (1, N, N, model.dim), (1, on[r + 1] - on[r], N, model.dim)
+        if tuple(pair.shape) not in (whole, rows):
+            raise ValueError(f"recyclables.pairwise_repr must be the whole {list(whole)} or this rank's pair rows {list(rows)}, got "
+                             f"{tuple(pair.shape)}")
     if model.disable_token_embed:
         raise ValueError("pair_rows mode embeds tokens with the fused pair-init kernel: disable_token_embed is not supported")
     d = model.dim
@@ -1146,7 +1158,6 @@ def _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclable
     if extra_msa is not None and (extra_msa_mask is None or extra_msa_mask.dim() != 3):
         raise ValueError("extra_msa_mask must be given with shape [b, n_msa, n] (the reference's default, alphafold2.py:791, has "
                          "the wrong rank and fails in einops too)")
-    pair = getattr(recyclables, "pairwise_repr", None)
     if not seq.is_cuda or (msa is not None and not msa.is_cuda) or (torch.is_tensor(pair) and not pair.is_cuda):
         raise ValueError("pair_rows mode runs on CUDA tensors (seq, msa and recyclables on the GPU)")
 
@@ -1158,15 +1169,19 @@ def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=Non
     """Alphafold2.forward of a model under shard_alphafold2(pair_rows=True): every pair-tensor stage runs on this rank's pair rows
     [n0, n1) = shard_offsets(N, P)[r:r + 2] and no rank holds the whole pair tensor.  Pair init rows -> recycling rows ->
     template branch on the rows -> template angles into m -> extra-MSA stack rows -> trunk rows -> one rows -> columns exchange
-    of x -> distogram and angle heads on the rows.  Returns this rank's rows: ret.distance [1, n1 - n0, N, 37], theta / phi /
-    omega_logits the same rows, ret.pair_rows = (n0, n1).  Each is bitwise those rows of the default shard_alphafold2 forward.
-    The inputs stay replicated (every rank passes the same tensors and reads its rows of them); so does the MSA tensor m."""
-    from .alphafold2 import ReturnValues
+    of x -> distogram and angle heads on the rows -> with predict_coords, the structure module (structure_module_rows).  Returns
+    this rank's rows: ret.distance [1, n1 - n0, N, 37], theta / phi / omega_logits the same rows, ret.pair_rows = (n0, n1).  Each
+    is bitwise those rows of the default shard_alphafold2 forward; so are the coordinates and confidence, which are whole.
+    The inputs stay replicated (every rank passes the same tensors and reads its rows of them); so does the MSA tensor m.
+    recyclables.pairwise_repr may be the whole [1, N, N, d] or this rank's rows [1, n1 - n0, N, d], as the rows forward returns it."""
+    from .alphafold2 import ReturnValues, _forward_only
     _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclables, return_trunk)
-    model._check_inputs(seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, recyclables)
+    model._check_inputs(seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, None)
     P, r, N = dist.get_world_size(group), dist.get_rank(group), seq.shape[1]
     on = shard_offsets(N, P)
     n0, n1 = on[r], on[r + 1]
+    if recyclables is not None:
+        _forward_only(*model._check_recyclables(1, N, seq.device, recyclables, pair_rows=n1 - n0))
     with torch.no_grad():
         if msa is None:                                                # alphafold2.py:656-658
             msa = seq[:, None, :]
@@ -1188,7 +1203,7 @@ def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=Non
             extra_m, em = model.extra_msa_inputs(msa, extra_msa_mask)
             x, _ = model.extra_msa_evoformer(x, extra_m, mask=x_mask, msa_mask=em, rows_in=True)
             x = x[None]
-        x_row, _ = model.net(x, m, mask=x_mask, msa_mask=msa_mask, rows_in=True)      # [n1 - n0, N, d]
+        x_row, m_row = model.net(x, m, mask=x_mask, msa_mask=msa_mask, rows_in=True)    # [n1 - n0, N, d], this rank's MSA rows
         del x, m
         counts = shard_counts(N, P) if N % P else None
         x_col = rows_to_cols(x_row, group, counts, counts)                       # [N, n1 - n0, d]: the same rows as columns
@@ -1199,14 +1214,60 @@ def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=Non
             ret.theta_logits, ret.phi_logits, ret.omega_logits = _ops.angle_heads_rows(model.angle_heads().packed(), x_row, x_col,
                                                                                        model.symmetrize_omega)
         ret.pair_rows = (n0, n1)
-    return ret
+        if not model.predict_coords or return_trunk:
+            return ret
+        del x_col                                                                # the heads were its only readers
+        m0 = m_row[:1].clone() if r == 0 else m_row.new_empty(1, N, model.dim)   # MSA row 0 (:845) is on rank 0
+        del m_row
+        dist.broadcast(m0, group=group, group_src=0)
+        return structure_module_rows(model, group, x_row, m0, mask, ret, return_confidence, return_recyclables, return_aux_logits)
+
+
+def structure_module_rows(model, group, x_row: torch.Tensor, single_msa_repr_row: torch.Tensor, mask: Optional[torch.Tensor], ret,
+                          return_confidence: bool, return_recyclables: bool, return_aux_logits: bool):
+    """Alphafold2._structure_module (alphafold2.py:841-905) for a rank that holds only the trunk's pair rows x_row [n1 - n0, N, d]
+    (its own buffer) and the whole single_msa_repr_row [1, N, d].  Invariant point attention for query i reads only pair row i,
+    and everything else in the module is per residue, so each layer runs the O(N^2) part on the rank's rows and exchanges N x d:
+      * single = msa_to_single_repr_dim(single_msa_repr_row), whole on every rank;
+      * pairwise_repr = trunk_to_pairwise_repr_dim written over x_row in bands (ops.pair_projection_rows_): no second pair tensor;
+      * per layer: structure_layer_rows_begin_ on the rank's query rows -> all-gather of the [n1 - n0, d] to_out rows ->
+        structure_layer_rows_end_ on all N (with depth 0, to_points and lddt_linear alone, no collective).
+    Returns what Alphafold2.forward returns, each value bitwise the default shard_alphafold2 forward's: coords [1, N, 3] and
+    confidence [1, N, 1] whole, ret.distance and the angle logits this rank's rows, and ret.recyclables = (coords,
+    single_msa_repr_row, this rank's rows of pairwise_repr [1, n1 - n0, N, d])."""
+    from .alphafold2 import structure_frames, structure_result
+    P, r = dist.get_world_size(group), dist.get_rank(group)
+    N = x_row.shape[1]
+    n0 = shard_offsets(N, P)[r]
+    single = _ops.structure_linear(single_msa_repr_row, model.msa_to_single_repr_dim.weight, model.msa_to_single_repr_dim.bias)
+    pair = _ops.pair_projection_rows_(model.pair_projection().packed(), x_row[None])       # :848
+    quat, trans, rot, coords, confidence = structure_frames(1, N, x_row.device)
+    mk = mask.bool() if mask is not None else None
+    depth = model.structure_module_depth
+    pk = model.structure_weights().packed()
+    counts = shard_counts(N, P) if N % P else None
+    o_rows = None
+    for i in range(depth):                                                               # :872-885
+        last = i == depth - 1
+        o_rows = _ops.structure_layer_rows_begin_(pk, single, pair, mk, quat, trans, rot, n0, out=o_rows)
+        o = all_gather_cat0(o_rows[0], group, counts)[None]
+        _ops.structure_layer_rows_end_(pk, single, o, quat, trans, rot, coords if last else None, confidence if last else None)
+        del o
+    if depth == 0:                                                                       # :889-891 with q = (1, 0, 0, 0), t = 0
+        _ops.structure_linear(single, model.to_points.weight, model.to_points.bias, out=coords)
+        _ops.structure_linear(single, model.lddt_linear.weight, model.lddt_linear.bias, out=confidence)
+    return structure_result(ret, coords, confidence, single_msa_repr_row, pair, return_confidence, return_recyclables,
+                            return_aux_logits)
 
 
 def pair_rows_bytes(N: int, S: int, d: int, heads: int, dim_head: int, P: int) -> int:
     """Device bytes one rank allocates in a shard_alphafold2(pair_rows=True) forward at its peak (the trunk's blocks), for the rank
     with the most pair rows, Rn = ceil(N / P), and an MSA of S rows (template angle rows included).  Not counted: the caller's
-    replicated inputs (recyclables.pairwise_repr is a whole fp32 pair tensor, templates_feats T of them at templates_dim) and
-    the weights.  Counted, from the library's workspace queries and the schedule's shapes:
+    replicated inputs (templates_feats, T pair tensors at templates_dim; a whole recyclables.pairwise_repr, where the caller
+    passes one instead of the rank's rows that the rows forward returns) and the weights.  The structure module (predict_coords)
+    is not counted either: it runs after the trunk has released its operands, writes pairwise_repr over the rank's rows and
+    adds only a scratch band and per-residue buffers, so a rank keeps only its rows of pairwise_repr for recycling.
+    Counted, from the library's workspace queries and the schedule's shapes:
       * the pair rows: the forward's x_rows, the trunk's working shard and its output, the peer arena's row and column buffers
         (4 fp32 [Rn, N, d] and one [N, Rn, d]), the replicated m and its arena buffers, the pair mask;
       * the operands a pair stage keeps: the gathered triangle operand (bf16 [d, N, align8(N)]) and the copy it is merged into

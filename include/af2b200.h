@@ -589,6 +589,13 @@ int af2_ipa_frames(float* proj, const float* rot, const float* trans, long long 
 int af2_ipa_attention(const float* proj, const float* pair, const float* w_bias, const float* b_bias, const float* point_weights,
                       const unsigned char* mask, const float* rot, const float* trans, float* out, int B, int n, int heads, int d,
                       af2_stream_t stream);
+/* af2_ipa_attention of the query rows [row0, row0 + rows) at batch 1, for a rank that holds only those pair rows:
+ * pair_rows [rows][n][d] (16-byte aligned) holds pair rows row0 .. row0 + rows - 1; proj [n][84 heads], mask [n], rot [n][9] and
+ * trans [n][3] cover all n residues (every query attends over all n keys); out [rows][heads (32 + d)].  Bitwise those rows of
+ * af2_ipa_attention.  AF2_ERR_BAD_ARG on a null argument, misalignment, row0 < 0, rows < 1, row0 + rows > n or the shapes above. */
+int af2_ipa_attention_rows(const float* proj, const float* pair_rows, const float* w_bias, const float* b_bias,
+                           const float* point_weights, const unsigned char* mask, const float* rot, const float* trans, float* out,
+                           int n, int row0, int rows, int heads, int d, af2_stream_t stream);
 /* single [rows][d] <- LayerNorm(single + o) (gamma, beta, eps).  With w_qu: (u, v) = to_quaternion_update(single);
  * q <- q (x) (1, u) negated where its real part is < 0; t <- t + v R (R before the update); R <- quat_to_matrix(q).
  * With coords (needs w_qu): coords [rows][3] = to_points(single) R + t with the new q, t; confidence [rows] = lddt_linear(single). */
@@ -603,6 +610,23 @@ long long af2_structure_layer_workspace(int B, int n, int d, int heads);
 int af2_structure_layer(const af2_structure_weights* w, float* single, const float* pair, const unsigned char* mask, float* quat,
                         float* trans, float* rot, float* coords, float* confidence, int B, int n, int d, int heads, float eps,
                         void* workspace, long long workspace_bytes, af2_stream_t stream);
+/* af2_structure_layer at batch 1 for a rank that holds only the pair rows [row0, row0 + rows), split around one exchange:
+ *   _begin: proj and its frames for all n residues, attention of the rank's query rows, o_rows [rows][d] = to_out of those rows;
+ *     single, q, t and R are read, not written;
+ *   (the caller gathers every rank's o_rows in row order: o [n][d])
+ *   _end: single = attn_norm(single + o), the three ff linears, ff_norm with the frame update of q, t and R, and on the last layer
+ *     (coords non-null) the coordinates and confidence, all for n residues.
+ * Both take workspaces of af2_structure_layer_rows_workspace(n, rows, d, heads) bytes (one may serve both: _end does not read
+ * what _begin left there).  With row0 = 0 and rows = n, _begin then _end is bitwise af2_structure_layer; split over row shards
+ * and gathered, likewise.  AF2_ERR_BAD_ARG as af2_structure_layer, and on a null workspace or a row window outside [0, n). */
+long long af2_structure_layer_rows_workspace(int n, int rows, int d, int heads);
+int af2_structure_layer_rows_begin(const af2_structure_weights* w, const float* single, const float* pair_rows,
+                                   const unsigned char* mask, const float* quat, const float* trans, const float* rot, float* o_rows,
+                                   int n, int row0, int rows, int d, int heads, void* workspace, long long workspace_bytes,
+                                   af2_stream_t stream);
+int af2_structure_layer_rows_end(const af2_structure_weights* w, float* single, const float* o, float* quat, float* trans, float* rot,
+                                 float* coords, float* confidence, int n, int d, int heads, float eps, void* workspace,
+                                 long long workspace_bytes, af2_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -5,7 +5,7 @@
 from .alphafold2 import (Alphafold2, Evoformer, EvoformerBlock, PairwiseAttentionBlock, MsaAttentionBlock,
                          AxialAttention, Attention, TriangleMultiplicativeModule, OuterMean, FeedForward,
                          ReturnValues, Recyclables, invalidate_packed, IPABlock, InvariantPointAttention,
-                         attach_structure_module)
+                         attach_structure_module, recycle)
 from .ops import set_precision
 from .rotary import apply_rotary_pos_emb, rotate_every_two, FixedPositionalEmbedding, AxialRotaryEmbedding
 
@@ -13,4 +13,4 @@ __all__ = ["Alphafold2", "Evoformer", "EvoformerBlock", "PairwiseAttentionBlock"
            "AxialAttention", "Attention", "TriangleMultiplicativeModule", "OuterMean", "FeedForward",
            "ReturnValues", "Recyclables", "apply_rotary_pos_emb", "rotate_every_two",
            "FixedPositionalEmbedding", "AxialRotaryEmbedding", "invalidate_packed", "set_precision", "IPABlock",
-           "InvariantPointAttention", "attach_structure_module"]
+           "InvariantPointAttention", "attach_structure_module", "recycle"]

@@ -672,6 +672,11 @@ class _PairProjection(_Packable):
         return ops.pack_linear(self.lin.weight, self.lin.bias, strict=ops.precision_of(self.lin) == "strict")
 
 
+NO_STRUCTURE_MODULE = (
+    "predict_coords=True needs the structure module (IPABlock, alphafold2.py:19-20, 841-905), which the constructor leaves "
+    "out because the reference's block is third-party: call alphafold2_b200.attach_structure_module(model) first")
+
+
 def attach_structure_module(model: "Alphafold2") -> "Alphafold2":
     """Register model.ipa_block = IPABlock(dim=model.dim, heads=structure_module_heads) with ipa_block.attn.to_out zeroed
     (alphafold2.py:608-615), so that predict_coords=True runs and a reference predict_coords checkpoint loads strictly.  The
@@ -864,6 +869,28 @@ class Alphafold2(nn.Module):
             del t, tm2                                   # free this group's t before the next one is embedded
         return x
 
+    def _embed_templates_reused_(self, x, x_mask, templates_feats, templates_mask, cache, stack_rows):
+        """embed_templates_ for the iterations of recycle(), which share templates_feats and templates_mask.  The pair stack
+        reads neither x nor the recyclables, so on the first iteration, when the branch runs whole (G = T, band = n) and
+        ops.template_reuse_fits says that t and the crossed mask fit beside the whole-tensor plan of every later pair stack
+        (stack_rows: their MSA rows), they are kept in `cache`; later iterations run only the pointwise attention on them,
+        which only reads t.  Otherwise every iteration runs embed_templates_.  The decision is kept in self.last_template_reuse."""
+        if "t" not in cache:
+            b, T, n = templates_feats.shape[:3]
+            G, band = self._template_plan(x, templates_feats, None, None)
+            tri = self.template_pairwise_embedder.triangle_attention_ingoing.attn
+            budget = int(ops.device_budget(x.device) * 0.85)         # the planners' headroom (_template_plan, _pair_band)
+            keep = G == T and band == n and ops.template_reuse_fits(b, T, n, x.shape[3], tri.heads, tri.dim_head, stack_rows,
+                                                                     budget)
+            self.last_template_reuse = keep
+            cache["t"] = self.template_pair_stack(templates_feats, templates_mask) if keep else None
+            if keep:
+                self.last_template_group, self.last_template_band = T, n
+        if cache["t"] is None:
+            return self.embed_templates_(x, x_mask, templates_feats, templates_mask)
+        t, tm2 = cache["t"]
+        return self.template_pointwise_attn.add_context_(x, t, x_mask, tm2)
+
     def _check_recyclables(self, b, n, device, recyclables, pair_rows=None):
         """Duck-typed like the reference (alphafold2.py:730-739 reads three attributes): its Recyclables and ours are both
         accepted.  Returns (coords, single_msa_repr_row, pairwise_repr); raises before any device work.  pair_rows: pairwise_repr
@@ -946,9 +973,30 @@ class Alphafold2(nn.Module):
         embedds=None, recyclables=None, return_trunk=False, return_confidence=False, return_recyclables=False,
         return_aux_logits=False
     ):
+        return self._forward(seq, msa, mask, msa_mask, extra_msa, extra_msa_mask, seq_index, seq_embed, msa_embed, templates_feats,
+                             templates_mask, templates_angles, embedds, recyclables, return_trunk, return_confidence,
+                             return_recyclables, return_aux_logits)
+
+    def _forward(
+        self, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None, seq_index=None,
+        seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None, templates_angles=None,
+        embedds=None, recyclables=None, return_trunk=False, return_confidence=False, return_recyclables=False,
+        return_aux_logits=False, *, owned=None, template_cache=None
+    ):
+        """forward, with the two hooks of recycle() (both None in forward):
+          owned: a one-element list [recyclables] given instead of `recyclables`, whose tensors the caller references nowhere
+            else.  The list is emptied before this iteration's x and m exist, after a copy of single_msa_repr_row (a view of the
+            previous MSA tensor, which is freed then); the pair tensor and coordinates are dropped once embed_recyclables_ has
+            read them, before the templates, the extra-MSA stack and the trunk run.
+          template_cache: a dict kept across the iterations of one prediction (_embed_templates_reused_)."""
+        if owned is not None:
+            recyclables = owned[0]
         self._check_inputs(seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, recyclables)
 
         with torch.no_grad():
+            if owned is not None and exists(recyclables):
+                recyclables = Recyclables(recyclables.coords, recyclables.single_msa_repr_row.clone(), recyclables.pairwise_repr)
+                owned.clear()
             if not exists(msa):                                        # alphafold2.py:656-658
                 msa = seq[:, None, :]
                 msa_mask = mask[:, None, :] if exists(mask) else None
@@ -993,7 +1041,12 @@ class Alphafold2(nn.Module):
 
             if exists(recyclables):                                    # alphafold2.py:730-739, before the templates read x
                 self.embed_recyclables_(x, m, recyclables)
-            if exists(templates_feats):                                # alphafold2.py:743-785
+                if owned is not None:
+                    recyclables = None
+            if exists(templates_feats) and template_cache is not None:
+                self._embed_templates_reused_(x, x_mask, templates_feats, templates_mask, template_cache,
+                                              (m.shape[1],) + ((msa.shape[1],) if exists(extra_msa) else ()))
+            elif exists(templates_feats):                              # alphafold2.py:743-785
                 self.embed_templates_(x, x_mask, templates_feats, templates_mask)
             if exists(templates_angles):                               # alphafold2.py:787-792
                 msa_mask = self.embed_template_angles_(m, msa_mask, templates_angles, templates_mask)
@@ -1031,9 +1084,7 @@ class Alphafold2(nn.Module):
             if getattr(self, "ipa_block", None) is not None:
                 return self._structure_module(x, m, mask, ret, x_private=x is x_trunk_in, return_confidence=return_confidence,
                                               return_recyclables=return_recyclables, return_aux_logits=return_aux_logits)
-        raise NotImplementedError(
-            "predict_coords=True needs the structure module (IPABlock, alphafold2.py:19-20, 841-905), which the constructor leaves "
-            "out because the reference's block is third-party: call alphafold2_b200.attach_structure_module(model) first")
+        raise NotImplementedError(NO_STRUCTURE_MODULE)
 
     def structure_weights(self) -> _StructureWeights:
         """The packed-weight cache of the attached ipa_block with to_quaternion_update, to_points and lddt_linear."""
@@ -1100,3 +1151,55 @@ def structure_result(ret, coords, confidence, single_msa_repr_row, pairwise_repr
     if return_confidence:                                                      # :902-903
         return coords, confidence
     return coords                                                              # :905 (return_recyclables alone: just coords)
+
+
+def _sharded(model: Alphafold2) -> bool:
+    """Whether parallel.shard_evoformer / shard_alphafold2 replaced a part of model's forward."""
+    return any(getattr(evo, "_af2_sharded", False) for evo in (model.net, model.extra_msa_evoformer)) or \
+        "forward" in model.__dict__ or "embed_templates_" in model.__dict__
+
+
+def recycle(model: Alphafold2, seq, msa=None, *, num_recycles: int = 3, **forward_kwargs):
+    """AlphaFold inference with recycling: what the last call of
+
+        coords, ret = model(seq, msa, **kw, return_aux_logits=True, return_recyclables=True)
+        for _ in range(num_recycles):
+            coords, ret = model(seq, msa, **kw, recyclables=ret.recyclables, return_aux_logits=True, return_recyclables=True)
+
+    returns, bitwise, where the caller's return_* flags in forward_kwargs (Alphafold2.forward's keyword arguments, an initial
+    `recyclables` included) apply to the last call only.  num_recycles = 0 is one model(seq, msa, **forward_kwargs) call.
+
+    On one GPU the loop does less than the one above, with the same bits:
+      * the template pair stack runs once, when its output fits beside the later stages' whole-tensor plans
+        (Alphafold2._embed_templates_reused_, ops.template_reuse_fits), and again on every iteration otherwise;
+      * each iteration's recyclables (the pair tensor, the coordinates, the MSA tensor behind single_msa_repr_row) and heads'
+        outputs are freed as soon as the next iteration's recycling embedder has read them, so the trunk of that iteration
+        runs without a second pair tensor beside it.
+    A sharded model (parallel.shard_evoformer, shard_alphafold2) runs the loop above as written.
+
+    Refused before any device work: num_recycles < 0, and with num_recycles >= 1: predict_coords=False, return_trunk=True
+    (no coordinates to recycle; ValueError) and an unattached structure module (NotImplementedError)."""
+    if isinstance(num_recycles, bool) or not isinstance(num_recycles, int) or num_recycles < 0:
+        raise ValueError(f"num_recycles must be a non-negative integer, got {num_recycles!r}")
+    if num_recycles == 0:
+        return model(seq, msa, **forward_kwargs)
+    if not model.predict_coords:
+        raise ValueError("recycling feeds back the structure module's coordinates: it needs Alphafold2(predict_coords=True)")
+    if forward_kwargs.get("return_trunk", False):
+        raise ValueError("return_trunk=True returns before the structure module, so there is nothing to recycle")
+    if getattr(model, "ipa_block", None) is None:
+        raise NotImplementedError(NO_STRUCTURE_MODULE)
+    flags = ("return_confidence", "return_recyclables", "return_aux_logits")
+    last_flags = {k: forward_kwargs.pop(k, False) for k in flags}
+    inner = dict(return_recyclables=True, return_aux_logits=True)
+    rec = forward_kwargs.pop("recyclables", None)
+    if _sharded(model):
+        for _ in range(num_recycles):
+            rec = model(seq, msa, recyclables=rec, **inner, **forward_kwargs)[1].recyclables
+        return model(seq, msa, recyclables=rec, **last_flags, **forward_kwargs)
+    held, cache = [rec], {}
+    del rec
+    for _ in range(num_recycles):
+        # only `held` references the recyclables: _forward empties it once they are read (the heads' outputs go with the tuple)
+        held = [model._forward(seq, msa, owned=held, template_cache=cache, **inner, **forward_kwargs)[1].recyclables]
+    return model._forward(seq, msa, owned=held, template_cache=cache, **last_flags, **forward_kwargs)

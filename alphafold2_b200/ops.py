@@ -1122,6 +1122,16 @@ def plan_template_branch(b: int, T: int, n: int, d: int, heads: int, dim_head: i
                       f"{budget / 2**30:.2f} GiB can be allocated")
 
 
+def template_reuse_fits(b: int, T: int, n: int, d: int, heads: int, dim_head: int, stack_rows, budget: int) -> bool:
+    """Whether a recycling loop may keep the template pair stack's output t [b * T, n, n, d] fp32 and its crossed mask
+    [b * T, n, n] bool across its iterations: they must fit `budget` (bytes) beside the whole-tensor plan of every pair stack
+    that runs after the templates, one per entry of stack_rows (its MSA rows: the trunk's, and the extra-MSA stack's when
+    there is one), so that keeping t moves none of them into bands.  That is a matter of correctness as well as speed: the
+    extra-MSA stack's tied-query column attention cannot run in pair bands at all."""
+    t_bytes = b * T * n * n * (d * 4 + 1)
+    return all(t_bytes + pair_block_bytes(b, n, S, d, heads, dim_head, n) <= budget for S in stack_rows)
+
+
 PAIR_BAND_ALIGN = 256      # band boundaries: every band call then picks the whole-tensor call's GEMM tile and chan_to_token kernel
 
 

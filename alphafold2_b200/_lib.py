@@ -191,6 +191,7 @@ _SIGNATURES = {
     "af2_template_angles_strict_workspace": (ll, [ci, ci, ci, ci, ci]),
     # structure module (alphafold2.py:841-891)
     "af2_structure_linear": (ci, [vp, vp, vp, vp, ll, ci, ci, ci, vp]),
+    "af2_ipa_tile_rows": (ci, [ci, ci, C.POINTER(ci)]),
     "af2_ipa_frames": (ci, [vp, vp, vp, ll, ci, vp]),
     "af2_ipa_attention": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]),
     "af2_structure_tail": (ci, [vp, vp, vp, vp, cf, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ll, ci, vp]),

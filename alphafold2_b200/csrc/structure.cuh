@@ -13,6 +13,7 @@ namespace af2 {
 
 constexpr int IPA_THREADS = 256;
 constexpr int IPA_MAX_HEADS = 16;
+constexpr int IPA_MAX_BATCH = 65535;     // one CTA row of the grid per batch element: gridDim.y
 constexpr int IPA_SD = 16;                 // scalar key / value width per head
 constexpr int IPA_PT = 4;                  // point keys / values per head
 constexpr int IPA_PROJ = 84;               // projection width per head: 3 * 16 + 3 * 12
@@ -43,9 +44,11 @@ __device__ __forceinline__ void quat_to_matrix(const float q[4], float R[9]) {
 
 // ------------------------------------------------------------------------------------------------ fp32 linear
 // y[M, N] = act(x[M, K] W^T + b), W [N, K] row-major (nn.Linear).  32 x 32 output tile per CTA, 2 x 2 per thread, K in slices of 16.
+// Row tiles on gridDim.x (so up to 2^31 - 1 rows), the few column tiles on gridDim.y.
 // The per-residue projections of the structure module: M = b * n rows, small N and K, so small tiles for enough CTAs (64 x 64
 // tiles gave 16 CTAs at C2 and measured 39 us per call).
 constexpr int SL_BM = 32, SL_BN = 32, SL_BK = 16, SL_R = 2;
+constexpr int SL_MAX_N = 65535 * SL_BN;   // column tiles on gridDim.y
 
 __global__ void __launch_bounds__(256) structure_linear_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                                const float* __restrict__ bias, float* __restrict__ y, int M,
@@ -53,12 +56,13 @@ __global__ void __launch_bounds__(256) structure_linear_kernel(const float* __re
   __shared__ float xs[SL_BK][SL_BM + 4];
   __shared__ float ws[SL_BK][SL_BN + 4];
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-  const int m0 = blockIdx.y * SL_BM, n0 = blockIdx.x * SL_BN;
+  const long long m0 = (long long)blockIdx.x * SL_BM;
+  const int n0 = blockIdx.y * SL_BN;
   float acc[SL_R][SL_R] = {};
   for (int k0 = 0; k0 < K; k0 += SL_BK) {
     for (int e = tid; e < SL_BM * SL_BK; e += 256) {
       const int r = e / SL_BK, k = e % SL_BK;
-      xs[k][r] = (m0 + r < M && k0 + k < K) ? x[(long long)(m0 + r) * K + k0 + k] : 0.f;
+      xs[k][r] = (m0 + r < M && k0 + k < K) ? x[(m0 + r) * K + k0 + k] : 0.f;
       ws[k][r] = (n0 + r < N && k0 + k < K) ? w[(long long)(n0 + r) * K + k0 + k] : 0.f;
     }
     __syncthreads();
@@ -79,14 +83,14 @@ __global__ void __launch_bounds__(256) structure_linear_kernel(const float* __re
   }
 #pragma unroll
   for (int u = 0; u < SL_R; ++u) {
-    const int r = m0 + ty + 16 * u;
+    const long long r = m0 + ty + 16 * u;
     if (r >= M) continue;
 #pragma unroll
     for (int v = 0; v < SL_R; ++v) {
       const int c = n0 + tx + 16 * v;
       if (c >= N) continue;
       float o = acc[u][v] + (bias ? bias[c] : 0.f);
-      y[(long long)r * N + c] = relu ? fmaxf(o, 0.f) : o;
+      y[r * N + c] = relu ? fmaxf(o, 0.f) : o;
     }
   }
 }

@@ -1341,19 +1341,28 @@ def template_pointwise(q: torch.Tensor, gate: torch.Tensor, kv: torch.Tensor, B:
 # structure module (alphafold2.py:841-891): fp32 in both precision modes, except the pair projection (pair_projection_)
 # --------------------------------------------------------------------------------------------------
 IPA_MAX_HEADS = 16        # csrc/structure.cuh: IPA_MAX_HEADS
+IPA_MAX_BATCH = 65535     # csrc/structure.cuh: IPA_MAX_BATCH (the attention grid's y dimension)
 IPA_PROJ = 84             # projection floats per head: q|k|v scalars (3 x 16) and q|k|v points (3 x 4 x 3)
 PAIR_PROJECTION_BAND_BYTES = 16 << 20     # scratch band of pair_projection_: pair rows of at most this many bytes
 
 
 def ipa_shape_ok(B: int, n: int, heads: int, d: int) -> bool:
     """The shapes af2_ipa_attention and af2_structure_layer take (the C side rejects the others with ValueError, unlaunched)."""
-    return B >= 1 and n >= 1 and 1 <= heads <= IPA_MAX_HEADS and d >= 4 and d % 4 == 0 and d <= 1024
+    return 1 <= B <= IPA_MAX_BATCH and n >= 1 and 1 <= heads <= IPA_MAX_HEADS and d >= 4 and d % 4 == 0 and d <= 1024
 
 
 def _check_ipa_shape(B: int, n: int, heads: int, d: int):
     if not ipa_shape_ok(B, n, heads, d):
-        raise ValueError(f"invariant point attention takes batch >= 1, n >= 1, 1 <= heads <= {IPA_MAX_HEADS} and dim a multiple of 4 "
-                         f"up to 1024; got batch {B}, n {n}, heads {heads}, dim {d}")
+        raise ValueError(f"invariant point attention takes 1 <= batch <= {IPA_MAX_BATCH}, n >= 1, 1 <= heads <= {IPA_MAX_HEADS} and dim "
+                         f"a multiple of 4 up to 1024; got batch {B}, n {n}, heads {heads}, dim {d}")
+
+
+def ipa_tile_rows(heads: int, d: int):
+    """(key rows per tile, dynamic shared memory bytes) of af2_ipa_attention's CTA for (heads, d) (af2_ipa_tile_rows); (0, 0) for
+    a shape it does not take."""
+    smem = C.c_int(0)
+    tj = _lib.load().af2_ipa_tile_rows(int(heads), int(d), C.byref(smem))
+    return int(tj), int(smem.value)
 
 
 def pack_structure(block, to_quaternion_update, to_points, lddt_linear) -> Packed:

@@ -564,7 +564,8 @@ int af2_peer_exchange_chunks(const void* src, long long src_row_stride, const af
  * Per residue r: q[r] [4] quaternion (r, i, j, k), never normalised; R[r] [9] = quat_to_matrix(q[r]) row-major; t[r] [3].
  * proj row (84 heads floats): [q_scalar 16H | k_scalar 16H | v_scalar 16H | q_point 12H | k_point 12H | v_point 12H], points (h p c).
  * to_out input row (heads (32 + d) floats): [o_scalar (h 16) | o_point local (h p c) | |o_point| (h p) | o_pair (h d)].
- * Shapes: B >= 1, n >= 1, 1 <= heads <= 16, d % 4 == 0 and 4 <= d <= 1024; otherwise AF2_ERR_BAD_ARG and nothing is launched. */
+ * Shapes: 1 <= B <= 65535, n >= 1, 1 <= heads <= 16, d % 4 == 0 and 4 <= d <= 1024; otherwise AF2_ERR_BAD_ARG and nothing is
+ * launched. */
 typedef struct {
   const float* w_proj;          /* [84 heads][d]: to_scalar_q, _k, _v, to_point_q, _k, _v weights stacked in that order */
   const float *w_bias, *b_bias; /* to_pairwise_attn_bias.0: [heads][d], [heads] */
@@ -576,9 +577,13 @@ typedef struct {
   const float *w_qu, *b_qu;     /* to_quaternion_update: [6][d], [6] */
   const float *w_points, *b_points, *w_lddt, *b_lddt;  /* to_points [3][d], [3]; lddt_linear [1][d], [1] (last layer only) */
 } af2_structure_weights;
-/* y[rows][n_out] = act(x[rows][k] W^T + bias), W [n_out][k] (nn.Linear), bias may be null, relu 0 / 1.  fp32 SIMT. */
+/* y[rows][n_out] = act(x[rows][k] W^T + bias), W [n_out][k] (nn.Linear), bias may be null, relu 0 / 1.  fp32 SIMT.
+ * rows <= 2^31 - 1, n_out <= 65535 * 32. */
 int af2_structure_linear(const float* x, const float* w, const float* bias, float* y, long long rows, int n_out, int k, int relu,
                          af2_stream_t stream);
+/* The key rows per tile af2_ipa_attention streams for (heads, d), and in *smem_bytes (if not null) the dynamic shared memory of
+ * its CTA; 0 (and 0 bytes) for a shape it does not take.  Reads nothing on the device. */
+int af2_ipa_tile_rows(int heads, int d, int* smem_bytes);
 /* The q / k / v point columns of proj [rows][84 heads] taken to the global frame in place: X <- X R[r] + t[r]. */
 int af2_ipa_frames(float* proj, const float* rot, const float* trans, long long rows, int heads, af2_stream_t stream);
 /* Invariant point attention of every query row, one streaming pass over pair [B][n][n][d] (16-byte aligned): per head h,

@@ -114,6 +114,8 @@ _SIGNATURES = {
     "af2_gemm_bf16_f32": (ci, [vp, ll, ll, vp, ll, ll, vp, ll, ll, ci, ci, ci, ci, ci, vp]),
     "af2_gemm_bf16_epilogue": (ci, [vp, ll, ll, vp, ll, ll, ci, ci, ci, ci, ci, C.POINTER(GemmEpilogue), vp]),
     "af2_attention_bf16": (ci, [vp, vp, vp, vp, vp, ci, ci, ci, ci, ll, ll, vp]),
+    "af2_attention_proj_bf16": (ci, [vp, ci, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ll, ll, vp]),
+    "af2_attention_proj_max_n": (ci, [ci]),
     "af2_gemm_bf16_f32_gathered": (ci, [vp, ll, ll, vp, ll, ll, vp, ll, ll, ci, ci, ci, ci, ci, ci, ci, ll, ci, ll, vp]),
     "af2_chan_to_token": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, vp, cf, cf, vp, ci, C.POINTER(ci), vp]),
     "af2_chan_to_token_select": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, vp, cf, cf, vp]),

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/af2b200.h"
+#include "attention_proj.cuh"
 #include "attention_tc.cuh"
 #include "chan2tok_tma.cuh"
 #include "ff_fused.cuh"
@@ -663,6 +664,76 @@ int launch_attention(const __nv_bfloat16* qkv, int heads, int dh, int n, int nba
   }
 }
 
+// -------------------------------------------------------------------------------------------------
+// attention with the projections inside (attention_proj.cuh), one folded batch group
+// -------------------------------------------------------------------------------------------------
+// the longest sequence attention_proj_kernel<dh> keeps resident (0: no such kernel for this head width)
+int attn_proj_max_n(int dh) {
+  int best = 0;
+  for (int n = APROJ_KB; n <= 4096; n += APROJ_KB) {
+    const int st = dh == 64 ? AttnProjSmem<64>::stages_for(n) : (dh == 32 ? AttnProjSmem<32>::stages_for(n) : 0);
+    if (st) best = n;
+  }
+  return best;
+}
+
+// Whether an attention call can take the fused kernel: head width 32 or 64, every key resident in shared memory, and the
+// TMA operands 16-byte aligned.  The rest (and the tied-query and strict paths, which never ask) run the projection GEMMs
+// and attention_tc_kernel.
+bool attn_proj_ok(int dh, int n, const void* xn, const void* w_qkv, const void* w_gate) {
+  return (dh == 32 || dh == 64) && n >= 1 && n <= attn_proj_max_n(dh) && aligned16(xn) && aligned16(w_qkv) && aligned16(w_gate);
+}
+
+template <int DH>
+int launch_attention_proj_inst(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tg, AttnProjParams p,
+                               cudaStream_t s) {
+  using L = AttnProjSmem<DH>;
+  static int configured[MAX_DEVICES] = {0};
+  auto kern = attention_proj_kernel<DH>;
+  p.stages = L::stages_for(p.n);
+  if (p.stages == 0) return fail(AF2_ERR_BAD_ARG, "attention_proj: sequence length %d too long", p.n);
+  const int smem = L::bytes(p.n, p.stages);
+  if (smem > configured[cur_dev()]) {
+    CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured[cur_dev()] = smem;
+  }
+  const long long items = (long long)p.heads * p.nbatch;
+  if (items <= 0) return AF2_OK;
+  const int grid = (int)(items < sm_count() ? items : sm_count());
+  if (items > 0x7fffffffLL - grid) return fail(AF2_ERR_BAD_ARG, "attention_proj: too many work items");
+  // algorithmic: the four projections (q, k, v, gate) plus QK^T and PV; xn read once, og written once, the bias once
+  const double tokens = (double)p.n * p.nbatch, I = (double)p.heads * DH;
+  ProfScope ps(s, KC_ATTENTION, 2.0 * tokens * p.d * 4.0 * I + 4.0 * tokens * p.n * I,
+               tokens * p.d * 2.0 + tokens * I * 2.0 + 4.0 * I * p.d * 2.0 + (p.has_bias ? (double)p.heads * p.n * p.n * 2 : 0));
+  CUDA_OK(launch_pdl(kern, dim3(grid), dim3(APROJ_THREADS), smem, s, tx, tw, tg, p));
+  return AF2_OK;
+}
+
+// xn: bf16 [tokens, d] (the LayerNorm output), token(b', i) = b' * tok_sb + i * tok_si; w_qkv bf16 [3I, d] (q rows pre-scaled),
+// w_gate bf16 [I, d], b_gate fp32 [I] or null; out bf16 [tokens, I].  The caller checks attn_proj_ok.
+int launch_attention_proj(const __nv_bfloat16* xn, int d, const __nv_bfloat16* w_qkv, const __nv_bfloat16* w_gate,
+                          const float* b_gate, int heads, int dh, int n, int nbatch, long long tok_sb, long long tok_si,
+                          const __nv_bfloat16* bias, int npad, const uint8_t* mask, __nv_bfloat16* out, cudaStream_t s) {
+  const long long I = (long long)heads * dh;
+  CUtensorMap tx, tw, tg;
+  const unsigned long long dx[3] = {(unsigned long long)d, (unsigned long long)n, (unsigned long long)nbatch};
+  const unsigned long long sx[2] = {(unsigned long long)(tok_si * d * 2), (unsigned long long)(tok_sb * d * 2)};
+  const unsigned bx[3] = {64, APROJ_TOK, 1};
+  AF2_TRY(make_tmap(&tx, xn, 3, dx, sx, bx, CU_TENSOR_MAP_SWIZZLE_128B));
+  const unsigned long long dw[2] = {(unsigned long long)d, (unsigned long long)(3 * I)}, dg[2] = {(unsigned long long)d, (unsigned long long)I};
+  const unsigned long long sw[1] = {(unsigned long long)d * 2};
+  const unsigned bw[2] = {64, (unsigned)dh};
+  AF2_TRY(make_tmap(&tw, w_qkv, 2, dw, sw, bw, CU_TENSOR_MAP_SWIZZLE_128B));
+  AF2_TRY(make_tmap(&tg, w_gate, 2, dg, sw, bw, CU_TENSOR_MAP_SWIZZLE_128B));
+  if (bias && npad % 2 != 0) return fail(AF2_ERR_BAD_ARG, "attention_proj: bias pitch %d must be even", npad);
+  AttnProjParams p;
+  memset(&p, 0, sizeof(p));
+  p.n = n; p.heads = heads; p.nbatch = nbatch; p.d = d; p.has_bias = bias != nullptr; p.bias = bias; p.npad = npad;
+  p.mask = mask; p.mask_sb = tok_sb; p.mask_si = tok_si; p.b_gate = b_gate;
+  p.out = out; p.tok_sb = tok_sb; p.tok_si = tok_si; p.ld_out = I;
+  return dh == 64 ? launch_attention_proj_inst<64>(tx, tw, tg, p, s) : launch_attention_proj_inst<32>(tx, tw, tg, p, s);
+}
+
 // OuterMean normaliser of pair rows [row0, row0 + rows) of one batch element (quirk Q3): bit-packed kernel when the packed
 // mask fits in shared memory, else the byte-loop kernel
 // variant: 0 the choice above, 1 the byte-loop kernel, 2 the bit-packed pair (needs `words` and the shared-memory fit);
@@ -908,6 +979,7 @@ struct AxialPlan {
   long long T, I;
   int n, nb, npad;
   bool has_bias;
+  bool fused;   // attention_proj_kernel projects q, k, v and the gate: the q|k|v and gate slices stay unused
   __nv_bfloat16 *xn, *qkv, *gate, *og, *bias;
 };
 
@@ -922,6 +994,7 @@ static int axial_plan(AxialPlan& p, const af2_attn_weights* w, const float* x, c
   p.nb = row_attn ? h : wdim;
   p.npad = (int)align_up(p.n, 8);
   p.has_bias = pre_bias != nullptr || (edges != nullptr && w->w_edge != nullptr);
+  p.fused = false;
   Arena ar(workspace, workspace_bytes);
   p.xn = ar.take<__nv_bfloat16>(p.T * d);
   p.qkv = ar.take<__nv_bfloat16>(p.T * 3 * p.I);
@@ -968,7 +1041,8 @@ static int axial_project(const AxialPlan& p, const af2_attn_weights* w, float* x
       AF2_TRY(launch_layernorm(bp, s));
     }
   }
-  // 2. projections
+  // 2. projections (the fused attention kernel makes its own)
+  if (p.fused) return AF2_OK;
   GemmCall cq = linear_call(xn, d, w->w_qkv, d, (int)T, (int)(3 * I), d);
   cq.mode = EPI_STORE_BF16; cq.layout = LAYOUT_TOKEN; cq.out = qkv; cq.ld_out = 3 * I;
   AF2_TRY(launch_gemm(cq, s));
@@ -977,7 +1051,8 @@ static int axial_project(const AxialPlan& p, const af2_attn_weights* w, float* x
   return launch_gemm(cg, s);
 }
 
-// 3. attention per batch element (queries tied first when `tied`) and 4. to_out + bias + residual into x
+// 3. attention per batch element (queries tied first when `tied`; projected inside the kernel when the plan is fused) and
+// 4. to_out + bias + residual into x
 static int axial_attend(const AxialPlan& p, const af2_attn_weights* w, float* x, const unsigned char* mask, int B, int h,
                         int wdim, int d, int heads, int dim_head, int row_attn, int tied, cudaStream_t s) {
   const long long T = p.T, I = p.I;
@@ -986,6 +1061,13 @@ static int axial_attend(const AxialPlan& p, const af2_attn_weights* w, float* x,
   for (int b = 0; b < B; ++b) {
     const long long t0 = (long long)b * h * wdim;
     // MSAColumnGlobalAttention-style tied queries (alphafold2.py:142-151): q <- mean over the folded batch
+    if (p.fused) {
+      AF2_TRY(launch_attention_proj(p.xn + t0 * d, d, static_cast<const __nv_bfloat16*>(w->w_qkv),
+                                    static_cast<const __nv_bfloat16*>(w->w_gate), w->b_gate, heads, dim_head, n, nb, tok_sb, tok_si,
+                                    p.has_bias ? p.bias + (long long)b * heads * n * npad : nullptr, npad, mask ? mask + t0 : nullptr,
+                                    p.og + t0 * I, s));
+      continue;
+    }
     if (tied) AF2_TRY(tie_queries<__nv_bfloat16>(p.qkv + t0 * 3 * I, 3 * I, (int)I, n, nb, tok_sb, tok_si, s));
     AF2_TRY(launch_attention(p.qkv + t0 * 3 * I, heads, dim_head, n, nb, tok_sb, tok_si,
                              p.has_bias ? p.bias + (long long)b * heads * n * npad : nullptr, npad,
@@ -1005,6 +1087,7 @@ static int axial_attention_impl(const af2_attn_weights* w, float* x, const float
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AxialPlan p;
   AF2_TRY(axial_plan(p, w, x, edges, pre_bias, B, h, wdim, d, heads, dim_head, row_attn, workspace, workspace_bytes));
+  p.fused = !tied && attn_proj_ok(dim_head, p.n, p.xn, w->w_qkv, w->w_gate);
   AF2_TRY(axial_project(p, w, x, edges, pre_bias, B, d, heads, s));
   return axial_attend(p, w, x, mask, B, h, wdim, d, heads, dim_head, row_attn, tied, s);
 }
@@ -1465,6 +1548,23 @@ int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, cons
                           static_cast<const __nv_bfloat16*>(bias), (int)align_up(n, 8), mask,
                           static_cast<const __nv_bfloat16*>(gate), static_cast<__nv_bfloat16*>(out),
                           static_cast<cudaStream_t>(stream));
+}
+
+int af2_attention_proj_max_n(int dim_head) { return attn_proj_max_n(dim_head); }
+
+int af2_attention_proj_bf16(const void* xn, int d, const void* w_qkv, const void* w_gate, const float* b_gate, const void* bias,
+                            const unsigned char* mask, void* out, int n, int nbatch, int heads, int dim_head, long long tok_sb,
+                            long long tok_si, af2_stream_t stream) {
+  if (!xn || !w_qkv || !w_gate || !out) return fail(AF2_ERR_BAD_ARG, "attention_proj: null argument");
+  if (d < 8 || d % 8) return fail(AF2_ERR_BAD_ARG, "attention_proj: dim %d must be a positive multiple of 8", d);
+  if (n <= 0 || nbatch <= 0 || heads <= 0) return AF2_OK;
+  if (!attn_proj_ok(dim_head, n, xn, w_qkv, w_gate))
+    return fail(AF2_ERR_BAD_ARG, "attention_proj: dim_head %d, n %d (at most %d) or a misaligned operand", dim_head, n,
+                attn_proj_max_n(dim_head));
+  return launch_attention_proj(static_cast<const __nv_bfloat16*>(xn), d, static_cast<const __nv_bfloat16*>(w_qkv),
+                               static_cast<const __nv_bfloat16*>(w_gate), b_gate, heads, dim_head, n, nbatch, tok_sb, tok_si,
+                               static_cast<const __nv_bfloat16*>(bias), (int)align_up(n, 8), mask, static_cast<__nv_bfloat16*>(out),
+                               static_cast<cudaStream_t>(stream));
 }
 
 int af2_gemm_bf16_f32_gathered(const void* A, long long lda, long long a_batch, const void* Bm, long long ldb, long long b_batch,

@@ -728,6 +728,39 @@ def attention_bf16(qkv: torch.Tensor, gate: torch.Tensor, n: int, nbatch: int, h
     return out
 
 
+def attention_proj_bf16(xn: torch.Tensor, w_qkv: torch.Tensor, w_gate: torch.Tensor, b_gate: Optional[torch.Tensor], n: int,
+                        nbatch: int, heads: int, dim_head: int, tok_sb: int, tok_si: int, bias: Optional[torch.Tensor] = None,
+                        mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """attention_bf16 with the projections inside the kernel: xn bf16 [tokens, d], w_qkv bf16 [3 * heads * dim_head, d],
+    w_gate bf16 [heads * dim_head, d], b_gate fp32 [heads * dim_head] or None; bias and mask as attention_bf16.  Returns bf16
+    [tokens, heads * dim_head]."""
+    _require(xn, torch.bfloat16, "xn")
+    _require(w_qkv, torch.bfloat16, "w_qkv")
+    _require(w_gate, torch.bfloat16, "w_gate")
+    I = heads * dim_head
+    d = xn.shape[-1]
+    if tuple(w_qkv.shape) != (3 * I, d) or tuple(w_gate.shape) != (I, d):
+        raise ValueError(f"w_qkv must be [{3 * I}, {d}] and w_gate [{I}, {d}]")
+    if b_gate is not None:
+        _require(b_gate, torch.float32, "b_gate")
+    if bias is not None:
+        _require(bias, torch.bfloat16, "bias")
+        if tuple(bias.shape) != (heads, n, (n + 7) // 8 * 8):
+            raise ValueError(f"bias must have shape {(heads, n, (n + 7) // 8 * 8)}, got {tuple(bias.shape)}")
+    T = xn.numel() // d
+    mask = _mask_u8(mask, (T,), "mask")
+    out = torch.empty(T, I, dtype=torch.bfloat16, device=xn.device)
+    _lib.check(_lib.load().af2_attention_proj_bf16(xn.data_ptr(), d, w_qkv.data_ptr(), w_gate.data_ptr(), _ptr(b_gate), _ptr(bias),
+                                                   _ptr(mask), out.data_ptr(), n, nbatch, heads, dim_head, tok_sb, tok_si,
+                                                   _stream_ptr()))
+    return out
+
+
+def attention_proj_max_n(dim_head: int) -> int:
+    """the longest sequence the fused projection + attention kernel keeps in shared memory (0: no kernel at this dim_head)"""
+    return int(_lib.load().af2_attention_proj_max_n(dim_head))
+
+
 def _addr(t: torch.Tensor, offset: int = 0) -> int:
     """device address of element `offset` of the flat buffer t"""
     return t.data_ptr() + offset * t.element_size()

@@ -207,6 +207,18 @@ int af2_gemm_bf16_epilogue(const void* A, long long lda, long long a_batch, cons
  * strict-mode forms take any multiple of 4). */
 int af2_attention_bf16(const void* qkv, const void* gate, const void* bias, const unsigned char* mask, void* out, int n,
                        int nbatch, int heads, int dim_head, long long tok_sb, long long tok_si, af2_stream_t stream);
+/* af2_attention_bf16 with the projections inside: q|k|v = xn w_qkv^T (bf16 store) and gate = sigmoid(xn w_gate^T + b_gate)
+ * are computed on chip from xn bf16 [tokens, d] (token (b, i) = b * tok_sb + i * tok_si), w_qkv bf16 [3 * heads * dim_head, d],
+ * w_gate bf16 [heads * dim_head, d] and b_gate fp32 [heads * dim_head] (or NULL), and never stored.  Bitwise equal to
+ * af2_gemm_bf16_epilogue (mode 0, then mode 0 with act 1 and the bias) followed by af2_attention_bf16 on the same inputs.
+ * dim_head 32 or 64, 1 <= n <= af2_attention_proj_max_n(dim_head), d % 8 == 0, 16-byte aligned xn and weights; otherwise
+ * AF2_ERR_BAD_ARG and nothing is launched.  af2_axial_attention{,_ex,_prebias} take this path whenever a call fits it and its
+ * queries are not tied. */
+int af2_attention_proj_bf16(const void* xn, int d, const void* w_qkv, const void* w_gate, const float* b_gate, const void* bias,
+                            const unsigned char* mask, void* out, int n, int nbatch, int heads, int dim_head, long long tok_sb,
+                            long long tok_si, af2_stream_t stream);
+/* the longest sequence af2_attention_proj_bf16 takes at this dim_head (0: none) */
+int af2_attention_proj_max_n(int dim_head);
 /* af2_gemm_bf16_f32 with the tile width `bn` (64 / 128 / 256) as given and gathered operands, as the sharded contractions
  * issue it: a_pr > 0 makes A `a_pr`-row (K-major) or -column (MN-major) pieces `a_piece` elements apart, row / column
  * r = p * a_pr + rr of piece p; b_pr / b_piece likewise for B.  0 = a plain operand.  K-major A pieces must be a multiple

@@ -11,7 +11,12 @@ Each launch is timed by the library's per-launch CUDA events (the ones behind be
 before it.  Algorithmic bytes are q, k, v, gate and output (tokens * heads * dim_head * 2 B * 5) plus the bias
 (heads * n * n * 2 B), the figure the library's profile records; FLOPs are 4 * tokens * n * heads * dim_head.  The GB/s
 fraction is of the H100 SXM data sheet's 3.35 TB/s, the TFLOP/s fraction of its 989 dense BF16 TFLOP/s.  The card name
-and power limit are read in the same run."""
+and power limit are read in the same run.
+
+--projected times each call from the fp32 residual stream instead: LayerNorm -> the fused projection + attention kernel
+against LayerNorm -> q|k|v GEMM -> gate GEMM -> attention kernel (time_projected), and reports both with the speedup; the
+summary's ms_per_block is then the fused sequences' and unfused_ms_per_block the unfused ones'.  A call whose n is above
+ops.attention_proj_max_n is refused by the fused kernel."""
 import argparse
 import ctypes as C
 import json
@@ -116,6 +121,60 @@ def time_eager(flush, qkv, gate, bt, mask, n, nbatch, row, launches, heads, dh):
     return rates(total / launches, b, f)
 
 
+def time_projected(flush, n, nbatch, row, bias, launches, heads, dh, d):
+    """LayerNorm -> fused projection + attention kernel (ops.attention_proj_bf16) against LayerNorm -> q|k|v GEMM -> gate GEMM
+    -> attention kernel, the two sequences the module entries run; CUDA events around each sequence, L2 flushed before it.
+    Algorithmic bytes: x read (fp32), xn written and read, the output written, the bias once, plus for the unfused sequence
+    q|k|v and the gate written and read back.  FLOPs: the four projections plus QK^T and PV."""
+    g = torch.Generator(device="cuda").manual_seed(n * 31 + nbatch)
+    I = heads * dh
+    T = n * nbatch
+    x = torch.randn(T, d, device="cuda", generator=g)
+    gamma, beta = torch.ones(d, device="cuda"), torch.zeros(d, device="cuda")
+    wqkv = (torch.randn(3 * I, d, device="cuda", generator=g) * d ** -0.5).to(torch.bfloat16)
+    wg = (torch.randn(I, d, device="cuda", generator=g) * d ** -0.5).to(torch.bfloat16)
+    bg = torch.randn(I, device="cuda", generator=g)
+    npad = (n + 7) // 8 * 8
+    bt = torch.randn(heads, n, npad, device="cuda", generator=g).to(torch.bfloat16) if bias else None
+    mask = torch.ones(T, dtype=torch.bool, device="cuda")
+    tok_sb, tok_si = (n, 1) if row else (1, nbatch)
+    qkv = torch.empty(T, 3 * I, dtype=torch.bfloat16, device="cuda")
+    gate = torch.empty(T, I, dtype=torch.bfloat16, device="cuda")
+    bn = lambda c: 256 if c > 128 else (128 if c > 64 else 64)   # noqa: E731  (csrc/api.cu pick_bn)
+
+    def fused():
+        xn = ops.layernorm_bf16(x, gamma, beta)
+        return ops.attention_proj_bf16(xn, wqkv, wg, bg, n, nbatch, heads, dh, tok_sb, tok_si, bias=bt, mask=mask)
+
+    def unfused():
+        xn = ops.layernorm_bf16(x, gamma, beta)
+        ops.gemm_bf16_epilogue(xn[None], wqkv[None], qkv, bn=bn(3 * I), mode=ops.EPI_STORE_BF16, ld_out=3 * I)
+        ops.gemm_bf16_epilogue(xn[None], wg[None], gate, bn=bn(I), mode=ops.EPI_STORE_BF16, act=ops.ACT_SIGMOID, bias=bg, ld_out=I)
+        return ops.attention_bf16(qkv, gate, n, nbatch, heads, dh, tok_sb, tok_si, bias=bt, mask=mask)
+
+    f = 2.0 * T * d * 4 * I + 4.0 * T * n * I
+    b_f = 4.0 * T * d + 4.0 * T * d + 2.0 * T * I + 4.0 * I * d * 2 + (heads * n * n * 2.0 if bias else 0.0)
+    b_u = b_f + 2.0 * T * 4 * I * 2
+    out = {"fused": None}
+    for name, run, b in (("fused", fused, b_f), ("unfused", unfused, b_u)):
+        if name == "fused" and n > ops.attention_proj_max_n(dh):
+            continue                     # the module entries run the unfused sequence for this call
+        for _ in range(3):
+            run()
+        torch.cuda.synchronize()
+        total = 0.0
+        for _ in range(launches):
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            run()
+            e1.record()
+            e1.synchronize()
+            total += e0.elapsed_time(e1)
+        out[name] = rates(total / launches, b, f)
+    return out
+
+
 def rates(t, b, f):
     return dict(ms=t, algorithmic_bytes=b, gbs=b / (t * 1e-3) / 1e9, frac_of_hbm_datasheet=b / (t * 1e-3) / HBM_DATASHEET,
                 flops=f, tflops=f / (t * 1e-3) / 1e12, frac_of_bf16_datasheet=f / (t * 1e-3) / BF16_DATASHEET)
@@ -128,6 +187,9 @@ def main():
     ap.add_argument("--heads", type=int, default=CFG["heads"])
     ap.add_argument("--dim-head", type=int, default=CFG["dim_head"], help="16, 32, 64 or 128")
     ap.add_argument("--eager", action="store_true", help="time the reference's eager PyTorch bf16 lines instead of the kernel")
+    ap.add_argument("--projected", action="store_true",
+                    help="time LayerNorm + the fused projection + attention kernel against LayerNorm + the q|k|v and gate GEMMs "
+                         "+ the attention kernel, from the fp32 residual stream (dim 256)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("time_attention.py needs a CUDA device")
@@ -140,6 +202,15 @@ def main():
         N, S = WORKLOADS[wl]
         total = 0.0
         for name, n, nbatch, row, bias in calls(N, S):
+            if args.projected:
+                r = time_projected(flush, n, nbatch, row, bias, args.launches, heads, dh, CFG["dim"])
+                r["speedup"] = r["unfused"]["ms"] / r["fused"]["ms"] if r["fused"] else None
+                total += (r["fused"] or r["unfused"])["ms"]
+                summary.setdefault("unfused_ms_per_block", {}).setdefault(wl, 0.0)
+                summary["unfused_ms_per_block"][wl] += r["unfused"]["ms"]
+                print(json.dumps(dict(workload=wl, call=name, n=n, nbatch=nbatch, heads=heads, dim_head=dh, bias=bias, **r)),
+                      flush=True)
+                continue
             r = time_call(lib, flush, n, nbatch, row, bias, args.launches, heads, dh, args.eager)
             total += r["ms"]
             extra = {"impl": "eager_pytorch_bf16"} if args.eager else {}

@@ -4,7 +4,10 @@
 AF2_PROFILE=1 adds a torch.profiler pass (CUDA activities, after the timed loop) that groups kernel time by name and, for
 the linear GEMMs (K-major, BN 256), by epilogue kind: ms per block, us per 128 x 256 output tile on one SM (kernel time x
 SM count / tiles), and TFLOP/s and GB/s from algorithmic FLOPs and bytes.  The fused feed-forward kernel has a row of its
-own: ms per block, TFLOP/s, HBM GB/s and the L2->SM rate of its weight reads (W1 and W2 once per 128-row tile).  The card name, power limit and max SM clock are read in the same run.  AF2_PROFILE_OUT=path also
+own: ms per block, TFLOP/s, HBM GB/s and the L2->SM rate of its weight reads (W1 and W2 once per 128-row tile), and so do
+the two axial attention kernels (the fused projection + attention kernel and the unfused one).  The linear GEMMs expected
+follow the library's path: attention calls that fit the fused kernel launch no q|k|v or gate GEMM.  The card name, power
+limit and max SM clock are read in the same run.  AF2_PROFILE_OUT=path also
 writes the result as JSON."""
 import json
 import os
@@ -16,7 +19,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import alphafold2_b200 as A  # noqa: E402
-from alphafold2_b200 import _lib  # noqa: E402
+from alphafold2_b200 import _lib, ops  # noqa: E402
 from bench import CFG, flops_per_block, randomize_zero_init_  # noqa: E402
 
 N = int(os.environ.get("AF2_N", 256))
@@ -56,12 +59,21 @@ EK_NAMES = {0: "GENERIC", 1: "STORE_TOK", 2: "STORE_TOK_SIG", 3: "STORE_CH", 4: 
             6: "RESID_F32", 7: "STORE_F32", 8: "STORE_CH_SIG", 9: "RESID_F32_W"}
 
 
-def linear_gemms(N, S, d, I):
-    """(epilogue kind, M, accumulator columns, K) of every linear GEMM launch of one block (module path)."""
+def attention_calls(N, S):
+    """(tokens, n) of the four axial attention calls of one block: MSA row / column, triangle attention start / end"""
+    return [(S * N, N), (S * N, S), (N * N, N), (N * N, N)]
+
+
+def linear_gemms(N, S, d, I, dim_head):
+    """(epilogue kind, M, accumulator columns, K) of every linear GEMM launch of one block (module path).  An attention call
+    whose n fits the fused projection + attention kernel (ops.attention_proj_max_n) launches no q|k|v or gate GEMM."""
     Tm, Tx = S * N, N * N
+    bound = ops.attention_proj_max_n(dim_head)
     out = []
-    for T in (Tm, Tm, Tx, Tx):        # MSA row / column attention, triangle attention start / end
-        out += [(1, T, 3 * I, d), (2, T, I, d), (6, T, d, I)]
+    for T, n in attention_calls(N, S):
+        if n > bound:
+            out += [(1, T, 3 * I, d), (2, T, I, d)]
+        out += [(6, T, d, I)]
     out += [(3, Tm, 2 * d, d), (6, Tx, d, d)]                        # outer mean: left|right, out
     for _ in range(2):                # triangle multiply outgoing / ingoing: left, right, out gate, out
         out += [(5, Tx, 2 * d, d), (5, Tx, 2 * d, d), (2, Tx, d, d), (6, Tx, d, d)]
@@ -121,7 +133,7 @@ if os.environ.get("AF2_PROFILE") == "1":
             by_ek[int(mt.group(4))][0] += ms_
             by_ek[int(mt.group(4))][1] += cnt // it
     cost = {}
-    for ek, M, Nacc, K in linear_gemms(N, S, CFG["dim"], CFG["heads"] * CFG["dim_head"]):
+    for ek, M, Nacc, K in linear_gemms(N, S, CFG["dim"], CFG["heads"] * CFG["dim_head"], CFG["dim_head"]):
         f, b_, tl = gemm_cost(ek, M, Nacc, K)
         c = cost.setdefault(ek, [0.0, 0.0, 0.0, 0])
         c[0] += f; c[1] += b_; c[2] += tl; c[3] += 1
@@ -143,9 +155,17 @@ if os.environ.get("AF2_PROFILE") == "1":
     ff_row = dict(kernel="ff_fused", launches=ff_n, launches_expected=len(ff_launches(N, S, CFG["dim"])), ms_per_block=ff_ms,
                   tflops=f / (ff_ms * 1e-3) / 1e12 if ff_ms else None, hbm_gbs=hb / (ff_ms * 1e-3) / 1e9 if ff_ms else None,
                   weight_l2_gbs=wb / (ff_ms * 1e-3) / 1e9 if ff_ms else None)
+    # axial attention: the fused projection + attention kernel and the unfused attention kernel, per block
+    attn = {}
+    for name, (ms_, cnt) in kernels.items():
+        for kname in ("attention_proj_kernel", "attention_tc_kernel"):
+            if kname in name:
+                a = attn.setdefault(kname, dict(kernel=kname, launches=0, ms_per_block=0.0))
+                a["launches"] += cnt // it
+                a["ms_per_block"] += ms_
     res = dict(N=N, S=S, iters=it, card=card(), lib=_lib.LIB_PATH,
                linear_gemm_ms_per_block=sum(r["ms_per_block"] for r in rows) + ff_ms, linear_gemm_by_epilogue=rows,
-               feed_forward=ff_row,
+               feed_forward=ff_row, attention=list(attn.values()),
                kernels_ms_per_block=dict(sorted(((k, v[0]) for k, v in kernels.items()), key=lambda kv: -kv[1])[:25]))
     print(json.dumps(res))
     if os.environ.get("AF2_PROFILE_OUT"):

@@ -119,6 +119,7 @@ _SIGNATURES = {
     "af2_gemm_bf16_f32_gathered": (ci, [vp, ll, ll, vp, ll, ll, vp, ll, ll, ci, ci, ci, ci, ci, ci, ci, ll, ci, ll, vp]),
     "af2_chan_to_token": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, vp, cf, cf, vp, ci, C.POINTER(ci), vp]),
     "af2_chan_to_token_select": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, vp, cf, cf, vp]),
+    "af2_contract_tail": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, vp, cf, cf, vp, vp, vp, vp, vp, vp, vp, ci, C.POINTER(ci), vp]),
     "af2_outer_scale": (ci, [vp, vp, vp, ci, ci, ci, ci, cf, ci, C.POINTER(ci), vp]),
     # strict precision mode (split-bf16 x3 operands)
     "af2_feed_forward_strict": (ci, [C.POINTER(FFWeightsStrict), vp, ll, ci, ci, vp, ll, vp]),

@@ -15,6 +15,7 @@
 #include "attention_proj.cuh"
 #include "attention_tc.cuh"
 #include "chan2tok_tma.cuh"
+#include "contract_tail.cuh"
 #include "ff_fused.cuh"
 #include "gemm_tc.cuh"
 #include "simt_kernels.cuh"
@@ -794,8 +795,17 @@ int launch_outer_scale(const uint8_t* mask, float* scale, uint32_t* words, int r
 // TriangleMultiply front of `tokens` tokens of x (a grid of rows x inner): LN(x) -> xn; left / right = (proj + b) * mask *
 // sigmoid(gate + b) -> channel-major Lc, Rc [c][chan_stride] (token t at (t / inner) * pitch + t % inner, pad columns zeroed);
 // sigmoid(out_gate) -> gate [tokens][d].  xn [tokens][d] and maskf [tokens] are workspace.
+// gate = bf16(sigmoid(xn w_ogate^T + b_ogate)) [tokens][d]: the triangle out gate (EK_STORE_TOK_SIG)
+int launch_out_gate(const void* xn, const void* w_ogate, const float* b_ogate, long long tokens, int d, void* gate, cudaStream_t s) {
+  GemmCall cg = linear_call(xn, d, w_ogate, d, (int)tokens, d, d);
+  cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = d; cg.bias = b_ogate;
+  return launch_gemm(cg, s);
+}
+
+// out_gate = false: the out gate is left to the tail (contract_tail with a TailGateProj), which projects it from xn itself
 int triangle_front(const af2_trimul_weights* w, const float* x, const unsigned char* mask, long long tokens, int inner, int pitch,
-                   int d, __nv_bfloat16* xn, float* maskf, void* Lc, void* Rc, long long chan_stride, void* gate, cudaStream_t s) {
+                   int d, __nv_bfloat16* xn, float* maskf, void* Lc, void* Rc, long long chan_stride, void* gate, cudaStream_t s,
+                   bool out_gate = true) {
   LnParams lp;
   memset(&lp, 0, sizeof(lp));
   lp.x = x; lp.gamma = w->ln_gamma; lp.beta = w->ln_beta; lp.y = xn; lp.T = tokens; lp.d = d; lp.eps = 1e-5f;
@@ -823,9 +833,7 @@ int triangle_front(const af2_trimul_weights* w, const float* x, const unsigned c
     c.use_rowscale = mask != nullptr; c.rowscale = maskf; c.cm_inner = inner; c.cm_pitch = pitch; c.out_cols = d;
     AF2_TRY(launch_gemm(c, s));
   }
-  GemmCall cg = linear_call(xn, d, w->w_ogate, d, (int)tokens, d, d);
-  cg.mode = EPI_STORE_BF16; cg.act = ACT_SIGMOID; cg.layout = LAYOUT_TOKEN; cg.out = gate; cg.ld_out = d; cg.bias = w->b_ogate;
-  return launch_gemm(cg, s);
+  return out_gate ? launch_out_gate(xn, w->w_ogate, w->b_ogate, tokens, d, gate, s) : AF2_OK;
 }
 
 // OuterMean front of `tokens` MSA tokens of m (a grid of rows x inner): [left | right] = (LN(m) W^T + b) * mask ->
@@ -865,12 +873,94 @@ ChanLnParams chan_ln_params(const float* src, long long chan_stride, int pitch, 
   return p;
 }
 
-// tail of the triangle / outer-product contractions: channel-major O -> token-major bf16 cp.y (launch_chan_to_token), then
-// x [rows * n][d] += cp.y w_out^T + b_out
-int contract_tail(const ChanLnParams& cp, const void* w_out, const float* b_out, float* x, cudaStream_t s) {
-  AF2_TRY(launch_chan_to_token(cp, s));
+// The out gate of a whole-module triangle multiply, projected by the tail from the front's LayerNorm output:
+// gate = bf16(sigmoid(xn w^T + b)).  The unfused tail launches that GEMM into cp.gate first.
+struct TailGateProj {
+  const void* xn;     // [tokens][d] bf16
+  const void* w;      // [d][d] bf16
+  const float* b;     // [d] or nullptr
+};
+
+template <int D, int V>
+int launch_contract_tail(const ChanLnParams& cp, const TailGateProj* gp, const void* w_out, const float* b_out, float* x,
+                         long long T, cudaStream_t s) {
+  using L = CtailSmem<D>;
+  static bool configured[MAX_DEVICES] = {false};
+  auto kern = contract_tail_kernel<D, V>;
+  if (!configured[cur_dev()]) {
+    CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+    configured[cur_dev()] = true;
+  }
+  const void* g = V == CT_GATE_PROJECT ? gp->xn : (V == CT_GATE_LOAD ? static_cast<const void*>(cp.gate) : nullptr);
+  CUtensorMap to, tg, twg, two;
+  {
+    const unsigned long long dO[2] = {(unsigned long long)T, (unsigned long long)D}, sO[1] = {(unsigned long long)cp.chan_stride * 4};
+    const unsigned bO[2] = {CT_TOK, (unsigned)D};
+    AF2_TRY(make_tmap(&to, cp.src, 2, dO, sO, bO, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_DATA_TYPE_FLOAT32));
+    const unsigned long long dW[2] = {(unsigned long long)D, (unsigned long long)D}, sW[1] = {(unsigned long long)D * 2};
+    const unsigned bW[2] = {64, (unsigned)D};
+    AF2_TRY(make_tmap(&two, w_out, 2, dW, sW, bW, CU_TENSOR_MAP_SWIZZLE_128B));
+    if (V == CT_GATE_PROJECT) AF2_TRY(make_tmap(&twg, gp->w, 2, dW, sW, bW, CU_TENSOR_MAP_SWIZZLE_128B));
+    else twg = two;
+    if (g) {
+      const unsigned long long dG[2] = {(unsigned long long)D, (unsigned long long)T}, sG[1] = {(unsigned long long)D * 2};
+      const unsigned bG[2] = {64, CT_TOK};
+      AF2_TRY(make_tmap(&tg, g, 2, dG, sG, bG, CU_TENSOR_MAP_SWIZZLE_128B));
+    } else {
+      tg = to;
+    }
+  }
+  CtailParams q;
+  q.x = x; q.b_ogate = V == CT_GATE_PROJECT ? gp->b : nullptr; q.b_out = b_out; q.gamma = cp.gamma; q.beta = cp.beta;
+  q.scale = cp.scale; q.scale_const = cp.scale_const; q.eps = cp.eps; q.T = (int)T;
+  const long long tiles = (T + CT_TOK - 1) / CT_TOK;
+  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
+  const int ngemm = V == CT_GATE_PROJECT ? 2 : 1;
+  const double flops = 2.0 * ngemm * T * D * (double)D;
+  // O, xn / gate, x read + written, the weights once
+  const double bytes = (double)T * D * (4.0 + (V == CT_SCALE ? 0.0 : 2.0) + 8.0) + ngemm * (double)D * D * 2;
+  ProfScope ps(s, KC_GEMM_LINEAR, flops, bytes);
+  CUDA_OK(launch_pdl(kern, dim3(grid), dim3(CT_THREADS), L::TOTAL, s, to, tg, twg, two, q));
+  return AF2_OK;
+}
+
+// The fused tail runs exactly where launch_chan_to_token would take the TMA kernel and the weights, x and (projected
+// gate) xn are TMA-addressable; every other call keeps the chan_to_token + to_out GEMM launches.
+bool contract_tail_fused_ok(const ChanLnParams& cp, const void* w_out, const float* x, const TailGateProj* gp) {
+  return c2t_variant_ok(cp, C2T_TMA) && aligned16(w_out) && aligned16(x) && (!gp || (aligned16(gp->xn) && aligned16(gp->w)));
+}
+
+enum CtailPath { CTAIL_AUTO = 0, CTAIL_UNFUSED = 1, CTAIL_FUSED = 2 };
+
+// tail of the triangle / outer-product contractions: x [rows * n][d] += tail(O) w_out^T + b_out, tail(O) as
+// launch_chan_to_token makes it (with the out gate projected from gp->xn first when gp is given).  Fused: one
+// contract_tail_kernel launch; unfused: [out-gate GEMM,] chan_to_token into cp.y, to_out GEMM.  *ran <- the path taken.
+int contract_tail(const ChanLnParams& cp, const void* w_out, const float* b_out, float* x, cudaStream_t s,
+                  const TailGateProj* gp = nullptr, int path = CTAIL_AUTO, int* ran = nullptr) {
+  if (ran) *ran = 0;
+  const long long T = (long long)cp.rows * cp.n;
+  const bool fused_ok = contract_tail_fused_ok(cp, w_out, x, gp);
+  if (path == CTAIL_FUSED && !fused_ok)
+    return fail(AF2_ERR_BAD_ARG, "contract_tail: the fused tail cannot run d=%d rows=%d n=%d pitch=%d chan_stride=%lld", cp.d,
+                cp.rows, cp.n, cp.pitch, cp.chan_stride);
+  if (gp && cp.mode != 0) return fail(AF2_ERR_BAD_ARG, "contract_tail: a projected gate needs mode 0");
   const int d = cp.d;
-  GemmCall co = linear_call(cp.y, d, w_out, d, (int)((long long)cp.rows * cp.n), d, d);
+  if (path != CTAIL_UNFUSED && fused_ok) {
+    if (ran) *ran = CTAIL_FUSED;
+    if (T <= 0) return AF2_OK;
+    if (cp.mode == 1)
+      return d == 256 ? launch_contract_tail<256, CT_SCALE>(cp, gp, w_out, b_out, x, T, s)
+                      : launch_contract_tail<128, CT_SCALE>(cp, gp, w_out, b_out, x, T, s);
+    if (gp)
+      return d == 256 ? launch_contract_tail<256, CT_GATE_PROJECT>(cp, gp, w_out, b_out, x, T, s)
+                      : launch_contract_tail<128, CT_GATE_PROJECT>(cp, gp, w_out, b_out, x, T, s);
+    return d == 256 ? launch_contract_tail<256, CT_GATE_LOAD>(cp, gp, w_out, b_out, x, T, s)
+                    : launch_contract_tail<128, CT_GATE_LOAD>(cp, gp, w_out, b_out, x, T, s);
+  }
+  if (ran) *ran = CTAIL_UNFUSED;
+  if (gp) AF2_TRY(launch_out_gate(gp->xn, gp->w, gp->b, T, d, const_cast<__nv_bfloat16*>(cp.gate), s));
+  AF2_TRY(launch_chan_to_token(cp, s));
+  GemmCall co = linear_call(cp.y, d, w_out, d, (int)T, d, d);
   co.mode = EPI_RESID_F32; co.out = x; co.ld_out = d; co.bias = b_out; co.resid = x; co.ld_resid = d;
   return launch_gemm(co, s);
 }
@@ -1130,7 +1220,11 @@ int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned 
   float* maskf = ar.take<float>(T);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_multiply: workspace too small");
 
-  AF2_TRY(triangle_front(w, x, mask, T, N, np8, d, xn, maskf, Lc, Rc, cs_lr, gate, s));
+  // the tail projects the out gate itself when it runs fused: decided here, before the front, with the tail's own predicate
+  const ChanLnParams cp = chan_ln_params(Oc, cs_o, np4, B * N, N, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn);
+  const TailGateProj gp = {xn, w->w_ogate, w->b_ogate};
+  const bool project = contract_tail_fused_ok(cp, w->w_out, x, &gp);
+  AF2_TRY(triangle_front(w, x, mask, T, N, np8, d, xn, maskf, Lc, Rc, cs_lr, gate, s, !project));
   // per-channel contraction, batch = channels
   for (int b = 0; b < B; ++b) {
     GemmCall c;
@@ -1146,9 +1240,8 @@ int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned 
     c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = Oc + (long long)b * N * np4; c.ld_out = np4; c.out_batch = cs_o;
     AF2_TRY(launch_gemm(c, s));
   }
-  // LN over channels * out_gate -> token-major bf16
-  return contract_tail(chan_ln_params(Oc, cs_o, np4, B * N, N, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
-                       w->w_out, w->b_out, x, s);
+  // LN over channels * out_gate -> to_out + residual
+  return contract_tail(cp, w->w_out, w->b_out, x, s, project ? &gp : nullptr, project ? CTAIL_FUSED : CTAIL_AUTO);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1618,6 +1711,23 @@ int af2_outer_scale(const unsigned char* mask, float* scale, void* words, int ro
   if (variant < 0 || variant > 2) return fail(AF2_ERR_BAD_ARG, "outer_scale: variant %d (0..2)", variant);
   return launch_outer_scale(mask, scale, static_cast<uint32_t*>(words), row0, rows, S, N, eps, static_cast<cudaStream_t>(stream),
                             variant, ran);
+}
+
+// The tail of the triangle / outer-product contractions on its own (see include/af2b200.h)
+int af2_contract_tail(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode, const float* gamma,
+                      const float* beta, const void* gate, const float* scale, float scale_const, float eps, const void* xn,
+                      const void* w_ogate, const float* b_ogate, const void* w_out, const float* b_out, float* x, void* y,
+                      int variant, int* ran, af2_stream_t stream) {
+  if (ran) *ran = 0;
+  const ChanLnParams p = chan_ln_params(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y);
+  AF2_TRY(chan_ln_check(p));
+  if (!w_out || !x) return fail(AF2_ERR_BAD_ARG, "contract_tail: null argument");
+  if ((xn != nullptr) != (w_ogate != nullptr)) return fail(AF2_ERR_BAD_ARG, "contract_tail: xn and w_ogate go together");
+  if (d % 8) return fail(AF2_ERR_BAD_ARG, "contract_tail: dim %d must be a multiple of 8", d);
+  if ((long long)rows * n > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "contract_tail: too many tokens");
+  if (variant < CTAIL_AUTO || variant > CTAIL_FUSED) return fail(AF2_ERR_BAD_ARG, "contract_tail: variant %d (0..2)", variant);
+  const TailGateProj gp = {xn, w_ogate, b_ogate};
+  return contract_tail(p, w_out, b_out, x, static_cast<cudaStream_t>(stream), xn ? &gp : nullptr, variant, ran);
 }
 
 }  // extern "C"

@@ -128,6 +128,11 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, in
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1)
+               : "memory");
+}
 
 // L2 prefetch of `bytes` (a multiple of 16) contiguous bytes at a 16-byte aligned global address
 __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes) {

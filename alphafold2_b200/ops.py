@@ -810,6 +810,31 @@ def chan_to_token(src: torch.Tensor, y: torch.Tensor, *, chan_stride: int, pitch
     return ran.value
 
 
+CTAIL_AUTO, CTAIL_UNFUSED, CTAIL_FUSED = 0, 1, 2
+
+
+def contract_tail(src: torch.Tensor, x: torch.Tensor, w_out: torch.Tensor, b_out: Optional[torch.Tensor], y: torch.Tensor, *,
+                  chan_stride: int, pitch: int, rows: int, n: int, d: int, mode: int,
+                  gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None,
+                  gate: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None, scale_const: float = 1.0,
+                  eps: float = 1e-5, xn: Optional[torch.Tensor] = None, w_ogate: Optional[torch.Tensor] = None,
+                  b_ogate: Optional[torch.Tensor] = None, variant: int = CTAIL_AUTO, src_off: int = 0, gate_off: int = 0,
+                  x_off: int = 0) -> int:
+    """af2_contract_tail: x[t] (fp32 [tokens][d] at x_off, in place) += tail(src)[t] w_out^T + b_out with the tail of
+    chan_to_token (mode 0 LayerNorm over channels * gate, mode 1 * scale); with xn / w_ogate the gate is projected first,
+    gate = sigmoid(xn w_ogate^T + b_ogate).  y: bf16 workspace of the unfused path.  Returns the path that ran
+    (CTAIL_UNFUSED or CTAIL_FUSED)."""
+    for t, name in ((x, "x"), (w_out, "w_out")):
+        if not t.is_cuda or not t.is_contiguous():
+            raise ValueError(f"contract_tail: {name} must be a contiguous CUDA tensor")
+    ran = C.c_int(0)
+    args = _c2t_args(src, chan_stride, pitch, rows, n, d, mode, gamma, beta, gate, scale, scale_const, eps, y, src_off,
+                     gate_off, 0)
+    _lib.check(_lib.load().af2_contract_tail(*args[:13], _ptr(xn), _ptr(w_ogate), _ptr(b_ogate), w_out.data_ptr(),
+                                             _ptr(b_out), _addr(x, x_off), args[13], variant, C.byref(ran), _stream_ptr()))
+    return ran.value
+
+
 def chan_to_token_select(src: torch.Tensor, y: torch.Tensor, *, chan_stride: int, pitch: int, rows: int, n: int, d: int,
                          mode: int, gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None,
                          gate: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None, scale_const: float = 1.0,

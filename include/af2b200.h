@@ -239,6 +239,16 @@ int af2_chan_to_token(const float* src, long long chan_stride, int pitch, int ro
 int af2_chan_to_token_select(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode,
                              const float* gamma, const float* beta, const void* gate, const float* scale, float scale_const,
                              float eps, void* y);
+/* The whole tail of a contraction: x [rows * n][d] (fp32, in place) += y w_out^T + b_out, y as af2_chan_to_token makes it
+ * (modes, src and gate as there; y is the token-major bf16 workspace of the unfused path).  With xn and w_ogate (mode 0)
+ * the gate is first projected: gate = bf16(sigmoid(xn w_ogate^T + b_ogate)), xn bf16 [tokens][d] (the unfused path
+ * writes it into gate).  variant: 0 the modules' choice (fused wherever it can run), 1 unfused (chan_to_token, then the to_out GEMM), 2 fused
+ * (one kernel; d 128 or 256 where af2_chan_to_token would take its TMA kernel, 16-byte aligned x and weights; otherwise
+ * AF2_ERR_BAD_ARG and no launch).  Both give the same bits.  *ran (may be NULL) receives the path taken (1 or 2). */
+int af2_contract_tail(const float* src, long long chan_stride, int pitch, int rows, int n, int d, int mode, const float* gamma,
+                      const float* beta, const void* gate, const float* scale, float scale_const, float eps, const void* xn,
+                      const void* w_ogate, const float* b_ogate, const void* w_out, const float* b_out, float* x, void* y,
+                      int variant, int* ran, af2_stream_t stream);
 /* OuterMean normaliser of pair rows [row0, row0 + rows): scale[(i - row0) * N + j] = 1 / (S * (count_ij + eps)), count_ij =
  * sum_s (mask[s][i] & mask[s][j]), mask bool [S][N].  words: workspace of ceil(S / 32) * N uint32 for the bit-packed
  * kernel, or NULL.  variant: 0 the modules' choice (bit-packed when words is given and ceil(S / 32) * N * 4 <= 160 KB),

@@ -6,7 +6,9 @@ the linear GEMMs (K-major, BN 256), by epilogue kind: ms per block, us per 128 x
 SM count / tiles), and TFLOP/s and GB/s from algorithmic FLOPs and bytes.  The fused feed-forward kernel has a row of its
 own: ms per block, TFLOP/s, HBM GB/s and the L2->SM rate of its weight reads (W1 and W2 once per 128-row tile), and so do
 the two axial attention kernels (the fused projection + attention kernel and the unfused one).  The linear GEMMs expected
-follow the library's path: attention calls that fit the fused kernel launch no q|k|v or gate GEMM.  The card name, power
+follow the library's path: attention calls that fit the fused kernel launch no q|k|v or gate GEMM, and where the contraction
+tail is fused (contract_tail_kernel, its own row) the triangle multiplications launch no out-gate GEMM and neither they nor
+the outer mean launch a to_out GEMM.  The card name, power
 limit and max SM clock are read in the same run.  AF2_PROFILE_OUT=path also
 writes the result as JSON."""
 import json
@@ -74,10 +76,30 @@ def linear_gemms(N, S, d, I, dim_head):
         if n > bound:
             out += [(1, T, 3 * I, d), (2, T, I, d)]
         out += [(6, T, d, I)]
-    out += [(3, Tm, 2 * d, d), (6, Tx, d, d)]                        # outer mean: left|right, out
+    tail = tail_fused(N, d)
+    out += [(3, Tm, 2 * d, d)] + ([] if tail else [(6, Tx, d, d)])   # outer mean: left|right, out
     for _ in range(2):                # triangle multiply outgoing / ingoing: left, right, out gate, out
-        out += [(5, Tx, 2 * d, d), (5, Tx, 2 * d, d), (2, Tx, d, d), (6, Tx, d, d)]
+        out += [(5, Tx, 2 * d, d), (5, Tx, 2 * d, d)] + ([] if tail else [(2, Tx, d, d), (6, Tx, d, d)])
     return out
+
+
+def tail_fused(N, d):
+    """whether the module tails run as contract_tail_kernel: d 128 / 256 and an unpadded channel-major O (N % 4 == 0)"""
+    return d in (128, 256) and N % 4 == 0
+
+
+def tail_launches(N, S, d):
+    """(gemms, T, d) of the fused contraction-tail launches of one block: the outer mean (to_out only) and the two triangle
+    multiplications (out gate and to_out)"""
+    return [(1, N * N, d), (2, N * N, d), (2, N * N, d)] if tail_fused(N, d) else []
+
+
+def tail_cost(gemms, T, d):
+    """Algorithmic FLOPs, HBM bytes (O fp32, xn when the gate is projected, x read and written, the weights once) and L2->SM
+    weight bytes (every weight once per 64-token tile) of one contract_tail_kernel launch"""
+    wbytes = gemms * d * d * 2
+    return 2.0 * gemms * T * d * d, float(4 * T * d + (2 * T * d if gemms == 2 else 0) + 8 * T * d + wbytes), \
+        float(-(-T // 64) * wbytes)
 
 
 def ff_launches(N, S, d):
@@ -155,6 +177,16 @@ if os.environ.get("AF2_PROFILE") == "1":
     ff_row = dict(kernel="ff_fused", launches=ff_n, launches_expected=len(ff_launches(N, S, CFG["dim"])), ms_per_block=ff_ms,
                   tflops=f / (ff_ms * 1e-3) / 1e12 if ff_ms else None, hbm_gbs=hb / (ff_ms * 1e-3) / 1e9 if ff_ms else None,
                   weight_l2_gbs=wb / (ff_ms * 1e-3) / 1e9 if ff_ms else None)
+    ct_ms, ct_n = 0.0, 0
+    for name, (ms_, cnt) in kernels.items():
+        if "contract_tail_kernel" in name:
+            ct_ms += ms_
+            ct_n += cnt // it
+    tl_ = tail_launches(N, S, CFG["dim"])
+    f, hb, wb = (sum(v) for v in zip(*(tail_cost(*a) for a in tl_))) if tl_ else (0.0, 0.0, 0.0)
+    ct_row = dict(kernel="contract_tail", launches=ct_n, launches_expected=len(tl_), ms_per_block=ct_ms,
+                  tflops=f / (ct_ms * 1e-3) / 1e12 if ct_ms else None, hbm_gbs=hb / (ct_ms * 1e-3) / 1e9 if ct_ms else None,
+                  weight_l2_gbs=wb / (ct_ms * 1e-3) / 1e9 if ct_ms else None)
     # axial attention: the fused projection + attention kernel and the unfused attention kernel, per block
     attn = {}
     for name, (ms_, cnt) in kernels.items():
@@ -164,8 +196,8 @@ if os.environ.get("AF2_PROFILE") == "1":
                 a["launches"] += cnt // it
                 a["ms_per_block"] += ms_
     res = dict(N=N, S=S, iters=it, card=card(), lib=_lib.LIB_PATH,
-               linear_gemm_ms_per_block=sum(r["ms_per_block"] for r in rows) + ff_ms, linear_gemm_by_epilogue=rows,
-               feed_forward=ff_row, attention=list(attn.values()),
+               linear_gemm_ms_per_block=sum(r["ms_per_block"] for r in rows) + ff_ms + ct_ms, linear_gemm_by_epilogue=rows,
+               feed_forward=ff_row, contract_tail=ct_row, attention=list(attn.values()),
                kernels_ms_per_block=dict(sorted(((k, v[0]) for k, v in kernels.items()), key=lambda kv: -kv[1])[:25]))
     print(json.dumps(res))
     if os.environ.get("AF2_PROFILE_OUT"):

@@ -184,6 +184,13 @@ _SIGNATURES = {
                                                vp, vp, ci, ci, vp, ll, vp]),
     "af2_template_pointwise_rows_end_workspace": (ll, [ll, ci, ci]),
     "af2_template_pointwise_rows_end": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, ll, ci, ci, ci, vp, ll, vp]),
+    # Attention.forward on its own (alphafold2.py:125-190)
+    "af2_attention_forward_workspace": (ll, [ci, ci, ci, ci, ci, ci, ci, ci]),
+    "af2_attention_forward": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, vp, vp, ll, ll, ll, ll, ci, ci, ci, ci, ci, ci, ci, vp,
+                                   vp, ll, vp]),
+    "af2_attention_forward_strict_workspace": (ll, [ci, ci, ci, ci, ci, ci, ci, ci]),
+    "af2_attention_forward_strict": (ci, [C.POINTER(TemplateAttnWeightsStrict), vp, vp, vp, vp, vp, ll, ll, ll, ll, ci, ci, ci, ci, ci, ci,
+                                          ci, vp, vp, ll, vp]),
     "af2_template_embed": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),
     "af2_template_embed_workspace": (ll, [ll, ci]),
     "af2_template_embed_strict": (ci, [vp, vp, vp, vp, ll, ci, ci, vp, ll, vp]),

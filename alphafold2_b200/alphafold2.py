@@ -176,8 +176,8 @@ class FeedForward(_Packable):
 # Attention / AxialAttention (alphafold2.py:98-255)
 # ------------------------------------------------------------------------------------------------------
 class Attention(_Packable):
-    """Parameters with the reference's layout.  Self-attention runs inside AxialAttention's kernel call; the packed weights of
-    this module itself serve the pointwise template attention (Attention with `context`, alphafold2.py:764-777)."""
+    """Parameters with the reference's layout.  Inside the model, self-attention runs in AxialAttention's kernel call and the
+    pointwise template attention through add_context_; forward() runs any standalone call (alphafold2.py:125-190)."""
 
     def __init__(self, dim, seq_len=None, heads=8, dim_head=64, dropout=0., gating=True):
         super().__init__()
@@ -211,9 +211,14 @@ class Attention(_Packable):
         return ops.TemplateAttentionGroups(self.packed(), x, x_mask, self.heads, self.dim_head)
 
     def forward(self, x, mask=None, attn_bias=None, context=None, context_mask=None, tie_dim=None):
-        raise NotImplementedError(
-            "alphafold2_b200.Attention runs through AxialAttention (self-attention) or Alphafold2's template branch "
-            "(pointwise attention over the templates, Attention.add_context_); a standalone call is not on the hot path")
+        """alphafold2.py:125-190 on the GPU: gated self- or cross-attention (no LayerNorm, no residual), result in x.dtype.
+        One query per batch element without a bias runs the pointwise template kernel; the rest the tensor-core attention
+        (strict mode: the split-bf16 attention)."""
+        _forward_only(x, context, attn_bias)
+        with torch.no_grad():
+            out = ops.attention_forward(self.packed(), x, self.heads, self.dim_head, mask=mask, attn_bias=attn_bias, context=context,
+                                        context_mask=context_mask, tie_dim=tie_dim)
+            return out.to(x.dtype)
 
 
 class _TemplateEmbed(_Packable, nn.Linear):

@@ -14,6 +14,7 @@
 #include "../../include/af2b200.h"
 #include "attention_proj.cuh"
 #include "attention_tc.cuh"
+#include "attention_fwd.cuh"
 #include "chan2tok_tma.cuh"
 #include "contract_tail.cuh"
 #include "ff_fused.cuh"
@@ -1735,5 +1736,6 @@ int af2_contract_tail(const float* src, long long chan_stride, int pitch, int ro
 #include "strict_api.inl"
 #include "peer_api.inl"
 #include "template_api.inl"
+#include "attention_api.inl"
 #include "heads_api.inl"
 #include "structure_api.inl"

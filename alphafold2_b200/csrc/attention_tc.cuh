@@ -51,6 +51,19 @@ struct AttnParams {
   const __nv_bfloat16* gate;  // [token, heads*DH], pitch ld_out: read directly by the DH 128 epilogue (the others TMA it)
 };
 
+// The general form (attention_tc_kernel<DH, true>, Attention.forward with i != j or a context): AttnParams::n is the query length i,
+// `mask` the key mask, and the bias is fbias, fp32 [Bb][heads][n][npad] (npad = align8(nk)) with a batch stride (0 when one
+// bias serves every batch element); AttnParams::bias is not read.  The bias stays fp32 because it is the caller's own fp32
+// tensor, which the reference adds unrounded: a bf16 copy would add an error of 2^-9 of the bias to every logit.  A logit is
+// replaced by -FLT_MAX where !(qmask[q] & mask[k]); a null mask counts as all valid.
+struct AttnXParams : AttnParams {
+  int nk;                     // key length j
+  const uint8_t* qmask;       // nullptr or bool query mask; element (b', i) at qmask[b'*qmask_sb + i*qmask_si]
+  long long qmask_sb, qmask_si;
+  const float* fbias;         // fp32 bias (log2 domain) when has_bias
+  long long bias_sb;          // elements between the biases of consecutive batch elements
+};
+
 constexpr int ATTN_THREADS = 384;
 constexpr int ATTN_STAGES = 4;
 constexpr int ATTN_KB = 128;                        // keys per block
@@ -84,13 +97,24 @@ __device__ __forceinline__ AttnItem attn_item(int item, int heads, int nqb) {
   return {item - r * heads, r % nqb, r / nqb};
 }
 
+// key length: n for self-attention, nk for the general form
+__device__ __forceinline__ int attn_keys(const AttnParams& p) { return p.n; }
+__device__ __forceinline__ int attn_keys(const AttnXParams& p) { return p.nk; }
+
+template <bool X> struct AttnParamsOf { using type = AttnParams; };
+template <> struct AttnParamsOf<true> { using type = AttnXParams; };
+
 // tmQ/tmK/tmV/tmG: 4-D maps over the projection buffer (Q, K, V) and the gate, dims (e [DH], i [n], h [heads],
 // b' [nbatch]), box (min(DH, 64), 128, 1, 1), swizzle = the box row's bytes.  tmG is not read at DH 128.
-template <int DH>
+// X = true, the general form (AttnXParams): tmQ and tmG run over the q and gate buffers with dims (e, i, h, b'), tmK and
+// tmV over the k|v buffer with dims (e, j, h, b'); the query blocks cover n = i, the key blocks nk = j, the key codes come
+// from the key mask and the query validity from the query mask.  X = false compiles to the same code as before the
+// general form existed.
+template <int DH, bool X = false>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmG,
-                    const __grid_constant__ AttnParams p) {
+                    const __grid_constant__ typename AttnParamsOf<X>::type p) {
   using L = AttnSmem<DH>;
   constexpr uint32_t SWZ = (DH >= 64) ? SWZ_128 : (DH == 32 ? SWZ_64 : SWZ_32);
   constexpr uint32_t ROWB = L::ATOM_B;              // bytes per row of a Q/K/V/gate swizzle atom
@@ -105,8 +129,9 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   uint64_t* empty_bar = full_bar + L::STAGES;                            // [L::STAGES] K / V consumed
 
   const int n = p.n;
+  const int nk = X ? attn_keys(p) : n;
   const int nqb = (n + 127) / 128;
-  const int nkb = (n + ATTN_KB - 1) / ATTN_KB;
+  const int nkb = (nk + ATTN_KB - 1) / ATTN_KB;
   const int kpad = nkb * ATTN_KB;
   const int items = nqb * p.heads * p.nbatch;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
@@ -171,7 +196,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         uint8_t* kcode = smem + L::KM_OFF + slot * kpad;
         const uint8_t* mrow = p.mask ? p.mask + static_cast<long long>(w.b) * p.mask_sb : nullptr;
         for (int k = lane; k < kpad; k += 32)
-          kcode[k] = k >= n ? 0 : ((mrow && !mrow[static_cast<long long>(k) * p.mask_si]) ? 1 : 2);
+          kcode[k] = k >= nk ? 0 : ((mrow && !mrow[static_cast<long long>(k) * p.mask_si]) ? 1 : 2);
         mbar_arrive(&code_full[slot]);
       }
     }
@@ -191,12 +216,21 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     int rows[2];
     bool qvalid[2];
     const __nv_bfloat16* brow[2];
+    const float* browf[2];
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       rows[hf] = w.qb * 128 + h * 64 + wq * 16 + (lane >> 2) + 8 * hf;
-      qvalid[hf] = kcode[rows[hf]] != 1;   // rows < nqb * 128 = kpad; pad rows (code 0) count as valid queries
       // pad rows (>= n) read the bias of row n - 1: their results are never stored and never mix with other rows
-      brow[hf] = p.has_bias ? p.bias + (static_cast<long long>(w.h) * n + min(rows[hf], n - 1)) * p.npad : nullptr;
+      if constexpr (X) {
+        qvalid[hf] = !p.qmask || rows[hf] >= n ||
+                     p.qmask[static_cast<long long>(w.b) * p.qmask_sb + static_cast<long long>(rows[hf]) * p.qmask_si];
+        browf[hf] = p.has_bias ? p.fbias + static_cast<long long>(w.b) * p.bias_sb +
+                                     (static_cast<long long>(w.h) * n + min(rows[hf], n - 1)) * p.npad
+                               : nullptr;
+      } else {
+        qvalid[hf] = kcode[rows[hf]] != 1;   // rows < nqb * 128 = kpad; pad rows (code 0) count as valid queries
+        brow[hf] = p.has_bias ? p.bias + (static_cast<long long>(w.h) * n + min(rows[hf], n - 1)) * p.npad : nullptr;
+      }
     }
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     float o[DH / 2];
@@ -226,7 +260,16 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       // the pair bias of this key block, read without branches: pad keys (>= n) read a word inside the row, which the key
       // code then discards
       uint32_t bw[ATTN_KB / 8][2] = {};
-      if (p.has_bias) {
+      float2 bwf[X ? ATTN_KB / 8 : 1][2];
+      if constexpr (X) {
+#pragma unroll
+        for (int j = 0; j < ATTN_KB / 8; ++j) {
+          const int key = min(kb * ATTN_KB + 8 * j + 2 * (lane & 3), p.npad - 2);
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf)
+            bwf[j][hf] = p.has_bias ? __ldg(reinterpret_cast<const float2*>(browf[hf] + key)) : make_float2(0.f, 0.f);
+        }
+      } else if (p.has_bias) {
 #pragma unroll
         for (int j = 0; j < ATTN_KB / 8; ++j) {
           const int key = min(kb * ATTN_KB + 8 * j + 2 * (lane & 3), p.npad - 2);
@@ -243,7 +286,14 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         const uint32_t c0 = kcode[key], c1 = kcode[key + 1];
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
-          const float b0 = bf16lo_to_f32(bw[j][hf]), b1 = bf16hi_to_f32(bw[j][hf]);
+          float b0, b1;
+          if constexpr (X) {
+            b0 = bwf[j][hf].x;
+            b1 = bwf[j][hf].y;
+          } else {
+            b0 = bf16lo_to_f32(bw[j][hf]);
+            b1 = bf16hi_to_f32(bw[j][hf]);
+          }
           float& v0 = s[4 * j + 2 * hf];
           float& v1 = s[4 * j + 2 * hf + 1];
           // computed unconditionally and then selected, so that the compiler emits selects rather than branches

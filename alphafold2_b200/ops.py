@@ -960,6 +960,67 @@ def template_pointwise_attention_(pk: Packed, x: torch.Tensor, t: torch.Tensor, 
     return x
 
 
+def attention_forward(pk: Packed, x: torch.Tensor, heads: int, dim_head: int, mask: Optional[torch.Tensor] = None,
+                      attn_bias: Optional[torch.Tensor] = None, context: Optional[torch.Tensor] = None,
+                      context_mask: Optional[torch.Tensor] = None, tie_dim: Optional[int] = None) -> torch.Tensor:
+    """Attention.forward (alphafold2.py:125-190) with the packed weights of pack_template_attention{,_strict}: x [B, i, d],
+    context [B, j, d] or None (self-attention), mask [B, i] and context_mask [B, j] bool or None, attn_bias any float tensor
+    that broadcasts to [B, heads, i, j], tie_dim r (queries averaged over groups of r batch elements) or None.  Masking
+    happens only when mask is given.  Returns fp32 [B, i, d].  Every shape rule is checked before anything runs on the
+    device (ValueError)."""
+    if not torch.is_tensor(x) or x.dim() != 3 or not x.is_floating_point():
+        raise ValueError(f"x must be a float tensor [B, i, d], got {tuple(x.shape) if torch.is_tensor(x) else type(x)}")
+    B, i, d = x.shape
+    j = i
+    if context is not None:
+        if not torch.is_tensor(context) or context.dim() != 3 or not context.is_floating_point() or context.shape[0] != B \
+                or context.shape[2] != d or context.device != x.device:
+            raise ValueError(f"context must be a float tensor [{B}, j, {d}] on {x.device}, got {tuple(context.shape)}")
+        j = context.shape[1]
+    if tie_dim is not None and (int(tie_dim) != tie_dim or tie_dim < 1 or B % tie_dim):
+        raise ValueError(f"tie_dim {tie_dim} must be a positive divisor of the batch {B}")
+    for name, m, n in (("mask", mask, i), ("context_mask", context_mask, j)):
+        if m is not None and (not torch.is_tensor(m) or tuple(m.shape) != (B, n) or m.device != x.device):
+            raise ValueError(f"{name} must be [{B}, {n}] on {x.device}, got {tuple(m.shape) if torch.is_tensor(m) else type(m)}")
+    strides, bias_batch = (0, 0, 0, 0), 0
+    if attn_bias is not None:
+        if not torch.is_tensor(attn_bias) or not attn_bias.is_floating_point() or attn_bias.device != x.device:
+            raise ValueError(f"attn_bias must be a float tensor on {x.device}")
+        try:
+            ok = torch.broadcast_shapes(attn_bias.shape, (B, heads, i, j)) == (B, heads, i, j)
+        except RuntimeError:
+            ok = False
+        if not ok:
+            raise ValueError(f"attn_bias of shape {tuple(attn_bias.shape)} does not broadcast to {(B, heads, i, j)}")
+        # one bias slab per batch element, or one for all of them (batch stride 0)
+        bias_batch = B if attn_bias.dim() == 4 and attn_bias.shape[0] == B and B > 1 else 1
+    strict = pk.kind == "strict"
+    lib = _lib.load()
+    wsfn = lib.af2_attention_forward_strict_workspace if strict else lib.af2_attention_forward_workspace
+    tie = int(tie_dim) if tie_dim is not None else 0
+    # the workspace query checks every shape rule of the C entry point (negative: refused, nothing launched)
+    nbytes = wsfn(B, i, j, d, heads, dim_head, tie, bias_batch)
+    if nbytes < 0:
+        _lib.check(int(nbytes))
+    if not x.is_cuda:
+        raise RuntimeError("x must be a CUDA tensor (alphafold2_b200 has no CPU fallback)")
+    xf = x.detach().to(torch.float32).contiguous()
+    _require(xf, torch.float32, "x")
+    cf = None if context is None else context.detach().to(torch.float32).contiguous()
+    bias = None
+    if attn_bias is not None:
+        bias = attn_bias.detach().to(torch.float32).expand(B, heads, i, j)
+        strides = (bias.stride(0) if bias_batch > 1 else 0,) + tuple(bias.stride()[1:])
+    xm = _mask_u8(mask, (B, i), "mask")
+    cm = _mask_u8(context_mask, (B, j), "context_mask")
+    out = torch.empty(B, i, d, dtype=torch.float32, device=x.device)
+    ws = workspace(nbytes, x.device)
+    fn = lib.af2_attention_forward_strict if strict else lib.af2_attention_forward
+    _lib.check(fn(C.byref(pk.struct), xf.data_ptr(), _ptr(cf), _ptr(xm), _ptr(cm), _ptr(bias), *strides, B, i, j, d, heads, dim_head, tie,
+                  out.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
+    return out
+
+
 class TemplateAttentionGroups:
     """template_pointwise_attention_ over the templates one group at a time (af2_template_pointwise_begin / _group / _end):
         g = TemplateAttentionGroups(pk, x, x_mask, heads, dim_head)

@@ -445,6 +445,30 @@ long long af2_template_pointwise_attention_strict_workspace(int B, int T, int n,
 int af2_template_pointwise_attention_strict(const af2_template_attn_weights_strict* w, float* x, const float* t,
                                             const unsigned char* x_mask, const unsigned char* t_mask, int B, int T, int n, int d,
                                             int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
+/* af2_attention_forward: Attention.forward (alphafold2.py:125-190) on its own, with the weights of the template attention:
+ *     q = to_q(x) * dim_head^-0.5, [k | v] = to_kv(context, or x when context is NULL), out = to_out(softmax(q k^T + bias) v *
+ *     sigmoid(gating(x))) + b_out;  no LayerNorm, no residual.  x fp32 [B][i][d], context fp32 [B][j][d] (NULL: j must equal i),
+ *     out fp32 [B][i][d].  Masking only when mask [B][i] is given: the key mask is then context_mask [B][j] (context given; NULL:
+ *     all keys valid) or mask (self-attention), and logits where !(mask[q] & key_mask[k]) are -FLT_MAX, so a masked query
+ *     averages all j values; context_mask without mask is ignored.  bias fp32 or NULL, added before masking, element (b, h, q, k)
+ *     at bias[b bias_sb + h bias_sh + q bias_si + k bias_sj] (bias_sb = 0: one bias for every batch element).  tie_dim r > 0:
+ *     q is averaged over each group of r consecutive batch elements (alphafold2.py:142-151), B % r == 0; 0: no tying.
+ *     i == 1 without a bias runs the pointwise template kernel (B pair positions, T = j templates); the rest runs the
+ *     projections as GEMMs, attention_tc_kernel<dim_head, true> on a log2(e)-scaled fp32 copy of the bias and to_out.  dim_head
+ *     16, 32, 64 or 128, d % 8 == 0, and j small enough for the attention kernel's shared memory.
+ * The strict twin: dim_head any multiple of 4, split-bf16 GEMMs around an fp32 softmax with the bias read in place.
+ * The _workspace queries take bias_batch = 0 (no bias), 1 (bias_sb = 0) or B; they return AF2_ERR_BAD_ARG (negative) for a
+ * shape the call refuses, and the calls refuse it before launching anything. */
+long long af2_attention_forward_workspace(int B, int i, int j, int d, int heads, int dim_head, int tie_dim, int bias_batch);
+int af2_attention_forward(const af2_template_attn_weights* w, const float* x, const float* context, const unsigned char* mask,
+                          const unsigned char* context_mask, const float* bias, long long bias_sb, long long bias_sh, long long bias_si,
+                          long long bias_sj, int B, int i, int j, int d, int heads, int dim_head, int tie_dim, float* out,
+                          void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_attention_forward_strict_workspace(int B, int i, int j, int d, int heads, int dim_head, int tie_dim, int bias_batch);
+int af2_attention_forward_strict(const af2_template_attn_weights_strict* w, const float* x, const float* context,
+                                 const unsigned char* mask, const unsigned char* context_mask, const float* bias, long long bias_sb,
+                                 long long bias_sh, long long bias_si, long long bias_sj, int B, int i, int j, int d, int heads,
+                                 int dim_head, int tie_dim, float* out, void* workspace, long long workspace_bytes, af2_stream_t stream);
 /* The pointwise kernel alone, on P = B * pairs pair positions:  out[p] = gate[p] * sum_t softmax_t(q[p] . k) v,  k | v = kv row
  * (b T + t) * pairs + (p % pairs), kv [B T pairs][2I] (k | v); pooled fp32 [P] = any_t t_mask; masks as above (t_mask indexed
  * like the kv rows).  _bf16: q [P][I] pre-scaled by dim_head^-0.5 * log2(e) (exp2-domain softmax), gate [P][I] with the sigmoid

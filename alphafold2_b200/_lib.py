@@ -153,6 +153,11 @@ _SIGNATURES = {
     "af2_strict_chan_to_token": (ci, [vp, ll, ci, ci, ci, ci, ci, vp, vp, vp, ll, ci, vp, cf, cf, vp, vp]),
     "af2_tie_queries_f32": (ci, [vp, ll, ci, ci, ci, ll, ll, vp]),
     "af2_tie_queries_bf16": (ci, [vp, ll, ci, ci, ci, ll, ll, vp]),
+    "af2_attention_x_bf16": (ci, [vp, vp, vp, vp, ll, vp, vp, ci, ci, ci, ci, ci, vp, vp]),
+    "af2_attn_bias_log2": (ci, [vp, ll, ll, ll, ll, vp, ci, ci, ci, ci, vp]),
+    "af2_strict_xqkv_split": (ci, [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
+    "af2_strict_xsoftmax_split": (ci, [vp, ll, vp, ll, ll, ll, ll, vp, vp, vp, ci, ci, ci, ci, ci, vp]),
+    "af2_strict_xgate_split": (ci, [vp, vp, vp, ci, ci, ci, ci, ci, vp]),
     # template embedder (alphafold2.py:743-792)
     "af2_template_pointwise_attention": (ci, [C.POINTER(TemplateAttnWeights), vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, ll, vp]),
     "af2_template_pointwise_attention_workspace": (ll, [ci, ci, ci, ci, ci, ci]),

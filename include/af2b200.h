@@ -354,6 +354,35 @@ int af2_strict_chan_to_token(const float* src, long long chan_stride, int pitch,
                              float scale_const, float eps, void* y, af2_stream_t stream);
 int af2_tie_queries_f32(float* buf, long long ld, int cols, int n, int nbatch, long long tok_sb, long long tok_si, af2_stream_t stream);
 int af2_tie_queries_bf16(void* buf, long long ld, int cols, int n, int nbatch, long long tok_sb, long long tok_si, af2_stream_t stream);
+/* The kernels of af2_attention_forward{,_strict} through the launchers those entries use (batch elements b < B, I = heads *
+ * dim_head):
+ * af2_attention_x_bf16: attention_tc_kernel<dim_head, true>: out bf16 [B i][I] = (softmax_k(2^(q . k + bias)) v) * gate over the
+ *   keys of the same batch element; q and gate (sigmoid applied) bf16 [B i][I], q pre-scaled by dim_head^-0.5 log2(e); kv bf16
+ *   [B j][2I] (k | v); bias_log2 fp32 [Bb][heads][i][align8(j)] or NULL, batch element b at bias_log2 + b * bias_sb (bias_sb = 0:
+ *   one slab for all); qmask [B][i] and kmask [B][j] bool or NULL (all valid): where !(qmask[q] & kmask[k]) the logit is
+ *   -FLT_MAX.  The shape rules of af2_attention_forward, with the key-length rule applied for every i, are checked before
+ *   anything is launched.
+ * af2_attn_bias_log2: out fp32 [Bb][heads][i][align8(j)] = bias[b sb + h sh + q si + k sj] * log2(e), pad columns 0.
+ * af2_strict_xqkv_split: for b' < nb, b = b0 + b': Q split [nb heads][i][3][align8(dim_head)] from qg fp32 [B i][2I] (q |
+ *   gate logits), K split [nb heads][j][3][align8(dim_head)] and Vt split [nb heads][dim_head][3][align8(j)] from kv fp32
+ *   [B j][2I] (k | v).
+ * af2_strict_xsoftmax_split: P split [nb heads][i][3][align8(j)] = softmax_k(S[r][k] + bias[b sb + h sh + q si + k sj]) of
+ *   the logits S fp32 [nb heads][i][lds] (bias NULL: none); when qmask [B][i] is given, logits where !(qmask[q] & kmask[k])
+ *   are -FLT_MAX (kmask [B][j] NULL: all keys valid); kmask alone is ignored.
+ * af2_strict_xgate_split: og split rows (b i + q) of [B i][3][align8(I)] = O[(b' heads + h) i + q][e] (O fp32 [nb heads][i]
+ *   [dim_head]) * sigmoid(qg[b i + q][I + h dim_head + e]); the rows of other batch elements are not written. */
+int af2_attention_x_bf16(const void* q, const void* gate, const void* kv, const float* bias_log2, long long bias_sb,
+                         const unsigned char* qmask, const unsigned char* kmask, int B, int i, int j, int heads, int dim_head, void* out,
+                         af2_stream_t stream);
+int af2_attn_bias_log2(const float* bias, long long sb, long long sh, long long si, long long sj, float* out, int Bb, int heads, int i,
+                       int j, af2_stream_t stream);
+int af2_strict_xqkv_split(const float* qg, const float* kv, void* Q, void* K, void* Vt, int b0, int nb, int heads, int i, int j,
+                          int dim_head, af2_stream_t stream);
+int af2_strict_xsoftmax_split(const float* S, long long lds, const float* bias, long long sb, long long sh, long long si, long long sj,
+                              const unsigned char* qmask, const unsigned char* kmask, void* P, int b0, int nb, int heads, int i, int j,
+                              af2_stream_t stream);
+int af2_strict_xgate_split(const float* O, const float* qg, void* og, int b0, int nb, int heads, int i, int dim_head,
+                           af2_stream_t stream);
 
 /* ---------------- pre- / post-trunk glue as fused kernels (SURVEY.md 8f n1) -------------------------------------------
  * af2_embed_pair_init: alphafold2.py:676-726 -- token embedding gather, m = (emb[msa] + msa_embed) + emb[seq],

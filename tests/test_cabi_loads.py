@@ -38,6 +38,30 @@ def test_workspace_queries(lib):
     assert lib.af2_outer_mean_workspace(1, 128, 256, 256) > 0
 
 
+def _attn_smem(dh, nk):
+    """AttnSmem<DH>::bytes(nk) of attention_tc.cuh: two item slots (Q | gate; Q only at DH 128, which reads the gate from
+    global memory), 4 K | V stages of 128 keys (2 at DH 128), 128 B of barriers and two slots of key codes, one byte per key
+    rounded up to the 128-key block"""
+    stages = 2 if dh == 128 else 4
+    tile = 128 * dh * 2
+    slot = tile if dh == 128 else 2 * tile
+    return 2 * slot + stages * 2 * tile + 128 + 2 * ((nk + 127) // 128 * 128)
+
+
+def test_attention_forward_key_length_rule(lib):
+    """the longest key length af2_attention_forward accepts is the last 128-key block that fits the 232,448 B of shared memory
+    a CTA can use; one query without a bias (the pointwise template kernel) has no such limit"""
+    limit = 232448
+    for dh in (16, 32, 64, 128):
+        jmax = (limit - _attn_smem(dh, 0)) // 2 // 128 * 128
+        assert _attn_smem(dh, jmax) <= limit < _attn_smem(dh, jmax + 1)
+        for bias_batch in (0, 1, 2):
+            assert lib.af2_attention_forward_workspace(2, 2, jmax, 64, 4, dh, 0, bias_batch) > 0, (dh, jmax)
+            assert lib.af2_attention_forward_workspace(2, 2, jmax + 1, 64, 4, dh, 0, bias_batch) < 0, (dh, jmax + 1)
+        assert lib.af2_attention_forward_workspace(2, 1, 4 * jmax, 64, 4, dh, 0, 0) > 0, "one query without bias: pointwise"
+        assert lib.af2_attention_forward_workspace(2, 1, jmax + 1, 64, 4, dh, 0, 1) < 0, "one query with a bias: general kernel"
+
+
 def test_product_never_imports_oracle():
     for dirpath, _, files in os.walk(os.path.join(ROOT, "alphafold2_b200")):
         for f in files:

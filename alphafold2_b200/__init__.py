@@ -8,9 +8,10 @@ from .alphafold2 import (Alphafold2, Evoformer, EvoformerBlock, PairwiseAttentio
                          attach_structure_module, recycle)
 from .ops import set_precision
 from .rotary import apply_rotary_pos_emb, rotate_every_two, FixedPositionalEmbedding, AxialRotaryEmbedding
+from . import utils
 
 __all__ = ["Alphafold2", "Evoformer", "EvoformerBlock", "PairwiseAttentionBlock", "MsaAttentionBlock",
            "AxialAttention", "Attention", "TriangleMultiplicativeModule", "OuterMean", "FeedForward",
            "ReturnValues", "Recyclables", "apply_rotary_pos_emb", "rotate_every_two",
            "FixedPositionalEmbedding", "AxialRotaryEmbedding", "invalidate_packed", "set_precision", "IPABlock",
-           "InvariantPointAttention", "attach_structure_module", "recycle"]
+           "InvariantPointAttention", "attach_structure_module", "recycle", "utils"]

@@ -227,6 +227,10 @@ _SIGNATURES = {
     "af2_peer_error": (ci, [vp]),
     "af2_peer_exchange": (ci, [vp, ll, ll, vp, ll, ll, ci, ll, ci, ci, ci, vp]),
     "af2_peer_exchange_chunks": (ci, [vp, ll, C.POINTER(PeerChunk), vp, ci, ci, ci, vp]),
+    # distogram to coordinates (utils.py:718-833)
+    "af2_center_distogram": (ci, [vp, vp, cf, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
+    "af2_mds_workspace": (ll, [ci, ci, ci]),
+    "af2_mds_iterate": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, C.c_double, vp, ll, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

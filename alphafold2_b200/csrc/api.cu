@@ -25,6 +25,7 @@
 #include "template_attn.cuh"
 #include "heads.cuh"
 #include "structure.cuh"
+#include "geometry.cuh"
 
 using namespace af2;
 
@@ -1739,3 +1740,4 @@ int af2_contract_tail(const float* src, long long chan_stride, int pitch, int ro
 #include "attention_api.inl"
 #include "heads_api.inl"
 #include "structure_api.inl"
+#include "geometry_api.inl"

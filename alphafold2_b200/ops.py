@@ -1757,3 +1757,96 @@ def _pair_projection(pk: Packed, x: torch.Tensor, out: torch.Tensor, band: Optio
         if scratch is not None:
             os_[r0:r1].copy_(dst)
     return out
+
+
+# --------------------------------------------------------------------------------------------------
+# distogram to coordinates (alphafold2_pytorch/utils.py:718-833)
+# --------------------------------------------------------------------------------------------------
+CENTER_MODES = {"mean": 0, "median": 1}
+MAX_BINS = 128           # csrc/geometry.cuh: CD_MAX_BINS
+MDS_MAX_N = 12288        # csrc/geometry.cuh: MDS_MAX_N
+
+
+def wide_mode(wide) -> int:
+    """0 std, 1 var, 2 none: like the reference, any other value means no dispersion (utils.py:751-756)."""
+    return {"std": 0, "var": 1}.get(wide, 2) if isinstance(wide, str) else 2
+
+
+def bin_centres(bins: torch.Tensor, device) -> torch.Tensor:
+    """utils.py:733-735, the same torch lines: bins - half a bin width, the first centre 1.5 and the last 1.33 * bins[-1]."""
+    c = (bins - 0.5 * (bins[2] - bins[1])).to(device)
+    c[0] = 1.5
+    c[-1] = 1.33 * bins[-1]
+    return c.float().contiguous()
+
+
+def check_bins(bins: torch.Tensor, nb: int):
+    if bins.dim() != 1 or bins.shape[0] != nb:
+        raise ValueError(f"bins must be a 1-D tensor of the distogram's {nb} buckets, got {tuple(bins.shape)}")
+    if not 3 <= nb <= MAX_BINS:
+        raise ValueError(f"the distogram kernel takes 3 to {MAX_BINS} bins, got {nb}")
+
+
+def center_distogram(dist: torch.Tensor, bins: torch.Tensor, center: str = "mean", wide="std", softmax: bool = False,
+                     mask: Optional[torch.Tensor] = None):
+    """center_distogram_torch (utils.py:718-764) in one pass over dist [B, N, N, nb] fp32 -> (central, weights) [B, N, N] fp32.
+    softmax: dist holds logits, normalised on chip.  mask [B, N]: a pair with a masked residue gets weight 0."""
+    if dist.dim() != 4 or dist.shape[1] != dist.shape[2]:
+        raise ValueError(f"distogram must be [b, N, N, bins], got {tuple(dist.shape)}")
+    B, n, _, nb = dist.shape
+    check_bins(bins, nb)
+    if center not in CENTER_MODES:
+        raise ValueError(f"center must be one of {tuple(CENTER_MODES)}, got {center!r}")
+    mask = _mask_u8(mask, (B, n), "mask")
+    _require(dist, torch.float32, "distogram")
+    thr = float(bins[-2])
+    centres = bin_centres(bins, dist.device)
+    if mask is not None:
+        mask = mask.to(dist.device)
+    central = torch.empty(B, n, n, dtype=torch.float32, device=dist.device)
+    weights = torch.empty_like(central)
+    _lib.check(_lib.load().af2_center_distogram(dist.data_ptr(), centres.data_ptr(), thr, _ptr(mask), central.data_ptr(),
+                                                weights.data_ptr(), B, n, nb, CENTER_MODES[center], wide_mode(wide), int(bool(softmax)),
+                                                _stream_ptr()))
+    return central, weights
+
+
+def mds_init(pre_dist_mat: torch.Tensor) -> torch.Tensor:
+    """mds_torch's initialisation (utils.py:789-798), the same torch lines on the device: the top singular vectors of
+    M = 0.5 (D[:, :1, :] + D[:, :, :1] - D), D = pre_dist_mat^2, by torch.svd_lowrank (randomised: it draws from the RNG of
+    the tensor's device), scaled by sqrt|s| -> [B, N, 3] fp32.  Below 3 points svd_lowrank gives fewer columns: the rest are 0."""
+    D = pre_dist_mat ** 2
+    M = 0.5 * (D[:, :1, :] + D[:, :, :1] - D)
+    svds = [torch.svd_lowrank(mi) for mi in M]
+    u = torch.stack([s[0] for s in svds], dim=0)
+    s = torch.stack([s[1] for s in svds], dim=0)
+    x = torch.bmm(u, torch.diag_embed(s).abs().sqrt())[..., :3]
+    if x.shape[-1] < 3:
+        x = torch.nn.functional.pad(x, (0, 3 - x.shape[-1]))
+    return x.float().contiguous()
+
+
+def mds_iterate_(delta: torch.Tensor, weights: Optional[torch.Tensor], x: torch.Tensor, iters: int, tol: float):
+    """The SMACOF loop of mds_torch (utils.py:805-831) in one cooperative launch with no host synchronisation inside: delta and
+    weights [B, N, N] fp32 (weights None: all ones), x [B, N, 3] fp32 in: the init, out (in place): the coords the reference
+    returns.  Reads the step count once at the end and returns (steps, stopped, his [steps + 1 + stopped, B] fp64,
+    stress [steps + stopped, B] fp64): his[0] = inf, his[k + 1] = stress_k / |X_k'|; the last row is that of the iteration
+    that stopped the loop when stopped."""
+    _require(delta, torch.float32, "pre_dist_mat")
+    _require(x, torch.float32, "x")
+    if weights is not None:
+        _require(weights, torch.float32, "weights")
+    B, n, _ = delta.shape
+    lib = _lib.load()
+    need = lib.af2_mds_workspace(B, n, int(iters))
+    if need < 0:
+        _lib.check(-1)
+    dev = delta.device
+    his = torch.empty(int(iters) + 1, B, dtype=torch.float64, device=dev)
+    stress = torch.empty(max(int(iters), 1), B, dtype=torch.float64, device=dev)
+    steps = torch.empty(2, dtype=torch.int32, device=dev)
+    ws = workspace(need, dev)
+    _lib.check(lib.af2_mds_iterate(delta.data_ptr(), _ptr(weights), x.data_ptr(), his.data_ptr(), stress.data_ptr(), steps.data_ptr(),
+                                   B, n, int(iters), float(tol), ws.data_ptr(), ws.numel(), _stream_ptr()))
+    k, stopped = (int(v) for v in steps.tolist())
+    return k, bool(stopped), his[:k + 1 + stopped], stress[:k + stopped]

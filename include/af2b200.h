@@ -708,6 +708,29 @@ int af2_structure_layer_rows_end(const af2_structure_weights* w, float* single, 
                                  float* coords, float* confidence, int n, int d, int heads, float eps, void* workspace,
                                  long long workspace_bytes, af2_stream_t stream);
 
+/* Distogram to coordinates (alphafold2_pytorch/utils.py:718-833, center_distogram_torch and mds_torch).
+ * af2_center_distogram: one pass over dist [B][n][n][nb] fp32 (probabilities; logits when softmax != 0, normalised on chip)
+ *   -> central, weights [B][n][n] fp32.  centres [nb] are the bin centres (the reference's n_bins), thr = bins[nb - 2].
+ *   center 0 mean (sum p c / sum p), 1 median (first bin whose running sum reaches half the total, clamped to the last bin);
+ *   wide 0 std, 1 var, 2 none.  weight = (central <= thr) / (1 + dispersion); on the diagonal central and weight are
+ *   multiplied by 0 (a NaN stays NaN, as in the reference: a pair whose bins sum to 0 has NaN mean and weight).
+ *   mask [B][n] (1-byte bools) or NULL: a pair with a masked residue gets weight 0.  3 <= nb <= 128, dist 16-byte aligned;
+ *   otherwise AF2_ERR_BAD_ARG.  No workspace.
+ * af2_mds_iterate: the SMACOF loop of mds_torch, one cooperative launch, no host synchronisation.  delta, w [B][n][n] fp32
+ *   (w NULL: all ones); x [B][n][3] fp32, in: the init, out: the coords the loop returns (the last accepted ones).
+ *   Iteration k: dist_ij = |x_i - x_j| from direct differences, stress = 0.5 sum_ij w (dist - delta)^2 (diagonal included),
+ *   x'_i = (1 / n) sum_j r_ij (x_i - x_j) with r_ij = w_ij (delta_ij / dist'_ij), dist' = dist + 1e-7 where dist <= 0;
+ *   val = stress / |X'|_F (fp64 sums in a fixed order: bitwise reproducible).  The loop stops at k when
+ *   mean_b(his[k] - val) <= tol, keeping the previous coords; otherwise his[k + 1] = val and X = X'.
+ *   his [iters + 1][B] fp64 (his[0] = inf; row k + 1 is written for every evaluated iteration k, including the one that
+ *   stops), stress [iters][B] fp64 (same rows), steps [2] int: accepted iterations and 1 if the loop stopped on tol.
+ *   1 <= n <= 12288, B >= 1, iters >= 0; workspace af2_mds_workspace(B, n, iters) bytes (negative: shape refused). */
+int af2_center_distogram(const float* dist, const float* centres, float thr, const unsigned char* mask, float* central, float* weights,
+                         int B, int n, int nb, int center, int wide, int softmax, af2_stream_t stream);
+long long af2_mds_workspace(int B, int n, int iters);
+int af2_mds_iterate(const float* delta, const float* w, float* x, double* his, double* stress, int* steps, int B, int n, int iters,
+                    double tol, void* workspace, long long workspace_bytes, af2_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

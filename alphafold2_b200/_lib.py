@@ -76,6 +76,15 @@ class StructureWeights(C.Structure):
                                   "b_points", "w_lddt", "b_lddt")]
 
 
+class Points(C.Structure):
+    """af2_points: coordinate k of point i of element e at p[e * sb + i * sn + k * sk]."""
+    _fields_ = [("p", vp), ("sb", ll), ("sn", ll), ("sk", ll)]
+
+
+class GdtSpec(C.Structure):
+    _fields_ = [("out", vp), ("k", ci), ("idx", ci * 8), ("w", cf * 8)]
+
+
 class PeerChunk(C.Structure):
     _fields_ = [("src_off", ll), ("dst_off", ll), ("dst_row_stride", ll), ("row_bytes", ll), ("rows", ci), ("reserved", ci)]
 
@@ -231,6 +240,12 @@ _SIGNATURES = {
     "af2_center_distogram": (ci, [vp, vp, cf, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
     "af2_mds_workspace": (ll, [ci, ci, ci]),
     "af2_mds_iterate": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, C.c_double, vp, ll, vp]),
+    # structure scores (utils.py:999-1247)
+    "af2_metrics_workspace": (ll, [ci, ci]),
+    "af2_pair_distance_scores": (ci, [ci, C.POINTER(Points), ci, C.POINTER(Points), ci, vp, ll, ll, ci, ci, cf, cf, cf, cf, vp, vp, ll,
+                                      vp]),
+    "af2_superpose_scores": (ci, [C.POINTER(Points), C.POINTER(Points), vp, ll, ll, ci, ci, ci, ci, C.POINTER(Points),
+                                  C.POINTER(Points), vp, vp, vp, ci, C.POINTER(cf), C.POINTER(GdtSpec), ci, vp, vp, vp, ll, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -26,6 +26,7 @@
 #include "heads.cuh"
 #include "structure.cuh"
 #include "geometry.cuh"
+#include "metrics.cuh"
 
 using namespace af2;
 
@@ -1741,3 +1742,4 @@ int af2_contract_tail(const float* src, long long chan_stride, int pitch, int ro
 #include "heads_api.inl"
 #include "structure_api.inl"
 #include "geometry_api.inl"
+#include "metrics_api.inl"

@@ -1850,3 +1850,93 @@ def mds_iterate_(delta: torch.Tensor, weights: Optional[torch.Tensor], x: torch.
                                    B, n, int(iters), float(tol), ws.data_ptr(), ws.numel(), _stream_ptr()))
     k, stopped = (int(v) for v in steps.tolist())
     return k, bool(stopped), his[:k + 1 + stopped], stress[:k + stopped]
+
+
+# --------------------------------------------------------------------------------------------------
+# structure scores (alphafold2_pytorch/utils.py:999-1247)
+# --------------------------------------------------------------------------------------------------
+MAX_CUTOFFS = 8          # csrc/metrics.cuh: SS_MAX_CUT
+
+
+def _points(t: Optional[torch.Tensor], strides=None):
+    """af2_points of a [B, n, 3]-like view: strides (sb, sn, sk) in elements, default the view's own."""
+    if t is None:
+        return None
+    sb, sn, sk = t.stride() if strides is None else strides
+    return _lib.Points(t.data_ptr(), sb, sn, sk)
+
+
+def _byref(s):
+    return None if s is None else C.byref(s)
+
+
+def _f32_view(t: torch.Tensor, name: str):
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor (alphafold2_b200 has no CPU fallback)")
+    if t.dtype != torch.float32:
+        raise TypeError(f"{name} must be float32, got {t.dtype}")
+
+
+def metrics_workspace(B: int, n: int, device) -> torch.Tensor:
+    need = _lib.load().af2_metrics_workspace(int(B), int(n))
+    if need < 0:
+        _lib.check(-1)
+    return workspace(need, device)
+
+
+def superpose_scores(x, y, B: int, n: int, *, mask=None, mask_strides=(0, 0), align=False, shift=False, out_x=None, out_y=None,
+                     rot=None, rmsd=None, tm=None, cutoffs=(), gdt=(), lddt=None, lddt_mean=None, lddt_points=None, r0=15.0):
+    """af2_superpose_scores, preceded by the lDDT pair pass when lddt_points = (true, predicted) is given, on one workspace.
+    x, y: fp32 CUDA views [B, n, 3] (any strides; the [B, 3, n] layouts are passed as their transposes), or None for lDDT
+    alone.  mask: uint8/bool [B, n]-strided selection (mask_strides in elements) or None.  Outputs are preallocated
+    tensors written in place: out_x / out_y [B, n, 3] views, rot [B, 3, 3] fp64, rmsd / tm / lddt_mean [B] fp32,
+    lddt [B, n] fp32.  gdt: up to two (out [B] fp32, cutoff indices, weights)."""
+    for t, name in ((x, "x"), (y, "y")):
+        if t is not None:
+            _f32_view(t, name)
+    outs = [t for t in (rmsd, tm, lddt, lddt_mean) if t is not None] + [g[0] for g in gdt]
+    for t in outs:
+        _require(t, torch.float32, "output")
+    dev = (x if x is not None else lddt_points[0]).device
+    lib = _lib.load()
+    ws = metrics_workspace(B, n, dev)
+    mptr = _ptr(mask)
+    if lddt_points is not None:
+        tp, pp = lddt_points
+        _f32_view(tp, "true_coords")
+        _f32_view(pp, "pred_coords")
+        _lib.check(lib.af2_pair_distance_scores(0, C.byref(_points(tp)), 0, C.byref(_points(pp)), 0, mptr, mask_strides[0],
+                                                mask_strides[1], B, n, float(r0), float("-inf"), float("inf"), 2.0, None,
+                                                ws.data_ptr(), ws.numel(), _stream_ptr()))
+    cut = (C.c_float * MAX_CUTOFFS)(*[float(c) for c in cutoffs])
+    specs = (_lib.GdtSpec * 2)()
+    for g, (out, idx, w) in enumerate(gdt):
+        specs[g].out = out.data_ptr()
+        specs[g].k = len(idx)
+        for k, (i, wk) in enumerate(zip(idx, w)):
+            specs[g].idx[k] = int(i)
+            specs[g].w[k] = float(wk)
+    _lib.check(lib.af2_superpose_scores(_byref(_points(x)), _byref(_points(y)), mptr, mask_strides[0], mask_strides[1], B, n,
+                                        int(bool(align)), int(bool(shift)), _byref(_points(out_x)), _byref(_points(out_y)),
+                                        _ptr(rot), _ptr(rmsd), _ptr(tm), len(cutoffs), cut, specs, int(lddt is not None),
+                                        _ptr(lddt), _ptr(lddt_mean), ws.data_ptr(), ws.numel(), _stream_ptr()))
+
+
+def distmat_loss(a, a_matrix: bool, b, b_matrix: bool, B: int, n: int, mask=None, lo=float("-inf"), hi=float("inf"), q=2.0):
+    """af2_pair_distance_scores in loss mode: a, b are fp32 CUDA views, coordinates [Bx, n, 3] or matrices [Bx, n, n] with
+    Bx 1 (shared by the batch) or B; mask bool [B, n, n] contiguous or None -> the mean loss, a 0-d fp32 tensor."""
+    _f32_view(a, "X")
+    _f32_view(b, "Y")
+    out = torch.empty((), dtype=torch.float32, device=a.device)
+    _require(out, torch.float32, "loss")
+    if mask is not None and not mask.is_contiguous():
+        mask = mask.contiguous()
+
+    def pts(t, mat):
+        sb = 0 if t.shape[0] == 1 else t.stride(0)
+        return _lib.Points(t.data_ptr(), sb, t.stride(1), 0 if mat else t.stride(2))
+    ws = metrics_workspace(B, n, a.device)
+    _lib.check(_lib.load().af2_pair_distance_scores(1, C.byref(pts(a, a_matrix)), int(a_matrix), C.byref(pts(b, b_matrix)),
+                                                    int(b_matrix), _ptr(mask), n * n, n, B, n, 15.0, float(lo), float(hi),
+                                                    float(q), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
+    return out

@@ -6,15 +6,24 @@ The centring runs as one kernel over the distogram and the SMACOF loop as one co
 on the device (csrc/geometry.cuh).  Return values, shapes and the reference's numerical quirks are kept (DESIGN.md §14).
 Differences: per-iteration lines are printed after the loop from the recorded history, the mirror check stays on the
 device, and inputs the reference would crash on raise ValueError before any device work.  ``coords_from_distogram`` is
-the one addition: distogram logits straight to coordinates.
+one addition: distogram logits straight to coordinates.
+
+The structure scores of utils.py:999-1247 (kabsch_torch / Kabsch, rmsd_torch / RMSD, gdt_torch / GDT, tmscore_torch /
+TMscore, lddt_ca_torch, distmat_loss_torch) run as two kernels (csrc/metrics.cuh): a pass over the pairs for lDDT and the
+loss, and one CTA per structure for the superposition and the per-point scores.  Names, layouts, return dtypes and the
+reference's quirks are kept (DESIGN.md §4d); ``score_coords`` scores a batch of predictions in the model's layout.
 """
+from dataclasses import dataclass
+
 import torch
 
 from . import ops
-from .alphafold2 import DISTOGRAM_BUCKETS
+from .alphafold2 import DISTOGRAM_BUCKETS, _forward_only
 
 __all__ = ["DISTANCE_THRESHOLDS", "center_distogram_torch", "mds_torch", "mdscaling_torch", "get_dihedral_torch",
-           "calc_phis_torch", "MDScaling", "coords_from_distogram"]
+           "calc_phis_torch", "MDScaling", "coords_from_distogram", "kabsch_torch", "Kabsch", "rmsd_torch", "RMSD",
+           "gdt_torch", "GDT", "tmscore_torch", "TMscore", "lddt_ca_torch", "distmat_loss_torch", "StructureScores",
+           "score_coords"]
 
 DISTANCE_THRESHOLDS = torch.linspace(2, 20, steps=DISTOGRAM_BUCKETS)
 
@@ -168,3 +177,259 @@ def coords_from_distogram(distance_logits, mask=None, iters=10, tol=1e-5, center
     bins = torch.linspace(2, 20, steps=nb)
     central, weights = ops.center_distogram(_f32(logits), bins, center=center, wide=wide, softmax=True, mask=mask)
     return _smacof(central, weights, int(iters), tol, 0)
+
+
+# --------------------------------------------------------------------------------------------------
+# structure scores (utils.py:999-1247)
+# --------------------------------------------------------------------------------------------------
+GDT_TS_CUTOFFS = (1, 2, 4, 8)
+GDT_HA_CUTOFFS = (0.5, 1, 2, 4)
+
+
+def _scored(t, name: str) -> torch.Tensor:
+    """The fp32 tensor the kernels read (a view when t is already fp32); CPU tensors and autograd inputs are refused."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor (alphafold2_b200 has no CPU fallback)")
+    if not t.is_floating_point():
+        raise TypeError(f"{name} must be a floating tensor, got {t.dtype}")
+    _forward_only(t)
+    return t.detach() if t.dtype == torch.float32 else t.detach().float()
+
+
+def _bdn(X, Y):
+    """expand_arg_dims (utils.py:68-81): A, B of equal rank, [3, N] -> [1, 3, N]; then [B, 3, N] with N >= 1."""
+    if not isinstance(X, torch.Tensor) or not isinstance(Y, torch.Tensor):
+        raise TypeError("A and B must be torch.Tensors")
+    if X.dim() != Y.dim():
+        raise ValueError(f"Shapes of A and B must match: {tuple(X.shape)} and {tuple(Y.shape)}")
+    if X.dim() == 2:
+        X, Y = X[None], Y[None]
+    if X.dim() != 3 or X.shape != Y.shape or X.shape[1] != 3:
+        raise ValueError(f"A and B must both be [B, 3, N] or [3, N], got {tuple(X.shape)} and {tuple(Y.shape)}")
+    if X.shape[-1] == 0:
+        raise ValueError("A and B have no points")
+    return X, Y
+
+
+def _backend(A, backend):
+    if backend == "auto":
+        backend = "torch" if isinstance(A, torch.Tensor) else "numpy"
+    if backend != "torch":
+        raise NotImplementedError(f"only the torch backend runs here (got {backend!r})")
+
+
+def kabsch_torch(X, Y, cpu=True):
+    """utils.py:999-1029 -- Kabsch alignment of X into Y, both [3, N] -> (X centred and rotated, Y centred), each [3, N].
+    C = X_ Y_^T = V S W; when det V det W < 0 the last column of V is negated; U = V W; X_aligned = U^T X_.  The covariance
+    and the SVD are fp64 on the device; ``cpu`` is accepted and has no effect (nothing goes to the host)."""
+    if not isinstance(X, torch.Tensor) or not isinstance(Y, torch.Tensor):
+        raise TypeError("X and Y must be torch.Tensors")
+    if X.dim() != 2 or X.shape != Y.shape or X.shape[0] != 3:
+        raise ValueError(f"X and Y must both be [3, N], got {tuple(X.shape)} and {tuple(Y.shape)}")
+    if X.shape[1] == 0:
+        raise ValueError("X and Y have no points")
+    x, y = _scored(X, "X"), _scored(Y, "Y")
+    n = X.shape[1]
+    ax = torch.empty(3, n, dtype=torch.float32, device=x.device)
+    ay = torch.empty_like(ax)
+    ops.superpose_scores(x.t()[None], y.t()[None], 1, n, align=True, out_x=ax.t()[None], out_y=ay.t()[None])
+    return ax.to(X.dtype), ay.to(Y.dtype)
+
+
+def Kabsch(A, B, backend="auto"):
+    """utils.py:1281-1294 -- kabsch_torch on A, B [3, N].  Only 2-D input: any other rank raises ValueError."""
+    _backend(A, backend)
+    if not isinstance(B, torch.Tensor) or A.dim() != B.dim():
+        raise ValueError("Shapes of A and B must match.")
+    return kabsch_torch(A, B)
+
+
+def _scores(X, Y, *, rmsd=False, tm=False, cutoffs=(), weights=None):
+    """One superpose_scores launch over [B, 3, N] pairs as given (no alignment)."""
+    X, Y = _bdn(X, Y)
+    x, y = _scored(X, "X"), _scored(Y, "Y")
+    b, n = X.shape[0], X.shape[2]
+    new = lambda: torch.empty(b, dtype=torch.float32, device=x.device)  # noqa: E731
+    out = {"rmsd": new() if rmsd else None, "tm": new() if tm else None, "gdt": new() if cutoffs else None}
+    gdt = ()
+    if cutoffs:
+        gdt = ((out["gdt"], range(len(cutoffs)), [1.0] * len(cutoffs) if weights is None else weights),)
+    ops.superpose_scores(x.transpose(1, 2), y.transpose(1, 2), b, n, rmsd=out["rmsd"], tm=out["tm"], cutoffs=cutoffs, gdt=gdt)
+    return out
+
+
+def rmsd_torch(X, Y):
+    """utils.py:1098-1100 -- sqrt of the mean of (X - Y)^2 over both the 3 and the N axes (the usual RMSD over sqrt 3), for
+    X, Y [B, 3, N] (or [3, N]) -> [B] in X's dtype."""
+    return _scores(X, Y, rmsd=True)["rmsd"].to(X.dtype)
+
+
+def RMSD(A, B, backend="auto"):
+    """utils.py:1296-1308 -- rmsd_torch on [B, 3, N] or [3, N] -> [B]."""
+    _backend(A, backend)
+    return rmsd_torch(A, B)
+
+
+def gdt_torch(X, Y, cutoffs, weights=None):
+    """utils.py:1106-1123 -- sum_k w_k GDT_k / K with GDT_k the fraction of points with |X - Y| <= cutoffs[k] (not normalised
+    by the weights: it can exceed 1), X, Y [B, 3, N] (or [3, N]) -> [B] fp32.  weights: K numbers or None for ones."""
+    cutoffs = [float(c) for c in cutoffs]
+    if not 1 <= len(cutoffs) <= ops.MAX_CUTOFFS:
+        raise ValueError(f"GDT takes 1 to {ops.MAX_CUTOFFS} cutoffs, got {len(cutoffs)}")
+    if weights is not None:
+        weights = [float(w) for w in (weights.tolist() if isinstance(weights, torch.Tensor) else weights)]
+        if len(weights) != len(cutoffs):
+            raise ValueError(f"{len(weights)} GDT weights for {len(cutoffs)} cutoffs")
+    return _scores(X, Y, cutoffs=cutoffs, weights=weights)["gdt"]
+
+
+def GDT(A, B, *, mode="TS", cutoffs=[1, 2, 4, 8], weights=None, backend="auto"):  # noqa: B006 (the reference's signature)
+    """utils.py:1310-1327 -- gdt_torch with the cutoffs of ``mode``: "HA" / "ha" 0.5, 1, 2, 4, anything else 1, 2, 4, 8.
+    The ``cutoffs`` argument is ignored, as in the reference."""
+    _backend(A, backend)
+    return gdt_torch(A, B, GDT_HA_CUTOFFS if mode in ["HA", "ha"] else GDT_TS_CUTOFFS, weights=weights)
+
+
+def tmscore_torch(X, Y):
+    """utils.py:1143-1150 -- mean of 1 / (1 + (d / d0)^2), L = max(15, N), d0 = 1.24 (L - 15)^(1/3) - 1.8 without a lower
+    clamp (negative for N <= 18), on the points as given (no superposition search), X, Y [B, 3, N] -> [B] in X's dtype."""
+    return _scores(X, Y, tm=True)["tm"].to(X.dtype)
+
+
+def TMscore(A, B, backend="auto"):
+    """utils.py:1329-1344 -- tmscore_torch on [B, 3, N] or [3, N] -> [B]."""
+    _backend(A, backend)
+    return tmscore_torch(A, B)
+
+
+def _bool_mask(mask, shape, name, device):
+    if not isinstance(mask, torch.Tensor):
+        mask = torch.as_tensor(mask)
+    if mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"{name} must be a bool mask, got {mask.dtype}")
+    if tuple(mask.shape) != tuple(shape):
+        raise ValueError(f"{name} must have shape {tuple(shape)}, got {tuple(mask.shape)}")
+    return mask.to(device=device, dtype=torch.bool)
+
+
+def lddt_ca_torch(true_coords, pred_coords, cloud_mask, r_0=15.):
+    """utils.py:1204-1247 -- lDDT of each C-alpha (atom 1) of sidechainnet-layout coordinates [b, L, C, 3] with cloud_mask
+    [b, L, C] -> [b, L] in true_coords' dtype.  Only CAs present in the mask take part.  Residue i: the pairs with a true
+    distance < r_0 (itself included) each score #{t in 0.5, 1, 2, 4 : |d_pred - d_true| <= t}; lddt = (sum - 4) /
+    (4 count - 4) in fp32.  A residue without a CA scores 0; one with no other CA within r_0 scores NaN."""
+    for t, name in ((true_coords, "true_coords"), (pred_coords, "pred_coords")):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+    if true_coords.dim() != 4 or true_coords.shape != pred_coords.shape or true_coords.shape[-1] != 3:
+        raise ValueError(f"true_coords and pred_coords must both be [b, L, C, 3], got {tuple(true_coords.shape)} and "
+                         f"{tuple(pred_coords.shape)}")
+    b, n, c, _ = true_coords.shape
+    if c < 2:
+        raise ValueError(f"lddt_ca_torch reads the CA as atom 1: C must be at least 2, got {c}")
+    if n == 0 or b == 0:
+        raise ValueError("true_coords has no residues")
+    t, p = _scored(true_coords, "true_coords"), _scored(pred_coords, "pred_coords")
+    cm = _bool_mask(cloud_mask, (b, n, c), "cloud_mask", t.device)
+    lddt = torch.empty(b, n, dtype=torch.float32, device=t.device)
+    ca = cm[:, :, 1]
+    ops.superpose_scores(None, None, b, n, mask=ca, mask_strides=ca.stride(), lddt=lddt,
+                         lddt_points=(t[:, :, 1], p[:, :, 1]), r0=float(r_0))
+    return lddt.to(true_coords.dtype)
+
+
+def _loss_operand(coords, mat, name):
+    """-> (fp32 view [Bx, N, 3] or [Bx, N, N], is_matrix, rank of the distance matrix the reference builds, dtype)."""
+    if mat is None:
+        if not isinstance(coords, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+        t = coords.squeeze()
+        if t.dim() not in (2, 3) or t.shape[-1] != 3:
+            raise ValueError(f"{name} must be [N, 3] or [B, N, 3] after squeeze(), got {tuple(coords.shape)}")
+        return t if t.dim() == 3 else t[None], False, t.dim(), coords.dtype
+    if not isinstance(mat, torch.Tensor):
+        raise TypeError(f"{name}_mat must be a torch.Tensor")
+    if mat.dim() not in (2, 3) or mat.shape[-1] != mat.shape[-2]:
+        raise ValueError(f"{name}_mat must be [N, N] or [B, N, N], got {tuple(mat.shape)}")
+    return mat if mat.dim() == 3 else mat[None], True, mat.dim(), mat.dtype
+
+
+def distmat_loss_torch(X=None, Y=None, X_mat=None, Y_mat=None, p=2, q=2, custom=None, distmat_mask=None, clamp=None):
+    """utils.py:1057-1096 -- mean over the True entries of distmat_mask (all of them by default, diagonal included, across
+    the batch) of ((D_X - D_Y)^2)^(q / 2).  Each operand is coordinates X [N, 3] / [B, N, 3] (squeeze() applied, clamp
+    clamping the coordinates) whose Euclidean distances are computed on the fly, or a distance matrix X_mat [N, N] /
+    [B, N, N].  Returns a 0-d tensor.  No N x N matrix is built."""
+    if (X is None and X_mat is None) or (Y is None and Y_mat is None):
+        raise ValueError("The true and predicted coords or dist mats must be provided")
+    if custom is not None:
+        raise NotImplementedError("distmat_loss_torch: a custom loss is a Python callable, which cannot run inside the kernel")
+    if (X_mat is None or Y_mat is None) and p != 2:
+        raise NotImplementedError(f"distmat_loss_torch: only the Euclidean distance (p=2) is built, got p={p}")
+    a, a_mat, a_rank, a_dtype = _loss_operand(X, X_mat, "X")
+    b, b_mat, b_rank, b_dtype = _loss_operand(Y, Y_mat, "Y")
+    n = a.shape[1]
+    if b.shape[1] != n or n == 0:
+        raise ValueError(f"the two operands must have the same N >= 1, got {tuple(a.shape)} and {tuple(b.shape)}")
+    if a.shape[0] != b.shape[0] and 1 not in (a.shape[0], b.shape[0]):
+        raise ValueError(f"batch sizes {a.shape[0]} and {b.shape[0]} do not broadcast")
+    B = max(a.shape[0], b.shape[0])
+    shape = (B, n, n) if max(a_rank, b_rank) == 3 else (n, n)
+    va, vb = _scored(a, "X"), _scored(b, "Y")
+    if a_mat and va.stride(-1) != 1:
+        va = va.contiguous()
+    if b_mat and vb.stride(-1) != 1:
+        vb = vb.contiguous()
+    mask = None
+    if distmat_mask is not None:
+        mask = _bool_mask(distmat_mask, shape, "distmat_mask", va.device).reshape(B, n, n)
+    lo, hi = (float("-inf"), float("inf")) if clamp is None else clamp
+    lo = float("-inf") if lo is None else float(lo)
+    hi = float("inf") if hi is None else float(hi)
+    out = ops.distmat_loss(va, a_mat, vb, b_mat, B, n, mask=mask, lo=lo, hi=hi, q=float(q))
+    return out.to(torch.promote_types(a_dtype, b_dtype))
+
+
+@dataclass
+class StructureScores:
+    """score_coords' result.  rmsd, gdt_ts, gdt_ha, tm_score, lddt_mean [b]; lddt [b, N]; aligned [b, N, 3]."""
+    rmsd: torch.Tensor
+    gdt_ts: torch.Tensor
+    gdt_ha: torch.Tensor
+    tm_score: torch.Tensor
+    lddt: torch.Tensor
+    lddt_mean: torch.Tensor
+    aligned: torch.Tensor
+
+
+def score_coords(pred, true, mask=None) -> StructureScores:
+    """Score predicted coordinates against the true structure, per element of the batch: pred, true [b, N, 3] (or [N, 3]),
+    mask [b, N] bool selecting the residues S to score (all when None).  The composition of the mirrors on S:
+    ``A, B = Kabsch(pred[S].T, true[S].T)``; ``rmsd = RMSD(A, B)`` (the reference's: it divides by 3N, so it is the usual
+    RMSD over sqrt 3); ``gdt_ts = GDT(A, B)``, ``gdt_ha = GDT(A, B, mode="HA")``; ``tm_score = TMscore(A, B)`` (the
+    reference's formula on the RMSD-optimal superposition, not the TM-score program's search); ``lddt`` = lddt_ca_torch
+    over S with 0 outside S; ``lddt_mean`` the mean of the finite lddt over S.  ``aligned`` is the whole predicted chain
+    moved by the superposition fitted on S, in the true structure's frame.  An element with no selected residue gets NaN.
+    Two kernel launches."""
+    if not isinstance(pred, torch.Tensor) or not isinstance(true, torch.Tensor):
+        raise TypeError("pred and true must be torch.Tensors")
+    if pred.dim() == 2 and true.dim() == 2:
+        pred, true = pred[None], true[None]
+        if mask is not None and isinstance(mask, torch.Tensor) and mask.dim() == 1:
+            mask = mask[None]
+    if pred.dim() != 3 or pred.shape != true.shape or pred.shape[-1] != 3:
+        raise ValueError(f"pred and true must both be [b, N, 3] or [N, 3], got {tuple(pred.shape)} and {tuple(true.shape)}")
+    b, n, _ = pred.shape
+    if n == 0 or b == 0:
+        raise ValueError("pred has no residues")
+    x, y = _scored(pred, "pred"), _scored(true, "true")
+    m = None if mask is None else _bool_mask(mask, (b, n), "mask", x.device)
+    dev = x.device
+    new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+    rmsd, ts, ha, tm, lddt, mean, aligned = new(b), new(b), new(b), new(b), new(b, n), new(b), new(b, n, 3)
+    ops.superpose_scores(x, y, b, n, mask=m, mask_strides=(0, 0) if m is None else m.stride(), align=True, shift=True,
+                         out_x=aligned, rmsd=rmsd, tm=tm, cutoffs=GDT_TS_CUTOFFS + (0.5,),
+                         gdt=((ts, (0, 1, 2, 3), (1.0,) * 4), (ha, (4, 0, 1, 2), (1.0,) * 4)), lddt=lddt, lddt_mean=mean,
+                         lddt_points=(y, x))
+    dt = pred.dtype
+    return StructureScores(rmsd.to(dt), ts, ha, tm.to(dt), lddt.to(dt), mean.to(dt), aligned.to(dt))

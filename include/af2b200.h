@@ -731,6 +731,43 @@ long long af2_mds_workspace(int B, int n, int iters);
 int af2_mds_iterate(const float* delta, const float* w, float* x, double* his, double* stress, int* steps, int B, int n, int iters,
                     double tol, void* workspace, long long workspace_bytes, af2_stream_t stream);
 
+/* Structure scores (alphafold2_pytorch/utils.py:999-1247: kabsch_torch, rmsd_torch, gdt_torch, tmscore_torch, lddt_ca_torch and
+ * distmat_loss_torch).  af2_points: coordinate k of point i of element e at p[e * sb + i * sn + k * sk] (sb 0: one structure
+ * for the whole batch); a distance matrix operand: entry (i, j) of element e at p[e * sb + i * sn + j].
+ * Every threshold decision is taken on dist(a, b) = sqrt((dx * dx + dy * dy) + dz * dz), dx = double(a_x) - double(b_x),
+ * each operation rounded in fp64 (no FMA contraction): exactly what fp64 arithmetic decides on the fp32 inputs.
+ * af2_metrics_workspace(B, n): bytes of workspace both calls take, O(B n) (negative: shape refused).  lDDT passes its
+ *   counters from af2_pair_distance_scores to af2_superpose_scores through this workspace: give both the same buffer.
+ * af2_pair_distance_scores: one pass over the B n^2 pairs; no n x n matrix is written.
+ *   mode 0, lDDT-CA: a = true, b = predicted coordinates; mask [B][n] (strides mask_sb, mask_sn; NULL: all present) selects
+ *     the CAs that take part as i and j.  Per residue i: count = #{j : dist_true(i, j) < r0}, score = sum over those j of
+ *     #{t in 0.5, 1, 2, 4 : |dist_pred - dist_true| <= t} (j = i included), as exact int32 sums.  One launch.
+ *   mode 1, loss: a = X, b = Y, each coordinates (clamped to [lo, hi] first) or, with a_matrix / b_matrix, a stored fp32
+ *     distance matrix; mask [B][n][n] (row stride mask_sn) or NULL.  *loss = mean over the selected pairs of all elements
+ *     (diagonal included) of ((D_X - D_Y)^2)^(q / 2), in fp64 with a fixed summation order (bitwise reproducible), stored
+ *     as fp32; NaN when no pair is selected.  Two launches.
+ * af2_superpose_scores: one CTA per element over the points selected by mask (or all n), in order.
+ *   align: the reference's Kabsch: centroids and C = X_ Y_^T in fp64, C = V S W by a 3 x 3 Jacobi SVD, the last column of
+ *     V negated when det V det W < 0, U = V W; x is moved to U^T (x - mean x) and y to y - mean y, each rounded to fp32.
+ *     xo / yo (or NULL) receive them for every one of the n points, xo with mean y added back when shift; rot [B][9] (or
+ *     NULL) receives U row-major in fp64.  Without align x and y are scored as given.
+ *   Then over the selected points with d = dist(x, y): rmsd = sqrt(sum d^2 / 3 n_sel), tm = mean 1 / (1 + (d / d0)^2) with
+ *     d0 = 1.24 (max(15, n_sel) - 15)^(1/3) - 1.8 (no clamp), and per gdt[g] with out non-NULL:
+ *     out = (sum_k w_k * (#{d <= cut[idx_k]} / n_sel)) / k in fp32.  An element with no selected point gets NaN.
+ *   lddt: lddt_out [B][n] = (score - 4) / (4 count - 4) in fp32 from the counters a mode 0 call of the same (B, n) left in
+ *     the workspace, 0 where mask is 0 (NaN where no other CA lies within r0); lddt_mean [B] (or NULL) = the mean of the
+ *     finite ones among the selected points.  x may be NULL for lDDT alone.  One launch; ncut <= 8. */
+typedef struct { float* p; long long sb, sn, sk; } af2_points;
+typedef struct { float* out; int k; int idx[8]; float w[8]; } af2_gdt_spec;
+long long af2_metrics_workspace(int B, int n);
+int af2_pair_distance_scores(int mode, const af2_points* a, int a_matrix, const af2_points* b, int b_matrix,
+                             const unsigned char* mask, long long mask_sb, long long mask_sn, int B, int n, float r0, float lo,
+                             float hi, float q, float* loss, void* workspace, long long workspace_bytes, af2_stream_t stream);
+int af2_superpose_scores(const af2_points* x, const af2_points* y, const unsigned char* mask, long long mask_sb, long long mask_sn,
+                         int B, int n, int align, int shift, const af2_points* xo, const af2_points* yo, double* rot, float* rmsd,
+                         float* tm, int ncut, const float* cut, const af2_gdt_spec* gdt, int lddt, float* lddt_out,
+                         float* lddt_mean, void* workspace, long long workspace_bytes, af2_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

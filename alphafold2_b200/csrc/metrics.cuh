@@ -383,6 +383,8 @@ __global__ void __launch_bounds__(SS_THREADS) superpose_scores_kernel(SuperposeP
       }
       __syncthreads();
       if (p.rot && tid < 9) p.rot[(long long)e * 9 + tid] = rot[tid / 3][tid % 3];
+    } else if (p.align && p.rot && tid < 9) {  // no selected point: no rotation, and none of the caller's memory left stale
+      p.rot[(long long)e * 9 + tid] = __longlong_as_double(0x7ff8000000000000LL);
     }
     // 3. d0 of the reference's TM-score on the selected points: L = max(15, n), no lower clamp
     const double d0 = 1.24 * pow((double)((nsel > 15 ? nsel : 15) - 15), 1.0 / 3.0) - 1.8;

@@ -750,7 +750,8 @@ int af2_mds_iterate(const float* delta, const float* w, float* x, double* his, d
  *   align: the reference's Kabsch: centroids and C = X_ Y_^T in fp64, C = V S W by a 3 x 3 Jacobi SVD, the last column of
  *     V negated when det V det W < 0, U = V W; x is moved to U^T (x - mean x) and y to y - mean y, each rounded to fp32.
  *     xo / yo (or NULL) receive them for every one of the n points, xo with mean y added back when shift; rot [B][9] (or
- *     NULL) receives U row-major in fp64.  Without align x and y are scored as given.
+ *     NULL) receives U row-major in fp64, nine NaNs for an element with no selected point.  Without align x and y are
+ *     scored as given, and a non-NULL rot is refused (AF2_ERR_BAD_ARG, nothing launched).
  *   Then over the selected points with d = dist(x, y): rmsd = sqrt(sum d^2 / 3 n_sel), tm = mean 1 / (1 + (d / d0)^2) with
  *     d0 = 1.24 (max(15, n_sel) - 15)^(1/3) - 1.8 (no clamp), and per gdt[g] with out non-NULL:
  *     out = (sum_k w_k * (#{d <= cut[idx_k]} / n_sel)) / k in fp32.  An element with no selected point gets NaN.

@@ -22,8 +22,9 @@
 // query phase (after a generic -> async proxy fence), and the previous item's reads from the next item's stores.
 // Keys and queries past n read zero xn rows (TMA fill), so pad keys are K = V = 0 exactly as the attention kernel's
 // zero-filled K / V tiles; the key codes discard them.
-// Head widths 32 and 64.  Shared memory holds the K / V of all kpad keys (4 DH bytes per key) and the stage ring: at DH 64
-// n <= 384 runs with 4 stages and n <= 512 with 3 (attn_proj_max_n).
+// Head widths 32 and 64.  Shared memory holds the K / V of all kpad keys (4 DH bytes per key) and the stage ring
+// (AttnProjSmem::stages_for): at DH 64 n <= 256 runs with 4 stages and 256 < n <= 384 with 3, at DH 32 n <= 896 with 4
+// and 896 < n <= 1024 with 3 (attn_proj_max_n).
 #pragma once
 #include <float.h>
 #include "common.cuh"

@@ -20,7 +20,8 @@ from typing import Optional
 import torch
 from torch import nn
 
-from . import ops
+from . import banded, ops
+from .stages import CudaStageOps
 
 # constants of alphafold2_pytorch/constants.py:5-15 that the constructor defaults depend on
 MAX_NUM_MSA = 20
@@ -451,8 +452,6 @@ class PairwiseAttentionBlock(nn.Module):
         if not x.is_cuda or ops.precision_of(self.outer_mean) == "strict":
             msa_rows = None                       # strict mode (a parity mode) runs whole
         if band < x.shape[1] or msa_rows is not None:
-            from . import banded
-            from .parallel import CudaStageOps
             st = CudaStageOps()
             mask = mask.bool().contiguous() if exists(mask) else None
             msa_mask = msa_mask.bool().contiguous() if exists(msa_mask) else None
@@ -518,8 +517,6 @@ class EvoformerBlock(nn.Module):
         self.last_pair_band = band
         self.last_msa_band = msa_band
         if msa_band < m.shape[1]:
-            from . import banded
-            from .parallel import CudaStageOps
             mmk = msa_mask.bool().contiguous() if exists(msa_mask) else None
             for b in range(x.shape[0]):
                 banded.msa_track_(msa_attn, msa_ff, m[b], None if mmk is None else mmk[b], x[b], msa_band, CudaStageOps())
@@ -528,8 +525,6 @@ class EvoformerBlock(nn.Module):
             msa_ff.add_to_(m)
         attn.update_(x, mask, m, msa_mask, band=band, msa_band=msa_band)
         if band < x.shape[1]:
-            from . import banded
-            from .parallel import CudaStageOps
             for b in range(x.shape[0]):
                 banded.feed_forward_(ff, x[b], band, CudaStageOps())
         else:

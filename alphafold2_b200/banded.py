@@ -8,7 +8,8 @@ its workspace for one band only, and the stages keep between bands just what the
                      af2_outer_contract(row0, rows), which computes the band's normaliser rows itself
   triangle multiply  L, R and the output gate of EVERY band first (they all read the pre-update x), into whole-tensor
                      operands; then the contraction band by band.  Outgoing: the band's rows of L against all of R.
-                     Ingoing: all of L against the column window R[c][k][i0:i1] (af2_triangle_contract_pitched)
+                     Ingoing: all of L against the column window R[c][k][i0:i1], read in place (af2_triangle_contract
+                     takes the operands' pitches)
   row attention      the pair bias of the whole x once, before any band updates x; then each row band
   column attention   the bias once; per column band a compact copy of x[:, j0:j1] (and its mask), attended and copied back
   pair transition    per row band (pointwise)
@@ -20,7 +21,7 @@ result is bitwise that of the whole-tensor schedule.  No FLOP is added.
 For deep MSAs the MSA track runs in bands of MSA rows as well (msa_track_): row attention per row band, column attention per
 column band after the last row band, the transition per row band, and the outer mean's projection per chunk of MSA rows.
 
-`ops` is the stage-op provider (parallel.CudaStageOps, the C ABI); tests/ drive the same schedule with oracle stage ops.
+`ops` is the stage-op provider (stages.CudaStageOps, the C ABI); tests/ drive the same schedule with oracle stage ops.
 """
 from __future__ import annotations
 
@@ -117,7 +118,7 @@ def pair_block_(pair, x: torch.Tensor, mask: Optional[torch.Tensor], m: Optional
             ops.tri_project(tm, x[i0:i1], rows_mask(i0, i1), out=(L[:, i0:i1], R[:, i0:i1], G[i0 * N:i1 * N]))
         for i0, i1 in bands:
             if ingoing:
-                ops.tri_contract_window_(tm, x[i0:i1], L, R[:, :, i0:i1], G[i0 * N:i1 * N])
+                ops.tri_contract_(tm, x[i0:i1], L[:, :, :N], R[:, :, i0:i1], G[i0 * N:i1 * N], True, 1)
             else:
                 ops.tri_contract_(tm, x[i0:i1], L[:, i0:i1], R, G[i0 * N:i1 * N], False, 1)
     del L, R, G

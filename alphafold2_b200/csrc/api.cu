@@ -976,7 +976,7 @@ int contract_tail(const ChanLnParams& cp, const void* w_out, const float* b_out,
 extern "C" {
 
 const char* af2_last_error(void) { return g_err; }
-int af2_abi_version(void) { return 3; }
+int af2_abi_version(void) { return 4; }
 
 unsigned long long af2_launch_count(void) { return g_launches; }
 
@@ -1193,6 +1193,52 @@ static int tied_args_ok(const af2_attn_weights* w, const float* x, const void* s
 }
 
 // ------------------------------------------------------------------------------------------------
+// per-channel contractions of the triangle multiplications and the outer mean
+// ------------------------------------------------------------------------------------------------
+// The contraction's fp32 product Oc [d][rows][pitch] (pitch = align4(cols), channel stride cs) and the tail's bf16 tokens
+// tn [rows * cols][d], taken from the workspace in this order.
+struct ContractOut {
+  float* Oc; __nv_bfloat16* tn; int pitch; long long cs;
+};
+
+static ContractOut take_contract_out(Arena& ar, int rows, int cols, int d) {
+  ContractOut o;
+  o.pitch = (int)align_up(cols, 4);
+  o.cs = (long long)rows * o.pitch;
+  o.Oc = ar.take<float>(d * o.cs);
+  o.tn = ar.take<__nv_bfloat16>((long long)rows * cols * d);
+  return o;
+}
+
+// O_c = A_c B_c^T for every channel c < d into Oc [c][M][ld_o] (channel stride cs_o), one batched GEMM over the channels.
+//   K-major (mn_major = 0): A [c][M][lda], B [c][N][ldb], k < K;   MN-major: A [c][K][lda] (i < M), B [c][K][ldb] (j < N).
+// Channel c of A (B) starts cs_a (cs_b) elements after channel c - 1.  A (gather_a) or B may be `pieces` gathered shards,
+// piece_stride elements apart, each holding M / pieces rows (A) or N / pieces columns (B) of O with the pitch lda (ldb).
+// One launch addresses all pieces through rank-4 tensor maps when a piece tiles the kernel's boxes (MN-major pieces of whole
+// 64-wide boxes, K-major B pieces of a multiple of 8 rows that tile BN); otherwise each piece is its own launch.
+static int launch_contract(const void* A, long long lda, long long cs_a, const void* B, long long ldb, long long cs_b,
+                           bool mn_major, int M, int N, int K, int d, int pieces, bool gather_a, long long piece_stride,
+                           float* Oc, int ld_o, long long cs_o, cudaStream_t s) {
+  GemmCall c;
+  memset(&c, 0, sizeof(c));
+  c.A = A; c.lda = lda; c.a_batch = cs_a; c.Bm = B; c.ldb = ldb; c.b_batch = cs_b; c.mn_major = mn_major;
+  c.M = M; c.N = N; c.K = K; c.batch = d; c.bn = pick_bn(N);
+  c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = Oc; c.ld_out = ld_o; c.out_batch = cs_o;
+  const int pw = (gather_a ? M : N) / pieces;
+  if (pieces > 1 && (mn_major ? pw % 64 == 0 : !gather_a && pw % 8 == 0 && (pw % c.bn == 0 || c.bn % pw == 0))) {
+    if (gather_a) { c.a_pr = pw; c.a_piece = piece_stride; }
+    else { c.b_pr = pw; c.b_piece = piece_stride; }
+    return launch_gemm(c, s);
+  }
+  const __nv_bfloat16* g = static_cast<const __nv_bfloat16*>(gather_a ? A : B);
+  for (int p = 0; p < pieces; ++p) {
+    if (gather_a) { c.A = g + p * piece_stride; c.M = pw; c.out = Oc + (long long)p * pw * ld_o; }
+    else { c.Bm = g + p * piece_stride; c.N = pw; c.bn = pick_bn(pw); c.out = Oc + (long long)p * pw; }
+    AF2_TRY(launch_gemm(c, s));
+  }
+  return AF2_OK;
+}
+
 long long af2_triangle_multiply_workspace(int B, int N, int d) {
   const long long T = (long long)B * N * N;
   const long long np8 = align_up(N, 8), np4 = align_up(N, 4);
@@ -1210,38 +1256,27 @@ int af2_triangle_multiply(const af2_trimul_weights* w, float* x, const unsigned 
   if (d % 32) return fail(AF2_ERR_BAD_ARG, "triangle_multiply: dim %d must be a multiple of 32", d);
   const long long T = (long long)B * N * N;
   if (T > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "triangle_multiply: too many tokens");
-  const int np8 = (int)align_up(N, 8), np4 = (int)align_up(N, 4);
+  const int np8 = (int)align_up(N, 8);
   const long long cs_lr = (long long)B * N * np8;   // channel stride of Lc / Rc
-  const long long cs_o = (long long)B * N * np4;    // channel stride of Oc
   Arena ar(workspace, workspace_bytes);
   __nv_bfloat16* xn = ar.take<__nv_bfloat16>(T * d);
   __nv_bfloat16* gate = ar.take<__nv_bfloat16>(T * d);
-  __nv_bfloat16* tn = ar.take<__nv_bfloat16>(T * d);
   __nv_bfloat16* Lc = ar.take<__nv_bfloat16>(d * cs_lr);
   __nv_bfloat16* Rc = ar.take<__nv_bfloat16>(d * cs_lr);
-  float* Oc = ar.take<float>(d * cs_o);
+  const ContractOut o = take_contract_out(ar, B * N, N, d);
   float* maskf = ar.take<float>(T);
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_multiply: workspace too small");
 
   // the tail projects the out gate itself when it runs fused: decided here, before the front, with the tail's own predicate
-  const ChanLnParams cp = chan_ln_params(Oc, cs_o, np4, B * N, N, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn);
+  const ChanLnParams cp = chan_ln_params(o.Oc, o.cs, o.pitch, B * N, N, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, o.tn);
   const TailGateProj gp = {xn, w->w_ogate, w->b_ogate};
   const bool project = contract_tail_fused_ok(cp, w->w_out, x, &gp);
   AF2_TRY(triangle_front(w, x, mask, T, N, np8, d, xn, maskf, Lc, Rc, cs_lr, gate, s, !project));
-  // per-channel contraction, batch = channels
+  // outgoing: O_c = L_c R_c^T, both K-major;  ingoing: O_c[i][j] = sum_k R_c[k][i] L_c[k][j], both MN-major
   for (int b = 0; b < B; ++b) {
-    GemmCall c;
-    memset(&c, 0, sizeof(c));
     const long long boff = (long long)b * N * np8;
-    if (!ingoing) {   // O_c = L_c R_c^T : both K-major (k contiguous)
-      c.A = Lc + boff; c.Bm = Rc + boff; c.mn_major = false;
-    } else {          // O_c[i][j] = sum_k R_c[k][i] L_c[k][j] : both MN-major
-      c.A = Rc + boff; c.Bm = Lc + boff; c.mn_major = true;
-    }
-    c.lda = np8; c.ldb = np8; c.a_batch = cs_lr; c.b_batch = cs_lr;
-    c.M = N; c.N = N; c.K = N; c.batch = d; c.bn = pick_bn(N);
-    c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = Oc + (long long)b * N * np4; c.ld_out = np4; c.out_batch = cs_o;
-    AF2_TRY(launch_gemm(c, s));
+    AF2_TRY(launch_contract((ingoing ? Rc : Lc) + boff, np8, cs_lr, (ingoing ? Lc : Rc) + boff, np8, cs_lr, ingoing, N, N, N, d, 1,
+                            false, 0, o.Oc + (long long)b * N * o.pitch, o.pitch, o.cs, s));
   }
   // LN over channels * out_gate -> to_out + residual
   return contract_tail(cp, w->w_out, w->b_out, x, s, project ? &gp : nullptr, project ? CTAIL_FUSED : CTAIL_AUTO);
@@ -1264,13 +1299,12 @@ int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const u
   if (d % 32) return fail(AF2_ERR_BAD_ARG, "outer_mean: dim %d must be a multiple of 32", d);
   const long long Tm = (long long)B * S * N, Tx = (long long)B * N * N;
   if (Tm > 0x7fffffffLL || Tx > 0x7fffffffLL) return fail(AF2_ERR_BAD_ARG, "outer_mean: too many tokens");
-  const int np8 = (int)align_up(N, 8), np4 = (int)align_up(N, 4);
-  const long long cs_lr = (long long)B * S * np8, cs_o = (long long)B * N * np4;
+  const int np8 = (int)align_up(N, 8);
+  const long long cs_lr = (long long)B * S * np8;
   Arena ar(workspace, workspace_bytes);
   __nv_bfloat16* mn = ar.take<__nv_bfloat16>(Tm * d);
   __nv_bfloat16* LRc = ar.take<__nv_bfloat16>(2LL * d * cs_lr);
-  float* Oc = ar.take<float>(d * cs_o);
-  __nv_bfloat16* tn = ar.take<__nv_bfloat16>(Tx * d);
+  const ContractOut o = take_contract_out(ar, B * N, N, d);
   float* maskf = ar.take<float>(Tm);
   float* scale = ar.take<float>(Tx);
   uint32_t* mwords = ar.take<uint32_t>((long long)((S + 31) / 32) * N);
@@ -1284,16 +1318,12 @@ int af2_outer_mean(const af2_outer_weights* w, float* x, const float* m, const u
   AF2_TRY(outer_front(w, m, msa_mask, Tm, N, np8, d, mn, maskf, LRc, cs_lr, s));
   // O_c[i][j] = sum_s L_c[s][i] R_c[s][j]  (MN-major operands, K = S)
   for (int b = 0; b < B; ++b) {
-    GemmCall g;
-    memset(&g, 0, sizeof(g));
-    g.A = LRc + (long long)b * S * np8; g.Bm = LRc + (long long)d * cs_lr + (long long)b * S * np8;
-    g.mn_major = true; g.lda = np8; g.ldb = np8; g.a_batch = cs_lr; g.b_batch = cs_lr;
-    g.M = N; g.N = N; g.K = S; g.batch = d; g.bn = pick_bn(N);
-    g.mode = EPI_STORE_F32; g.layout = LAYOUT_TOKEN; g.out = Oc + (long long)b * N * np4; g.ld_out = np4; g.out_batch = cs_o;
-    AF2_TRY(launch_gemm(g, s));
+    const __nv_bfloat16* Lb = LRc + (long long)b * S * np8;
+    AF2_TRY(launch_contract(Lb, np8, cs_lr, Lb + (long long)d * cs_lr, np8, cs_lr, true, N, N, S, d, 1, false, 0,
+                            o.Oc + (long long)b * N * o.pitch, o.pitch, o.cs, s));
   }
-  return contract_tail(chan_ln_params(Oc, cs_o, np4, B * N, N, d, 1, nullptr, nullptr, nullptr, msa_mask ? scale : nullptr,
-                                      1.0f / (float)S, 0.f, tn),
+  return contract_tail(chan_ln_params(o.Oc, o.cs, o.pitch, B * N, N, d, 1, nullptr, nullptr, nullptr, msa_mask ? scale : nullptr,
+                                      1.0f / (float)S, 0.f, o.tn),
                        w->w_out, w->b_out, x, s);
 }
 
@@ -1402,106 +1432,29 @@ long long af2_triangle_contract_workspace(int rows, int cols, int d) {
 }
 
 // x [rows, cols, d] (local shard, updated in place) += to_out(LN_c(O) * gate) with
-//   outgoing: O[i][j] = sum_k L[i][k] R[j][k]; L = Lc [c][rows][pitch(K)], piece p of Rg = [c][cols/pieces][pitch(K)]
-//   ingoing : O[i][j] = sum_k R[k][i] L[k][j]; L = Lc [c][K][pitch(cols)],  piece p of Rg = [c][K][pitch(rows/pieces)]
-int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, const void* Rg,
-                          long long cs_r, long long piece_stride, int pieces, const void* gate, int rows, int cols,
-                          int K, int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream) {
+//   outgoing: O[i][j] = sum_k L[i][k] R[j][k]; L = Lc [c][rows][ld_l], piece p of Rg = [c][cols/pieces][ld_r]
+//   ingoing : O[i][j] = sum_k R[k][i] L[k][j]; L = Lc [c][K][ld_l],    piece p of Rg = [c][K][ld_r] (i < rows/pieces)
+// Either operand may be a window into a larger channel-major tensor (the banded schedule's column window R[c][k][i0 .. i0 + rows)).
+int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, long long ld_l, const void* Rg,
+                          long long cs_r, long long ld_r, long long piece_stride, int pieces, const void* gate, int rows,
+                          int cols, int K, int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream) {
   NvtxRange nvtx_("af2_triangle_contract");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!w || !x || !Lc || !Rg || !gate || pieces < 1) return fail(AF2_ERR_BAD_ARG, "triangle_contract: bad argument");
+  if (rows <= 0 || cols <= 0 || K <= 0 || d % 32) return fail(AF2_ERR_BAD_ARG, "triangle_contract: rows %d cols %d K %d d %d", rows, cols, K, d);
   if ((!ingoing && cols % pieces) || (ingoing && rows % pieces)) return fail(AF2_ERR_BAD_ARG, "triangle_contract: pieces must divide the gathered axis");
-  const long long T = (long long)rows * cols;
-  const int cp4 = (int)align_up(cols, 4);
-  const long long cs_o = (long long)rows * cp4;
-  Arena ar(workspace, workspace_bytes);
-  float* Oc = ar.take<float>(d * cs_o);
-  __nv_bfloat16* tn = ar.take<__nv_bfloat16>(T * d);
-  if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_contract: workspace too small");
-  const __nv_bfloat16* L = static_cast<const __nv_bfloat16*>(Lc);
-  const __nv_bfloat16* R = static_cast<const __nv_bfloat16*>(Rg);
-  // one launch over all gathered pieces when their size tiles the kernel's boxes (rank-4 tensor maps), else one per piece
-  bool fused_pieces = false;
-  if (pieces > 1) {
-    GemmCall c;
-    memset(&c, 0, sizeof(c));
-    c.batch = d; c.K = K; c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.ld_out = cp4; c.out_batch = cs_o; c.out = Oc;
-    if (!ingoing) {
-      const int pc = cols / pieces, bn = pick_bn(cols);
-      if (pc % 8 == 0 && (pc % bn == 0 || bn % pc == 0)) {
-        c.A = L; c.lda = align_up(K, 8); c.a_batch = cs_l;
-        c.Bm = R; c.ldb = align_up(K, 8); c.b_batch = cs_r; c.b_pr = pc; c.b_piece = piece_stride;
-        c.mn_major = false; c.M = rows; c.N = cols; c.bn = bn;
-        fused_pieces = true;
-      }
-    } else {
-      const int pr = rows / pieces;
-      if (pr % 64 == 0) {
-        c.A = R; c.lda = align_up(pr, 8); c.a_batch = cs_r; c.a_pr = pr; c.a_piece = piece_stride;
-        c.Bm = L; c.ldb = align_up(cols, 8); c.b_batch = cs_l;
-        c.mn_major = true; c.M = rows; c.N = cols; c.bn = pick_bn(cols);
-        fused_pieces = true;
-      }
-    }
-    if (fused_pieces) AF2_TRY(launch_gemm(c, s));
-  }
-  for (int p = 0; p < pieces && !fused_pieces; ++p) {
-    GemmCall c;
-    memset(&c, 0, sizeof(c));
-    c.batch = d; c.K = K; c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.ld_out = cp4; c.out_batch = cs_o;
-    if (!ingoing) {
-      const int pc = cols / pieces;
-      c.A = L; c.lda = align_up(K, 8); c.a_batch = cs_l;
-      c.Bm = R + p * piece_stride; c.ldb = align_up(K, 8); c.b_batch = cs_r;
-      c.mn_major = false; c.M = rows; c.N = pc; c.bn = pick_bn(pc);
-      c.out = Oc + (long long)p * pc;
-    } else {
-      const int pr = rows / pieces;
-      c.A = R + p * piece_stride; c.lda = align_up(pr, 8); c.a_batch = cs_r;
-      c.Bm = L; c.ldb = align_up(cols, 8); c.b_batch = cs_l;
-      c.mn_major = true; c.M = pr; c.N = cols; c.bn = pick_bn(cols);
-      c.out = Oc + (long long)p * pr * cp4;
-    }
-    AF2_TRY(launch_gemm(c, s));
-  }
-  return contract_tail(chan_ln_params(Oc, cs_o, cp4, rows, cols, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
-                       w->w_out, w->b_out, x, s);
-}
-
-// af2_triangle_contract of one L / R pair with explicit pitches: the operands may be windows into larger channel-major
-// tensors (the banded single-GPU schedule contracts rows [i0, i0 + rows) of the ingoing product against the column window
-// R[c][k][i0 .. i0 + rows) of the whole R).  Same GEMM tile (pick_bn(cols)) and tail as the whole-tensor call.
-//   outgoing: L [c][rows][ld_l] (k < K), R [c][cols][ld_r] (k < K)
-//   ingoing : L [c][K][ld_l] (j < cols), R [c][K][ld_r] (i < rows)
-int af2_triangle_contract_pitched(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, long long ld_l,
-                                  const void* Rc, long long cs_r, long long ld_r, const void* gate, int rows, int cols, int K,
-                                  int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream) {
-  NvtxRange nvtx_("af2_triangle_contract_pitched");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!w || !x || !Lc || !Rc || !gate) return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: null argument");
-  if (rows <= 0 || cols <= 0 || K <= 0 || d % 32) return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: rows %d cols %d K %d d %d", rows, cols, K, d);
   if (ld_l % 8 || ld_r % 8 || cs_l % 8 || cs_r % 8)
-    return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: pitches and channel strides must be multiples of 8 elements");
-  const long long mn_l = ingoing ? cols : K, mn_r = ingoing ? rows : K;   // elements used along each operand's pitch
-  if (ld_l < mn_l || ld_r < mn_r) return fail(AF2_ERR_BAD_ARG, "triangle_contract_pitched: pitch shorter than the operand row");
-  const long long T = (long long)rows * cols;
-  const int cp4 = (int)align_up(cols, 4);
-  const long long cs_o = (long long)rows * cp4;
+    return fail(AF2_ERR_BAD_ARG, "triangle_contract: pitches and channel strides must be multiples of 8 elements");
+  const long long mn_l = ingoing ? cols : K, mn_r = ingoing ? rows / pieces : K;   // elements used along each operand's pitch
+  if (ld_l < mn_l || ld_r < mn_r) return fail(AF2_ERR_BAD_ARG, "triangle_contract: pitch shorter than the operand row");
   Arena ar(workspace, workspace_bytes);
-  float* Oc = ar.take<float>(d * cs_o);
-  __nv_bfloat16* tn = ar.take<__nv_bfloat16>(T * d);
-  if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_contract_pitched: workspace too small");
-  GemmCall c;
-  memset(&c, 0, sizeof(c));
-  c.batch = d; c.K = K; c.M = rows; c.N = cols; c.bn = pick_bn(cols);
-  c.mode = EPI_STORE_F32; c.layout = LAYOUT_TOKEN; c.out = Oc; c.ld_out = cp4; c.out_batch = cs_o;
-  if (!ingoing) {   // O_c = L_c R_c^T, both K-major
-    c.A = Lc; c.lda = ld_l; c.a_batch = cs_l; c.Bm = Rc; c.ldb = ld_r; c.b_batch = cs_r; c.mn_major = false;
-  } else {          // O_c[i][j] = sum_k R_c[k][i] L_c[k][j], both MN-major
-    c.A = Rc; c.lda = ld_r; c.a_batch = cs_r; c.Bm = Lc; c.ldb = ld_l; c.b_batch = cs_l; c.mn_major = true;
-  }
-  AF2_TRY(launch_gemm(c, s));
-  return contract_tail(chan_ln_params(Oc, cs_o, cp4, rows, cols, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, tn),
+  const ContractOut o = take_contract_out(ar, rows, cols, d);
+  if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "triangle_contract: workspace too small");
+  if (!ingoing)   // O_c = L_c R_c^T, both K-major, R gathered along j
+    AF2_TRY(launch_contract(Lc, ld_l, cs_l, Rg, ld_r, cs_r, false, rows, cols, K, d, pieces, false, piece_stride, o.Oc, o.pitch, o.cs, s));
+  else            // O_c[i][j] = sum_k R_c[k][i] L_c[k][j], both MN-major, R gathered along i
+    AF2_TRY(launch_contract(Rg, ld_r, cs_r, Lc, ld_l, cs_l, true, rows, cols, K, d, pieces, true, piece_stride, o.Oc, o.pitch, o.cs, s));
+  return contract_tail(chan_ln_params(o.Oc, o.cs, o.pitch, rows, cols, d, 0, w->on_gamma, w->on_beta, gate, nullptr, 0.f, 1e-5f, o.tn),
                        w->w_out, w->b_out, x, s);
 }
 
@@ -1545,40 +1498,17 @@ int af2_outer_contract(const af2_outer_weights* w, float* x, const void* Lc, lon
   NvtxRange nvtx_("af2_outer_contract");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!w || !x || !Lc || !Rg || pieces < 1 || N % pieces) return fail(AF2_ERR_BAD_ARG, "outer_contract: bad argument");
-  const long long T = (long long)rows * N;
-  const int np4 = (int)align_up(N, 4);
-  const long long cs_o = (long long)rows * np4;
   Arena ar(workspace, workspace_bytes);
-  float* Oc = ar.take<float>(d * cs_o);
-  __nv_bfloat16* tn = ar.take<__nv_bfloat16>(T * d);
-  float* scale = ar.take<float>(T);
+  const ContractOut o = take_contract_out(ar, rows, N, d);
+  float* scale = ar.take<float>((long long)rows * N);
   uint32_t* mwords = (S <= 4096) ? ar.take<uint32_t>((long long)((S + 31) / 32) * N) : nullptr;
   if (!ar.ok) return fail(AF2_ERR_WORKSPACE, "outer_contract: workspace too small");
   if (msa_mask_full) AF2_TRY(launch_outer_scale(msa_mask_full, scale, mwords, row0, rows, S, N, eps, s));
-  const __nv_bfloat16* L = static_cast<const __nv_bfloat16*>(Lc);
-  const __nv_bfloat16* R = static_cast<const __nv_bfloat16*>(Rg);
-  const int pc = N / pieces;
-  const bool fused_pieces = pieces > 1 && pc % 64 == 0;
-  if (fused_pieces) {   // one launch: B columns j = p * pc + jj addressed through a rank-4 map over the gathered pieces
-    GemmCall g;
-    memset(&g, 0, sizeof(g));
-    g.A = L; g.lda = align_up(rows, 8); g.a_batch = cs_l;
-    g.Bm = R; g.ldb = align_up(pc, 8); g.b_batch = cs_r; g.b_pr = pc; g.b_piece = piece_stride;
-    g.mn_major = true; g.M = rows; g.N = N; g.K = S; g.batch = d; g.bn = pick_bn(N);
-    g.mode = EPI_STORE_F32; g.layout = LAYOUT_TOKEN; g.out = Oc; g.ld_out = np4; g.out_batch = cs_o;
-    AF2_TRY(launch_gemm(g, s));
-  }
-  for (int p = 0; p < pieces && !fused_pieces; ++p) {
-    GemmCall g;
-    memset(&g, 0, sizeof(g));
-    g.A = L; g.lda = align_up(rows, 8); g.a_batch = cs_l;
-    g.Bm = R + p * piece_stride; g.ldb = align_up(pc, 8); g.b_batch = cs_r;
-    g.mn_major = true; g.M = rows; g.N = pc; g.K = S; g.batch = d; g.bn = pick_bn(pc);
-    g.mode = EPI_STORE_F32; g.layout = LAYOUT_TOKEN; g.out = Oc + (long long)p * pc; g.ld_out = np4; g.out_batch = cs_o;
-    AF2_TRY(launch_gemm(g, s));
-  }
-  return contract_tail(chan_ln_params(Oc, cs_o, np4, rows, N, d, 1, nullptr, nullptr, nullptr, msa_mask_full ? scale : nullptr,
-                                      1.0f / (float)S, 0.f, tn),
+  // both MN-major, R gathered along j
+  AF2_TRY(launch_contract(Lc, align_up(rows, 8), cs_l, Rg, align_up(N / pieces, 8), cs_r, true, rows, N, S, d, pieces, false,
+                          piece_stride, o.Oc, o.pitch, o.cs, s));
+  return contract_tail(chan_ln_params(o.Oc, o.cs, o.pitch, rows, N, d, 1, nullptr, nullptr, nullptr, msa_mask_full ? scale : nullptr,
+                                      1.0f / (float)S, 0.f, o.tn),
                        w->w_out, w->b_out, x, s);
 }
 

@@ -141,20 +141,18 @@ int af2_triangle_project(const af2_trimul_weights* w, const float* x, const unsi
                          int inner, int d, void* Lc, void* Rc, long long chan_stride, void* gate, void* workspace,
                          long long workspace_bytes, af2_stream_t stream);
 long long af2_triangle_project_workspace(long long tokens, int d);
-/* x [rows, cols, d] += to_out(LN_c(O) * gate);  Rg holds `pieces` gathered shards, piece_stride elements apart.
- *   outgoing: O[i][j] = sum_k L[i][k] R[j][k], L [c][rows][align8(K)], piece p = R rows j of shard p [c][cols/pieces][align8(K)]
- *   ingoing : O[i][j] = sum_k R[k][i] L[k][j], L [c][K][align8(cols)], piece p = R columns i of shard p [c][K][align8(rows/pieces)] */
-int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, const void* Rg,
-                          long long cs_r, long long piece_stride, int pieces, const void* gate, int rows, int cols,
-                          int K, int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);
+/* x [rows, cols, d] += to_out(LN_c(O) * gate).  L and R are channel-major: channel c starts cs_l / cs_r elements after
+ * channel c - 1, and each row of it ld_l / ld_r elements after the previous one.  Rg holds `pieces` gathered shards of R,
+ * piece_stride elements apart, each with the pitch ld_r (pieces = 1: R itself).  An operand may be a window into a larger
+ * channel-major tensor, e.g. the column window R[c][k][i0 .. i0 + rows) of a whole R.
+ *   outgoing: O[i][j] = sum_k L[i][k] R[j][k], L [c][rows][ld_l] (k < K), piece p = R rows j of shard p [c][cols/pieces][ld_r] (k < K)
+ *   ingoing : O[i][j] = sum_k R[k][i] L[k][j], L [c][K][ld_l] (j < cols), piece p = R columns i of shard p [c][K][ld_r] (i < rows/pieces)
+ * AF2_ERR_BAD_ARG on a null pointer, pieces < 1 or not dividing the gathered axis, rows / cols / K < 1, d not a multiple of
+ * 32, a pitch or channel stride not a multiple of 8 elements, or a pitch shorter than the operand row. */
+int af2_triangle_contract(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, long long ld_l, const void* Rg,
+                          long long cs_r, long long ld_r, long long piece_stride, int pieces, const void* gate, int rows,
+                          int cols, int K, int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);
 long long af2_triangle_contract_workspace(int rows, int cols, int d);
-/* af2_triangle_contract of one L / R pair with explicit pitches ld_l / ld_r (elements, multiples of 8) and channel strides
- * cs_l / cs_r: the operands may be windows into larger channel-major tensors.  Workspace: af2_triangle_contract_workspace.
- *   outgoing: L [c][rows][ld_l] (k < K), R [c][cols][ld_r] (k < K)
- *   ingoing : L [c][K][ld_l] (j < cols), R [c][K][ld_r] (i < rows; e.g. the column window R[c][k][i0 .. i0 + rows)) */
-int af2_triangle_contract_pitched(const af2_trimul_weights* w, float* x, const void* Lc, long long cs_l, long long ld_l,
-                                  const void* Rc, long long cs_r, long long ld_r, const void* gate, int rows, int cols, int K,
-                                  int d, int ingoing, void* workspace, long long workspace_bytes, af2_stream_t stream);
 /* LN + left|right projections of m [S, inner, d] (masked) -> channel-major LRc [2d][chan_stride] */
 int af2_outer_project(const af2_outer_weights* w, const float* m, const unsigned char* msa_mask, long long tokens,
                       int inner, int d, void* LRc, long long chan_stride, void* workspace, long long workspace_bytes,

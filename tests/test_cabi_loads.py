@@ -27,7 +27,7 @@ def test_header_symbols_exported(lib):
 
 
 def test_abi_version(lib):
-    assert lib.af2_abi_version() == 3
+    assert lib.af2_abi_version() == 4
     assert lib.af2_last_error() is not None
 
 
@@ -36,6 +36,43 @@ def test_workspace_queries(lib):
     assert lib.af2_axial_attention_workspace(1, 128, 256, 256, 8, 64, 1) > 0
     assert lib.af2_triangle_multiply_workspace(1, 256, 256) > 0
     assert lib.af2_outer_mean_workspace(1, 128, 256, 256) > 0
+
+
+def test_triangle_contract_refusals(lib):
+    """af2_triangle_contract refuses malformed operands with AF2_ERR_BAD_ARG before it touches them.  The pointers are never
+    read: a call that passes the argument checks stops at its empty workspace (AF2_ERR_WORKSPACE) before any launch, so the
+    well-formed controls below tell the two apart without a GPU."""
+    import ctypes as C
+    from alphafold2_b200 import _lib
+    w = _lib.TriMulWeights()
+    fake = 1 << 20
+    rows, cols, K, d = 16, 24, 24, 32
+
+    def call(ingoing=0, Lc=fake, Rg=fake, gate=fake, cs_l=None, ld_l=None, cs_r=None, ld_r=None, pieces=1, rows=rows,
+             cols=cols, K=K, d=d):
+        ld_l = ld_l if ld_l is not None else (cols if ingoing else K)
+        ld_r = ld_r if ld_r is not None else (rows // pieces if ingoing else K)
+        cs_l = cs_l if cs_l is not None else 8 * 1024
+        cs_r = cs_r if cs_r is not None else 8 * 1024
+        return lib.af2_triangle_contract(C.byref(w), fake, Lc, cs_l, ld_l, Rg, cs_r, ld_r, d * cs_r, pieces, gate, rows, cols,
+                                         K, d, ingoing, None, 0, None)
+
+    AF2_ERR_BAD_ARG, AF2_ERR_WORKSPACE = -1, -4
+    for ingoing in (0, 1):
+        assert call(ingoing) == AF2_ERR_WORKSPACE, ingoing
+        assert call(ingoing, pieces=2) == AF2_ERR_WORKSPACE, ingoing
+    assert call(1, ld_r=8, pieces=2) == AF2_ERR_WORKSPACE                  # a piece's pitch covers rows / pieces
+    bad = {
+        "null L": call(Lc=None), "null R": call(Rg=None), "null gate": call(gate=None), "pieces 0": call(pieces=0),
+        "pieces not dividing cols": call(pieces=5), "pieces not dividing rows": call(1, pieces=5),
+        "rows 0": call(rows=0), "cols 0": call(cols=0), "K 0": call(K=0), "rows -8": call(1, rows=-8), "d 48": call(d=48),
+        "ld_l 28": call(ld_l=28), "ld_r 28": call(ld_r=28), "ingoing ld_l 28": call(1, ld_l=28),
+        "cs_l 8196": call(cs_l=8196), "cs_r 8196": call(cs_r=8196),
+        "ld_l < K": call(ld_l=16), "ld_r < K": call(ld_r=16),
+        "ingoing ld_l < cols": call(1, ld_l=16), "ingoing ld_r < rows": call(1, ld_r=8),
+    }
+    wrong = {k: rc for k, rc in bad.items() if rc != AF2_ERR_BAD_ARG}
+    assert not wrong, f"expected AF2_ERR_BAD_ARG ({AF2_ERR_BAD_ARG}): {wrong}"
 
 
 def _attn_smem(dh, nk):

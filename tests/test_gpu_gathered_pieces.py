@@ -1,4 +1,4 @@
-"""The contractions the sharded schedule feeds with ALL-GATHERED operand pieces (alphafold2_b200/parallel.py CudaStageOps),
+"""The contractions the sharded schedule feeds with ALL-GATHERED operand pieces (alphafold2_b200/stages.py CudaStageOps),
 checked on ONE GPU against the oracle stage ops: pieces whose width is not a multiple of 8 carry alignment padding, narrow
 pieces are merged into one operand, wide ones are addressed in place through rank-4 tensor maps.  (The multi-GPU check in
 tests/parallel_check_multi_gpu.py covers the same code with real collectives; this one runs in the single-GPU suite.)"""
@@ -6,7 +6,8 @@ import pytest
 import torch
 
 import alphafold2_b200 as A
-from alphafold2_b200.parallel import CudaStageOps, _align8
+from alphafold2_b200.parallel import _align8
+from alphafold2_b200.stages import CudaStageOps
 from oracle import evoformer_oracle as O
 from stage_ops_oracle import OracleStageOps
 

@@ -25,7 +25,7 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # P, d, H, dh, N, S, masked.  The contraction paths follow from the piece width N/P (api.cu: af2_triangle_contract,
-# af2_outer_contract; parallel.py: CudaStageOps._merge_mn_pieces merges MN-major pieces narrower than 64 columns).
+# af2_outer_contract; stages.py: CudaStageOps._merge_mn_pieces merges MN-major pieces narrower than 64 columns).
 CASES = [
     (8, 64, 2, 32, 48, 8, True),      # 6 per piece: outer-mean and ingoing pieces merged into one operand (the padding bug
                                       # once seen at 8 GPUs), outgoing one launch per piece

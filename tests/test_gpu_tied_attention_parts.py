@@ -93,7 +93,7 @@ def _oracle_update(st, x, edges, mask, H):
 
 @pytest.mark.parametrize("d,H,dh,h,w,masked", CASES)
 def test_tied_parts(d, H, dh, h, w, masked):
-    from alphafold2_b200.parallel import CudaStageOps
+    from alphafold2_b200.stages import CudaStageOps
     from gpu_util import check
     ax, st, x, edges, mask = _setup(d, H, dh, h, w, masked)
     whole = _whole(ax, x, edges, mask)

@@ -4,12 +4,11 @@ before which update, and that every triangle projection runs before any contract
 the CUDA kernels themselves (tests/test_gpu_pair_bands.py checks those, bitwise against the whole-tensor calls)."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 import alphafold2_b200 as A
 from alphafold2_b200 import banded
 from oracle import evoformer_oracle as O
-from stage_ops_oracle import OracleStageOps, _w
+from stage_ops_oracle import OracleStageOps
 
 
 def _align8(n):
@@ -33,13 +32,6 @@ class BandOracleStageOps(OracleStageOps):
         Ro[..., :R.shape[2]] = R
         Go.copy_(G)
         return out
-
-    def tri_contract_window_(self, tm, x_rows, L, R_win, gate):
-        w = _w(tm, x_rows.dtype)
-        d, N = L.shape[0], x_rows.shape[1]
-        out = torch.einsum("cki,ckj->ijc", R_win, L[:, :, :N])
-        out = F.layer_norm(out, (d,), w["to_out_norm.weight"], w["to_out_norm.bias"], 1e-5) * gate.view(out.shape)
-        x_rows += F.linear(out, w["to_out.weight"], w["to_out.bias"])
 
     def outer_contract_(self, om, x_rows, L, Rg, msa_mask_full, row0, pieces):
         super().outer_contract_(om, x_rows, L[..., :x_rows.shape[0]], Rg, msa_mask_full, row0, pieces)

@@ -77,7 +77,8 @@ def test_merge_gathered_pieces_drops_alignment_padding():
     (they were kept once: wrong pair rows at 8 GPUs whenever N/P is not a multiple of 8)."""
     import torch
 
-    from alphafold2_b200.parallel import CudaStageOps, _align8
+    from alphafold2_b200.parallel import _align8
+    from alphafold2_b200.stages import CudaStageOps
     for (n_total, P, d, K) in [(48, 8, 4, 3), (40, 2, 3, 5), (64, 8, 2, 2), (256, 8, 2, 4)]:
         w = n_total // P
         full = torch.arange(d * K * n_total, dtype=torch.float32).view(d, K, n_total)

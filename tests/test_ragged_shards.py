@@ -101,7 +101,8 @@ def test_merge_uneven_pieces_is_the_concatenation_of_unpadded_pieces(N, P, d, K)
     """CudaStageOps._merge_mn_pieces / _merge_k_pieces with per-piece sizes (host logic, no GPU): pieces gathered the way
     the schedule gathers them (each padded with -1 to the widest piece's align8 width, or to the tallest piece's rows)
     become the concatenation of the unpadded pieces, and the MN result's alignment columns are zero."""
-    from alphafold2_b200.parallel import CudaStageOps, _align8, shard_counts, shard_offsets
+    from alphafold2_b200.parallel import _align8, shard_counts, shard_offsets
+    from alphafold2_b200.stages import CudaStageOps
     widths, off = shard_counts(N, P), shard_offsets(N, P)
     full = torch.arange(d * K * N, dtype=torch.float32).view(d, K, N)
     W = _align8(max(widths))

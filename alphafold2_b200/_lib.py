@@ -245,6 +245,10 @@ _SIGNATURES = {
                                       vp]),
     "af2_superpose_scores": (ci, [C.POINTER(Points), C.POINTER(Points), vp, ll, ll, ci, ci, ci, ci, C.POINTER(Points),
                                   C.POINTER(Points), vp, vp, vp, ci, C.POINTER(cf), C.POINTER(GdtSpec), ci, vp, vp, vp, ll, vp]),
+    # distogram loss (train_pre.py:76-90, utils.py:45-50)
+    "af2_distogram_xent_rows": (ci, [vp, vp, ci, vp, vp, ci, ci, ci, ci, ci, ll, vp, vp]),
+    "af2_distogram_xent_finish": (ci, [vp, ll, vp, vp]),
+    "af2_bucketed_distance": (ci, [vp, ci, vp, vp, ci, ci, ci, ll, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -27,6 +27,7 @@
 #include "structure.cuh"
 #include "geometry.cuh"
 #include "metrics.cuh"
+#include "distogram_loss.cuh"
 
 using namespace af2;
 
@@ -1673,3 +1674,4 @@ int af2_contract_tail(const float* src, long long chan_stride, int pitch, int ro
 #include "structure_api.inl"
 #include "geometry_api.inl"
 #include "metrics_api.inl"
+#include "distogram_loss_api.inl"

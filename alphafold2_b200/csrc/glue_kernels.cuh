@@ -160,6 +160,22 @@ __global__ void __launch_bounds__(256) glue_distogram_kernel(const float* __rest
 // coordinate differences in fp32, squares summed by fmaf over the c coordinates in order, IEEE sqrtf.  bucket = lower bound of
 // the distance in bnd[0 .. nb-2] under !(bnd >= v) (torch.bucketize, right=False): NaN -> nb - 1, nb == 1 -> 0.
 // Lane owns the float4 chunks lane, lane + 32, ... (NCH of them, d4 = d / 4 <= 32 NCH); every row 16-byte aligned.
+
+// The bucket of the distance between points ci and cj [c] (fp32, global memory) under the edges bnd[0 .. nb-2], as the
+// recycling embedder decides it; also the label of the distogram loss (distogram_loss.cuh), which must agree with it bit for bit.
+__device__ __forceinline__ int distance_bucket(const float* __restrict__ ci, const float* __restrict__ cj, int c,
+                                               const float* __restrict__ bnd, int nb) {
+  float s2 = 0.f;
+  for (int e = 0; e < c; ++e) { const float dl = __ldg(ci + e) - __ldg(cj + e); s2 = fmaf(dl, dl, s2); }
+  const float dist = sqrtf(s2);
+  int lo = 0, hi = nb - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (!(__ldg(bnd + mid) >= dist)) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
 template <int NCH>
 __device__ __forceinline__ void recycle_ln_row(const float* __restrict__ src, const float* __restrict__ g, const float* __restrict__ be,
                                                int d, int lane, float eps, float (&y)[4 * NCH]) {
@@ -221,16 +237,7 @@ __global__ void __launch_bounds__(256) glue_recycle_kernel(const float* __restri
       for (int k = 0; k < NCH; ++k)
         if (lane + 32 * k < d4) xv[k] = reinterpret_cast<const float4*>(x + t * d)[lane + 32 * k];
       recycle_ln_row<NCH>(pprev + t * d, pair_g, pair_b, d, lane, eps, y);
-      const float* ci = coords + (b * n + i) * c;
-      const float* cj = coords + (b * n + j) * c;
-      float s2 = 0.f;
-      for (int e = 0; e < c; ++e) { const float dl = __ldg(ci + e) - __ldg(cj + e); s2 = fmaf(dl, dl, s2); }
-      const float dist = sqrtf(s2);
-      int lo = 0, hi = nb - 1;
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (!(__ldg(bnd + mid) >= dist)) lo = mid + 1; else hi = mid;
-      }
+      const int lo = distance_bucket(coords + (b * n + i) * c, coords + (b * n + j) * c, c, bnd, nb);
       const float4* er = reinterpret_cast<const float4*>(table + static_cast<long long>(lo) * d);
 #pragma unroll
       for (int k = 0; k < NCH; ++k) {

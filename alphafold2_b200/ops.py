@@ -1940,3 +1940,52 @@ def distmat_loss(a, a_matrix: bool, b, b_matrix: bool, B: int, n: int, mask=None
                                                     int(b_matrix), _ptr(mask), n * n, n, B, n, 15.0, float(lo), float(hi),
                                                     float(q), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
     return out
+
+
+# --------------------------------------------------------------------------------------------------
+# distogram loss (train_pre.py:76-90 with get_bucketed_distance_matrix, alphafold2_pytorch/utils.py:45-50)
+# --------------------------------------------------------------------------------------------------
+XENT_MAX_BINS = 4096     # csrc/distogram_loss.cuh: DX_MAX_BINS
+
+
+def _label_inputs(coords: torch.Tensor, mask: Optional[torch.Tensor], nb: int):
+    """coords fp32 [B, n, c] contiguous on a CUDA device, mask bool [B, n] contiguous on it or None, and the bucket edges."""
+    _require(coords, torch.float32, "coords")
+    if mask is not None:
+        _require(mask, torch.bool, "mask")
+    return recycling_boundaries(nb, coords.device)
+
+
+def distogram_xent_rows(logits: torch.Tensor, coords: torch.Tensor, mask: Optional[torch.Tensor], ignore_index: int,
+                        row0: int = 0) -> torch.Tensor:
+    """af2_distogram_xent_rows: logits [B, rows, n, nb] fp32 contiguous (the distogram rows [row0, row0 + rows)), coords
+    [B, n, c] fp32, mask [B, n] bool or None -> the per-row partials [B, rows, 2] int64: column 0 holds the fp64 bits of the
+    row's sum (.view(torch.float64)), column 1 the number of counted pairs.  One launch; no other device memory."""
+    _require(logits, torch.float32, "distance_logits")
+    B, rows, n, nb = logits.shape
+    bnd = _label_inputs(coords, mask, nb)
+    part = torch.empty(B, rows, 2, dtype=torch.int64, device=logits.device)
+    if rows == 0:
+        return part
+    _lib.check(_lib.load().af2_distogram_xent_rows(logits.data_ptr(), coords.data_ptr(), coords.shape[-1], _ptr(mask), bnd.data_ptr(), B,
+                                                   n, nb, int(row0), rows, int(ignore_index), part.data_ptr(), _stream_ptr()))
+    return part
+
+
+def distogram_xent_finish(part: torch.Tensor) -> torch.Tensor:
+    """af2_distogram_xent_finish over partials [B, n, 2] int64 in row order (distogram_xent_rows of every row, joined along the
+    rows) -> the mean, a 0-d fp32 tensor on their device.  One launch."""
+    _require(part, torch.int64, "partials")
+    out = torch.empty((), dtype=torch.float32, device=part.device)
+    _lib.check(_lib.load().af2_distogram_xent_finish(part.data_ptr(), part.numel() // 2, out.data_ptr(), _stream_ptr()))
+    return out
+
+
+def bucketed_distance(coords: torch.Tensor, mask: Optional[torch.Tensor], nb: int, ignore_index: int) -> torch.Tensor:
+    """af2_bucketed_distance: coords [B, n, c] fp32, mask [B, n] bool or None -> labels [B, n, n] int64.  One launch."""
+    bnd = _label_inputs(coords, mask, nb)
+    B, n, c = coords.shape
+    labels = torch.empty(B, n, n, dtype=torch.int64, device=coords.device)
+    _lib.check(_lib.load().af2_bucketed_distance(coords.data_ptr(), c, _ptr(mask), bnd.data_ptr(), B, n, int(nb), int(ignore_index),
+                                                 labels.data_ptr(), _stream_ptr()))
+    return labels

@@ -927,6 +927,25 @@ def gather_pair_rows(t: torch.Tensor, group=None) -> torch.Tensor:
     return all_gather_cat0(t[0].contiguous(), group, shard_counts(N, P) if N % P else None)[None]
 
 
+def distogram_loss_rows(distance_rows, coords, mask=None, ignore_index=-100, group=None) -> torch.Tensor:
+    """utils.distogram_loss of the whole distogram from this rank's rows of it, without gathering the logits: distance_rows
+    [b, n1 - n0, N, buckets] (ret.distance of shard_alphafold2(pair_rows=True), n0 = shard_offsets(N, P)[r]), coords [b, N, c]
+    and mask [b, N] bool or None whole, as every rank holds them.  Each rank reduces its rows to per-row fp64 partials (16 bytes
+    per row), one all-gather joins them in row order, and each rank finishes the mean.  The partials of a row do not depend on
+    how the rows are split, so every rank returns the same 0-d fp32 tensor, bitwise utils.distogram_loss of the gathered
+    distogram.  Every rank must call it (it is a collective)."""
+    from .utils import _xent_args
+    P, r = dist.get_world_size(group), dist.get_rank(group)
+    N = distance_rows.shape[2] if torch.is_tensor(distance_rows) and distance_rows.dim() == 4 else None
+    if N is None:
+        raise ValueError(f"distance_rows must be [b, rows, N, buckets], got {getattr(distance_rows, 'shape', type(distance_rows))}")
+    on = shard_offsets(N, P)
+    logits, x, m, ii = _xent_args(distance_rows, coords, mask, ignore_index, rows=on[r + 1] - on[r])
+    part = _ops.distogram_xent_rows(logits, x, m, ii, row0=on[r])                        # [b, rows, 2]
+    whole = all_gather_cat0(part.transpose(0, 1), group, shard_counts(N, P) if N % P else None)   # [N, b, 2]
+    return _ops.distogram_xent_finish(whole.transpose(0, 1).contiguous())
+
+
 def _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclables, return_trunk):
     """What sharded_alphafold2_rows cannot run, raised before any device work or collective."""
     from .alphafold2 import DISTOGRAM_BUCKETS

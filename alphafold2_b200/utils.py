@@ -12,7 +12,11 @@ The structure scores of utils.py:999-1247 (kabsch_torch / Kabsch, rmsd_torch / R
 TMscore, lddt_ca_torch, distmat_loss_torch) run as two kernels (csrc/metrics.cuh): a pass over the pairs for lDDT and the
 loss, and one CTA per structure for the superposition and the per-point scores.  Names, layouts, return dtypes and the
 reference's quirks are kept (DESIGN.md §4d); ``score_coords`` scores a batch of predictions in the model's layout.
+
+The distogram loss of the reference's training script (train_pre.py:76-90) and its labels, get_bucketed_distance_matrix
+(utils.py:45-50), run as one pass over the logits and a fixed-order finish (csrc/distogram_loss.cuh, DESIGN.md §4e).
 """
+import numbers
 from dataclasses import dataclass
 
 import torch
@@ -23,7 +27,7 @@ from .alphafold2 import DISTOGRAM_BUCKETS, _forward_only
 __all__ = ["DISTANCE_THRESHOLDS", "center_distogram_torch", "mds_torch", "mdscaling_torch", "get_dihedral_torch",
            "calc_phis_torch", "MDScaling", "coords_from_distogram", "kabsch_torch", "Kabsch", "rmsd_torch", "RMSD",
            "gdt_torch", "GDT", "tmscore_torch", "TMscore", "lddt_ca_torch", "distmat_loss_torch", "StructureScores",
-           "score_coords"]
+           "score_coords", "get_bucketed_distance_matrix", "distogram_loss"]
 
 DISTANCE_THRESHOLDS = torch.linspace(2, 20, steps=DISTOGRAM_BUCKETS)
 
@@ -433,3 +437,103 @@ def score_coords(pred, true, mask=None) -> StructureScores:
                          lddt_points=(y, x))
     dt = pred.dtype
     return StructureScores(rmsd.to(dt), ts, ha, tm.to(dt), lddt.to(dt), mean.to(dt), aligned.to(dt))
+
+
+# --------------------------------------------------------------------------------------------------
+# distogram loss (train_pre.py:76-90 with get_bucketed_distance_matrix, utils.py:45-50)
+# --------------------------------------------------------------------------------------------------
+def _ignore_index(ignore_index) -> int:
+    if isinstance(ignore_index, bool) or not isinstance(ignore_index, numbers.Integral):
+        raise TypeError(f"ignore_index must be an integer, got {type(ignore_index).__name__}")
+    if not -2 ** 63 <= int(ignore_index) < 2 ** 63:
+        raise ValueError(f"ignore_index {int(ignore_index)} does not fit in int64")
+    return int(ignore_index)
+
+
+def _checked(t, name: str) -> torch.Tensor:
+    """_scored's refusals (not a tensor, on the CPU, not floating, requires grad) without its conversion."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor (alphafold2_b200 has no CPU fallback)")
+    if not t.is_floating_point():
+        raise TypeError(f"{name} must be a floating tensor, got {t.dtype}")
+    _forward_only(t)
+    return t
+
+
+def _label_args(coords, mask, b=None, n=None, device=None):
+    """Refusals of coords [b, N, c] and mask [b, N] bool (or None); nothing is converted or launched."""
+    _checked(coords, "coords")
+    if coords.dim() != 3 or coords.shape[-1] < 1:
+        raise ValueError(f"coords must be [b, N, c] with c >= 1, got {tuple(coords.shape)}")
+    if coords.shape[0] == 0 or coords.shape[1] == 0:
+        raise ValueError(f"coords has no residues: {tuple(coords.shape)}")
+    if b is not None and tuple(coords.shape[:2]) != (b, n):
+        raise ValueError(f"coords must be [{b}, {n}, c] to match the distogram, got {tuple(coords.shape)}")
+    if device is not None and coords.device != device:
+        raise RuntimeError(f"coords are on {coords.device}, distance_logits on {device}")
+    if mask is not None:
+        if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool:
+            raise TypeError(f"mask must be a bool tensor, got {getattr(mask, 'dtype', type(mask).__name__)}")
+        if tuple(mask.shape) != tuple(coords.shape[:2]):
+            raise ValueError(f"mask must have shape {tuple(coords.shape[:2])}, got {tuple(mask.shape)}")
+        if mask.device != coords.device:
+            raise RuntimeError(f"mask is on {mask.device}, coords on {coords.device}")
+
+
+def _f32c(t: torch.Tensor) -> torch.Tensor:
+    return (t.detach() if t.dtype == torch.float32 else t.detach().float()).contiguous()
+
+
+def get_bucketed_distance_matrix(coords, mask, num_buckets=DISTOGRAM_BUCKETS, ignore_index=-100):
+    """utils.py:45-50 -- the distogram labels: int64 [b, N, N] for coords [b, N, c] and mask [b, N] bool (or [N, N] for [N, c]
+    and [N]; mask None: every residue present).  Label = ignore_index where either residue is masked, otherwise the bucket of
+    |coords_i - coords_j| under torch.linspace(2, 20, num_buckets)[:-1] (torch.bucketize, right=False: a distance on an edge
+    goes below it, NaN to num_buckets - 1).  The distance is the direct one in fp32, as the recycling embedder takes it: above
+    25 points the reference's torch.cdist uses |a|^2 + |b|^2 - 2 a.b, which can put a pair near an edge into the next bucket
+    (DESIGN.md §2).  One kernel launch."""
+    flat = isinstance(coords, torch.Tensor) and coords.dim() == 2
+    if flat:
+        coords = coords[None]
+        mask = mask[None] if isinstance(mask, torch.Tensor) and mask.dim() == 1 else mask
+    ii = _ignore_index(ignore_index)
+    if isinstance(num_buckets, bool) or not isinstance(num_buckets, numbers.Integral) or num_buckets < 1:
+        raise ValueError(f"num_buckets must be a positive integer, got {num_buckets!r}")
+    _label_args(coords, mask)
+    labels = ops.bucketed_distance(_f32c(coords), None if mask is None else mask.contiguous(), int(num_buckets), ii)
+    return labels[0] if flat else labels
+
+
+def _xent_args(distance_logits, coords, mask, ignore_index, rows=None):
+    """The checks both loss entries share, all before any device work -> (logits, coords, mask, ignore_index) as the kernels
+    read them.  rows: the number of pair rows distance_logits must hold (the whole N when None)."""
+    ii = _ignore_index(ignore_index)
+    _checked(distance_logits, "distance_logits")
+    shape = tuple(distance_logits.shape)
+    if len(shape) != 4 or shape[-1] < 1 or (rows is None and shape[1] != shape[2]):
+        raise ValueError(f"distance_logits must be [b, N, N, buckets] with buckets >= 1, got {shape}")
+    b, r, n, nb = shape
+    if b == 0 or n == 0:
+        raise ValueError(f"distance_logits has no pairs: {shape}")
+    if rows is not None and r != rows:
+        raise ValueError(f"distance_rows must hold this rank's {rows} pair rows of N = {n}, got {shape}")
+    if nb > ops.XENT_MAX_BINS:
+        raise ValueError(f"the distogram loss kernel takes at most {ops.XENT_MAX_BINS} buckets, got {nb}")
+    _label_args(coords, mask, b, n, distance_logits.device)
+    return _f32c(distance_logits), _f32c(coords), None if mask is None else mask.contiguous(), ii
+
+
+def distogram_loss(distance_logits, coords, mask=None, ignore_index=-100):
+    """The reference's distogram training loss (train_pre.py:76-90) in two kernel launches with no host synchronisation:
+        labels = get_bucketed_distance_matrix(coords, mask, buckets, ignore_index)
+        F.cross_entropy(rearrange(distance_logits, 'b i j c -> b c i j'), labels, ignore_index=ignore_index)
+    for distance_logits [b, N, N, buckets] (Alphafold2's ret.distance), coords [b, N, c] (the C-alpha coordinates) and mask
+    [b, N] bool or None (every residue counts).  The mean runs over every pair of the batch whose label is not ignore_index,
+    diagonal included; an in-range ignore_index also drops the pairs in that bucket, and NaN is returned when nothing counts.
+    No label matrix and no softmaxed copy of the logits is made: the extra device memory is 16 bytes per (element, row).
+    Returns a 0-d fp32 tensor on the logits' device.  The labels are get_bucketed_distance_matrix's; each term is the fp32
+    log-sum-exp minus the label's logit, summed in fp64 in a fixed order (DESIGN.md §4e), so the result is reproducible bit
+    for bit and equal to parallel.distogram_loss_rows on the same distogram sharded by rows."""
+    logits, x, m, ii = _xent_args(distance_logits, coords, mask, ignore_index)
+    return ops.distogram_xent_finish(ops.distogram_xent_rows(logits, x, m, ii))

@@ -767,6 +767,30 @@ int af2_superpose_scores(const af2_points* x, const af2_points* y, const unsigne
                          float* tm, int ncut, const float* cut, const af2_gdt_spec* gdt, int lddt, float* lddt_out,
                          float* lddt_mean, void* workspace, long long workspace_bytes, af2_stream_t stream);
 
+/* Distogram loss (the training objective of train_pre.py:76-90: F.cross_entropy of the distogram logits against
+ * get_bucketed_distance_matrix, alphafold2_pytorch/utils.py:45-50, with ignore_index).  coords [B][n][c] fp32 (c >= 1), mask
+ * [B][n] (1-byte bools) or NULL (every residue present), bnd [nb] the bucket edges torch.linspace(2, 20, nb) (the first nb - 1
+ * are searched).  The label of pair (i, j): ignore_index when mask[i] & mask[j] is false, otherwise the bucket of the direct
+ * distance, decided exactly as af2_recycle_embed decides it: fp32 coordinate differences, squares summed by fmaf over c in
+ * order, IEEE sqrtf, then the lower bound in bnd[0 .. nb-2] under !(bnd >= d) (torch.bucketize, right = False): a distance
+ * on an edge goes below it, NaN goes to nb - 1, and nb == 1 puts every pair in bucket 0.
+ * af2_distogram_xent_rows: one pass over the logits rows [row0, row0 + rows) of the distogram, logits [B][rows][n][nb] fp32
+ *   (any alignment), 1 <= nb <= 4096.  Per counted pair (label != ignore_index, so an in-range ignore_index also drops the
+ *   pairs in that bucket): term = (max + logf(sum expf(l - max))) - l[label] in fp32 with IEEE expf / logf.  partials
+ *   [B][rows] of {double sum; long long count} (16 B each) receive each row's fp64 sum and count, in an order that depends
+ *   only on (n, nb): the partials of any split of the rows are bitwise those of the whole.  No workspace; one launch.
+ * af2_distogram_xent_finish: *loss = (sum of the parts' sums) / (sum of their counts) from parts >= 1 partials in row order
+ *   ([B][n] for the whole distogram), fp64 in a fixed order that depends only on parts, stored as fp32; NaN (0 / 0) when
+ *   nothing counts.  One launch.  Together: F.cross_entropy(logits.permute(0, 3, 1, 2), labels, ignore_index = ignore_index).
+ * af2_bucketed_distance: labels [B][n][n] int64 as above (get_bucketed_distance_matrix).  One launch.
+ * Each returns AF2_ERR_BAD_ARG and launches nothing on a null pointer, B or n < 1, c < 1, nb < 1 (or > 4096 for the loss)
+ * or rows outside [0, n). */
+int af2_distogram_xent_rows(const float* logits, const float* coords, int c, const unsigned char* mask, const float* bnd, int B, int n,
+                            int nb, int row0, int rows, long long ignore_index, void* partials, af2_stream_t stream);
+int af2_distogram_xent_finish(const void* partials, long long parts, float* loss, af2_stream_t stream);
+int af2_bucketed_distance(const float* coords, int c, const unsigned char* mask, const float* bnd, int B, int n, int nb,
+                          long long ignore_index, long long* labels, af2_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -207,10 +207,6 @@ class Attention(_Packable):
         the pointwise template attention of alphafold2.py:764-785 (t [b * T, n, n, d], t_mask [b * T, n, n] crossed)."""
         return ops.template_pointwise_attention_(self.packed(), x, t, x_mask, t_mask, self.heads, self.dim_head)
 
-    def context_groups(self, x, x_mask):
-        """add_context_ with the templates given one group at a time (ops.TemplateAttentionGroups): same result, bitwise."""
-        return ops.TemplateAttentionGroups(self.packed(), x, x_mask, self.heads, self.dim_head)
-
     def forward(self, x, mask=None, attn_bias=None, context=None, context_mask=None, tie_dim=None):
         """alphafold2.py:125-190 on the GPU: gated self- or cross-attention (no LayerNorm, no residual), result in x.dtype.
         One query per batch element without a bias runs the pointwise template kernel; the rest the tensor-core attention
@@ -837,8 +833,8 @@ class Alphafold2(nn.Module):
         `group` forces G (tests).  The G used is kept in self.last_template_group.
 
         When not even one template fits (bf16 mode), the pointwise attention runs in bands of pair rows as well
-        (ops.plan_template_branch, ops.TemplateAttentionRows): per group the pair stack, in the same bands, then per batch
-        element and band q and gate of the band's rows of x, the group's k|v of those rows and the state-carrying kernel,
+        (ops.plan_template_branch, ops.TemplateAttentionGroups with band): per group the pair stack, in the same bands, then
+        per batch element and band q and gate of the band's rows of x, the group's k|v of those rows and the state-carrying kernel,
         and after the last group to_out into the band's rows of x.  Only the softmax state is kept for every pair; the result
         is bitwise the same.  `band` forces the rows per band (tests: a positive multiple of 8).  The band used is kept in
         self.last_template_band (n: the whole-tensor calls)."""
@@ -848,23 +844,17 @@ class Alphafold2(nn.Module):
         G, band = self._template_plan(x, templates_feats, group, band)
         self.last_template_group = G
         self.last_template_band = band
-        if band < n:
-            ops.release_workspace(x.device)          # the plan counted it as free: the softmax state may need its memory
-            acc = ops.TemplateAttentionRows(attn.packed(), x, x_mask, attn.heads, attn.dim_head, band)
-            for t0 in range(0, T, G):
-                t1 = min(t0 + G, T)
-                t, tm2 = self.template_pair_stack(templates_feats[:, t0:t1], templates_mask[:, t0:t1], band=band)
-                acc.add(t, tm2, last=t1 == T)
-                del t, tm2
-            return x
-        if G == T:
+        if G == T and band == n:
             t, tm2 = self.template_pair_stack(templates_feats, templates_mask)
             attn.add_context_(x, t, x_mask, tm2)
             return x
-        acc = attn.context_groups(x, x_mask)
+        if band < n:
+            ops.release_workspace(x.device)          # the plan counted it as free: the softmax state may need its memory
+        stack_band = band if band < n else None          # None: the pair stack keeps its own band planner
+        acc = ops.TemplateAttentionGroups(attn.packed(), x, x_mask, attn.heads, attn.dim_head, stack_band)
         for t0 in range(0, T, G):
             t1 = min(t0 + G, T)
-            t, tm2 = self.template_pair_stack(templates_feats[:, t0:t1], templates_mask[:, t0:t1])
+            t, tm2 = self.template_pair_stack(templates_feats[:, t0:t1], templates_mask[:, t0:t1], band=stack_band)
             acc.add(t, tm2, last=t1 == T)
             del t, tm2                                   # free this group's t before the next one is embedded
         return x

@@ -977,7 +977,7 @@ int contract_tail(const ChanLnParams& cp, const void* w_out, const float* b_out,
 extern "C" {
 
 const char* af2_last_error(void) { return g_err; }
-int af2_abi_version(void) { return 4; }
+int af2_abi_version(void) { return 5; }
 
 unsigned long long af2_launch_count(void) { return g_launches; }
 

@@ -1023,135 +1023,98 @@ def attention_forward(pk: Packed, x: torch.Tensor, heads: int, dim_head: int, ma
 
 class TemplateAttentionGroups:
     """template_pointwise_attention_ over the templates one group at a time (af2_template_pointwise_begin / _group / _end):
-        g = TemplateAttentionGroups(pk, x, x_mask, heads, dim_head)
-        g.add(t, t_mask, last=False) ...; g.add(t, t_mask, last=True)     # t [B * G, n, n, d], t_mask [B * G, n, n] per group
-    adds to x exactly what one template_pointwise_attention_ over the concatenated groups adds (bitwise).  Between the calls
-    it holds q and gate of x and the fp32 online-softmax state; a group's t may be freed as soon as its add() returns."""
+        g = TemplateAttentionGroups(pk, x, x_mask, heads, dim_head, band=None)
+        g.add(t, t_mask, last=False) ...; g.add(t, t_mask, last=True)     # t [B * G, R, C, d], t_mask [B * G, R, C] per group
+    x [B, R, C, d] is R rows of C pairs per batch element (the pair tensor, or a rank's rows of it).  Adds to x exactly what
+    one template_pointwise_attention_ over the concatenated groups adds (bitwise).  Between the calls it holds the fp32
+    online-softmax state of every pair; a group's t may be freed as soon as its add() returns.
+      band None or >= R: one window of all B * R * C pairs.  q and gate of x are made here, each add() is one group step and
+        the last one adds to_out to x.
+      band < R (bf16 only): each add() runs, per batch element and band of `band` pair rows, q and gate of the band's rows of
+        x, the group step on those rows and, on the last add(), to_out into them, so q, gate and k|v exist for one band at a
+        time.  x changes only in the last add(), band by band, after the band's own q and gate are made."""
 
-    def __init__(self, pk: Packed, x: torch.Tensor, x_mask: Optional[torch.Tensor], heads: int, dim_head: int):
+    def __init__(self, pk: Packed, x: torch.Tensor, x_mask: Optional[torch.Tensor], heads: int, dim_head: int,
+                 band: Optional[int] = None):
         _require(x, torch.float32, "x")
-        if x.dim() != 4 or x.shape[1] != x.shape[2]:
-            raise ValueError(f"x must be [B, n, n, d], got {tuple(x.shape)}")
-        B, n, _, d = x.shape
-        self.pk, self.x, self.heads, self.dim_head = pk, x, heads, dim_head
-        self.xm = _mask_u8(x_mask, (B, n, n), "x_mask")
-        self.first, self.done = True, False
-        P, I, dev = B * n * n, heads * dim_head, x.device
-        lib = _lib.load()
+        if x.dim() != 4:
+            raise ValueError(f"x must be [B, R, C, d], got {tuple(x.shape)}")
+        B, R, Cn, d = x.shape
         self.strict = pk.kind == "strict"
+        if band is not None and int(band) < R:
+            if self.strict:
+                raise NotImplementedError("the pointwise template attention runs in bands of pair rows in bf16 mode only")
+            if int(band) <= 0 or int(band) % 8:
+                raise ValueError(f"template band {band} must be a positive multiple of 8")
+        self.pk, self.x, self.heads, self.dim_head = pk, x, heads, dim_head
+        self.band = R if band is None else min(int(band), R)
+        self.xm = _mask_u8(x_mask, (B, R, Cn), "x_mask")
+        self.first, self.done = True, False
+        P, I, dev = B * R * Cn, heads * dim_head, x.device
+        W = P if self.band == R else self.band * Cn              # pairs of one window
         self.run_max = torch.empty(P, heads, dtype=torch.float32, device=dev)
         self.run_sum = torch.empty(P, heads, dtype=torch.float32, device=dev)
         self.acc = torch.empty(P, I, dtype=torch.float32, device=dev)
         self.pooled = torch.empty(P, dtype=torch.float32, device=dev)
+        # the last group writes the gated output of a window from the start of q (one window's rows), or of the accumulator in
+        # strict mode, which runs as one window
         if self.strict:
-            self.qg = torch.empty(P, 2 * I, dtype=torch.float32, device=dev)
-            self.out = self.acc                     # the last group writes the gated output over the accumulator
-            ws = workspace(lib.af2_template_pointwise_begin_strict_workspace(B, n, d), dev)
-            _lib.check(lib.af2_template_pointwise_begin_strict(C.byref(pk.struct), x.data_ptr(), B, n, d, heads, dim_head,
-                                                               self.qg.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
+            qg = torch.empty(W, 2 * I, dtype=torch.float32, device=dev)
+            self.qgate, self.out = (qg,), self.acc
         else:
-            self.q = torch.empty(P, I, dtype=torch.bfloat16, device=dev)
-            self.gate = torch.empty(P, I, dtype=torch.bfloat16, device=dev)
-            self.out = self.q                       # ... over q
-            ws = workspace(lib.af2_template_pointwise_begin_workspace(B, n, d), dev)
-            _lib.check(lib.af2_template_pointwise_begin(C.byref(pk.struct), x.data_ptr(), B, n, d, heads, dim_head, self.q.data_ptr(),
-                                                        self.gate.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr()))
+            q = torch.empty(W, I, dtype=torch.bfloat16, device=dev)
+            self.qgate, self.out = (q, torch.empty(W, I, dtype=torch.bfloat16, device=dev)), q
+        lib, sfx = _lib.load(), "_strict" if self.strict else ""
+        self.fn = {s: getattr(lib, f"af2_template_pointwise_{s}{sfx}") for s in ("begin", "group", "end")}
+        self.ws_fn = {s: getattr(lib, f"af2_template_pointwise_{s}{sfx}_workspace") for s in ("begin", "group", "end")}
+        self.w, self.qgate_ptrs = C.byref(pk.struct), [v.data_ptr() for v in self.qgate]
+        if self.band == R:
+            self._begin(_stream_ptr(), workspace(self.ws_fn["begin"](P, d), dev), 0, P)
+
+    def _begin(self, s, ws, o, P):
+        d = self.x.shape[3]
+        _lib.check(self.fn["begin"](self.w, _addr(self.x, o * d), P, d, self.heads, self.dim_head, *self.qgate_ptrs, ws.data_ptr(),
+                                    ws.numel(), s))
+
+    def _group(self, s, ws, t, tm, o, ot, B, G, pairs, t_stride, last):
+        d, h, I = self.x.shape[3], self.heads, self.heads * self.dim_head
+        _lib.check(self.fn["group"](
+            self.w, _addr(t, ot * d), None if self.xm is None else _addr(self.xm, o), None if tm is None else _addr(tm, ot), B, G,
+            pairs, t_stride, d, h, self.dim_head, *self.qgate_ptrs, _addr(self.run_max, o * h), _addr(self.run_sum, o * h),
+            _addr(self.acc, o * I), _addr(self.pooled, o), self.out.data_ptr(), int(self.first), int(last), ws.data_ptr(),
+            ws.numel(), s))
+
+    def _end(self, s, ws, o, P):
+        d = self.x.shape[3]
+        _lib.check(self.fn["end"](self.w, _addr(self.x, o * d), self.out.data_ptr(), _addr(self.pooled, o), P, d, self.heads,
+                                  self.dim_head, ws.data_ptr(), ws.numel(), s))
 
     def add(self, t: torch.Tensor, t_mask: Optional[torch.Tensor], last: bool) -> None:
         """One group of templates; on the last one (last=True) x gets the attention output."""
         if self.done:
             raise RuntimeError("TemplateAttentionGroups: the last group has already been added")
         _require(t, torch.float32, "t")
-        B, n, _, d = self.x.shape
-        if t.dim() != 4 or t.shape[0] % B or t.shape[0] == 0 or tuple(t.shape[1:]) != (n, n, d):
-            raise ValueError(f"t must be [B * G, {n}, {n}, {d}], got {tuple(t.shape)}")
+        B, R, Cn, d = self.x.shape
+        if t.dim() != 4 or t.shape[0] % B or t.shape[0] == 0 or tuple(t.shape[1:]) != (R, Cn, d):
+            raise ValueError(f"t must be [B * G, {R}, {Cn}, {d}], got {tuple(t.shape)}")
         G = t.shape[0] // B
-        tm = _mask_u8(t_mask, (B * G, n, n), "t_mask")
-        lib = _lib.load()
-        h, dh = self.heads, self.dim_head
-        if self.strict:
-            ws = workspace(lib.af2_template_pointwise_group_strict_workspace(B, G, n, d, h, dh), t.device)
-            fn, qg = lib.af2_template_pointwise_group_strict, (self.qg.data_ptr(),)
+        tm = _mask_u8(t_mask, (B * G, R, Cn), "t_mask")
+        h, dh, RC, s = self.heads, self.dim_head, R * Cn, _stream_ptr()
+        if self.band == R:
+            self._group(s, workspace(self.ws_fn["group"](B, G, RC, RC, d, h, dh), t.device), t, tm, 0, 0, B, G, RC, RC, last)
+            if last:
+                self._end(s, workspace(self.ws_fn["end"](B * RC, h, dh), t.device), 0, B * RC)
         else:
-            ws = workspace(lib.af2_template_pointwise_group_workspace(B, G, n, d, h, dh), t.device)
-            fn, qg = lib.af2_template_pointwise_group, (self.q.data_ptr(), self.gate.data_ptr())
-        _lib.check(fn(C.byref(self.pk.struct), t.data_ptr(), _ptr(self.xm), _ptr(tm), B, G, n, d, h, dh, *qg, self.run_max.data_ptr(),
-                      self.run_sum.data_ptr(), self.acc.data_ptr(), self.pooled.data_ptr(), self.out.data_ptr(), int(self.first),
-                      int(last), ws.data_ptr(), ws.numel(), _stream_ptr()))
-        self.first = False
-        if last:
-            self.done = True
-            if self.strict:
-                ws = workspace(lib.af2_template_pointwise_end_strict_workspace(B, n, h, dh), t.device)
-                fn = lib.af2_template_pointwise_end_strict
-            else:
-                ws = workspace(lib.af2_template_pointwise_end_workspace(B, n, h, dh), t.device)
-                fn = lib.af2_template_pointwise_end
-            _lib.check(fn(C.byref(self.pk.struct), self.x.data_ptr(), self.out.data_ptr(), self.pooled.data_ptr(), B, n, d, h, dh,
-                          ws.data_ptr(), ws.numel(), _stream_ptr()))
-
-
-class TemplateAttentionRows:
-    """TemplateAttentionGroups one band of pair rows at a time (af2_template_pointwise_rows_begin / _group / _end, bf16 only):
-        r = TemplateAttentionRows(pk, x, x_mask, heads, dim_head, band)
-        r.add(t, t_mask, last=False) ...; r.add(t, t_mask, last=True)      # t [B * G, n, n, d], t_mask [B * G, n, n] per group
-    Each add() runs, per batch element and band of `band` pair rows, q and gate of the band's rows of x, the k|v projection of
-    the band's rows of the group's templates and the state-carrying kernel; the last one also adds to_out to the band's rows of
-    x.  Between the calls only the fp32 softmax state is kept for every pair; q, gate and k|v exist for one band at a time.
-    x changes only in the last add(), band by band, after the band's own q and gate are made, so the result is bitwise that of
-    TemplateAttentionGroups."""
-
-    def __init__(self, pk: Packed, x: torch.Tensor, x_mask: Optional[torch.Tensor], heads: int, dim_head: int, band: int):
-        _require(x, torch.float32, "x")
-        if pk.kind == "strict":
-            raise NotImplementedError("the pointwise template attention runs in bands of pair rows in bf16 mode only")
-        if x.dim() != 4 or x.shape[1] != x.shape[2]:
-            raise ValueError(f"x must be [B, n, n, d], got {tuple(x.shape)}")
-        B, n, _, d = x.shape
-        if int(band) <= 0 or (int(band) < n and int(band) % 8):
-            raise ValueError(f"template band {band} must be a positive multiple of 8")
-        self.pk, self.x, self.heads, self.dim_head, self.band = pk, x, heads, dim_head, min(int(band), n)
-        self.xm = _mask_u8(x_mask, (B, n, n), "x_mask")
-        self.first, self.done = True, False
-        P, I, dev = B * n * n, heads * dim_head, x.device
-        self.run_max = torch.empty(P, heads, dtype=torch.float32, device=dev)
-        self.run_sum = torch.empty(P, heads, dtype=torch.float32, device=dev)
-        self.acc = torch.empty(P, I, dtype=torch.float32, device=dev)
-        self.pooled = torch.empty(P, dtype=torch.float32, device=dev)
-        W = self.band * n
-        self.q = torch.empty(W, I, dtype=torch.bfloat16, device=dev)      # the last group writes the gated output over q
-        self.gate = torch.empty(W, I, dtype=torch.bfloat16, device=dev)
-
-    def add(self, t: torch.Tensor, t_mask: Optional[torch.Tensor], last: bool) -> None:
-        """One group of templates over every band; on the last one (last=True) x gets the attention output."""
-        if self.done:
-            raise RuntimeError("TemplateAttentionRows: the last group has already been added")
-        _require(t, torch.float32, "t")
-        x = self.x
-        B, n, _, d = x.shape
-        if t.dim() != 4 or t.shape[0] % B or t.shape[0] == 0 or tuple(t.shape[1:]) != (n, n, d):
-            raise ValueError(f"t must be [B * G, {n}, {n}, {d}], got {tuple(t.shape)}")
-        G = t.shape[0] // B
-        tm = _mask_u8(t_mask, (B * G, n, n), "t_mask")
-        lib = _lib.load()
-        h, dh, R, nn = self.heads, self.dim_head, self.band, n * n
-        W = R * n
-        ws = workspace(max(lib.af2_template_pointwise_rows_begin_workspace(W, d),
-                           lib.af2_template_pointwise_rows_group_workspace(G, W, d, h, dh),
-                           lib.af2_template_pointwise_rows_end_workspace(W, h, dh)), x.device)
-        I, q, gate, s, w = h * dh, self.q.data_ptr(), self.gate.data_ptr(), _stream_ptr(), C.byref(self.pk.struct)
-        for b in range(B):
-            for i0 in range(0, n, R):
-                P = (min(i0 + R, n) - i0) * n
-                o, ot = b * nn + i0 * n, b * G * nn + i0 * n             # window offsets in x and in template 0 of t
-                _lib.check(lib.af2_template_pointwise_rows_begin(w, _addr(x, o * d), P, d, h, dh, q, gate, ws.data_ptr(), ws.numel(), s))
-                _lib.check(lib.af2_template_pointwise_rows_group(
-                    w, _addr(t, ot * d), None if self.xm is None else _addr(self.xm, o), None if tm is None else _addr(tm, ot), G, P, nn,
-                    d, h, dh, q, gate, _addr(self.run_max, o * h), _addr(self.run_sum, o * h), _addr(self.acc, o * I),
-                    _addr(self.pooled, o), q, int(self.first), int(last), ws.data_ptr(), ws.numel(), s))
-                if last:
-                    _lib.check(lib.af2_template_pointwise_rows_end(w, _addr(x, o * d), q, _addr(self.pooled, o), P, d, h, dh,
-                                                                   ws.data_ptr(), ws.numel(), s))
+            W = self.band * Cn
+            ws = workspace(max(self.ws_fn["begin"](W, d), self.ws_fn["group"](1, G, W, RC, d, h, dh), self.ws_fn["end"](W, h, dh)),
+                           t.device)
+            for b in range(B):
+                for i0 in range(0, R, self.band):
+                    P, o = (min(i0 + self.band, R) - i0) * Cn, b * RC + i0 * Cn
+                    self._begin(s, ws, o, P)
+                    self._group(s, ws, t, tm, o, b * G * RC + i0 * Cn, 1, G, P, RC, last)
+                    if last:
+                        self._end(s, ws, o, P)
         self.first = False
         self.done = last
 
@@ -1168,29 +1131,30 @@ def template_branch_bytes(b: int, T: int, G: int, n: int, d: int, heads: int, di
     one group, that group's copy of templates_feats, q and gate of x and the fp32 softmax state.  Computed from the library's
     workspace queries: no GPU needed.
 
-    band < n (bf16 only): the branch in bands of `band` pair rows (TemplateAttentionRows, the pair stack in the same bands):
+    band < n (bf16 only): the branch in bands of `band` pair rows (TemplateAttentionGroups with band, the pair stack in the
+    same bands):
     the fp32 softmax state of every pair, one group's t, crossed mask and templates_feats copy, one band's q and gate, plus
     the larger of the banded pair block (pair_block_bytes with S = 0) and one band's begin / group / end workspace."""
     if precision not in PRECISIONS:
         raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
     lib = _lib.load()
     strict = precision == "strict"
+    sfx = "_strict" if strict else ""
+    begin, group, end = (getattr(lib, f"af2_template_pointwise_{step}{sfx}_workspace") for step in ("begin", "group", "end"))
     G = max(1, min(G, T))
-    bg, P, I = b * G, b * n * n, heads * dim_head
+    bg, P, I, nn = b * G, b * n * n, heads * dim_head, n * n
     rows = bg * n * n
     if band is not None and band < n:
         if strict:
             raise ValueError("strict mode runs the template branch whole: no band")
         W = band * n
-        ws = [lib.af2_template_embed_workspace(rows, templates_dim), lib.af2_template_pointwise_rows_begin_workspace(W, d),
-              lib.af2_template_pointwise_rows_group_workspace(G, W, d, heads, dim_head),
-              lib.af2_template_pointwise_rows_end_workspace(W, heads, dim_head)]
+        ws = [lib.af2_template_embed_workspace(rows, templates_dim), begin(W, d), group(1, G, W, nn, d, heads, dim_head),
+              end(W, heads, dim_head)]
         persist = rows * d * 4 + rows + rows * templates_dim * 4               # t, crossed mask, templates_feats copy
         persist += P * (2 * heads + I + 1) * 4 + W * 2 * I * 2                 # whole-tensor state, one band's q | gate
         # the workspace is grow-only: a band's window workspace larger than the pair block's stays beside the block's operands
         pair_ws, keep = _pair_block_parts(bg, n, 0, d, heads, dim_head, band)
         return _ws_alloc(max(pair_ws, *ws)) + keep + persist
-    sfx = "_strict" if strict else ""
     ax = lib.af2_axial_attention_strict_workspace if strict else lib.af2_axial_attention_workspace
     ws = [getattr(lib, f"af2_template_embed{sfx}_workspace")(rows, templates_dim),
           getattr(lib, f"af2_triangle_multiply{sfx}_workspace")(bg, n, d),
@@ -1199,9 +1163,7 @@ def template_branch_bytes(b: int, T: int, G: int, n: int, d: int, heads: int, di
     if G == T:
         ws.append(getattr(lib, f"af2_template_pointwise_attention{sfx}_workspace")(b, T, n, d, heads, dim_head))
     else:
-        ws += [getattr(lib, f"af2_template_pointwise_begin{sfx}_workspace")(b, n, d),
-               getattr(lib, f"af2_template_pointwise_group{sfx}_workspace")(b, G, n, d, heads, dim_head),
-               getattr(lib, f"af2_template_pointwise_end{sfx}_workspace")(b, n, heads, dim_head)]
+        ws += [begin(P, d), group(b, G, nn, nn, d, heads, dim_head), end(P, heads, dim_head)]
         persist += rows * templates_dim * 4                                # the group's contiguous templates_feats
         persist += P * 2 * I * (4 if strict else 2)                        # q | gate
         persist += P * (2 * heads + I + 1) * 4                             # run_max, run_sum, acc, pooled
@@ -1428,7 +1390,8 @@ def template_angle_features(pk: Packed, angles: torch.Tensor, m: torch.Tensor, r
 def template_pointwise(q: torch.Tensor, gate: torch.Tensor, kv: torch.Tensor, B: int, T: int, heads: int, dim_head: int,
                        x_mask: Optional[torch.Tensor] = None, t_mask: Optional[torch.Tensor] = None,
                        out: Optional[torch.Tensor] = None, pooled: Optional[torch.Tensor] = None):
-    """The pointwise template-attention kernel alone (include/af2b200.h, af2_template_pointwise_bf16 / _f32): q, gate [P, I],
+    """The pointwise template-attention kernel alone, one launch over all T templates (include/af2b200.h,
+    af2_template_pointwise_bf16_state / _f32_state with first = last = 1 and no state): q, gate [P, I],
     kv [B * T * pairs, 2I] with P = B * pairs; bf16 operands (q in the log2 domain, gate after the sigmoid) or fp32 operands
     (the strict instantiation: natural-log domain, gate logits).  x_mask bool [P], t_mask bool [B * T * pairs].
     out / pooled: caller-given output buffers (flat views of at least P * I / P elements) or None.
@@ -1450,9 +1413,9 @@ def template_pointwise(q: torch.Tensor, gate: torch.Tensor, kv: torch.Tensor, B:
     _require(pooled, torch.float32, "pooled")
     if out.numel() < P * I or pooled.numel() < P:
         raise ValueError("out / pooled too small")
-    fn = _lib.load().af2_template_pointwise_bf16 if dt == torch.bfloat16 else _lib.load().af2_template_pointwise_f32
-    _lib.check(fn(q.data_ptr(), gate.data_ptr(), kv.data_ptr(), _ptr(xm), _ptr(tm), out.data_ptr(), pooled.data_ptr(), B, T, P // B,
-                  heads, dim_head, _stream_ptr()))
+    fn = _lib.load().af2_template_pointwise_bf16_state if dt == torch.bfloat16 else _lib.load().af2_template_pointwise_f32_state
+    _lib.check(fn(q.data_ptr(), gate.data_ptr(), kv.data_ptr(), _ptr(xm), _ptr(tm), out.data_ptr(), pooled.data_ptr(), None, None,
+                  None, 1, 1, B, T, P // B, heads, dim_head, _stream_ptr()))
     return out, pooled
 
 

@@ -822,10 +822,10 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
     The templates run one at a time, so a rank's memory does not grow with T.  For template k: to_template_embed of this
     rank's rows of templates_feats[0, k] (GEMM rows are independent: bitwise the rows of the whole call), the crossed mask's
     row and column shards, templates_embed_layers passes of sharded_pair_track (no outer mean, no transition), then one step
-    of the state-carrying pointwise attention over this rank's pairs (af2_template_pointwise_rows_*, q and gate from
-    x[0, n0:n1]).  After the last template to_out adds into those rows and an all-gather of the rows gives every rank the full
-    x.  The row <-> column exchanges use the peer-memory arena the sharded trunk already holds for (n, d), when there is
-    one (from the second forward on), and NCCL all-to-alls otherwise: both move the same bytes.  Runs eagerly.
+    of the state-carrying pointwise attention over this rank's pairs (ops.TemplateAttentionGroups on x[0, n0:n1]).  After
+    the last template to_out adds into those rows and an all-gather of the rows gives every rank the full x.  The row <->
+    column exchanges use the peer-memory arena the sharded trunk already holds for (n, d), when there is one (from the
+    second forward on), and NCCL all-to-alls otherwise: both move the same bytes.  Runs eagerly.
     rows_in: x is this rank's pair rows [1, n1 - n0, n, d] (shard_alphafold2(pair_rows=True)); they are updated in place and
     nothing is gathered."""
     attn = model.template_pointwise_attn
@@ -840,10 +840,7 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
     if n < P:
         raise ValueError(f"N_res={n} is smaller than the number of ranks {P}: every rank needs at least one pair row")
     ops = CudaStageOps()
-    lib = _lib.load()
     pair = model.template_pairwise_embedder
-    H, dh = attn.heads, attn.dim_head
-    I = H * dh
     with torch.no_grad():
         on = shard_offsets(n, P)
         r = dist.get_rank(group)
@@ -856,22 +853,11 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
         else:
             to_cols = lambda t: rows_to_cols(t, group, counts, counts)  # noqa: E731
             to_rows = lambda t: cols_to_rows(t, group, counts, counts)  # noqa: E731
-        Pn = (n1 - n0) * n                                                  # this rank's pairs
         x_rows = x[0] if rows_in else x[0, n0:n1]                           # a contiguous window of x
-        xm = None if x_mask is None else x_mask[0, n0:n1].bool().contiguous()
         tm = templates_mask[0].bool()
         embed = model.to_template_embed.packed()
-        w = C.byref(attn.packed().struct)
-        s = _ops._stream_ptr()
-        run_max = torch.empty(Pn, H, dtype=torch.float32, device=x.device)
-        run_sum = torch.empty_like(run_max)
-        acc = torch.empty(Pn, I, dtype=torch.float32, device=x.device)
-        pooled = torch.empty(Pn, dtype=torch.float32, device=x.device)
-        q = torch.empty(Pn, I, dtype=torch.bfloat16, device=x.device)      # the last template writes the gated output over q
-        gate = torch.empty_like(q)
-        ws = _ops.workspace(lib.af2_template_pointwise_rows_begin_workspace(Pn, d), x.device)
-        _lib.check(lib.af2_template_pointwise_rows_begin(w, x_rows.data_ptr(), Pn, d, H, dh, q.data_ptr(), gate.data_ptr(),
-                                                         ws.data_ptr(), ws.numel(), s))
+        acc = _ops.TemplateAttentionGroups(attn.packed(), x_rows[None], None if x_mask is None else x_mask[:, n0:n1], attn.heads,
+                                           attn.dim_head)
         for k in range(T):
             t_row = _ops.template_embed(embed, templates_feats[0, k, n0:n1].detach().float().contiguous())   # [Rn, n, d]
             sh = _PairShards(group, n, tm[k][:, None] & tm[k][None, :], to_cols, to_rows)                     # crossed mask
@@ -879,16 +865,8 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
                 t_row = ex.buffer(PeerExchange.PAIR, "row").copy_(t_row)
             for _ in range(model.templates_embed_layers):
                 t_row = sharded_pair_track(ops, pair, t_row, sh)
-            t_row = t_row.contiguous()
-            ws = _ops.workspace(lib.af2_template_pointwise_rows_group_workspace(1, Pn, d, H, dh), x.device)
-            _lib.check(lib.af2_template_pointwise_rows_group(
-                w, t_row.data_ptr(), None if xm is None else xm.data_ptr(), sh.mask_rows.data_ptr(), 1, Pn, Pn, d, H, dh,
-                q.data_ptr(), gate.data_ptr(), run_max.data_ptr(), run_sum.data_ptr(), acc.data_ptr(), pooled.data_ptr(),
-                q.data_ptr(), int(k == 0), int(k == T - 1), ws.data_ptr(), ws.numel(), s))
+            acc.add(t_row.contiguous()[None], sh.mask_rows[None], last=k == T - 1)
             del t_row
-        ws = _ops.workspace(lib.af2_template_pointwise_rows_end_workspace(Pn, H, dh), x.device)
-        _lib.check(lib.af2_template_pointwise_rows_end(w, x_rows.data_ptr(), q.data_ptr(), pooled.data_ptr(), Pn, d, H, dh,
-                                                       ws.data_ptr(), ws.numel(), s))
         if not rows_in:
             x[0].copy_(all_gather_cat0(x_rows, group, counts))
     return x

@@ -496,85 +496,70 @@ int af2_attention_forward_strict(const af2_template_attn_weights_strict* w, cons
                                  const unsigned char* mask, const unsigned char* context_mask, const float* bias, long long bias_sb,
                                  long long bias_sh, long long bias_si, long long bias_sj, int B, int i, int j, int d, int heads,
                                  int dim_head, int tie_dim, float* out, void* workspace, long long workspace_bytes, af2_stream_t stream);
-/* The pointwise kernel alone, on P = B * pairs pair positions:  out[p] = gate[p] * sum_t softmax_t(q[p] . k) v,  k | v = kv row
- * (b T + t) * pairs + (p % pairs), kv [B T pairs][2I] (k | v); pooled fp32 [P] = any_t t_mask; masks as above (t_mask indexed
- * like the kv rows).  _bf16: q [P][I] pre-scaled by dim_head^-0.5 * log2(e) (exp2-domain softmax), gate [P][I] with the sigmoid
- * applied, out bf16 [P][I].  _f32 (the strict instantiation): q pre-scaled by dim_head^-0.5, gate_logits BEFORE the sigmoid,
- * out fp32.  q, gate, kv and out 16-byte aligned.  A shape the kernel does not support returns AF2_ERR_BAD_ARG and launches
- * nothing. */
-int af2_template_pointwise_bf16(const void* q, const void* gate, const void* kv, const unsigned char* x_mask,
-                                const unsigned char* t_mask, void* out, float* pooled, int B, int T, long long pairs, int heads,
-                                int dim_head, af2_stream_t stream);
-int af2_template_pointwise_f32(const float* q, const float* gate_logits, const float* kv, const unsigned char* x_mask,
-                               const unsigned char* t_mask, float* out, float* pooled, int B, int T, long long pairs, int heads,
-                               int dim_head, af2_stream_t stream);
-/* The same kernel over one group of templates, carrying the online-softmax state from launch to launch: kv / t_mask hold the
- * group's T templates only.  State, all fp32: run_max and run_sum [P][heads], acc [P][I] (16-byte aligned), and pooled [P],
- * which holds "any template valid" (0 / 1) between groups.  first = 1: start from no state (nothing is read);  last = 1: write out
- * and pooled as above (nothing else);  last = 0: write the state instead (out is not touched and may be NULL).  first = last = 1
- * is af2_template_pointwise_bf16 / _f32 and the state pointers may be NULL.  Running every group in order gives out and pooled
- * bitwise equal to one launch over all templates.  out may be q (_bf16) or acc (_f32): each element is read before it is
- * written, by the same thread. */
+/* The pointwise kernel alone, on P = B * pairs pair positions, over one group of T templates, carrying the online-softmax
+ * state from launch to launch:  out[p] = gate[p] * sum_t softmax_t(q[p] . k) v,  k | v = kv row (b T + t) * pairs + (p % pairs),
+ * kv [B T pairs][2I] (k | v); pooled fp32 [P] = any_t t_mask; masks as above (t_mask indexed like the kv rows).  _bf16: q [P][I]
+ * pre-scaled by dim_head^-0.5 * log2(e) (exp2-domain softmax), gate [P][I] with the sigmoid applied, out bf16 [P][I].  _f32 (the
+ * strict instantiation): q pre-scaled by dim_head^-0.5, gate_logits BEFORE the sigmoid, out fp32.  q, gate, kv and out 16-byte
+ * aligned.  State, all fp32: run_max and run_sum [P][heads], acc [P][I] (16-byte aligned), and pooled [P], which holds "any
+ * template valid" (0 / 1) between groups.  first = 1: start from no state (nothing is read);  last = 1: write out and pooled as
+ * above (nothing else);  last = 0: write the state instead (out is not touched and may be NULL).  first = last = 1 is one launch
+ * over all templates, and the state pointers may then be NULL.  Running every group in order gives out and pooled bitwise equal
+ * to that one launch.  out may be q (_bf16) or acc (_f32): each element is read before it is written, by the same thread.  A
+ * shape the kernel does not support returns AF2_ERR_BAD_ARG and launches nothing. */
 int af2_template_pointwise_bf16_state(const void* q, const void* gate, const void* kv, const unsigned char* x_mask,
                                       const unsigned char* t_mask, void* out, float* pooled, float* run_max, float* run_sum, float* acc,
                                       int first, int last, int B, int T, long long pairs, int heads, int dim_head, af2_stream_t stream);
 int af2_template_pointwise_f32_state(const float* q, const float* gate_logits, const float* kv, const unsigned char* x_mask,
                                      const unsigned char* t_mask, float* out, float* pooled, float* run_max, float* run_sum, float* acc,
                                      int first, int last, int B, int T, long long pairs, int heads, int dim_head, af2_stream_t stream);
-/* af2_template_pointwise_attention in groups of templates, so that only one group's t and k|v are in memory at a time
- * (af2_template_pointwise_attention{,_strict} is exactly begin, one group of all T with first = last = 1, end):
- *   begin: q, gate from x into caller-owned buffers: bf16 q [P][I] and gate [P][I] (sigmoid-ed);  strict: qg fp32 [P][2I]
- *     = [q * dim_head^-0.5 | gating logits].  P = B n^2.
- *   group: for G templates, t fp32 [B G][n][n][d] and their crossed mask t_mask [B G][n][n] (template g of pair (b, i, j) is
- *     row (b G + g) n^2 + i n + j), in order over the groups with first = 1 on the first and last = 1 on the last: the k|v
- *     projection and the state-carrying kernel above.  run_max, run_sum, acc, pooled: the caller-owned state (fp32; acc
- *     16-byte aligned; run_max / run_sum / acc may be NULL when first = last = 1).  On the last group the gated attention output
- *     goes to out: bf16 [P][I], which may be q;  strict fp32 [P][I], which may be acc.
- *   end: x += pooled * (to_out(out) + b_out).
- * The state lives in caller memory because each call draws its workspace afresh. */
-long long af2_template_pointwise_begin_workspace(int B, int n, int d);
-int af2_template_pointwise_begin(const af2_template_attn_weights* w, const float* x, int B, int n, int d, int heads, int dim_head,
+/* af2_template_pointwise_attention in steps on a window of pairs, so that only one group's t and k|v, and if need be only one
+ * band of pair rows' q and gate, are in memory at a time (af2_template_pointwise_attention{,_strict} is exactly begin, one group
+ * of all T with first = last = 1, end).  A window is B * pairs consecutive pairs of x, x_mask, q, gate, out and the state;
+ * every pointer points at the window's first pair:
+ *   begin: q, gate of the window's P pairs of x into caller-owned buffers: bf16 q [P][I] and gate [P][I] (sigmoid-ed);
+ *     strict: qg fp32 [P][2I] = [q * dim_head^-0.5 | gating logits].
+ *   group: for G templates, block (b, g) of t fp32 and of the crossed mask t_mask (pairs rows of d floats / of bytes each)
+ *     starts (b G + g) t_stride pairs after t / t_mask, t_stride >= pairs (t_stride = pairs: contiguous [B G pairs]); template
+ *     g of window pair b pairs + p is row p of block (b, g).  In order over the groups with first = 1 on the first and last = 1
+ *     on the last: the k|v projection and the state-carrying kernel above.  run_max, run_sum, acc, pooled: the caller-owned
+ *     state (fp32; acc 16-byte aligned; run_max / run_sum / acc may be NULL when first = last = 1).  On the last group the
+ *     gated attention output goes to out: bf16 [B pairs][I], which may be q;  strict fp32 [B pairs][I], which may be acc.
+ *   end: x += pooled * (to_out(out) + b_out) on the window's P pairs.
+ * Whole tensors x [B][n][n][d], t [B G][n][n][d]: P = B n^2, pairs = t_stride = n^2.  A band of pair rows [i0, i1) of batch
+ * element b: B = 1, P = pairs = (i1 - i0) n, window offset o = b n^2 + i0 n (x + o d, x_mask + o, run_max + o heads,
+ * run_sum + o heads, acc + o I, pooled + o), t + (b G n^2 + i0 n) d, t_mask + b G n^2 + i0 n and t_stride = n^2.  Running, for
+ * every group in order, every window's begin and group, and end after the last group, gives x bitwise equal to the
+ * whole-tensor calls: each pair's q, gate, k|v and to_out are GEMM rows and the kernel resumes the state exactly.
+ * Workspaces are sized for the window only; group's counts the compacted mask rows when t_stride != pairs.  The state lives
+ * in caller memory because each call draws its workspace afresh.  x, t, q, gate, out and acc 16-byte aligned; d a multiple
+ * of 8; B, G >= 1; B G pairs < 2^31. */
+long long af2_template_pointwise_begin_workspace(long long P, int d);
+int af2_template_pointwise_begin(const af2_template_attn_weights* w, const float* x, long long P, int d, int heads, int dim_head,
                                  void* q, void* gate, void* workspace, long long workspace_bytes, af2_stream_t stream);
-long long af2_template_pointwise_group_workspace(int B, int G, int n, int d, int heads, int dim_head);
+long long af2_template_pointwise_group_workspace(int B, int G, long long pairs, long long t_stride, int d, int heads, int dim_head);
 int af2_template_pointwise_group(const af2_template_attn_weights* w, const float* t, const unsigned char* x_mask,
-                                 const unsigned char* t_mask, int B, int G, int n, int d, int heads, int dim_head, const void* q,
-                                 const void* gate, float* run_max, float* run_sum, float* acc, float* pooled, void* out, int first,
-                                 int last, void* workspace, long long workspace_bytes, af2_stream_t stream);
-long long af2_template_pointwise_end_workspace(int B, int n, int heads, int dim_head);
-int af2_template_pointwise_end(const af2_template_attn_weights* w, float* x, const void* out, const float* pooled, int B, int n, int d,
-                               int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
-long long af2_template_pointwise_begin_strict_workspace(int B, int n, int d);
-int af2_template_pointwise_begin_strict(const af2_template_attn_weights_strict* w, const float* x, int B, int n, int d, int heads,
+                                 const unsigned char* t_mask, int B, int G, long long pairs, long long t_stride, int d, int heads,
+                                 int dim_head, const void* q, const void* gate, float* run_max, float* run_sum, float* acc,
+                                 float* pooled, void* out, int first, int last, void* workspace, long long workspace_bytes,
+                                 af2_stream_t stream);
+long long af2_template_pointwise_end_workspace(long long P, int heads, int dim_head);
+int af2_template_pointwise_end(const af2_template_attn_weights* w, float* x, const void* out, const float* pooled, long long P,
+                               int d, int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
+long long af2_template_pointwise_begin_strict_workspace(long long P, int d);
+int af2_template_pointwise_begin_strict(const af2_template_attn_weights_strict* w, const float* x, long long P, int d, int heads,
                                         int dim_head, float* qg, void* workspace, long long workspace_bytes, af2_stream_t stream);
-long long af2_template_pointwise_group_strict_workspace(int B, int G, int n, int d, int heads, int dim_head);
+long long af2_template_pointwise_group_strict_workspace(int B, int G, long long pairs, long long t_stride, int d, int heads,
+                                                       int dim_head);
 int af2_template_pointwise_group_strict(const af2_template_attn_weights_strict* w, const float* t, const unsigned char* x_mask,
-                                        const unsigned char* t_mask, int B, int G, int n, int d, int heads, int dim_head, const float* qg,
-                                        float* run_max, float* run_sum, float* acc, float* pooled, float* out, int first, int last,
-                                        void* workspace, long long workspace_bytes, af2_stream_t stream);
-long long af2_template_pointwise_end_strict_workspace(int B, int n, int heads, int dim_head);
-int af2_template_pointwise_end_strict(const af2_template_attn_weights_strict* w, float* x, const float* out, const float* pooled, int B,
-                                      int n, int d, int heads, int dim_head, void* workspace, long long workspace_bytes,
+                                        const unsigned char* t_mask, int B, int G, long long pairs, long long t_stride, int d, int heads,
+                                        int dim_head, const float* qg, float* run_max, float* run_sum, float* acc, float* pooled,
+                                        float* out, int first, int last, void* workspace, long long workspace_bytes,
+                                        af2_stream_t stream);
+long long af2_template_pointwise_end_strict_workspace(long long P, int heads, int dim_head);
+int af2_template_pointwise_end_strict(const af2_template_attn_weights_strict* w, float* x, const float* out, const float* pooled,
+                                      long long P, int d, int heads, int dim_head, void* workspace, long long workspace_bytes,
                                       af2_stream_t stream);
-/* begin / group / end (bf16) on a window of P consecutive pairs of one batch element, e.g. a band of pair rows [i0, i1) of
- * batch element b: P = (i1 - i0) n, window offset o = b n^2 + i0 n.  Every pointer points at the window: x + o d, q, gate and
- * out [P][I] (window-sized, caller-owned), x_mask + o, and the window's slice of the whole-tensor state: run_max + o heads,
- * run_sum + o heads, acc + o I, pooled + o.  group: t points at template 0's first window row, t_mask at its crossed-mask
- * entry; template g's rows start g t_stride pairs later (t_stride >= P; for t [B G][n][n][d] from the grouped entry points,
- * t + (b G n^2 + i0 n) d and t_stride = n^2).  Workspaces are sized for the window only.  Running, for every group in order,
- * every window's begin and group (first / last as above), and end after the last group, gives x bitwise equal to the
- * whole-tensor calls.  x, t, q, gate, out and acc 16-byte aligned; d a multiple of 8. */
-long long af2_template_pointwise_rows_begin_workspace(long long P, int d);
-int af2_template_pointwise_rows_begin(const af2_template_attn_weights* w, const float* x, long long P, int d, int heads, int dim_head,
-                                      void* q, void* gate, void* workspace, long long workspace_bytes, af2_stream_t stream);
-long long af2_template_pointwise_rows_group_workspace(int G, long long P, int d, int heads, int dim_head);
-int af2_template_pointwise_rows_group(const af2_template_attn_weights* w, const float* t, const unsigned char* x_mask,
-                                      const unsigned char* t_mask, int G, long long P, long long t_stride, int d, int heads,
-                                      int dim_head, const void* q, const void* gate, float* run_max, float* run_sum, float* acc,
-                                      float* pooled, void* out, int first, int last, void* workspace, long long workspace_bytes,
-                                      af2_stream_t stream);
-long long af2_template_pointwise_rows_end_workspace(long long P, int heads, int dim_head);
-int af2_template_pointwise_rows_end(const af2_template_attn_weights* w, float* x, const void* out, const float* pooled, long long P,
-                                    int d, int heads, int dim_head, void* workspace, long long workspace_bytes, af2_stream_t stream);
 /* to_template_embed (alphafold2.py:751): t fp32 [rows][d] = feats fp32 [rows][K] W^T + bias.  w bf16 [d][align8(K)] (zero pad
  * columns); _strict: w split [d][3][align8(K)]. */
 long long af2_template_embed_workspace(long long rows, int K);

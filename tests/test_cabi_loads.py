@@ -26,8 +26,8 @@ def test_header_symbols_exported(lib):
     assert names == set(_lib.EXPORTED_SYMBOLS)
 
 
-def test_abi_version(lib):
-    assert lib.af2_abi_version() == 4
+def test_abi_version_5(lib):
+    assert lib.af2_abi_version() == 5
     assert lib.af2_last_error() is not None
 
 

@@ -1,12 +1,12 @@
-"""-m gpu: the pointwise template attention in bands of pair rows (ops.TemplateAttentionRows through
-Alphafold2.embed_templates_, and af2_template_pointwise_rows_begin / _group / _end).
+"""-m gpu: the pointwise template attention in bands of pair rows (ops.TemplateAttentionGroups with band through
+Alphafold2.embed_templates_, and af2_template_pointwise_begin / _group / _end on a window).
 
 q, gate and k|v are GEMM rows, the carry kernel resumes the softmax state exactly and to_out works row by row, so every band
 computes each element from the same bits in the same order as the whole-tensor calls: bitwise equality, never a tolerance.
   * model: embed_templates_ with forced bands of 8, 16 and 64 rows and G in {1, 2, T} == band None, G = T, over batch, T, n
     (136: a ragged last band) and the "mixed" masks of test_gpu_template_groups.py; Alphafold2.forward on the
     alphafold2_templates.pt inputs with bands of 8;
-  * C ABI: the rows entry points on a window inside larger tensors == the whole-tensor call on those rows, NaN guards around
+  * C ABI: the window entry points on a window inside larger tensors == the whole-tensor call on those rows, NaN guards around
     the window's outputs and state untouched; bad arguments return AF2_ERR_BAD_ARG and launch nothing;
   * memory: at N_res 1024, 4 templates, bands of 256 rows lower the peak below the one-template-at-a-time peak by at least
     what template_branch_bytes computes, and stay within the planned bytes;
@@ -101,7 +101,7 @@ def test_alphafold2_templates_fixture_bands_of_8_bitwise():
 
 
 # ------------------------------------------------------------------------------------------------------------------------
-# C ABI: the rows entry points
+# C ABI: the window entry points
 # ------------------------------------------------------------------------------------------------------------------------
 def _attn_weights(d, heads, dh, seed):
     from alphafold2_b200 import ops
@@ -122,7 +122,7 @@ def _guarded(rows, cols, dtype):
 
 
 @pytest.mark.parametrize("groups", [(1,), (2,), (3,), (1, 2), (2, 1), (1, 1, 1)])
-def test_rows_entry_points_on_a_window(groups):
+def test_window_entry_points_on_a_band(groups):
     import ctypes as C
     from alphafold2_b200 import _lib, ops
     lib = _lib.load()
@@ -149,22 +149,22 @@ def test_rows_entry_points_on_a_window(groups):
     gb, gate = _guarded(P, I, torch.bfloat16)
     s = ops._stream_ptr()
     w = C.byref(pk.struct)
-    ws = ops.workspace(max(lib.af2_template_pointwise_rows_begin_workspace(P, d),
-                           lib.af2_template_pointwise_rows_group_workspace(max(groups), P, d, heads, dh)), "cuda")
+    ws = ops.workspace(max(lib.af2_template_pointwise_begin_workspace(P, d),
+                           lib.af2_template_pointwise_group_workspace(1, max(groups), P, nn, d, heads, dh)), "cuda")
     t0 = 0
     for k, G in enumerate(groups):
         first, last = int(k == 0), int(k == len(groups) - 1)
-        _lib.check(lib.af2_template_pointwise_rows_begin(w, ops._addr(xw, o * d), P, d, heads, dh, q.data_ptr(), gate.data_ptr(),
-                                                         ws.data_ptr(), ws.numel(), s))
+        _lib.check(lib.af2_template_pointwise_begin(w, ops._addr(xw, o * d), P, d, heads, dh, q.data_ptr(), gate.data_ptr(),
+                                                    ws.data_ptr(), ws.numel(), s))
         # template g of the group: t[b, t0 + g], i.e. a stride of n^2 pairs inside t [B, T, n, n, d]
         base = (b * T + t0) * nn + i0 * n
-        _lib.check(lib.af2_template_pointwise_rows_group(
-            w, ops._addr(t, base * d), ops._addr(xm, o), ops._addr(tm, base), G, P, nn, d, heads, dh, q.data_ptr(), gate.data_ptr(),
+        _lib.check(lib.af2_template_pointwise_group(
+            w, ops._addr(t, base * d), ops._addr(xm, o), ops._addr(tm, base), 1, G, P, nn, d, heads, dh, q.data_ptr(), gate.data_ptr(),
             win["run_max"][1], win["run_sum"][1], win["acc"][1], win["pooled"][1], q.data_ptr(), first, last, ws.data_ptr(),
             ws.numel(), s))
         t0 += G
-    _lib.check(lib.af2_template_pointwise_rows_end(w, ops._addr(xw, o * d), q.data_ptr(), win["pooled"][1], P, d, heads, dh,
-                                                   ws.data_ptr(), 0, s))
+    _lib.check(lib.af2_template_pointwise_end(w, ops._addr(xw, o * d), q.data_ptr(), win["pooled"][1], P, d, heads, dh,
+                                              ws.data_ptr(), 0, s))
     torch.cuda.synchronize()
     flat, rflat, x0 = xw.view(-1, d), ref.view(-1, d), x.view(-1, d)
     assert torch.equal(_bits(flat[o:o + P]), _bits(rflat[o:o + P])), \
@@ -181,7 +181,7 @@ def test_rows_entry_points_on_a_window(groups):
     assert pooled.isfinite().all() and pooled.eq(tm[b].reshape(T, -1)[:, i0 * n:i1 * n].any(0).float()).all()
 
 
-def test_rows_entry_points_reject_bad_arguments():
+def test_window_entry_points_reject_bad_arguments():
     import ctypes as C
     from alphafold2_b200 import _lib, ops
     lib = _lib.load()
@@ -195,20 +195,20 @@ def test_rows_entry_points_reject_bad_arguments():
     gate = torch.full((P, I), float("nan"), dtype=torch.bfloat16, device="cuda")
     state = [torch.full((n * n, c), float("nan"), device="cuda") for c in (heads, heads, I, 1)]
     sp = [s.data_ptr() for s in state]
-    ws = ops.workspace(lib.af2_template_pointwise_rows_group_workspace(2, P, d, heads, dh), "cuda")
+    ws = ops.workspace(lib.af2_template_pointwise_group_workspace(1, 2, P, n * n, d, heads, dh), "cuda")
     s = ops._stream_ptr()
     w = C.byref(pk.struct)
     wsa = (ws.data_ptr(), ws.numel(), s)
 
     def begin(w=w, x=x.data_ptr(), P=P, q=q.data_ptr()):
-        return lib.af2_template_pointwise_rows_begin(w, x, P, d, heads, dh, q, gate.data_ptr(), *wsa)
+        return lib.af2_template_pointwise_begin(w, x, P, d, heads, dh, q, gate.data_ptr(), *wsa)
 
-    def group(w=w, t=t.data_ptr(), G=2, P=P, stride=n * n, q=q.data_ptr(), st=sp, first=0, last=0):
-        return lib.af2_template_pointwise_rows_group(w, t, None, None, G, P, stride, d, heads, dh, q, gate.data_ptr(), *st,
-                                                     q, first, last, *wsa)
+    def group(w=w, t=t.data_ptr(), B=1, G=2, P=P, stride=n * n, q=q.data_ptr(), st=sp, first=0, last=0):
+        return lib.af2_template_pointwise_group(w, t, None, None, B, G, P, stride, d, heads, dh, q, gate.data_ptr(), *st,
+                                                q, first, last, *wsa)
 
     def end(w=w, x=x.data_ptr(), P=P, out=q.data_ptr(), pooled=sp[3]):
-        return lib.af2_template_pointwise_rows_end(w, x, out, pooled, P, d, heads, dh, *wsa)
+        return lib.af2_template_pointwise_end(w, x, out, pooled, P, d, heads, dh, *wsa)
 
     bad = {
         "begin null weights": begin(w=None), "begin null x": begin(x=None), "begin negative P": begin(P=-1),
@@ -216,7 +216,8 @@ def test_rows_entry_points_reject_bad_arguments():
         "group null weights": group(w=None), "group null t": group(t=None), "group negative P": group(P=-n),
         "group misaligned t": group(t=t.data_ptr() + 4), "group misaligned q": group(q=q.data_ptr() + 2),
         "group first = 2": group(first=2), "group last = -1": group(last=-1), "group G = 0": group(G=0),
-        "group stride below the window": group(stride=P - 1), "group null state": group(st=[None, None, None, sp[3]]),
+        "group B = 0": group(B=0), "group B = -1": group(B=-1), "group stride below the window": group(stride=P - 1),
+        "group B = 2, stride below the window": group(B=2, G=1, stride=P - 1), "group null state": group(st=[None, None, None, sp[3]]),
         "group null pooled": group(st=sp[:3] + [None]), "group misaligned acc": group(st=sp[:2] + [sp[2] + 4, sp[3]]),
         "end null weights": end(w=None), "end null x": end(x=None), "end negative P": end(P=-1),
         "end misaligned out": end(out=q.data_ptr() + 2), "end null pooled": end(pooled=None),

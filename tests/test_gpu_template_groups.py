@@ -3,7 +3,8 @@
 The online softmax of the pointwise template attention carries its fp32 state (running max, running sum, accumulator, "any
 template valid") from one group to the next, and every other step acts on each template alone, so the result must not depend
 on G at all: bitwise equality against G = T, never a tolerance.
-  * kernel: af2_template_pointwise_{bf16,f32}_state over groups == one af2_template_pointwise_{bf16,f32} launch, out and pooled;
+  * kernel: af2_template_pointwise_{bf16,f32}_state over groups == one launch of the same entry with first = last = 1 and no
+    state, out and pooled;
   * model: embed_templates_ with G in {1, 2, T} == G = T, bf16 and strict, over batch, T, n and masks that leave pairs with
     every template masked (their templates then fall into different groups), a fully masked template and a partial x_mask;
   * Alphafold2.forward with G = 1 against the alphafold2_templates.pt fixture with the gates of test_alphafold2_templates_golden;
@@ -31,7 +32,7 @@ def _bits(t):
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
 @pytest.mark.parametrize("groups", [(1, 1, 1, 1, 1), (2, 2, 1), (1, 4), (3, 2)])
-def test_state_carry_kernel_bitwise(dtype, groups):
+def test_state_carry_over_groups_equals_one_state_launch(dtype, groups):
     from alphafold2_b200 import _lib
     lib = _lib.load()
     g = torch.Generator().manual_seed(sum(groups) * 10 + len(groups))
@@ -48,13 +49,12 @@ def test_state_carry_kernel_bitwise(dtype, groups):
     tm[:, :, 200:260] = False
     tm[:, T - 1, 200:260] = True                          # valid only in the last group
     tm = tm.cuda()
-    single = lib.af2_template_pointwise_bf16 if dtype == torch.bfloat16 else lib.af2_template_pointwise_f32
     state = lib.af2_template_pointwise_bf16_state if dtype == torch.bfloat16 else lib.af2_template_pointwise_f32_state
     stream = torch.cuda.current_stream().cuda_stream
     out1 = torch.full((P, I), float("nan"), dtype=dtype, device="cuda")
     pooled1 = torch.full((P,), float("nan"), device="cuda")
-    _lib.check(single(q.data_ptr(), gate.data_ptr(), kv.data_ptr(), xm.data_ptr(), tm.data_ptr(), out1.data_ptr(), pooled1.data_ptr(),
-                      B, T, pairs, heads, dh, stream))
+    _lib.check(state(q.data_ptr(), gate.data_ptr(), kv.data_ptr(), xm.data_ptr(), tm.data_ptr(), out1.data_ptr(), pooled1.data_ptr(),
+                     None, None, None, 1, 1, B, T, pairs, heads, dh, stream))
     out2 = torch.full((P, I), float("nan"), dtype=dtype, device="cuda")
     pooled2 = torch.full((P,), float("nan"), device="cuda")
     run_max = torch.full((P, heads), float("nan"), device="cuda")

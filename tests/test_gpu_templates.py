@@ -1,7 +1,7 @@
 """-m gpu: the template embedder (alphafold2.py:743-792, SURVEY.md 8f n3).
 
-Kernel alone (template_pointwise_kernel through af2_template_pointwise_bf16 / _f32) against fp64 math on the exact operands the
-kernel was given, element-wise with `check_bound`.  For pair p, head h, templates t = 0..T-1 (s_t the logits in the kernel's
+Kernel alone (template_pointwise_kernel through af2_template_pointwise_{bf16,f32}_state, one launch over all templates) against
+fp64 math on the exact operands the kernel was given, element-wise with `check_bound`.  For pair p, head h, templates t = 0..T-1 (s_t the logits in the kernel's
 domain: log2 for the bf16 instantiation, natural log for the fp32 one; w_t = softmax weights of the valid templates, or 1/T
 each when none is valid; o = sum_t w_t v_t; ref = gate * o):
   * each logit is an fp32 dot product of dh terms:              |ds_t| <= E_s = dh 2^-24 sum_e |q_e k_e|

@@ -59,14 +59,14 @@ def test_bytes_do_not_decrease_with_the_band(n):
     assert _bytes(n, 1, band=256) < 0.65 * _bytes(n, 1), "bands of 256 rows must need far less than one whole template"
 
 
-def test_banded_bytes_count_state_template_and_window():
+def test_banded_bytes_count_state_template_and_window_workspaces():
     """State of every pair, one template's t / crossed mask / templates_feats copy and one band's q | gate, plus the larger
     of the banded pair block and the band's workspace (as the grow-only workspace allocates it)."""
     lib = _lib.load()
     n, R, I = 2048, 512, H * DH
     P, rows, W = n * n, n * n, R * n
-    ws = max(lib.af2_template_embed_workspace(rows, K), lib.af2_template_pointwise_rows_begin_workspace(W, D),
-             lib.af2_template_pointwise_rows_group_workspace(1, W, D, H, DH), lib.af2_template_pointwise_rows_end_workspace(W, H, DH))
+    ws = max(lib.af2_template_embed_workspace(rows, K), lib.af2_template_pointwise_begin_workspace(W, D),
+             lib.af2_template_pointwise_group_workspace(1, 1, W, n * n, D, H, DH), lib.af2_template_pointwise_end_workspace(W, H, DH))
     persist = rows * D * 4 + rows + rows * K * 4 + P * (2 * H + I + 1) * 4 + W * 2 * I * 2
     got = _bytes(n, 1, band=R)
     assert got >= ops.pair_block_bytes(1, n, 0, D, H, DH, R) + persist

@@ -240,6 +240,10 @@ _SIGNATURES = {
     "af2_distogram_xent_rows": (ci, [vp, vp, ci, vp, vp, ci, ci, ci, ci, ci, ll, vp, vp]),
     "af2_distogram_xent_finish": (ci, [vp, ll, vp, vp]),
     "af2_bucketed_distance": (ci, [vp, ci, vp, vp, ci, ci, ci, ll, vp, vp]),
+    # angle-head labels and loss (trRosetta orientations from the backbone, DESIGN.md §4f)
+    "af2_angle_xent_rows": (ci, [vp, vp, vp, vp, ci, vp, vp, ci, ci, ci, ci, ll, vp, vp]),
+    "af2_angle_xent_finish": (ci, [vp, ll, vp, vp]),
+    "af2_bucketed_angles": (ci, [vp, ci, vp, vp, ci, ci, ll, vp, vp, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

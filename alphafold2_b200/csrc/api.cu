@@ -28,6 +28,7 @@
 #include "geometry.cuh"
 #include "metrics.cuh"
 #include "distogram_loss.cuh"
+#include "angle_loss.cuh"
 
 using namespace af2;
 
@@ -1675,3 +1676,4 @@ int af2_contract_tail(const float* src, long long chan_stride, int pitch, int ro
 #include "geometry_api.inl"
 #include "metrics_api.inl"
 #include "distogram_loss_api.inl"
+#include "angle_loss_api.inl"

@@ -1952,3 +1952,54 @@ def bucketed_distance(coords: torch.Tensor, mask: Optional[torch.Tensor], nb: in
     _lib.check(_lib.load().af2_bucketed_distance(coords.data_ptr(), c, _ptr(mask), bnd.data_ptr(), B, n, int(nb), int(ignore_index),
                                                  labels.data_ptr(), _stream_ptr()))
     return labels
+
+
+# --------------------------------------------------------------------------------------------------
+# angle-head labels and loss (the trRosetta orientations from the backbone, DESIGN.md §4f)
+# --------------------------------------------------------------------------------------------------
+def _angle_nb(nb) -> C.Array:
+    return (C.c_int * 3)(*(int(v) for v in nb))
+
+
+def angle_xent_rows(theta: torch.Tensor, phi: torch.Tensor, omega: torch.Tensor, backbone: torch.Tensor,
+                    mask: Optional[torch.Tensor], ignore_index: int, row0: int = 0) -> torch.Tensor:
+    """af2_angle_xent_rows: theta / phi / omega [B, rows, n, nb_h] fp32 contiguous (the heads' rows [row0, row0 + rows)),
+    backbone [B, n, A, 3] fp32 contiguous, mask [B, n] bool or None -> the per-row partials [B, rows, 3, 2] int64: per head
+    (theta, phi, omega) column 0 holds the fp64 bits of the row's sum (.view(torch.float64)), column 1 the number of counted
+    pairs.  One launch; no other device memory."""
+    for t, name in ((theta, "theta_logits"), (phi, "phi_logits"), (omega, "omega_logits")):
+        _require(t, torch.float32, name)
+    _require(backbone, torch.float32, "backbone")
+    if mask is not None:
+        _require(mask, torch.bool, "mask")
+    B, rows, n = theta.shape[:3]
+    part = torch.empty(B, rows, 3, 2, dtype=torch.int64, device=theta.device)
+    if rows == 0:
+        return part
+    nb = _angle_nb((theta.shape[-1], phi.shape[-1], omega.shape[-1]))
+    _lib.check(_lib.load().af2_angle_xent_rows(theta.data_ptr(), phi.data_ptr(), omega.data_ptr(), backbone.data_ptr(),
+                                               backbone.shape[2], _ptr(mask), nb, B, n, int(row0), rows, int(ignore_index),
+                                               part.data_ptr(), _stream_ptr()))
+    return part
+
+
+def angle_xent_finish(part: torch.Tensor) -> torch.Tensor:
+    """af2_angle_xent_finish over partials [B, n, 3, 2] int64 in row order (angle_xent_rows of every row, joined along the
+    rows) -> the three heads' mean terms, fp32 [3] (theta, phi, omega) on their device.  One launch."""
+    _require(part, torch.int64, "partials")
+    out = torch.empty(3, dtype=torch.float32, device=part.device)
+    _lib.check(_lib.load().af2_angle_xent_finish(part.data_ptr(), part.numel() // 6, out.data_ptr(), _stream_ptr()))
+    return out
+
+
+def bucketed_angles(backbone: torch.Tensor, mask: Optional[torch.Tensor], nb, ignore_index: int):
+    """af2_bucketed_angles: backbone [B, n, A, 3] fp32, mask [B, n] bool or None, nb the three bucket counts -> the labels
+    (theta, phi, omega), each [B, n, n] int64.  One launch."""
+    _require(backbone, torch.float32, "backbone")
+    if mask is not None:
+        _require(mask, torch.bool, "mask")
+    B, n, A = backbone.shape[:3]
+    out = [torch.empty(B, n, n, dtype=torch.int64, device=backbone.device) for _ in range(3)]
+    _lib.check(_lib.load().af2_bucketed_angles(backbone.data_ptr(), A, _ptr(mask), _angle_nb(nb), B, n, int(ignore_index),
+                                               out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(), _stream_ptr()))
+    return tuple(out)

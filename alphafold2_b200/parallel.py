@@ -924,6 +924,25 @@ def distogram_loss_rows(distance_rows, coords, mask=None, ignore_index=-100, gro
     return _ops.distogram_xent_finish(whole.transpose(0, 1).contiguous())
 
 
+def angle_loss_rows(theta_rows, phi_rows, omega_rows, backbone, mask=None, ignore_index=-100, group=None):
+    """utils.angle_loss of the whole angle logits from this rank's rows of them, without gathering the logits: theta_rows,
+    phi_rows and omega_rows [b, n1 - n0, N, buckets] (ret.theta_logits, ret.phi_logits and ret.omega_logits of
+    shard_alphafold2(pair_rows=True), n0 = shard_offsets(N, P)[r]), backbone [b, N, A, 3] and mask [b, N] bool or None whole,
+    as every rank holds them.  Each rank reduces its rows to per-row fp64 partials (48 bytes per row), one all-gather joins
+    them in row order, and each rank finishes the three means, so every rank returns the same utils.AngleLoss, bitwise
+    utils.angle_loss of the gathered logits.  Every rank must call it (it is a collective)."""
+    from .utils import _angle_args, _angle_result
+    P, r = dist.get_world_size(group), dist.get_rank(group)
+    N = theta_rows.shape[2] if torch.is_tensor(theta_rows) and theta_rows.dim() == 4 else None
+    if N is None:
+        raise ValueError(f"theta_rows must be [b, rows, N, buckets], got {getattr(theta_rows, 'shape', type(theta_rows))}")
+    on = shard_offsets(N, P)
+    *heads, x, m, ii = _angle_args(theta_rows, phi_rows, omega_rows, backbone, mask, ignore_index, rows=on[r + 1] - on[r])
+    part = _ops.angle_xent_rows(*heads, x, m, ii, row0=on[r])                             # [b, rows, 3, 2]
+    whole = all_gather_cat0(part.transpose(0, 1).contiguous(), group, shard_counts(N, P) if N % P else None)   # [N, b, 3, 2]
+    return _angle_result(_ops.angle_xent_finish(whole.transpose(0, 1).contiguous()))
+
+
 def _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclables, return_trunk):
     """What sharded_alphafold2_rows cannot run, raised before any device work or collective."""
     from .alphafold2 import DISTOGRAM_BUCKETS

@@ -15,6 +15,8 @@ reference's quirks are kept (DESIGN.md §4d); ``score_coords`` scores a batch of
 
 The distogram loss of the reference's training script (train_pre.py:76-90) and its labels, get_bucketed_distance_matrix
 (utils.py:45-50), run as one pass over the logits and a fixed-order finish (csrc/distogram_loss.cuh, DESIGN.md §4e).
+The angle heads are scored the same way against the trRosetta orientations of the true backbone (csrc/angle_loss.cuh,
+DESIGN.md §4f).
 """
 import numbers
 from dataclasses import dataclass
@@ -22,12 +24,13 @@ from dataclasses import dataclass
 import torch
 
 from . import ops
-from .alphafold2 import DISTOGRAM_BUCKETS, _forward_only
+from .alphafold2 import DISTOGRAM_BUCKETS, OMEGA_BUCKETS, PHI_BUCKETS, THETA_BUCKETS, _forward_only
 
 __all__ = ["DISTANCE_THRESHOLDS", "center_distogram_torch", "mds_torch", "mdscaling_torch", "get_dihedral_torch",
            "calc_phis_torch", "MDScaling", "coords_from_distogram", "kabsch_torch", "Kabsch", "rmsd_torch", "RMSD",
            "gdt_torch", "GDT", "tmscore_torch", "TMscore", "lddt_ca_torch", "distmat_loss_torch", "StructureScores",
-           "score_coords", "get_bucketed_distance_matrix", "distogram_loss"]
+           "score_coords", "get_bucketed_distance_matrix", "distogram_loss", "get_bucketed_angle_matrices", "AngleLoss",
+           "angle_loss"]
 
 DISTANCE_THRESHOLDS = torch.linspace(2, 20, steps=DISTOGRAM_BUCKETS)
 
@@ -537,3 +540,111 @@ def distogram_loss(distance_logits, coords, mask=None, ignore_index=-100):
     for bit and equal to parallel.distogram_loss_rows on the same distogram sharded by rows."""
     logits, x, m, ii = _xent_args(distance_logits, coords, mask, ignore_index)
     return ops.distogram_xent_finish(ops.distogram_xent_rows(logits, x, m, ii))
+
+
+# --------------------------------------------------------------------------------------------------
+# angle-head labels and loss (the trRosetta inter-residue orientations, DESIGN.md §4f)
+# --------------------------------------------------------------------------------------------------
+ANGLE_HEADS = ("theta", "phi", "omega")
+
+
+@dataclass
+class AngleLoss:
+    """angle_loss's result: each head's mean cross-entropy over its counted pairs, a 0-d fp32 tensor on the logits' device."""
+    theta: torch.Tensor
+    phi: torch.Tensor
+    omega: torch.Tensor
+
+
+def _backbone_args(backbone, mask, b=None, n=None, device=None):
+    """Refusals of backbone [b, N, A, 3] (A >= 3) and mask [b, N] bool (or None); nothing is converted or launched."""
+    _checked(backbone, "backbone")
+    if backbone.dim() != 4 or backbone.shape[-1] != 3 or backbone.shape[2] < 3:
+        raise ValueError(f"backbone must be [b, N, A, 3] with A >= 3 (atoms N, CA, C first), got {tuple(backbone.shape)}")
+    if backbone.shape[0] == 0 or backbone.shape[1] == 0:
+        raise ValueError(f"backbone has no residues: {tuple(backbone.shape)}")
+    if b is not None and tuple(backbone.shape[:2]) != (b, n):
+        raise ValueError(f"backbone must be [{b}, {n}, A, 3] to match the angle logits, got {tuple(backbone.shape)}")
+    if device is not None and backbone.device != device:
+        raise RuntimeError(f"backbone is on {backbone.device}, the angle logits on {device}")
+    if mask is not None:
+        if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool:
+            raise TypeError(f"mask must be a bool tensor, got {getattr(mask, 'dtype', type(mask).__name__)}")
+        if tuple(mask.shape) != tuple(backbone.shape[:2]):
+            raise ValueError(f"mask must have shape {tuple(backbone.shape[:2])}, got {tuple(mask.shape)}")
+        if mask.device != backbone.device:
+            raise RuntimeError(f"mask is on {mask.device}, backbone on {backbone.device}")
+
+
+def _bucket_count(nb, name: str) -> int:
+    if isinstance(nb, bool) or not isinstance(nb, numbers.Integral) or nb < 2:
+        raise ValueError(f"{name} needs at least 2 buckets (one angular bin and no contact), got {nb!r}")
+    return int(nb)
+
+
+def get_bucketed_angle_matrices(backbone, mask, num_buckets=(THETA_BUCKETS, PHI_BUCKETS, OMEGA_BUCKETS), ignore_index=-100):
+    """The angle heads' labels: the trRosetta orientations theta, phi and omega of every residue pair, bucketed, for backbone
+    [b, N, A, 3] (A >= 3; atoms 0, 1, 2 are N, CA, C, sidechainnet's order, so the reference's 14-atom layout passes as it is)
+    and mask [b, N] bool or None (every residue present); [N, A, 3] and [N] give [N, N].  Returns (theta, phi, omega), each
+    int64 [b, N, N].  In fp64 on the fp32 atoms: the virtual CB of every residue, a contact is i != j with |CB_i - CB_j| <=
+    20 A, and for a contact theta = dihedral(N_i, CA_i, CB_i, CB_j), omega = dihedral(CA_i, CB_i, CB_j, CA_j) in [-pi, pi] and
+    phi = angle(CA_i, CB_i, CB_j) in [0, pi].  A head of nb buckets has nb - 1 bins of equal width (torch.bucketize, right=False:
+    an angle on an edge goes below it) and puts no contact (the diagonal, farther pairs, missing atoms) in the last bucket,
+    nb - 1; a pair with a masked residue gets ignore_index.  One kernel launch."""
+    flat = isinstance(backbone, torch.Tensor) and backbone.dim() == 3
+    if flat:
+        backbone = backbone[None]
+        mask = mask[None] if isinstance(mask, torch.Tensor) and mask.dim() == 1 else mask
+    ii = _ignore_index(ignore_index)
+    if not isinstance(num_buckets, (tuple, list)) or len(num_buckets) != 3:
+        raise ValueError(f"num_buckets must be three bucket counts (theta, phi, omega), got {num_buckets!r}")
+    nb = tuple(_bucket_count(v, h) for v, h in zip(num_buckets, ANGLE_HEADS))
+    _backbone_args(backbone, mask)
+    labels = ops.bucketed_angles(_f32c(backbone), None if mask is None else mask.contiguous(), nb, ii)
+    return tuple(t[0] for t in labels) if flat else labels
+
+
+def _angle_args(theta_logits, phi_logits, omega_logits, backbone, mask, ignore_index, rows=None):
+    """The checks angle_loss and parallel.angle_loss_rows share, all before any device work -> (theta, phi, omega, backbone,
+    mask, ignore_index) as the kernels read them.  rows: the number of pair rows the logits must hold (the whole N when None)."""
+    ii = _ignore_index(ignore_index)
+    heads = (theta_logits, phi_logits, omega_logits)
+    for t, h in zip(heads, ANGLE_HEADS):
+        _checked(t, f"{h}_logits")
+    shape = tuple(theta_logits.shape)
+    if len(shape) != 4 or (rows is None and shape[1] != shape[2]):
+        raise ValueError(f"theta_logits must be [b, N, N, buckets], got {shape}")
+    b, r, n, _ = shape
+    if b == 0 or n == 0:
+        raise ValueError(f"theta_logits has no pairs: {shape}")
+    if rows is not None and r != rows:
+        raise ValueError(f"the angle logits must hold this rank's {rows} pair rows of N = {n}, got {shape}")
+    for t, h in zip(heads, ANGLE_HEADS):
+        if t.dim() != 4 or tuple(t.shape[:3]) != (b, r, n):
+            raise ValueError(f"{h}_logits must be [{b}, {r}, {n}, buckets] like theta_logits, got {tuple(t.shape)}")
+        if t.device != theta_logits.device:
+            raise RuntimeError(f"{h}_logits are on {t.device}, theta_logits on {theta_logits.device}")
+        _bucket_count(t.shape[-1], f"{h}_logits")
+    nbs = sum(t.shape[-1] for t in heads)
+    if nbs > ops.XENT_MAX_BINS:
+        raise ValueError(f"the angle loss kernel takes at most {ops.XENT_MAX_BINS} buckets over the three heads, got {nbs}")
+    _backbone_args(backbone, mask, b, n, theta_logits.device)
+    return (*(_f32c(t) for t in heads), _f32c(backbone), None if mask is None else mask.contiguous(), ii)
+
+
+def _angle_result(losses: torch.Tensor) -> AngleLoss:
+    return AngleLoss(losses[0], losses[1], losses[2])
+
+
+def angle_loss(theta_logits, phi_logits, omega_logits, backbone, mask=None, ignore_index=-100) -> AngleLoss:
+    """The angle heads scored against a true structure in two kernel launches with no host synchronisation: for each head,
+        F.cross_entropy(rearrange(logits, 'b i j c -> b c i j'), labels, ignore_index=ignore_index)
+    with (theta, phi, omega) labels = get_bucketed_angle_matrices(backbone, mask, (their bucket counts), ignore_index), for
+    the logits [b, N, N, nb_h] of Alphafold2(predict_angles=True) (ret.theta_logits, ret.phi_logits, ret.omega_logits; each
+    nb_h >= 2), backbone [b, N, A, 3] and mask [b, N] bool or None.  The F.cross_entropy conventions of distogram_loss hold:
+    the diagonal counts (as no contact), an in-range ignore_index also drops that bucket, NaN when nothing counts.  No label
+    matrix and no softmaxed copy is made: the extra device memory is 48 bytes per (element, row).  Returns an AngleLoss whose
+    .theta, .phi and .omega are 0-d fp32 tensors on the logits' device, reproducible bit for bit and equal to
+    parallel.angle_loss_rows on the same logits sharded by rows."""
+    *heads, x, m, ii = _angle_args(theta_logits, phi_logits, omega_logits, backbone, mask, ignore_index)
+    return _angle_result(ops.angle_xent_finish(ops.angle_xent_rows(*heads, x, m, ii)))

@@ -776,6 +776,31 @@ int af2_distogram_xent_finish(const void* partials, long long parts, float* loss
 int af2_bucketed_distance(const float* coords, int c, const unsigned char* mask, const float* bnd, int B, int n, int nb,
                           long long ignore_index, long long* labels, af2_stream_t stream);
 
+/* Angle-head labels and loss: the trRosetta inter-residue orientations (Yang et al., PNAS 2020) of a true structure as labels
+ * for theta_logits, phi_logits and omega_logits (af2_angle_heads), and each head's cross-entropy against them (DESIGN.md §4f).
+ * backbone [B][n][A][3] fp32, A >= 3, atoms 0, 1, 2 of a residue its N, CA and C; mask [B][n] (1-byte bools) or NULL; nb[3]
+ * (a host array) the bucket counts of theta, phi and omega, each >= 2.  In fp64 on the fp32 atoms, every operation rounded
+ * on its own: the virtual CB = ((-0.58273431 a + 0.56802827 b) - 0.54067466 c) + CA with b = CA - N, c = C - CA, a = b x c;
+ * a contact is i != j with |CB_i - CB_j| <= 20; then theta = dihedral(N_i, CA_i, CB_i, CB_j), omega = dihedral(CA_i, CB_i,
+ * CB_j, CA_j) (the reference's get_dihedral_torch, operation for operation) and phi = atan2(|v x w|, v . w) with v = CA_i -
+ * CB_i, w = CB_j - CB_i.  A head of nb buckets has K = nb - 1 bins: the label is the number of edges below the angle
+ * (torch.bucketize, right = False) among -pi + (k + 1) (2 pi / K) for theta and omega, (k + 1) (pi / K) for phi, with the
+ * last edge pi; no contact (the diagonal, farther pairs, NaN atoms) is nb - 1.  A pair with a masked residue is ignore_index.
+ * af2_angle_xent_rows: one pass over the rows [row0, row0 + rows) of the three heads, each [B][rows][n][nb[h]] fp32 (any
+ *   alignment), nb[0] + nb[1] + nb[2] <= 4096; the per-pair term of af2_distogram_xent_rows per head.  partials [B][rows][3]
+ *   of {double sum; long long count} (48 B per (element, row)), bitwise the same for any split of the rows.  One launch.
+ * af2_angle_xent_finish: loss[h] = the mean term of head h (theta, phi, omega) from parts >= 1 partial triples in row order,
+ *   as af2_distogram_xent_finish sums them; NaN when nothing counts.  One launch.
+ * af2_bucketed_angles: the labels theta, phi, omega, each [B][n][n] int64.  One launch.
+ * Each returns AF2_ERR_BAD_ARG and launches nothing on a null pointer, B or n < 1, A < 3, a head with fewer than 2 buckets
+ * (or more than 4096 in all, for the loss) or rows outside [0, n). */
+int af2_angle_xent_rows(const float* theta, const float* phi, const float* omega, const float* backbone, int A,
+                        const unsigned char* mask, const int* nb, int B, int n, int row0, int rows, long long ignore_index,
+                        void* partials, af2_stream_t stream);
+int af2_angle_xent_finish(const void* partials, long long parts, float* loss, af2_stream_t stream);
+int af2_bucketed_angles(const float* backbone, int A, const unsigned char* mask, const int* nb, int B, int n, long long ignore_index,
+                        long long* theta, long long* phi, long long* omega, af2_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1143,12 +1143,6 @@ def structure_result(ret, coords, confidence, single_msa_repr_row, pairwise_repr
     return coords                                                              # :905 (return_recyclables alone: just coords)
 
 
-def _sharded(model: Alphafold2) -> bool:
-    """Whether parallel.shard_evoformer / shard_alphafold2 replaced a part of model's forward."""
-    return any(getattr(evo, "_af2_sharded", False) for evo in (model.net, model.extra_msa_evoformer)) or \
-        "forward" in model.__dict__ or "embed_templates_" in model.__dict__
-
-
 def recycle(model: Alphafold2, seq, msa=None, *, num_recycles: int = 3, **forward_kwargs):
     """AlphaFold inference with recycling: what the last call of
 
@@ -1165,7 +1159,14 @@ def recycle(model: Alphafold2, seq, msa=None, *, num_recycles: int = 3, **forwar
       * each iteration's recyclables (the pair tensor, the coordinates, the MSA tensor behind single_msa_repr_row) and heads'
         outputs are freed as soon as the next iteration's recycling embedder has read them, so the trunk of that iteration
         runs without a second pair tensor beside it.
-    A sharded model (parallel.shard_evoformer, shard_alphafold2) runs the loop above as written.
+    Sharded models do the same:
+      * under parallel.shard_evoformer(model) the template branch runs whole on every rank, as on one GPU, and the reuse
+        rule above applies on each rank;
+      * under parallel.shard_alphafold2(model), default and pair_rows=True, each rank keeps its rows of every template's pair
+        stack output (parallel.sharded_embed_templates_) when parallel.template_reuse_rows_fits allows it on every rank of the
+        group (the ranks reduce their decisions, so they all take the same branch), and later iterations run only the
+        pointwise attention over the kept rows; the recyclables (in pair_rows mode the rank's pair rows) are freed as above.
+    The decision is kept in model.last_template_reuse.
 
     Refused before any device work: num_recycles < 0, and with num_recycles >= 1: predict_coords=False, return_trunk=True
     (no coordinates to recycle; ValueError) and an unattached structure module (NotImplementedError)."""
@@ -1183,12 +1184,9 @@ def recycle(model: Alphafold2, seq, msa=None, *, num_recycles: int = 3, **forwar
     last_flags = {k: forward_kwargs.pop(k, False) for k in flags}
     inner = dict(return_recyclables=True, return_aux_logits=True)
     rec = forward_kwargs.pop("recyclables", None)
-    if _sharded(model):
-        for _ in range(num_recycles):
-            rec = model(seq, msa, recyclables=rec, **inner, **forward_kwargs)[1].recyclables
-        return model(seq, msa, recyclables=rec, **last_flags, **forward_kwargs)
     held, cache = [rec], {}
     del rec
+    # model._forward is Alphafold2._forward, or sharded_alphafold2_rows under shard_alphafold2(pair_rows=True)
     for _ in range(num_recycles):
         # only `held` references the recyclables: _forward empties it once they are read (the heads' outputs go with the tuple)
         held = [model._forward(seq, msa, owned=held, template_cache=cache, **inner, **forward_kwargs)[1].recyclables]

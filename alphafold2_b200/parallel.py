@@ -814,20 +814,69 @@ def _pair_arena(group, device: torch.device, N: int, d: int):
     return None
 
 
+def sharded_template_pair_stack(model, templates_feats_rows: torch.Tensor, template_mask: torch.Tensor, group, to_cols, to_rows,
+                                ex=None):
+    """The template pair stack (alphafold2.py:751-760) of ONE template over the ranks of `group`: to_template_embed of this rank's
+    rows of the template's features templates_feats_rows [n1 - n0, n, templates_dim] (GEMM rows are independent: bitwise the
+    rows of the whole call), then templates_embed_layers passes of sharded_pair_track (no outer mean, no transition) under the
+    crossed mask of template_mask [n] bool.  Returns (t_row [1, n1 - n0, n, d], the crossed mask's rows [1, n1 - n0, n]), both
+    this rank's rows.  With the peer arena ex, t_row is the arena's row buffer, which the next exchange overwrites.
+    A collective: every rank calls it for the same template."""
+    n = template_mask.shape[0]
+    t_row = _ops.template_embed(model.to_template_embed.packed(), templates_feats_rows.detach().float().contiguous())   # [Rn, n, d]
+    sh = _PairShards(group, n, template_mask[:, None] & template_mask[None, :], to_cols, to_rows)
+    if ex is not None:
+        t_row = ex.buffer(PeerExchange.PAIR, "row").copy_(t_row)
+    ops = CudaStageOps()
+    for _ in range(model.templates_embed_layers):
+        t_row = sharded_pair_track(ops, model.template_pairwise_embedder, t_row, sh)
+    return t_row.contiguous()[None], sh.mask_rows[None]
+
+
+def template_reuse_rows_fits(T: int, rows: int, N: int, d: int, heads: int, dim_head: int, P: int, stack_rows, budget: int,
+                             whole_pair: bool = False) -> bool:
+    """The rows counterpart of ops.template_reuse_fits: whether a rank of shard_alphafold2 may keep its rows of the template
+    pair stack's output across the iterations of recycle(), T pairs (t_row [rows, N, d] fp32, crossed mask rows [rows, N] bool)
+    for its `rows` pair rows.  They must fit `budget` (bytes) beside every sharded stack that runs after the templates, one per
+    entry of stack_rows (its MSA rows: the trunk's, and the extra-MSA stack's when there is one), each counted by
+    pair_rows_bytes.  The structure module on rows needs less than the trunk beside the rows (pair_rows_bytes), so the trunk's
+    count covers it.  whole_pair: the default mode, where every rank also holds the whole fp32 pair tensor and, at a stack's
+    gather, the gathered output: two whole pair tensors more.  The sharded stacks have one plan each (no bands), so a cache that
+    does not fit beside one would make it run out of memory; refusing keeps every stage where it runs without the cache.
+    Ranks differ in rows and free memory: the caller reduces the decisions over the group (sharded_embed_templates_)."""
+    t_bytes = T * rows * N * (4 * d + 1)
+    held = 2 * N * N * d * 4 if whole_pair else 0
+    return all(t_bytes + held + pair_rows_bytes(N, S, d, heads, dim_head, P) <= budget for S in stack_rows)
+
+
+def _all_ranks_agree(ok: bool, device: torch.device, group) -> bool:
+    """ok on every rank of `group` (an all-reduce MIN): the ranks then take the same branch and make the same collectives."""
+    dev = torch.device("cpu") if dist.get_backend(group) == "gloo" else device
+    flag = torch.tensor([1 if ok else 0], dtype=torch.int32, device=dev)
+    dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=group)
+    return bool(flag.item())
+
+
 def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tensor], templates_feats: torch.Tensor,
-                             templates_mask: torch.Tensor, group=None, rows_in: bool = False) -> torch.Tensor:
+                             templates_mask: torch.Tensor, group=None, rows_in: bool = False, cache: Optional[dict] = None,
+                             stack_rows=()) -> torch.Tensor:
     """Alphafold2.embed_templates_ (alphafold2.py:743-785) with the pair work sharded over the ranks of `group`, in place on
     the full fp32 x [1, n, n, d] that every rank holds.  Rank r owns pair rows [n0, n1) = shard_offsets(n, P)[r:r + 2].
 
-    The templates run one at a time, so a rank's memory does not grow with T.  For template k: to_template_embed of this
-    rank's rows of templates_feats[0, k] (GEMM rows are independent: bitwise the rows of the whole call), the crossed mask's
-    row and column shards, templates_embed_layers passes of sharded_pair_track (no outer mean, no transition), then one step
-    of the state-carrying pointwise attention over this rank's pairs (ops.TemplateAttentionGroups on x[0, n0:n1]).  After
-    the last template to_out adds into those rows and an all-gather of the rows gives every rank the full x.  The row <->
-    column exchanges use the peer-memory arena the sharded trunk already holds for (n, d), when there is one (from the
-    second forward on), and NCCL all-to-alls otherwise: both move the same bytes.  Runs eagerly.
+    The templates run one at a time, so a rank's memory does not grow with T.  For template k: sharded_template_pair_stack
+    (the rank's rows of the template's pair stack and of its crossed mask), then one step of the state-carrying pointwise
+    attention over this rank's pairs (ops.TemplateAttentionGroups on x[0, n0:n1]).  After the last template to_out adds into
+    those rows and an all-gather of the rows gives every rank the full x.  The row <-> column exchanges use the peer-memory
+    arena the sharded trunk already holds for (n, d), when there is one (from the second forward on), and NCCL all-to-alls
+    otherwise: both move the same bytes.  Runs eagerly.
     rows_in: x is this rank's pair rows [1, n1 - n0, n, d] (shard_alphafold2(pair_rows=True)); they are updated in place and
-    nothing is gathered."""
+    nothing is gathered.
+    cache: a dict kept across the iterations of recycle(), which share templates_feats and templates_mask (the pair stack reads
+    neither x nor the recyclables).  On the first call the ranks decide together whether to keep the T (t_row, mask rows)
+    pairs: template_reuse_rows_fits on each rank for its rows and 85 % of its ops.device_budget (the planners' headroom), with
+    stack_rows the MSA rows of the later stacks, reduced over the group so that every rank takes the same branch.  When they
+    keep them, later calls run only the pointwise attention over the kept pairs, in the same template order, and the result is
+    bitwise that of running the stack again.  The decision is kept in model.last_template_reuse."""
     attn = model.template_pointwise_attn
     if _ops.precision_of(attn) == "strict":
         raise NotImplementedError("the strict precision mode runs on one GPU (it is a parity mode, not a throughput mode)")
@@ -839,8 +888,6 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
     T, n, d = templates_feats.shape[1], x.shape[2 if rows_in else 1], x.shape[3]
     if n < P:
         raise ValueError(f"N_res={n} is smaller than the number of ranks {P}: every rank needs at least one pair row")
-    ops = CudaStageOps()
-    pair = model.template_pairwise_embedder
     with torch.no_grad():
         on = shard_offsets(n, P)
         r = dist.get_rank(group)
@@ -854,19 +901,27 @@ def sharded_embed_templates_(model, x: torch.Tensor, x_mask: Optional[torch.Tens
             to_cols = lambda t: rows_to_cols(t, group, counts, counts)  # noqa: E731
             to_rows = lambda t: cols_to_rows(t, group, counts, counts)  # noqa: E731
         x_rows = x[0] if rows_in else x[0, n0:n1]                           # a contiguous window of x
+        if cache is not None and "t" not in cache:
+            tri = model.template_pairwise_embedder.triangle_attention_ingoing.attn
+            budget = int(_ops.device_budget(x.device) * 0.85)
+            keep = template_reuse_rows_fits(T, n1 - n0, n, d, tri.heads, tri.dim_head, P, stack_rows, budget, whole_pair=not rows_in)
+            keep = _all_ranks_agree(keep, x.device, group)
+            model.last_template_reuse = keep
+            cache["t"] = [] if keep else None
+        kept = None if cache is None else cache["t"]
         tm = templates_mask[0].bool()
-        embed = model.to_template_embed.packed()
         acc = _ops.TemplateAttentionGroups(attn.packed(), x_rows[None], None if x_mask is None else x_mask[:, n0:n1], attn.heads,
                                            attn.dim_head)
-        for k in range(T):
-            t_row = _ops.template_embed(embed, templates_feats[0, k, n0:n1].detach().float().contiguous())   # [Rn, n, d]
-            sh = _PairShards(group, n, tm[k][:, None] & tm[k][None, :], to_cols, to_rows)                     # crossed mask
-            if ex is not None:
-                t_row = ex.buffer(PeerExchange.PAIR, "row").copy_(t_row)
-            for _ in range(model.templates_embed_layers):
-                t_row = sharded_pair_track(ops, pair, t_row, sh)
-            acc.add(t_row.contiguous()[None], sh.mask_rows[None], last=k == T - 1)
-            del t_row
+        if kept:                                                            # a later iteration of recycle(): the stack is kept
+            for k, (t_row, mask_rows) in enumerate(kept):
+                acc.add(t_row, mask_rows, last=k == T - 1)
+        else:
+            for k in range(T):
+                t_row, mask_rows = sharded_template_pair_stack(model, templates_feats[0, k, n0:n1], tm[k], group, to_cols, to_rows, ex)
+                acc.add(t_row, mask_rows, last=k == T - 1)
+                if kept is not None:                                        # the arena's row buffer is the next template's
+                    kept.append((t_row.clone() if ex is not None else t_row, mask_rows))
+                del t_row
         if not rows_in:
             x[0].copy_(all_gather_cat0(x_rows, group, counts))
     return x
@@ -887,14 +942,19 @@ def shard_alphafold2(model, group=None, use_graph: Optional[bool] = None, pair_r
     def embed_templates_(x, x_mask, templates_feats, templates_mask):
         return sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group)
 
+    def embed_templates_reused_(x, x_mask, templates_feats, templates_mask, cache, stack_rows):
+        return sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group, cache=cache, stack_rows=stack_rows)
+
     model.embed_templates_ = embed_templates_
+    model._embed_templates_reused_ = embed_templates_reused_         # recycle()'s template cache (Alphafold2._forward)
     if pair_rows:
         def forward(*args, **kwargs):
             return sharded_alphafold2_rows(model, group, *args, **kwargs)
 
-        model.forward = forward
+        model.forward = model._forward = forward                     # _forward: recycle() passes its owned / template_cache hooks
     else:
-        model.__dict__.pop("forward", None)              # back to Alphafold2.forward, whatever an earlier call installed
+        for name in ("forward", "_forward"):             # back to Alphafold2's, whatever an earlier call installed
+            model.__dict__.pop(name, None)
     return model
 
 
@@ -984,7 +1044,7 @@ def _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclable
 def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=None, extra_msa=None, extra_msa_mask=None,
                             seq_index=None, seq_embed=None, msa_embed=None, templates_feats=None, templates_mask=None,
                             templates_angles=None, embedds=None, recyclables=None, return_trunk=False, return_confidence=False,
-                            return_recyclables=False, return_aux_logits=False):
+                            return_recyclables=False, return_aux_logits=False, *, owned=None, template_cache=None):
     """Alphafold2.forward of a model under shard_alphafold2(pair_rows=True): every pair-tensor stage runs on this rank's pair rows
     [n0, n1) = shard_offsets(N, P)[r:r + 2] and no rank holds the whole pair tensor.  Pair init rows -> recycling rows ->
     template branch on the rows -> template angles into m -> extra-MSA stack rows -> trunk rows -> one rows -> columns exchange
@@ -992,8 +1052,15 @@ def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=Non
     this rank's rows: ret.distance [1, n1 - n0, N, 37], theta / phi / omega_logits the same rows, ret.pair_rows = (n0, n1).  Each
     is bitwise those rows of the default shard_alphafold2 forward; so are the coordinates and confidence, which are whole.
     The inputs stay replicated (every rank passes the same tensors and reads its rows of them); so does the MSA tensor m.
-    recyclables.pairwise_repr may be the whole [1, N, N, d] or this rank's rows [1, n1 - n0, N, d], as the rows forward returns it."""
-    from .alphafold2 import ReturnValues, _forward_only
+    recyclables.pairwise_repr may be the whole [1, N, N, d] or this rank's rows [1, n1 - n0, N, d], as the rows forward returns it.
+    owned, template_cache: the hooks of recycle(), as in Alphafold2._forward.  owned is a one-element list [recyclables] whose
+    tensors the caller references nowhere else: it is emptied before this iteration's x and m exist, after a copy of
+    single_msa_repr_row, and the pair rows and coordinates are dropped once the recycling embedder has read them, before the
+    templates, the extra-MSA stack and the trunk run.  None of them is an input of a captured graph (_GraphedTrunk holds only
+    the x and m of its own forward).  template_cache: sharded_embed_templates_'s cache."""
+    from .alphafold2 import Recyclables, ReturnValues, _forward_only
+    if owned is not None:
+        recyclables = owned[0]
     _rows_refusals(model, group, seq, msa, extra_msa, extra_msa_mask, recyclables, return_trunk)
     model._check_inputs(seq, mask, seq_embed, msa_embed, embedds, templates_feats, templates_mask, templates_angles, None)
     P, r, N = dist.get_world_size(group), dist.get_rank(group), seq.shape[1]
@@ -1002,6 +1069,9 @@ def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=Non
     if recyclables is not None:
         _forward_only(*model._check_recyclables(1, N, seq.device, recyclables, pair_rows=n1 - n0))
     with torch.no_grad():
+        if owned is not None and recyclables is not None:
+            recyclables = Recyclables(recyclables.coords, recyclables.single_msa_repr_row.clone(), recyclables.pairwise_repr)
+            owned.clear()
         if msa is None:                                                # alphafold2.py:656-658
             msa = seq[:, None, :]
             msa_mask = mask[:, None, :] if mask is not None else None
@@ -1014,8 +1084,12 @@ def sharded_alphafold2_rows(model, group, seq, msa=None, mask=None, msa_mask=Non
         x_mask = (mask[:, :, None] & mask[:, None, :]) if mask is not None else None
         if recyclables is not None:
             model.embed_recyclables_(x, m, recyclables, row0=n0)
+            if owned is not None:
+                recyclables = None
         if templates_feats is not None:
-            sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group, rows_in=True)
+            stack_rows = (m.shape[1],) + ((msa.shape[1],) if extra_msa is not None else ())
+            sharded_embed_templates_(model, x, x_mask, templates_feats, templates_mask, group, rows_in=True, cache=template_cache,
+                                     stack_rows=stack_rows)
         if templates_angles is not None:
             msa_mask = model.embed_template_angles_(m, msa_mask, templates_angles, templates_mask)
         if extra_msa is not None:

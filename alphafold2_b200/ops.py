@@ -74,11 +74,14 @@ def _require(t: torch.Tensor, dtype, name: str):
 
 
 _WS_PRIVATE = None        # (dict device -> tensor, locked) while a CUDA graph owner captures (parallel._GraphedTrunk)
+_WS_CAPTURED: Dict[int, torch.Tensor] = {}     # shared workspaces handed out during a caller's CUDA-graph capture, by address
 
 
 def workspace(nbytes: int, device) -> torch.Tensor:
     """Grow-only per-device scratch buffer, reused by every op (ops on one stream are serialised).  Inside a
-    `private_workspace` scope the buffer belongs to the scope's owner (a captured CUDA graph keeps raw pointers into it)."""
+    `private_workspace` scope the buffer belongs to the scope's owner (a captured CUDA graph keeps raw pointers into it).
+    A shared buffer handed out while the current stream is capturing a CUDA graph is retained: growth and release_workspace
+    drop it from the store but do not free it, since the graph replays into it; release_captured_workspaces() frees it."""
     device = torch.device(device)
     store, locked = (_WORKSPACE, False) if _WS_PRIVATE is None else _WS_PRIVATE
     buf = store.get(device)
@@ -89,7 +92,17 @@ def workspace(nbytes: int, device) -> torch.Tensor:
         store.pop(device, None)
         buf = torch.empty(int(nbytes * 1.05) + 4096, dtype=torch.uint8, device=device)
         store[device] = buf
+    if store is _WORKSPACE and torch.cuda.is_current_stream_capturing():
+        _WS_CAPTURED[buf.data_ptr()] = buf
     return buf
+
+
+def release_captured_workspaces() -> None:
+    """Free the shared workspace buffers that ops used while a caller captured them in a CUDA graph (see workspace).  Call it
+    once the graphs that captured ops are dropped; a graph replayed after this call reads and writes freed memory."""
+    _WS_CAPTURED.clear()
+    if torch.cuda.is_available():
+        torch.cuda.empty_cache()
 
 
 class private_workspace:
@@ -1347,9 +1360,10 @@ def release_workspace(device) -> None:
     """Drop the grow-only workspace of `device` and return its memory to the driver, so that tensors which outlive single ops
     can use it; the next op allocates a workspace of the size it needs.  device_budget counts the workspace as available,
     which holds only once it is released (a workspace left at the trunk's whole-tensor size by an earlier forward would
-    otherwise stay beside them).  A no-op inside a locked private_workspace scope."""
+    otherwise stay beside them).  A no-op inside a locked private_workspace scope.  A buffer that a CUDA-graph capture used
+    stays allocated (workspace); while the current stream is capturing, nothing is returned to the driver."""
     store, locked = (_WORKSPACE, False) if _WS_PRIVATE is None else _WS_PRIVATE
-    if not locked and store.pop(torch.device(device), None) is not None:
+    if not locked and store.pop(torch.device(device), None) is not None and not torch.cuda.is_current_stream_capturing():
         torch.cuda.empty_cache()
 
 

@@ -741,8 +741,8 @@ class _GraphedTrunk:
                 _ops.pack_epoch(), _ops.precision_of(self.evo))
 
     def __call__(self, x, m, mask=None, msa_mask=None, rows_in=False):
-        if not GRAPH_ENABLED or self.failed is not None or not x.is_cuda:
-            return self._eager(x, m, mask, msa_mask, rows_in)
+        if not GRAPH_ENABLED or self.failed is not None or not x.is_cuda or _ops.precision_of(self.evo) == "strict":
+            return self._eager(x, m, mask, msa_mask, rows_in)       # strict: the eager schedule refuses it before any capture
         key = (tuple(x.shape), tuple(m.shape), x.dtype, m.dtype, None if mask is None else tuple(mask.shape),
                None if msa_mask is None else tuple(msa_mask.shape), x.device, self._weights_key(), rows_in)
         if key != self.key:
